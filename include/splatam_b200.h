@@ -44,7 +44,7 @@ extern "C" {
 #define SB_API
 #endif
 
-#define SB_ABI_VERSION 2
+#define SB_ABI_VERSION 3
 #define SB_TILE 16 /* BLOCK_X == BLOCK_Y == 16, X/cuda_rasterizer/config.h:16-17 (part of the key contract) */
 #define SB_CHANNELS 3 /* NUM_CHANNELS, X/cuda_rasterizer/config.h:15 */
 
@@ -235,14 +235,6 @@ SB_API size_t sb_adam_clock_bytes(void);
 SB_API int sb_adam_step_guarded(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, size_t n,
                                 const uint32_t* seg_end, const double* seg_lr, int num_segments, void* clock_dev,
                                 const float* skip_if_nonzero, double beta1, double beta2, double eps, void* stream);
-/* The two halves of sb_adam_step_guarded for a step applied in chunks (each chunk after its slice of the gradient
- * all-reduce has landed, so the update of chunk k overlaps the transfer of chunk k+1): advance the clock once per step,
- * then apply the update to the element range [first, first + count) of the flat buffers. */
-SB_API int sb_adam_clock_advance(const double* seg_lr, int num_segments, void* clock_dev, const float* skip_if_nonzero,
-                                 double beta1, double beta2, void* stream);
-SB_API int sb_adam_apply_guarded(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, size_t first,
-                                 size_t count, const uint32_t* seg_end, int num_segments, const void* clock_dev,
-                                 const float* skip_if_nonzero, double beta1, double beta2, double eps, void* stream);
 SB_API size_t sb_image_loss_workspace_floats(int C, int H, int W);
 SB_API int sb_image_loss_forward(const float* x, const float* y, int C, int H, int W, float* work,
                                  double* sums, void* stream);

@@ -70,9 +70,6 @@ _SIGNATURES = {
     "sb_adam_clock_bytes": (_sz, []),
     "sb_adam_step_guarded": (_i, [_vp, _vp, _vp, _vp, _sz, ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_double),
                                   _i, _vp, _vp, ctypes.c_double, ctypes.c_double, ctypes.c_double, _vp]),
-    "sb_adam_clock_advance": (_i, [ctypes.POINTER(ctypes.c_double), _i, _vp, _vp, ctypes.c_double, ctypes.c_double, _vp]),
-    "sb_adam_apply_guarded": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, ctypes.POINTER(ctypes.c_uint32), _i, _vp, _vp,
-                                   ctypes.c_double, ctypes.c_double, ctypes.c_double, _vp]),
     "sb_image_loss_workspace_floats": (_sz, [_i, _i, _i]),
     "sb_image_loss_forward": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "sb_image_loss_backward": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, ctypes.c_float, ctypes.c_float, _vp, _vp]),
@@ -115,7 +112,7 @@ def load():
         fn = getattr(lib, name)  # AttributeError if a declared symbol is not exported
         fn.restype = restype
         fn.argtypes = argtypes
-    if lib.sb_abi_version() != 2:
+    if lib.sb_abi_version() != 3:
         raise SplatamB200Error("libsplatam_b200.so ABI version mismatch")
     _lib = lib
     return lib

@@ -346,40 +346,6 @@ static GaussWin gauss_window() {
     return g;
 }
 
-/* The two halves of sb_adam_step_guarded, for a step whose update is applied in CHUNKS (each chunk after its slice of the
- * all-reduce has landed): sb_adam_clock_advance once per step, then sb_adam_apply_guarded per chunk with the chunk's
- * element range [first, first + count) of the flat buffers. */
-SB_API int sb_adam_clock_advance(const double* seg_lr, int num_segments, void* clock_dev, const float* skip_if_nonzero,
-                                 double beta1, double beta2, void* stream) {
-    if (!seg_lr || !clock_dev || num_segments < 1 || num_segments > kMaxSeg) return SB_ERR_BAD_ARG;
-    AdamLrs lrs;
-    lrs.n = num_segments;
-    for (int k = 0; k < num_segments; ++k) lrs.lr[k] = seg_lr[k];
-    adam_clock_kernel<<<1, 1, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<AdamClock*>(clock_dev), skip_if_nonzero,
-                                                                      lrs, beta1, beta2);
-    SB_LAUNCH_CHECK("adam_clock_kernel");
-    return SB_OK;
-}
-
-SB_API int sb_adam_apply_guarded(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, size_t first,
-                                 size_t count, const uint32_t* seg_end, int num_segments, const void* clock_dev,
-                                 const float* skip_if_nonzero, double beta1, double beta2, double eps, void* stream) {
-    if (!params || !grads || !exp_avg || !exp_avg_sq || !seg_end || !clock_dev || num_segments < 1 || num_segments > kMaxSeg)
-        return SB_ERR_BAD_ARG;
-    if (count == 0) return SB_OK;
-    AdamSegs segs;                 // segment ends relative to the chunk's first element
-    segs.n = num_segments;
-    for (int k = 0; k < num_segments; ++k) {
-        segs.end[k] = seg_end[k] > first ? (uint32_t)(seg_end[k] - first) : 0u;
-        segs.lr[k] = 0.f;
-    }
-    adam_kernel<true><<<(unsigned)((count + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        params + first, grads + first, exp_avg + first, exp_avg_sq + first, count, segs, (float)(1.0 - beta1), (float)beta2,
-        (float)(1.0 - beta2), (float)eps, 0.f, static_cast<const AdamClock*>(clock_dev), skip_if_nonzero);
-    SB_LAUNCH_CHECK("adam_kernel");
-    return SB_OK;
-}
-
 SB_API size_t sb_image_loss_workspace_floats(int C, int H, int W) { return (size_t)3 * C * H * W; }
 
 /* loss terms of  w_l1*mean|x-y| + w_ssim*(1-mean(SSIM(x,y))) : writes sums[0]=sum(ssim map), sums[1]=sum|x-y|

@@ -39,16 +39,28 @@ def quat_mult(q1, q2):
                         w1 * y2 - x1 * z2 + y1 * w2 + z1 * x2, w1 * z2 + x1 * y2 - y1 * x2 + z1 * w2]).T
 
 
-def transform_to_frame(params, time_idx, gaussians_grad, camera_grad):
-    """World -> camera-frame Gaussians for frame `time_idx` (R/utils/slam_helpers.py:252-304)."""
+def camera_w2c(rot, tran):
+    """(rel_w2c [4,4], normalised camera quaternion [1,4]) of an unnormalised camera quaternion [1,4] and a
+    translation [1,3] (R/utils/slam_helpers.py:266-275)."""
+    cam_rot = F.normalize(rot)
+    rel_w2c = torch.eye(4, device=rot.device, dtype=torch.float32)
+    rel_w2c[:3, :3] = build_rotation(cam_rot)
+    rel_w2c[:3, 3] = tran
+    return rel_w2c, cam_rot
+
+
+def pose_matrices(params, time_idx, camera_grad=False):
+    """camera_w2c of frame `time_idx`; the pose gets gradient only if `camera_grad`."""
     rot, tran = params["cam_unnorm_rots"][..., time_idx], params["cam_trans"][..., time_idx]
     if not camera_grad:
         rot, tran = rot.detach(), tran.detach()
-    cam_rot = F.normalize(rot)
+    return camera_w2c(rot, tran)
+
+
+def transform_to_frame(params, time_idx, gaussians_grad, camera_grad):
+    """World -> camera-frame Gaussians for frame `time_idx` (R/utils/slam_helpers.py:252-304)."""
+    rel_w2c, cam_rot = pose_matrices(params, time_idx, camera_grad)
     dev = params["means3D"].device
-    rel_w2c = torch.eye(4, device=dev, dtype=torch.float32)
-    rel_w2c[:3, :3] = build_rotation(cam_rot)
-    rel_w2c[:3, 3] = tran
     pts, unnorm = params["means3D"], params["unnorm_rotations"]
     if not gaussians_grad:
         pts, unnorm = pts.detach(), unnorm.detach()
@@ -115,30 +127,11 @@ def fused_pose_cached(params, time_idx):
     return hit
 
 
-def _last_num_rendered():
-    from . import rasterizer
-    return rasterizer._LAST_SYNC_R[0]
-
-
-def pose_matrices(params, time_idx, camera_grad=False):
-    """(rel_w2c [4,4], normalised camera quaternion [1,4]) of frame `time_idx` (slam_helpers.py:266-275)."""
-    rot, tran = params["cam_unnorm_rots"][..., time_idx], params["cam_trans"][..., time_idx]
-    if not camera_grad:
-        rot, tran = rot.detach(), tran.detach()
-    cam_rot = F.normalize(rot)
-    rel_w2c = torch.eye(4, device=params["means3D"].device, dtype=torch.float32)
-    rel_w2c[:3, :3] = build_rotation(cam_rot)
-    rel_w2c[:3, 3] = tran
-    return rel_w2c, cam_rot
-
-
 def fused_rendervars(params, time_idx, w2c0, camera_grad, pose=None):
     """Both rendervars of one frame from ONE fused kernel (splatam_b200/prepare.py); equals
     transform_to_frame + rgb_rendervar + depth_sil_rendervar above to float rounding.  `pose` = precomputed
     (rel_w2c, cam_rot) tensors (the CUDA-graph path keeps them in static buffers)."""
     from .prepare import prepare_gaussians
-    rots_all, trans_all = params["cam_unnorm_rots"], params["cam_trans"]
-    dev = params["means3D"].device
     if pose is not None:
         rel_w2c, cam_rot = pose
     elif not camera_grad:     # poses are constants of the mapping loop: build each frame's matrix once
@@ -174,22 +167,17 @@ def calc_ssim(img1, img2, window_size=11):
     return (((2 * mu12 + c1) * (2 * s12 + c2)) / ((mu1_sq + mu2_sq + c1) * (s1 + s2 + c2))).mean()
 
 
-def mapping_loss(params, frame, render, loss_weights=(0.5, 1.0), ignore_outlier_depth_loss=False, fused_loss=False,
-                 max_rendered=None, keep=None):
-    """SplaTAM get_loss(mapping=True): Gaussians get gradient, camera does not
-    (R/scripts/splatam.py:214-347 with tracking=False, mapping=True, do_ba=False, use_l1=True).
-    frame: dict(im [3,H,W], depth [1,H,W], cam settings, w2c [4,4] first-frame w2c, id time index).
-    render(settings, **rendervar) -> (image, radii, depth)."""
-    if fused_loss:      # fused glue: one kernel builds both rendervars (csrc/prepare.cu)
-        rv_rgb, rv_depth = fused_rendervars(params, frame["id"], frame["w2c"], camera_grad=False,
-                                            pose=frame.get("pose"))
+def _render_pair(params, frame, render, fused, camera_grad, max_rendered=None):
+    """The RGB and depth/silhouette renders of `frame` -> (image, depth_sil, radii, means2D of the RGB render).  Either
+    the Gaussians get gradient or, with `camera_grad`, only the camera pose.  fused: one kernel builds both rendervars
+    (csrc/prepare.cu) from frame["pose"] if given, and the product rasterizer blends both colour sets in one pass (N1),
+    with a fixed instance capacity if `max_rendered`; otherwise the PyTorch glue and two `render` calls."""
+    if fused:
+        rv_rgb, rv_depth = fused_rendervars(params, frame["id"], frame["w2c"], camera_grad, pose=frame.get("pose"))
     else:
-        tg = transform_to_frame(params, frame["id"], gaussians_grad=True, camera_grad=False)
+        tg = transform_to_frame(params, frame["id"], gaussians_grad=not camera_grad, camera_grad=camera_grad)
         rv_rgb, rv_depth = rgb_rendervar(params, tg), depth_sil_rendervar(params, frame["w2c"], tg)
-    if keep is not None:       # the caller wants d loss / d means2D of the RGB render (densification statistic)
-        rv_rgb["means2D"].retain_grad()
-        keep["means2D"] = rv_rgb["means2D"]
-    if fused_loss and render is default_render:      # N1: both colour sets in one raster pass
+    if fused and render is default_render:
         from .rasterizer import GaussianRasterizer
         im, depth_sil, radius, _ = GaussianRasterizer(raster_settings=frame["cam"], max_rendered=max_rendered).forward_fused(
             means3D=rv_rgb["means3D"], means2D=rv_rgb["means2D"], opacities=rv_rgb["opacities"],
@@ -198,6 +186,33 @@ def mapping_loss(params, frame, render, loss_weights=(0.5, 1.0), ignore_outlier_
     else:
         im, radius, _ = render(frame["cam"], **rv_rgb)
         depth_sil, _, _ = render(frame["cam"], **rv_depth)
+    return im, depth_sil, radius, rv_rgb["means2D"]
+
+
+def _capacity(params, frames, slack):
+    """Instance capacity of the sync-free rasterizer for renders like those of `frames`: one synchronous forward per
+    frame, slack x the largest num_rendered, plus 4096."""
+    from . import rasterizer
+    worst = 0
+    for fr in frames:
+        with torch.no_grad():
+            rgb, _ = fused_rendervars(params, fr["id"], fr["w2c"], camera_grad=False)
+            rasterizer.GaussianRasterizer(fr["cam"])(**rgb)
+        worst = max(worst, rasterizer._LAST_SYNC_R[0])
+    return int(worst * slack) + 4096
+
+
+def mapping_loss(params, frame, render, loss_weights=(0.5, 1.0), ignore_outlier_depth_loss=False, fused_loss=False,
+                 max_rendered=None, keep=None):
+    """SplaTAM get_loss(mapping=True): Gaussians get gradient, camera does not
+    (R/scripts/splatam.py:214-347 with tracking=False, mapping=True, do_ba=False, use_l1=True).
+    frame: dict(im [3,H,W], depth [1,H,W], cam settings, w2c [4,4] first-frame w2c, id time index).
+    render(settings, **rendervar) -> (image, radii, depth)."""
+    im, depth_sil, radius, means2D = _render_pair(params, frame, render, fused_loss, camera_grad=False,
+                                                  max_rendered=max_rendered)
+    if keep is not None:       # the caller wants d loss / d means2D of the RGB render (densification statistic)
+        means2D.retain_grad()
+        keep["means2D"] = means2D
     if fused_loss and not ignore_outlier_depth_loss:
         from .train_ops import masked_l1        # validity-masked mean |gt - depth| in one kernel (+ one backward)
         l_depth, _ = masked_l1(depth_sil, frame["depth"], depth_mean=True)
@@ -218,24 +233,11 @@ def mapping_loss(params, frame, render, loss_weights=(0.5, 1.0), ignore_outlier_
     return loss_weights[0] * l_im + loss_weights[1] * l_depth, radius
 
 
-def tracking_loss(params, frame, render, sil_thres=0.99, loss_weights=(0.5, 1.0), fused=False):
+def tracking_loss(params, frame, render, sil_thres=0.99, loss_weights=(0.5, 1.0), fused=False, max_rendered=None):
     """SplaTAM get_loss(tracking=True, use_sil_for_loss=True, use_l1=True): only the camera pose of frame
     `frame["id"]` gets gradient; L1 sums over pixels with silhouette > sil_thres and valid depth
     (R/scripts/splatam.py:220-224,254-288; weights R/configs/replica/splatam.py:65-68)."""
-    if fused:
-        rv_rgb, rv_depth = fused_rendervars(params, frame["id"], frame["w2c"], camera_grad=True)
-    else:
-        tg = transform_to_frame(params, frame["id"], gaussians_grad=False, camera_grad=True)
-        rv_rgb, rv_depth = rgb_rendervar(params, tg), depth_sil_rendervar(params, frame["w2c"], tg)
-    if fused and render is default_render:
-        from .rasterizer import GaussianRasterizer
-        im, depth_sil, radius, _ = GaussianRasterizer(raster_settings=frame["cam"]).forward_fused(
-            means3D=rv_rgb["means3D"], means2D=rv_rgb["means2D"], opacities=rv_rgb["opacities"],
-            colors_precomp=rv_rgb["colors_precomp"], colors_extra=rv_depth["colors_precomp"],
-            scales=rv_rgb["scales"], rotations=rv_rgb["rotations"])
-    else:
-        im, radius, _ = render(frame["cam"], **rv_rgb)
-        depth_sil, _, _ = render(frame["cam"], **rv_depth)
+    im, depth_sil, radius, _ = _render_pair(params, frame, render, fused, camera_grad=True, max_rendered=max_rendered)
     if fused:
         from .train_ops import masked_l1
         l_depth, l_im = masked_l1(depth_sil, frame["depth"], im, frame["im"], sil_thres=sil_thres, use_sil=True,
@@ -314,7 +316,6 @@ class _TrackingGraph:
 
     def __init__(self, params, frame, num_iters, lr_rot, lr_trans, slack=1.5):
         from .rasterizer import GaussianRasterizer
-        from .train_ops import masked_l1
         dev = params["means3D"].device
         self.dev, self.t, self.num_iters = dev, frame["id"], num_iters
         t = frame["id"]
@@ -322,16 +323,12 @@ class _TrackingGraph:
         self.gp = dict({k: params[k].detach() for k in GAUSSIAN_KEYS}, cam_unnorm_rots=rots.detach(), cam_trans=trans.detach())
         self.key = _tracking_key(params, frame, num_iters)
         gp = self.gp
-        with torch.no_grad():       # one synchronous forward at the starting pose sizes the capacity
-            rgb, _ = fused_rendervars(gp, t, frame["w2c"], camera_grad=False, pose=pose_matrices(gp, t))
-            GaussianRasterizer(frame["cam"])(means3D=rgb["means3D"], means2D=rgb["means2D"], opacities=rgb["opacities"],
-                                             colors_precomp=rgb["colors_precomp"], scales=rgb["scales"],
-                                             rotations=rgb["rotations"])
-        cap = int(_last_num_rendered() * slack) + 4096
+        cap = _capacity(gp, [frame], slack)         # sized at the starting pose
         self.side = torch.cuda.Stream(dev)
         self.side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(self.side):
             self.im, self.depth, self.w2c = frame["im"].clone(), frame["depth"].clone(), frame["w2c"].clone()
+            static = dict(id=t, cam=frame["cam"], w2c=self.w2c, im=self.im, depth=self.depth)
             self.q = rots[..., t].detach().clone().requires_grad_(True)      # [1,4], [1,3]: leaves born on the capture stream
             self.tr = trans[..., t].detach().clone().requires_grad_(True)
             q, tr = self.q, self.tr
@@ -343,21 +340,11 @@ class _TrackingGraph:
             self.hist = torch.zeros(num_iters, device=dev)
             self.it = torch.zeros(1, dtype=torch.long, device=dev)
             self.bad_any = torch.zeros(1, device=dev)
-            cam = frame["cam"]
 
             def body():
                 q.grad.zero_(); tr.grad.zero_()
-                cam_rot = F.normalize(q)
-                rel = torch.eye(4, device=dev, dtype=torch.float32)
-                rel[:3, :3] = build_rotation(cam_rot)
-                rel[:3, 3] = tr
-                rgb, dep = fused_rendervars(gp, t, self.w2c, camera_grad=True, pose=(rel, cam_rot))
-                im, depth_sil, _, _ = GaussianRasterizer(cam, max_rendered=cap).forward_fused(
-                    means3D=rgb["means3D"], means2D=rgb["means2D"], opacities=rgb["opacities"],
-                    colors_precomp=rgb["colors_precomp"], colors_extra=dep["colors_precomp"], scales=rgb["scales"],
-                    rotations=rgb["rotations"])
-                l_depth, l_im = masked_l1(depth_sil, self.depth, im, self.im, sil_thres=0.99, use_sil=True, depth_mean=False)
-                loss = 0.5 * l_im + 1.0 * l_depth
+                loss, _ = tracking_loss(gp, dict(static, pose=camera_w2c(q, tr)), default_render, fused=True,
+                                        max_rendered=cap)
                 loss.backward()
                 lossd = loss.detach().reshape(1)
                 bad = (GaussianRasterizer.last_state(dev).header()[2:3] != 0) | ~torch.isfinite(lossd)
@@ -448,14 +435,21 @@ class FlatGaussians:
         self.seen_f = self.bucket[n:n + P_]
         self.loss_slot = self.bucket[n + P_:n + P_ + 1]
         self.overflow_slot = self.bucket[n + P_ + 1:]
-        self.params, off = {}, 0
+        self.params, grads = self.views(self.flat), self.views(self.flat_grad)
+        for k, p in self.params.items():
+            p.copy_(tensors[k].detach().reshape(self.shapes[k]))
+            p.requires_grad_(True)
+            p.grad = grads[k]                   # autograd accumulates in place
+
+    def views(self, buf):
+        """{key: view of the key's segment of `buf`}, for any flat buffer of this layout (parameters, gradients, Adam
+        moments)."""
+        out, off = {}, 0
         for k in GAUSSIAN_KEYS:
             m = math.prod(self.shapes[k])
-            self.flat[off:off + m].copy_(tensors[k].detach().reshape(-1))
-            p = self.flat[off:off + m].view(self.shapes[k]).requires_grad_(True)
-            p.grad = self.flat_grad[off:off + m].view(self.shapes[k])   # autograd accumulates in place
-            self.params[k] = p
+            out[k] = buf[off:off + m].view(self.shapes[k])
             off += m
+        return out
 
     def zero_grad(self):
         self.bucket.zero_()
@@ -473,7 +467,9 @@ class ShardedMapper:
                        log_scales=0.001)
 
     def __init__(self, gaussians, cam_unnorm_rots, cam_trans, lrs=None, render=default_render, group=None, seed=0,
-                 fused=None):
+                 fused=None, track_means2D=False):
+        """track_means2D: keep d loss / d means2D of every eager step's RGB render and which Gaussians it saw (the
+        statistic of `densify`)."""
         import torch.distributed as dist
         self.dist = dist if (dist.is_available() and dist.is_initialized()) else None
         self.group = group
@@ -490,10 +486,15 @@ class ShardedMapper:
         self.render = render
         self.gen = torch.Generator().manual_seed(seed)   # shared seed -> identical schedule on every rank
         self.step_idx = 0
-        # graph mode, world > 1: the bucket is all-reduced in this many slices, the guarded Adam update of slice k
-        # overlapping the transfer of slice k+1 (1 = one collective, then one Adam launch)
-        import os as _os
-        self.overlap_chunks = int(_os.environ.get("SPLATAM_OVERLAP_CHUNKS", "1"))
+        self.track_means2D = bool(track_means2D)
+        self.last_means2D_grad = self.last_seen_local = None
+        self._dens = None                   # densification statistic: dict(accum, denom) per Gaussian
+        self._dev_gen = None                # shared-seed device generator of the split samples (world > 1)
+        # CUDA-graph mode (enable_graph): captured step, its static frame buffers, instance capacity, in-flight polls
+        self._graph = self._static = None
+        self._cap, self._slack = 0, 1.3
+        self._polls, self._pin = [], []
+        self.overflow_events = 0
 
     def params(self):
         return dict(self.g.params, **self.cam)
@@ -521,14 +522,30 @@ class ShardedMapper:
 
     # ---- map maintenance (prune / grow); every rank applies the same deterministic edit --------------------------
     def _make_optimizer(self, m=None, v=None, t=0):
+        """Adam over the current map whose two moments live in flat buffers of the parameter layout (zero by default)
+        and which has taken `t` steps."""
+        self.exp_avg = torch.zeros_like(self.g.flat) if m is None else m
+        self.exp_avg_sq = torch.zeros_like(self.g.flat) if v is None else v
         if self.fused:
             from .train_ops import FusedAdam
             sizes = [math.prod(self.g.shapes[k]) for k in GAUSSIAN_KEYS]
             self.opt = FusedAdam(self.g.flat, self.g.flat_grad, sizes, [self.lrs[k] for k in GAUSSIAN_KEYS], eps=1e-15,
-                                 exp_avg=m, exp_avg_sq=v, step=t)
+                                 exp_avg=self.exp_avg, exp_avg_sq=self.exp_avg_sq, step=t)
         else:
             self.opt = torch.optim.Adam([{"params": [self.g.params[k]], "name": k, "lr": self.lrs[k]}
                                          for k in GAUSSIAN_KEYS], lr=0.0, eps=1e-15)
+            for k, (mk, vk) in self.moments().items():    # the state torch.optim.Adam would create, on our buffers
+                self.opt.state[self.g.params[k]] = dict(step=torch.tensor(float(t)), exp_avg=mk, exp_avg_sq=vk)
+
+    def moments(self):
+        """{key: (exp_avg, exp_avg_sq)}: the Adam moments of each parameter tensor, for either optimizer."""
+        m, v = self.g.views(self.exp_avg), self.g.views(self.exp_avg_sq)
+        return {k: (m[k], v[k]) for k in GAUSSIAN_KEYS}
+
+    def _adam_steps(self):
+        if self.fused:
+            return self.opt.applied_steps()[0]
+        return int(self.opt.state[self.g.params["means3D"]]["step"])
 
     def reset_optimizer(self):
         """Fresh Adam state, as the reference re-creates its optimizer at the start of every frame's mapping
@@ -538,16 +555,15 @@ class ShardedMapper:
     def _widths(self):
         return [self.g.shapes[k][1] if len(self.g.shapes[k]) > 1 else 1 for k in GAUSSIAN_KEYS]
 
-    def _rebuild(self, flat, P_new, m=None, v=None, t=0, state=None):
+    def _rebuild(self, flat, P_new, m, v, t):
+        """The map becomes `P_new` rows: parameters `flat` and Adam moments `m`, `v` (flat buffers of the packed layout)
+        after `t` Adam steps."""
         tensors, off = {}, 0
         for k, w in zip(GAUSSIAN_KEYS, self._widths()):
             tensors[k] = flat[off:off + w * P_new].view(P_new, w)
             off += w * P_new
         self.g = FlatGaussians(tensors)
         self._make_optimizer(m, v, t)
-        if state is not None:                   # torch.optim path: carry the moments over
-            for k in GAUSSIAN_KEYS:
-                self.opt.state[self.g.params[k]] = state[k]
         self._graph = None                      # shapes changed: a captured graph is stale
 
     def remove_points(self, to_remove):
@@ -555,28 +571,24 @@ class ShardedMapper:
         (remove_points, R/utils/slam_external.py:144-167).  Returns the number of Gaussians kept."""
         P = self.g.shapes["means3D"][0]
         keep = ~to_remove.reshape(-1).bool()
-        if self.fused:
+        if self.fused:              # stream compaction kernels (csrc/map_ops.cu)
             from . import map_ops
             m8, dst, P_new = map_ops.compact_plan(keep)
-            if P_new == P:
-                return P
-            w = self._widths()
-            flat = map_ops.compact_flat(self.g.flat, P, w, m8, dst, P_new)
-            m = map_ops.compact_flat(self.opt.m, P, w, m8, dst, P_new)
-            v = map_ops.compact_flat(self.opt.v, P, w, m8, dst, P_new)
-            self._rebuild(flat, P_new, m, v, self.opt.applied_steps()[0])
-            return P_new
-        P_new = int(keep.sum())
+            compact = lambda buf: map_ops.compact_flat(buf, P, self._widths(), m8, dst, P_new)
+        else:
+            P_new = int(keep.sum())
+            compact = lambda buf: torch.cat([x[keep].reshape(-1) for x in self.g.views(buf).values()])
         if P_new == P:
             return P
-        state = {}
-        for k in GAUSSIAN_KEYS:
-            st = self.opt.state.get(self.g.params[k], None)
-            state[k] = {} if not st else dict(step=st["step"], exp_avg=st["exp_avg"][keep].clone(),
-                                              exp_avg_sq=st["exp_avg_sq"][keep].clone())
-        flat = torch.cat([self.g.params[k].detach()[keep].reshape(-1) for k in GAUSSIAN_KEYS])
-        self._rebuild(flat, P_new, state={k: s for k, s in state.items() if s} or None)
+        self._rebuild(compact(self.g.flat), P_new, compact(self.exp_avg), compact(self.exp_avg_sq), self._adam_steps())
         return P_new
+
+    def _reset_opacities(self):
+        """Every opacity to 0.01 (inverse_sigmoid(0.01)), its Adam moments to zero (R/utils/slam_external.py:184-186)."""
+        with torch.no_grad():
+            self.g.params["logit_opacities"].fill_(math.log(0.01 / 0.99))
+        for mom in self.moments()["logit_opacities"]:
+            mom.zero_()
 
     def prune_gaussians(self, iter, prune_dict, scene_radius):
         """prune_gaussians of the reference (R/utils/slam_external.py:170-197): same schedule keys
@@ -600,15 +612,7 @@ class ShardedMapper:
                 keep = ~remove
             P = self.remove_points(~keep)
         if iter > 0 and iter % prune_dict["reset_opacities_every"] == 0 and prune_dict["reset_opacities"]:
-            with torch.no_grad():                                  # inverse_sigmoid(0.01), moments zeroed
-                self.g.params["logit_opacities"].fill_(math.log(0.01 / 0.99))
-            if self.fused:
-                off = sum(math.prod(self.g.shapes[k]) for k in GAUSSIAN_KEYS[:3])
-                self.opt.m[off:off + P].zero_(); self.opt.v[off:off + P].zero_()
-            else:
-                st = self.opt.state.get(self.g.params["logit_opacities"], None)
-                if st:
-                    st["exp_avg"].zero_(); st["exp_avg_sq"].zero_()
+            self._reset_opacities()
         return P
 
     def add_gaussians(self, new):
@@ -618,25 +622,12 @@ class ShardedMapper:
         if n_new == 0:
             return P
         dev = self.g.flat.device
-        flat = torch.cat([torch.cat([self.g.params[k].detach(), new[k].to(dev).float().reshape(n_new, -1)], 0).reshape(-1)
-                          for k in GAUSSIAN_KEYS])
-        if self.fused:
-            def grown(buf):
-                parts, off = [], 0
-                for k, w in zip(GAUSSIAN_KEYS, self._widths()):
-                    parts += [buf[off:off + w * P], torch.zeros(w * n_new, device=dev)]
-                    off += w * P
-                return torch.cat(parts)
-            self._rebuild(flat, P + n_new, grown(self.opt.m), grown(self.opt.v), self.opt.applied_steps()[0])
-        else:
-            state = {}
-            for k in GAUSSIAN_KEYS:
-                st = self.opt.state.get(self.g.params[k], None)
-                if st:
-                    z = torch.zeros(n_new, *st["exp_avg"].shape[1:], device=dev)
-                    state[k] = dict(step=st["step"], exp_avg=torch.cat([st["exp_avg"], z], 0),
-                                    exp_avg_sq=torch.cat([st["exp_avg_sq"], z.clone()], 0))
-            self._rebuild(flat, P + n_new, state=state or None)
+
+        def grown(buf, rows):
+            return torch.cat([torch.cat([x, rows[k]], 0).reshape(-1) for k, x in self.g.views(buf).items()])
+        zeros = {k: torch.zeros(n_new, w, device=dev) for k, w in zip(GAUSSIAN_KEYS, self._widths())}
+        flat = grown(self.g.flat, {k: new[k].to(dev).float().reshape(n_new, -1) for k in GAUSSIAN_KEYS})
+        self._rebuild(flat, P + n_new, grown(self.exp_avg, zeros), grown(self.exp_avg_sq, zeros), self._adam_steps())
         return P + n_new
 
     def add_new_gaussians(self, frame, time_idx, intrinsics, sil_thres):
@@ -648,10 +639,7 @@ class ShardedMapper:
         with torch.no_grad():
             tg = transform_to_frame(p, time_idx, gaussians_grad=False, camera_grad=False)
             depth_sil, _, _ = self.render(frame["cam"], **depth_sil_rendervar(p, frame["w2c"], tg))
-            rot = F.normalize(p["cam_unnorm_rots"][..., time_idx].detach())
-            curr_w2c = torch.eye(4, device=depth_sil.device)
-            curr_w2c[:3, :3] = build_rotation(rot)[0]
-            curr_w2c[:3, 3] = p["cam_trans"][0, :, time_idx].detach()
+            curr_w2c, _ = pose_matrices(p, time_idx)
         new, n = map_ops.new_gaussians_from_frame(depth_sil, frame, intrinsics, curr_w2c, sil_thres,
                                                   scale_dim=self._widths()[4])
         if n:
@@ -675,19 +663,13 @@ class ShardedMapper:
         dev = self.g.flat.device
         f0 = window[0]
         if capacity is None:
-            worst = 0
+            # a few synchronous forwards size the capacity (an overflow later is safe: it skips the step and
+            # re-captures, see the docstring)
             probe = window if len(window) <= 3 else [window[0], window[len(window) // 2], window[-1]]
-            for fr in probe:             # a few synchronous forwards size the capacity (an overflow later is safe: it
-                                         # skips the step and re-captures, see the docstring)
-                with torch.no_grad():
-                    rgb, dep = fused_rendervars(self.params(), fr["id"], fr["w2c"], camera_grad=False)
-                    c, _, _ = GaussianRasterizer(fr["cam"])(**rgb)
-                worst = max(worst, _last_num_rendered())
-            capacity = int(worst * slack) + 4096
+            capacity = _capacity(self.params(), probe, slack)
         self._cap = int(capacity)
         self._slack = slack
         self._polls = []                 # (event, pinned copy of the overflow slot) of steps in flight
-        self.overflow_events = getattr(self, "overflow_events", 0)
         self._pin = [torch.empty(1, dtype=torch.float32, pin_memory=True) for _ in range(8)]
         self._static = dict(id=f0["id"], cam=f0["cam"], w2c=f0["w2c"].clone(), im=f0["im"].clone(), depth=f0["depth"].clone(),
                             pose=tuple(t.clone() for t in pose_matrices(self.params(), f0["id"])))
@@ -729,9 +711,12 @@ class ShardedMapper:
         """(Adam steps applied, steps skipped because a render overflowed the instance capacity); synchronises."""
         return self.opt.applied_steps() if self.fused else (self.step_idx, 0)
 
-    def _poll_overflow(self, window, block=False):
-        """Looks at the overflow flags of COMPLETED earlier steps (one-step lag: never waits for the step in flight
-        unless `block`); on overflow grows the capacity from the measured instance count and re-captures."""
+    def poll_overflow(self, window, block=False):
+        """Graph mode: looks at the overflow flags of COMPLETED earlier steps (one-step lag: never waits for the step in
+        flight unless `block`); on overflow grows the capacity from the measured instance count and re-captures.
+        Returns whether a step overflowed; False without a captured graph."""
+        if self._graph is None:
+            return False
         hit = False
         while self._polls and (block or len(self._polls) > 1 or self._polls[0][0].query()):
             ev, host = self._polls.pop(0)
@@ -773,7 +758,7 @@ class ShardedMapper:
 
     def accumulate(self, frame):
         """Local backward of one keyframe into the flat gradient bucket (no communication)."""
-        keep = {} if getattr(self, "track_means2D", False) else None
+        keep = {} if self.track_means2D else None
         loss, radius = mapping_loss(self.params(), frame, self.render, fused_loss=self.fused, keep=keep)
         loss.backward()
         if keep is not None:      # gradient of the RGB render's 2D means: the densification statistic (splatam.py:250)
@@ -793,13 +778,13 @@ class ShardedMapper:
         RNG, as the reference) draws the split samples.  Returns the Gaussian count afterwards."""
         P = self.g.shapes["means3D"][0]
         dev = self.g.flat.device
-        if not hasattr(self, "_dens") or self._dens["accum"].shape[0] != P:
+        if self._dens is None or self._dens["accum"].shape[0] != P:
             self._dens = dict(accum=torch.zeros(P, device=dev), denom=torch.zeros(P, device=dev))
         if iter > densify_dict["stop_after"]:
             return P
         means2D_grad = self.last_means2D_grad if means2D_grad is None else means2D_grad
         if seen is None:       # the Gaussians THIS rank's render saw (the bucket's seen flags are already summed over ranks)
-            seen = self.last_seen_local if getattr(self, "last_seen_local", None) is not None else (self.g.seen_f > 0)
+            seen = self.last_seen_local if self.last_seen_local is not None else (self.g.seen_f > 0)
         if self.dist and self.world > 1:
             # K ranks rendered K keyframes this step: the statistic of the step is the sum over the keyframes, exactly
             # what K sequential single-keyframe steps of the reference would have accumulated; summing it over the ranks
@@ -844,19 +829,11 @@ class ShardedMapper:
         P = self.remove_points(to_remove)
         self._dens = dict(accum=torch.zeros(P, device=dev), denom=torch.zeros(P, device=dev))
         if iter > 0 and iter % densify_dict["reset_opacities_every"] == 0 and densify_dict["reset_opacities"]:
-            with torch.no_grad():
-                self.g.params["logit_opacities"].fill_(math.log(0.01 / 0.99))
-            if self.fused:
-                off = sum(math.prod(self.g.shapes[k]) for k in GAUSSIAN_KEYS[:3])
-                self.opt.m[off:off + P].zero_(); self.opt.v[off:off + P].zero_()
-            else:
-                st = self.opt.state.get(self.g.params["logit_opacities"], None)
-                if st:
-                    st["exp_avg"].zero_(); st["exp_avg_sq"].zero_()
+            self._reset_opacities()
         return P
 
     def _device_generator(self):
-        if getattr(self, "_dev_gen", None) is None:
+        if self._dev_gen is None:
             self._dev_gen = torch.Generator(device=self.g.flat.device)
             self._dev_gen.manual_seed(12345)
         return self._dev_gen
@@ -864,39 +841,20 @@ class ShardedMapper:
     def step(self, window):
         """One sharded mapping step over `window` (list of keyframe dicts).  Returns the mean loss."""
         picks = self.schedule(len(window))
-        graphed = getattr(self, "_graph", None) is not None
+        graphed = self._graph is not None
         if graphed:
-            self._poll_overflow(window)
+            self.poll_overflow(window)
             self._replay(window[picks[self.rank]])
         else:
             self.g.zero_grad()
             loss, radius = self.accumulate(window[picks[self.rank]])
             self.g.seen_f.copy_(radius > 0)
             self.g.loss_slot.copy_(loss.reshape(1))
-        chunked = graphed and self.dist is not None and self.world > 1 and self.overlap_chunks > 1
-        if chunked:
-            # The bucket travels as K slices, the TAIL first (it carries the seen flags, the loss and the overflow flag
-            # that every later Adam chunk needs); the guarded Adam update of slice k runs on the compute stream as soon as
-            # its all-reduce has landed, while NCCL moves slice k+1: only the last slice's update is exposed.
-            n = self.g.flat.numel()
-            K = int(self.overlap_chunks)
-            cuts = [n * i // K for i in range(K)] + [n]
-            works = [self.dist.all_reduce(self.g.bucket[cuts[K - 1]:], op=self.dist.ReduceOp.SUM, group=self.group,
-                                          async_op=True)]
-            works += [self.dist.all_reduce(self.g.bucket[cuts[i]:cuts[i + 1]], op=self.dist.ReduceOp.SUM, group=self.group,
-                                           async_op=True) for i in range(K - 1)]
-            works[0].wait()
-            self.opt.advance_clock(self.g.overflow_slot)
-            self.opt.apply_range(cuts[K - 1], n - cuts[K - 1], self.g.overflow_slot)
-            for i in range(K - 1):
-                works[i + 1].wait()
-                self.opt.apply_range(cuts[i], cuts[i + 1] - cuts[i], self.g.overflow_slot)
-        elif self.dist and self.world > 1:
+        if self.dist and self.world > 1:
             # ONE collective per step: gradients, seen flags (sum of 0/1 > 0 == OR) and the loss travel together
             self.dist.all_reduce(self.g.bucket, op=self.dist.ReduceOp.SUM, group=self.group)
         if graphed:
-            if not chunked:
-                self.opt.step_guarded(self.g.overflow_slot)    # no-op on every rank if any rank's render overflowed
+            self.opt.step_guarded(self.g.overflow_slot)    # no-op on every rank if any rank's render overflowed
             host = self._pin[self.step_idx % len(self._pin)]
             host.copy_(self.g.overflow_slot, non_blocking=True)
             ev = torch.cuda.Event()

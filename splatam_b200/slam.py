@@ -56,10 +56,7 @@ def initialize_map(frame, intrinsics, scale_dim=1):
 
 
 def _curr_w2c(rots, trans, t):
-    w2c = torch.eye(4, device=rots.device)
-    w2c[:3, :3] = M.build_rotation(F.normalize(rots[..., t]))[0]
-    w2c[:3, 3] = trans[0, :, t]
-    return w2c
+    return M.camera_w2c(rots[..., t], trans[..., t])[0]
 
 
 def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_iters=8, keyframe_every=2,
@@ -90,8 +87,7 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     rots = torch.zeros(1, 4, T, device=dev); rots[:, 0] = 1.0
     trans = torch.zeros(1, 3, T, device=dev)
     kw = {} if render is None else {"render": render}
-    mapper = M.ShardedMapper(gauss_init, rots, trans, seed=seed, fused=fused, **kw)
-    mapper.track_means2D = densify_dict is not None
+    mapper = M.ShardedMapper(gauss_init, rots, trans, seed=seed, fused=fused, track_means2D=densify_dict is not None, **kw)
     keyframes = [dict(frames[0], est_w2c=torch.eye(4, device=dev))]
     counts = [mapper.g.shapes["means3D"][0]]
     for it in range(first_frame_iters):       # the reference maps frame 0 before it tracks frame 1 (splatam.py:777)
@@ -143,8 +139,7 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
                     mapper.prune_gaussians(it, prune_dict, scene_radius)
                 if densify_dict is not None:
                     mapper.densify(it, densify_dict, scene_radius)
-            if graph and getattr(mapper, "_graph", None) is not None:
-                mapper._poll_overflow(win, block=True)
+            mapper.poll_overflow(win, block=True)
             torch.cuda.synchronize(dev) if dev.type == "cuda" else None
             timing["mapping_s"] += time.perf_counter() - t0
             timing["mapping_iters"] += mapping_iters

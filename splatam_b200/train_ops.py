@@ -55,26 +55,6 @@ class FusedAdam:
                 None if skip_if_nonzero is None else skip_if_nonzero.data_ptr(), self.betas[0], self.betas[1], self.eps,
                 _stream(self.flat.device)), "sb_adam_step_guarded")
 
-    def advance_clock(self, skip_if_nonzero=None):
-        """First half of a chunked guarded step: the device clock ticks (unless the skip flag is set)."""
-        lib = _lib.load()
-        clk = self._clock()
-        with torch.cuda.device(self.flat.device):
-            _lib.check(lib.sb_adam_clock_advance(self.seg_lr, self.n, clk.data_ptr(),
-                                                 None if skip_if_nonzero is None else skip_if_nonzero.data_ptr(),
-                                                 self.betas[0], self.betas[1], _stream(self.flat.device)),
-                       "sb_adam_clock_advance")
-
-    def apply_range(self, first, count, skip_if_nonzero=None):
-        """Second half: the Adam update of flat elements [first, first + count) with the clock's current step sizes."""
-        lib = _lib.load()
-        clk = self._clock()
-        with torch.cuda.device(self.flat.device):
-            _lib.check(lib.sb_adam_apply_guarded(
-                self.flat.data_ptr(), self.flat_grad.data_ptr(), self.m.data_ptr(), self.v.data_ptr(), int(first), int(count),
-                self.seg_end, self.n, clk.data_ptr(), None if skip_if_nonzero is None else skip_if_nonzero.data_ptr(),
-                self.betas[0], self.betas[1], self.eps, _stream(self.flat.device)), "sb_adam_apply_guarded")
-
     def applied_steps(self):
         """(steps applied, steps skipped) of the guarded mode; synchronises."""
         if self.clock is None:

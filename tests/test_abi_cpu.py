@@ -25,7 +25,7 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), name
     assert sorted(_lib.EXPORTED_SYMBOLS) == declared, "python binding table out of sync with the header"
-    assert lib.sb_abi_version() == 2
+    assert lib.sb_abi_version() == 3
     assert lib.sb_status_string(0) == b"SB_OK" and lib.sb_status_string(3) == b"SB_ERR_CUDA"
 
 

@@ -104,11 +104,10 @@ def test_prune_torch_path_matches_reference(tag):
     prune_dict = ast.literal_eval(str(G[f"prune_{tag}_dict"][0]))
     P_new = m.prune_gaussians(int(G[f"prune_{tag}_iter"]), prune_dict, float(G["prune_scene_radius"]))
     assert P_new == G[f"prune_{tag}_means3D"].shape[0] and 0 < P_new < 400
-    for k in KEYS:
+    for k, (exp_avg, exp_avg_sq) in m.moments().items():
         assert np.allclose(m.g.params[k].detach().numpy(), G[f"prune_{tag}_{k}"], rtol=1e-6, atol=1e-7), k
-        st = m.opt.state[m.g.params[k]]
-        assert np.allclose(st["exp_avg"].numpy(), G[f"prune_{tag}_{k}_exp_avg"], rtol=1e-6, atol=1e-9), k
-        assert np.allclose(st["exp_avg_sq"].numpy(), G[f"prune_{tag}_{k}_exp_avg_sq"], rtol=1e-6, atol=1e-12), k
+        assert np.allclose(exp_avg.numpy(), G[f"prune_{tag}_{k}_exp_avg"], rtol=1e-6, atol=1e-9), k
+        assert np.allclose(exp_avg_sq.numpy(), G[f"prune_{tag}_{k}_exp_avg_sq"], rtol=1e-6, atol=1e-12), k
     # the mapper keeps working on the smaller map: gradient views and the bucket follow the new size
     assert m.g.bucket.numel() == sum(p.numel() for p in m.g.params.values()) + P_new + 2
     m.g.flat_grad.fill_(0.5)
@@ -121,12 +120,11 @@ def test_grow_torch_path_appends_rows_with_zero_moments():
     n = new["means3D"].shape[0]
     before = {k: m.g.params[k].detach().clone() for k in KEYS}
     assert m.add_gaussians(new) == 400 + n
-    for k in KEYS:
+    for k, (exp_avg, _) in m.moments().items():
         p = m.g.params[k].detach()
         assert torch.equal(p[:400], before[k]) and torch.equal(p[400:], new[k].float().reshape(n, -1))
-        st = m.opt.state[m.g.params[k]]
-        assert st["exp_avg"].shape[0] == 400 + n and float(st["exp_avg"][400:].abs().sum()) == 0.0
-        assert float(st["exp_avg"][:400].abs().sum()) > 0.0
+        assert exp_avg.shape[0] == 400 + n and float(exp_avg[400:].abs().sum()) == 0.0
+        assert float(exp_avg[:400].abs().sum()) > 0.0
 
 
 def test_oracle_backproject_and_prune_mask_match_reference():
@@ -240,8 +238,7 @@ def test_densify_matches_reference():
         P = m.densify(int(G["iter_%d" % call]), dd, float(G["scene_radius"]), means2D_grad=torch.from_numpy(G["m2d_%d" % call]),
                       seen=torch.from_numpy(G["seen_%d" % call]))
     assert P == G["out_means3D"].shape[0] != 300
-    for k in keys:
+    for k, (exp_avg, exp_avg_sq) in m.moments().items():
         assert np.allclose(m.g.params[k].detach().numpy(), G["out_" + k], rtol=1e-6, atol=1e-7), k
-        st = m.opt.state[m.g.params[k]]
-        assert np.allclose(st["exp_avg"].numpy(), G["out_" + k + "_exp_avg"], rtol=1e-6, atol=1e-9), k
-        assert np.allclose(st["exp_avg_sq"].numpy(), G["out_" + k + "_exp_avg_sq"], rtol=1e-6, atol=1e-12), k
+        assert np.allclose(exp_avg.numpy(), G["out_" + k + "_exp_avg"], rtol=1e-6, atol=1e-9), k
+        assert np.allclose(exp_avg_sq.numpy(), G["out_" + k + "_exp_avg_sq"], rtol=1e-6, atol=1e-12), k

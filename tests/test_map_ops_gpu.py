@@ -72,13 +72,12 @@ def test_prune_fused_path_matches_reference(cuda_device, tag):
     P_new = m.prune_gaussians(int(G[f"prune_{tag}_iter"]), prune_dict, float(G["prune_scene_radius"]))
     assert P_new == G[f"prune_{tag}_means3D"].shape[0]
     off = 0
-    for k in KEYS:
+    for k, (exp_avg, exp_avg_sq) in m.moments().items():
         ref = G[f"prune_{tag}_{k}"]
         assert np.allclose(m.g.params[k].detach().cpu().numpy(), ref, rtol=2e-6, atol=1e-7), k
-        n = ref.size
-        assert np.allclose(m.opt.m[off:off + n].cpu().numpy().reshape(ref.shape), G[f"prune_{tag}_{k}_exp_avg"], rtol=2e-6, atol=1e-9), k
-        assert np.allclose(m.opt.v[off:off + n].cpu().numpy().reshape(ref.shape), G[f"prune_{tag}_{k}_exp_avg_sq"], rtol=2e-6, atol=1e-12), k
-        off += n
+        assert np.allclose(exp_avg.cpu().numpy().reshape(ref.shape), G[f"prune_{tag}_{k}_exp_avg"], rtol=2e-6, atol=1e-9), k
+        assert np.allclose(exp_avg_sq.cpu().numpy().reshape(ref.shape), G[f"prune_{tag}_{k}_exp_avg_sq"], rtol=2e-6, atol=1e-12), k
+        off += ref.size
     assert m.opt.t == 1 and m.opt.m.numel() == m.g.flat.numel() == off
     m.g.flat_grad.fill_(0.5)
     m.opt.step()                                   # the fused optimizer keeps working on the compacted buffers
@@ -142,7 +141,8 @@ def test_non_presence_mask_and_add_new_gaussians(cuda_device):
         a, b = m.g.params[k].detach()[P0:], ref_new[k]
         assert torch.allclose(a, b, rtol=2e-6, atol=2e-6), (k, float((a - b).abs().max()))
         assert torch.equal(m.g.params[k].detach()[:P0], part[k].reshape(P0, -1))
-    assert float(m.opt.m.abs().sum()) == 0.0 and m.opt.m.numel() == m.g.flat.numel()
+    assert all(float(exp_avg.abs().sum()) == 0.0 for exp_avg, _ in m.moments().values())
+    assert m.opt.m.numel() == m.g.flat.numel()
     # the grown map covers the frame: the silhouette hole is (mostly) gone, and mapping steps still run
     p = m.params()
     with torch.no_grad():
@@ -157,7 +157,7 @@ def test_non_presence_mask_and_add_new_gaussians(cuda_device):
     P1 = m.prune_gaussians(20, dict(start_after=0, remove_big_after=0, stop_after=20, prune_every=20,
                                     removal_opacity_threshold=0.005, final_removal_opacity_threshold=0.6,
                                     reset_opacities=False, reset_opacities_every=500), scene_radius=3.0)
-    assert 0 < P1 < P0 + n and getattr(m, "_graph", None) is None      # the opacity-0.5 newcomers go
+    assert 0 < P1 < P0 + n and m._graph is None      # the opacity-0.5 newcomers go
     loss, _, _ = m.step([frame])                      # eager again after the shape change
     assert np.isfinite(float(loss))
 
@@ -185,16 +185,9 @@ def test_densify_fused_path_matches_torch_path_and_reference_fixture(cuda_device
             P = m.densify(int(G["iter_%d" % call]), dd, float(G["scene_radius"]),
                           means2D_grad=torch.from_numpy(G["m2d_%d" % call]).to(dev),
                           seen=torch.from_numpy(G["seen_%d" % call]).to(dev), generator=gen)
-        if fused:
-            sizes = [int(np.prod(m.g.shapes[k])) for k in keys]
-            mom = dict(zip(keys, torch.split(m.opt.m, sizes))), dict(zip(keys, torch.split(m.opt.v, sizes)))
-            res[fused] = (P, {k: m.g.params[k].detach().clone() for k in keys},
-                          {k: mom[0][k].reshape(m.g.shapes[k]).clone() for k in keys},
-                          {k: mom[1][k].reshape(m.g.shapes[k]).clone() for k in keys})
-        else:
-            res[fused] = (P, {k: m.g.params[k].detach().clone() for k in keys},
-                          {k: m.opt.state[m.g.params[k]]["exp_avg"].clone() for k in keys},
-                          {k: m.opt.state[m.g.params[k]]["exp_avg_sq"].clone() for k in keys})
+        mom = m.moments()
+        res[fused] = (P, {k: m.g.params[k].detach().clone() for k in keys},
+                      {k: mom[k][0].clone() for k in keys}, {k: mom[k][1].clone() for k in keys})
     assert res[True][0] == res[False][0] == G["out_means3D"].shape[0]
     for k in keys:
         for i in (1, 2, 3):

@@ -165,8 +165,7 @@ def _worker_densify(rank, world, port, q):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     torch.set_num_threads(2)
     gauss, rots, trans, frames = _problem()
-    mapper = M.ShardedMapper(gauss, rots, trans, render=_cpu_render, seed=77)
-    mapper.track_means2D = True
+    mapper = M.ShardedMapper(gauss, rots, trans, render=_cpu_render, seed=77, track_means2D=True)
     dd = dict(start_after=0, remove_big_after=0, stop_after=10, densify_every=1, grad_thresh=1e-9, num_to_split_into=2,
               removal_opacity_threshold=0.05, final_removal_opacity_threshold=0.05, reset_opacities=False,
               reset_opacities_every=100)

@@ -105,51 +105,3 @@ def test_graph_mode_matches_eager(cuda_device):
         lg, seen, _ = graph.step(frames)
     n, overflow = graph.check_capacity()
     assert not overflow and 0 < n <= cap and bool(torch.isfinite(lg)) and bool(seen.any())
-
-
-def _worker_chunked(rank, world, port, q):
-    import torch.distributed as dist
-    from splatam_b200 import mapping as M
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-    dev = torch.device("cuda", rank)
-    torch.cuda.set_device(dev)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=dev)
-    gauss, rots, trans, frames = _problem(dev)
-    out = {}
-    for chunks in (1, 4):
-        m = M.ShardedMapper(gauss, rots, trans, seed=7)
-        m.overlap_chunks = chunks
-        m.enable_graph(frames)
-        losses = [float(m.step(frames)[0]) for _ in range(4)]
-        torch.cuda.synchronize()
-        out[chunks] = (m.g.flat.detach().cpu().numpy(), losses, m.effective_steps())
-    q.put((rank, out))
-    dist.barrier()
-    dist.destroy_process_group()
-
-
-def test_graph_mode_chunked_allreduce_overlap_two_gpus(cuda_device):
-    """Graph-replayed sharded step with the bucket all-reduced in 4 slices and the guarded Adam update applied slice by
-    slice (the update of slice k overlaps the transfer of slice k+1): replicas stay bit-identical, and the result equals
-    the single-collective step up to the float-atomics noise of two separate backward passes."""
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs")
-    import torch.multiprocessing as mp
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); port = s.getsockname()[1]; s.close()
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_worker_chunked, args=(r, 2, port, q)) for r in range(2)]
-    [p.start() for p in procs]
-    res = sorted([q.get(timeout=600) for _ in range(2)], key=lambda t: t[0])
-    [p.join(120) for p in procs]
-    r0, r1 = res[0][1], res[1][1]
-    gauss, _, _, _ = _problem(cuda_device)
-    init = torch.cat([gauss[k].reshape(-1) for k in ("means3D", "rgb_colors", "unnorm_rotations", "logit_opacities", "log_scales")]).cpu().numpy()
-    for chunks in (1, 4):
-        assert np.array_equal(r0[chunks][0], r1[chunks][0]), "replicas must stay bit-identical"
-        assert r0[chunks][2] == (4, 0) and np.allclose(r0[chunks][1], r1[chunks][1])
-    assert np.allclose(r0[1][1], r0[4][1], rtol=1e-3)
-    n_rot0 = 6 * gauss["means3D"].shape[0]
-    sig = np.r_[0:n_rot0, n_rot0 + 4 * gauss["means3D"].shape[0]:init.size]       # skip unnorm_rotations (pure noise, isotropic)
-    du, dr = (r0[4][0] - init)[sig], (r0[1][0] - init)[sig]
-    assert np.linalg.norm(du - dr) / np.linalg.norm(dr) < 0.05

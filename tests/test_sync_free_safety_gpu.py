@@ -58,7 +58,7 @@ def test_mapper_recovers_from_capacity_overflow(cuda_device):
     while graphed.effective_steps()[0] < n_steps and guard < 40:
         losses.append(float(graphed.step(frames)[0]))
         guard += 1
-    graphed._poll_overflow(frames, block=True)
+    graphed.poll_overflow(frames, block=True)
     applied, skipped = graphed.effective_steps()
     assert applied == n_steps and skipped >= 1 and graphed.overflow_events >= 1, (applied, skipped, graphed.overflow_events)
     assert any(np.isnan(l) for l in losses), "overflowed steps report a NaN loss"
