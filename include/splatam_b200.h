@@ -300,6 +300,26 @@ SB_API int sb_backproject(int H, int W, const float* color, const float* depth, 
                           const float* c2w_host, const uint8_t* mask, const uint32_t* dst_index, int scale_dim,
                           float* means3D, float* rgb, float* log_scales, float* mean_sq_dist, void* stream);
 
+/* ---- final evaluation metrics (SURVEY.md section 8(f) row N4; R/utils/eval_helpers.py:408-623) -----------------
+ * Forward only, deterministic (per-block partials reduced in a fixed order), no host synchronisation.
+ * sb_frame_metrics: im, gt_im [3,H,W], depth_sil [3,H,W] (depth, silhouette, depth^2), gt_depth [1,H,W].
+ * valid = gt_depth > 0, presence = silhouette > sil_thres, mask = presence*valid if use_presence else valid
+ * (use_presence = mapping_iters == 0 && !add_new_gaussians in the reference).  Writes weighted_im = im*mask and
+ * weighted_gt = gt_im*mask [3,H,W] and metrics[5] (device doubles) = {PSNR: mean over channels of the per-channel
+ * PSNR, each MSE over all H*W pixels; "depth RMSE": sum(sqrt(e^2)*valid)/sum(valid), i.e. a masked mean absolute
+ * error as the reference defines it; depth L1: sum(|e|*valid)/sum(valid); sum(valid); sum(mask)} with
+ * e = (depth*valid - gt_depth) [* presence when use_presence].  Rendered values are not clamped.
+ * sb_ms_ssim: pytorch_msssim.ms_ssim(x, y, data_range, 11-tap sigma-1.5 window, 5 levels) of [N,C,H,W] contiguous
+ * float images, computed in double; per_channel [N*C] and/or mean (device doubles, either may be NULL).
+ * min(H, W) must exceed 160.  Workspaces: the *_workspace_bytes queries (device memory, any content). */
+SB_API int sb_frame_metrics_workspace_bytes(int H, int W, size_t* bytes);
+SB_API int sb_frame_metrics(const float* im, const float* depth_sil, const float* gt_im, const float* gt_depth, int H,
+                            int W, float sil_thres, int use_presence, float* weighted_im, float* weighted_gt,
+                            void* workspace, size_t workspace_bytes, double* metrics, void* stream);
+SB_API int sb_ms_ssim_workspace_bytes(int N, int C, int H, int W, size_t* bytes);
+SB_API int sb_ms_ssim(const float* x, const float* y, int N, int C, int H, int W, double data_range, void* workspace,
+                      size_t workspace_bytes, double* per_channel, double* mean, void* stream);
+
 /* ---- per-stage device timing (measurement only; bench.py's roofline pass) -------------------
  * Between sb_profile_begin() and sb_profile_end() every stage launch of this process is bracketed
  * by CUDA events on its stream.  sb_profile_end synchronises, writes the summed milliseconds and call

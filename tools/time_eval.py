@@ -1,0 +1,140 @@
+#!/usr/bin/env python
+"""Times SplaTAM's final evaluation on one GPU: splatam_b200.evaluate over a 1200x680 view-filling map
+(scenes.view_filling, Replica intrinsics) and 200 frames along slam.look_trajectory, against the reference's metric
+path (R/utils/eval_helpers.py:463-507: PSNR and depth errors in PyTorch on the GPU, MS-SSIM by pytorch_msssim on the
+CPU after .cpu(); the float32 restatement in oracle/metrics_torch.py stands in for pytorch_msssim, which is not
+installed).  Prints the GPU name and power limit of the run and one JSON line:
+  evaluate_frames_per_s      whole evaluate() (two renders + metrics per frame, one read-back at the end)
+  metric_kernels_ms_per_frame  sb_frame_metrics + sb_ms_ssim on one frame, CUDA events over --reps calls
+  reference_metrics_ms_per_frame  the reference-style metric path for one frame (GPU PyTorch + .cpu() + CPU MS-SSIM)
+Run:  python tools/time_eval.py [--frames 200] [--reps 100] [--ref-frames 5]"""
+import argparse
+import ctypes
+import json
+import os
+import subprocess
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import torch  # noqa: E402
+
+import scenes  # noqa: E402
+
+
+def gpu_info():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                           text=True, check=True, timeout=30).stdout.strip().splitlines()[0]
+    except Exception as e:          # the name still comes from torch
+        q = "%s, power limit unknown (%s)" % (torch.cuda.get_device_name(0), e)
+    return q
+
+
+def reference_metrics(im, depth_sil, gt_im, gt_depth, sil_thres, use_presence):
+    """eval_helpers.py:465-507 as the reference runs it, with the float32 MS-SSIM restatement on the CPU."""
+    from oracle import metrics_torch as O
+    rastered_depth = depth_sil[0, :, :].unsqueeze(0)
+    valid = gt_depth > 0
+    rastered_depth = rastered_depth * valid
+    presence = depth_sil[1, :, :] > sil_thres
+    if use_presence:
+        w_im, w_gt = im * presence * valid, gt_im * presence * valid
+    else:
+        w_im, w_gt = im * valid, gt_im * valid
+    mse = ((w_im - w_gt) ** 2).view(3, -1).mean(1, keepdim=True)
+    psnr = (20 * torch.log10(1.0 / torch.sqrt(mse))).mean()
+    ssim = O.ms_ssim(w_im.unsqueeze(0).cpu(), w_gt.unsqueeze(0).cpu(), data_range=1.0, dtype=torch.float32)
+    e = (rastered_depth - gt_depth) * presence if use_presence else rastered_depth - gt_depth
+    rmse = (torch.sqrt(e ** 2) * valid).sum() / valid.sum()
+    l1 = (torch.abs(e) * valid).sum() / valid.sum()
+    return psnr.cpu(), ssim, rmse.cpu(), l1.cpu()
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--frames", type=int, default=200)
+    ap.add_argument("--reps", type=int, default=100)
+    ap.add_argument("--ref-frames", type=int, default=5)
+    ap.add_argument("--sil-thres", type=float, default=0.5)
+    args = ap.parse_args()
+    assert torch.cuda.is_available(), "time_eval.py measures on a CUDA device"
+    import splatam_b200 as S
+    from splatam_b200 import _lib, evaluate as EV, slam
+    from splatam_b200 import mapping as M
+    dev = torch.device("cuda:0")
+    print("GPU:", gpu_info(), flush=True)
+    sc = scenes.view_filling(margin=100)          # surface beyond the borders: the moving camera sees a covered view
+    cam = sc.settings(S.GaussianRasterizationSettings, dev)
+    gt = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
+              logit_opacities=torch.logit(sc.opacities.reshape(-1, 1)), log_scales=torch.log(sc.scales[:, :1]))
+    gt = {k: v.to(dev).contiguous() for k, v in gt.items()}
+    T = args.frames
+    rots, trans = slam.look_trajectory(T, dev, step=(0.002, -0.001, 0.001), rot_step=(0.0005, -0.0004, 0.0003))
+    frames = [slam.render_frame(gt, rots, trans, t, cam) for t in range(T)]
+    g = torch.Generator().manual_seed(1)
+    # the evaluated map: colours, sizes and poses a little off the generating scene, as after a SLAM run
+    noise = lambda t, s: t + s * torch.randn(t.shape, generator=g).to(dev)
+    params = dict(gt, cam_unnorm_rots=noise(rots, 0.0005), cam_trans=noise(trans, 0.001))
+    params["cam_unnorm_rots"][..., 0], params["cam_trans"][..., 0] = rots[..., 0], trans[..., 0]
+    params["rgb_colors"] = noise(gt["rgb_colors"], 0.05).clamp(0, 1)
+    params["log_scales"] = noise(gt["log_scales"], 0.05)
+    gt_w2c = slam.w2c_list(rots, trans)
+
+    # evaluate(): warm up on a few frames, then the whole sequence
+    EV.evaluate(params, frames[:4], cam, args.sil_thres, 0, False)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    out = EV.evaluate(params, frames, cam, args.sil_thres, 0, False, gt_w2c=gt_w2c)
+    torch.cuda.synchronize()
+    wall = time.perf_counter() - t0
+
+    # the metric kernels alone on frame 1's renders, CUDA events over --reps calls
+    lib = _lib.load()
+    H, W = sc.h, sc.w
+    with torch.no_grad():
+        im, ds, _, _ = M._render_pair(params, dict(frames[1], cam=cam), M.default_render, True, camera_grad=False)
+    im, ds = im.contiguous(), ds.contiguous()
+    gt_im, gt_d = frames[1]["im"].contiguous(), frames[1]["depth"].contiguous()
+    w_im, w_gt = torch.empty_like(im), torch.empty_like(im)
+    metrics = torch.zeros(6, dtype=torch.float64, device=dev)
+    ws_f = EV._workspace(lib.sb_frame_metrics_workspace_bytes, H, W, device=dev)
+    ws_s = EV._workspace(lib.sb_ms_ssim_workspace_bytes, 1, 3, H, W, device=dev)
+    st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+    def kernels():
+        _lib.check(lib.sb_frame_metrics(im.data_ptr(), ds.data_ptr(), gt_im.data_ptr(), gt_d.data_ptr(), H, W,
+                                        args.sil_thres, 1, w_im.data_ptr(), w_gt.data_ptr(), ws_f.data_ptr(),
+                                        ws_f.numel(), metrics.data_ptr(), st), "sb_frame_metrics")
+        EV._ms_ssim_into(w_im[None], w_gt[None], 1.0, None, metrics[5], ws_s)
+    for _ in range(10):
+        kernels()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(args.reps):
+        kernels()
+    e1.record()
+    torch.cuda.synchronize()
+    kernel_ms = e0.elapsed_time(e1) / args.reps
+
+    # the reference-style metric path on the same renders
+    reference_metrics(im, ds, gt_im, gt_d, args.sil_thres, True)          # warm-up
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for _ in range(args.ref_frames):
+        ref = reference_metrics(im, ds, gt_im, gt_d, args.sil_thres, True)
+    torch.cuda.synchronize()
+    ref_ms = (time.perf_counter() - t0) * 1e3 / args.ref_frames
+    print(json.dumps(dict(
+        gpu=gpu_info(), width=W, height=H, gaussians=sc.P, frames=T,
+        evaluate_frames_per_s=round(T / wall, 2), evaluate_wall_s=round(wall, 3),
+        metric_kernels_ms_per_frame=round(kernel_ms, 4), reference_metrics_ms_per_frame=round(ref_ms, 2),
+        cpu_threads=torch.get_num_threads(), psnr=round(out["psnr"], 4), ms_ssim=round(out["ms_ssim"], 6),
+        depth_rmse=round(out["depth_rmse"], 6), ate=out["ate"],
+        frame1_kernel_vs_reference_style=dict(psnr=[metrics[0].item(), float(ref[0])],
+                                              ms_ssim=[metrics[5].item(), float(ref[1])]))))
+
+
+if __name__ == "__main__":
+    main()
