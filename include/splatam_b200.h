@@ -44,7 +44,7 @@ extern "C" {
 #define SB_API
 #endif
 
-#define SB_ABI_VERSION 3
+#define SB_ABI_VERSION 4
 #define SB_TILE 16 /* BLOCK_X == BLOCK_Y == 16, X/cuda_rasterizer/config.h:16-17 (part of the key contract) */
 #define SB_CHANNELS 3 /* NUM_CHANNELS, X/cuda_rasterizer/config.h:15 */
 
@@ -55,7 +55,7 @@ typedef enum sb_status {
     SB_ERR_CUDA = 3,         /* a CUDA runtime call or kernel launch failed             */
     SB_ERR_UNSUPPORTED = 4,  /* feature of the reference API not built (see DESIGN.md)  */
     SB_ERR_BINNING_TOO_SMALL = 5 /* sb_forward only: stage 1 is complete and *num_rendered is set, but the guessed
-                                binning workspace cannot hold it -- finish with sb_forward_render_ex */
+                                binning workspace cannot hold it -- finish with sb_forward_render */
 } sb_status;
 
 /* Mirror of GaussianRasterizationSettings (X/diff_gaussian_rasterization/__init__.py:134-145).
@@ -84,8 +84,9 @@ SB_API const char* sb_last_cuda_error(void);
  *      X/cuda_rasterizer/rasterizer_impl.h:63-72) -------------------------------------- */
 SB_API int sb_geometry_workspace_bytes(int P, size_t* bytes);
 SB_API int sb_image_workspace_bytes(int width, int height, size_t* bytes);
-SB_API int sb_binning_workspace_bytes(int num_rendered, int width, int height, size_t* bytes);
-SB_API int sb_backward_workspace_bytes(int P, size_t* bytes);
+/* color_sets = 1, or 2 for a render with a second colour set (see sb_forward_render). */
+SB_API int sb_binning_workspace_bytes(int num_rendered, int width, int height, int color_sets, size_t* bytes);
+SB_API int sb_backward_workspace_bytes(int P, int color_sets, size_t* bytes);
 
 /* ---- forward, stage 1: per-Gaussian projection + depth ordering -----------------------
  * FORWARD::preprocess + InclusiveSum + num_rendered readback
@@ -104,20 +105,28 @@ SB_API int sb_forward_geometry(const sb_settings* s, int P,
 /* ---- forward, stage 2: tile duplication + sort + alpha-composite ------------------------
  * duplicateWithKeys + SortPairs + identifyTileRanges + FORWARD::render
  * (X/cuda_rasterizer/rasterizer_impl.cu:284-337, forward.cu:261-393).
- * colors [P,3] (colors_precomp).  out_color [3,H,W], out_depth [1,H,W]. */
+ * colors [P,3] (colors_precomp).  out_color [3,H,W], out_depth [1,H,W].
+ * Second colour set (SURVEY.md section 8(f) row N1): SplaTAM renders the SAME geometry twice per iteration with
+ * different colours_precomp, RGB and [depth, 1, depth^2] (R/scripts/splatam.py:249,253).  colors2 [P,3] /
+ * out_color2 [3,H,W] blend both sets in one pass over one projection and one sort; NULL for both is a plain
+ * render.  Outputs of the first set are bit-identical to a plain render.  The binning workspace must then be
+ * sized with color_sets = 2. */
 SB_API int sb_forward_render(const sb_settings* s, int P, int num_rendered,
-                      const float* colors,
+                      const float* colors, const float* colors2,
                       const void* geom_ws, size_t geom_ws_bytes,
                       void* binning_ws, size_t binning_ws_bytes,
                       void* image_ws, size_t image_ws_bytes,
-                      float* out_color, float* out_depth,
+                      float* out_color, float* out_color2, float* out_depth,
                       void* stream);
 
 /* ---- backward ---------------------------------------------------------------------------
  * BACKWARD::render + BACKWARD::preprocess (X/cuda_rasterizer/backward.cu:399-657).
  * dL_dout_color [3,H,W].  Outputs are fully overwritten (no pre-zeroing needed):
  * dL_dmeans3D [P,3], dL_dmeans2D [P,3], dL_dcolors [P,3], dL_dopacity [P],
- * dL_dscales [P,3], dL_drotations [P,4]; dL_dcov3D [P,6] may be NULL. */
+ * dL_dscales [P,3], dL_drotations [P,4]; dL_dcov3D [P,6] may be NULL.
+ * Second colour set: dL_dout_color2 [3,H,W] and dL_dcolors2 [P,3], both NULL for a plain render.  dL_dmeans2D
+ * then carries the FIRST set's share only (SplaTAM reads the means2D gradient of the RGB render,
+ * splatam.py:250); every other gradient is the sum over both sets.  bwd_ws is sized with color_sets = 2. */
 SB_API int sb_backward(const sb_settings* s, int P, int num_rendered,
                 const float* means3D, const float* colors,
                 const float* scales, const float* rotations,
@@ -127,18 +136,18 @@ SB_API int sb_backward(const sb_settings* s, int P, int num_rendered,
                 const void* binning_ws, size_t binning_ws_bytes,
                 const void* image_ws, size_t image_ws_bytes,
                 void* bwd_ws, size_t bwd_ws_bytes,
-                const float* dL_dout_color,
-                float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dcolors,
+                const float* dL_dout_color, const float* dL_dout_color2,
+                float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dcolors, float* dL_dcolors2,
                 float* dL_dopacity, float* dL_dscales, float* dL_drotations,
                 float* dL_dcov3D,
                 void* stream);
 
 /* ---- forward in one call ---------------------------------------------------------------------------------
- * sb_forward_geometry + sb_forward_render_ex back to back WITHOUT returning to the caller between them, so
+ * sb_forward_geometry + sb_forward_render back to back WITHOUT returning to the caller between them, so
  * the GPU is idle only for the num_rendered read-back itself.  The caller passes a binning workspace sized
  * from a guess (e.g. the previous call's num_rendered plus slack); if it is too small the call returns
  * SB_ERR_BINNING_TOO_SMALL with *num_rendered set and stage 1 complete -- the caller then allocates
- * sb_binning_workspace_bytes_ex(*num_rendered, ...) and finishes with sb_forward_render_ex. */
+ * sb_binning_workspace_bytes(*num_rendered, ...) and finishes with sb_forward_render. */
 SB_API int sb_forward(const sb_settings* s, int P, const float* means3D, const float* opacities, const float* scales,
                const float* rotations, const float* cov3D_precomp, const float* colors, const float* colors2,
                int32_t* radii, void* geom_ws, size_t geom_ws_bytes, void* binning_ws, size_t binning_ws_bytes,
@@ -147,10 +156,10 @@ SB_API int sb_forward(const sb_settings* s, int P, const float* means3D, const f
 
 /* ---- sync-free forward (CUDA-graph capturable) -------------------------------------------------------------
  * Same work as sb_forward but num_rendered never leaves the device: the caller fixes a CAPACITY (tile
- * instances) for the binning workspace (sb_binning_workspace_bytes_ex(capacity, ...)); the instance count is read
+ * instances) for the binning workspace (sb_binning_workspace_bytes(capacity, ...)); the instance count is read
  * on the device by the sort and the record gather, so only the live instances are processed.  No memcpy to the
  * host, no synchronisation, no allocation:
- * the call (and sb_backward_ex with num_rendered := capacity) can be captured into a CUDA graph.
+ * the call (and sb_backward with num_rendered := capacity) can be captured into a CUDA graph.
  * If the scene needs more than `capacity` instances the overflow flag (geometry workspace, int32 word 2) is set and
  * the images are written as NaN, so a truncated render cannot pass for a valid one;
  * sb_read_counts (which synchronises) returns the true count and the flag so the caller can grow and redo. */
@@ -161,28 +170,6 @@ SB_API int sb_forward_async(const sb_settings* s, int P, const float* means3D, c
                      float* out_color2, float* out_depth, void* stream);
 SB_API int sb_read_counts(const void* geom_ws, size_t geom_ws_bytes, int P, int* num_rendered, int* overflow,
                           void* stream);
-
-/* ---- fused two-colour-set render (SURVEY.md section 8(f) row N1) ---------------------------------------
- * SplaTAM renders the SAME geometry twice per iteration with different colours_precomp: RGB and
- * [depth, 1, depth^2] (R/scripts/splatam.py:249,253).  The _ex entry points blend both sets in one pass:
- * one projection, one sort, one forward and one backward blend.  colors2 / out_color2 / dL_dout_color2 /
- * dL_dcolors2 == NULL reduce them to the plain calls above.  Outputs of the first set are bit-identical
- * to a plain render; dL_dmeans2D carries the FIRST set's share only (SplaTAM reads the means2D gradient
- * of the RGB render, splatam.py:250), every other gradient is the sum over both sets.  Workspaces must be
- * sized with the _ex size functions (color_sets = 2). */
-SB_API int sb_binning_workspace_bytes_ex(int num_rendered, int width, int height, int color_sets, size_t* bytes);
-SB_API int sb_backward_workspace_bytes_ex(int P, int color_sets, size_t* bytes);
-SB_API int sb_forward_render_ex(const sb_settings* s, int P, int num_rendered, const float* colors,
-                         const float* colors2, const void* geom_ws, size_t geom_ws_bytes, void* binning_ws,
-                         size_t binning_ws_bytes, void* image_ws, size_t image_ws_bytes, float* out_color,
-                         float* out_color2, float* out_depth, void* stream);
-SB_API int sb_backward_ex(const sb_settings* s, int P, int num_rendered, const float* means3D, const float* colors,
-                   const float* scales, const float* rotations, const float* cov3D_precomp, const int32_t* radii,
-                   const void* geom_ws, size_t geom_ws_bytes, const void* binning_ws, size_t binning_ws_bytes,
-                   const void* image_ws, size_t image_ws_bytes, void* bwd_ws, size_t bwd_ws_bytes,
-                   const float* dL_dout_color, const float* dL_dout_color2, float* dL_dmeans3D,
-                   float* dL_dmeans2D, float* dL_dcolors, float* dL_dcolors2, float* dL_dopacity,
-                   float* dL_dscales, float* dL_drotations, float* dL_dcov3D, void* stream);
 
 /* ---- spherical-harmonics colour branch (shs / sh_degree, X/cuda_rasterizer/forward.cu:20-71,
  *      backward.cu:20-139).  sb_sh_forward turns shs [P,max_coeffs,3] into the rgb [P,3] the render consumes

@@ -2,9 +2,13 @@
 
 The product path has NO fallback: if ``libsplatam_b200.so`` is missing or fails to load, importing
 the rasterizer raises.  Build it with ``python -c "import __graft_entry__ as g; g.build()"`` or ``make``.
+Every wrapper module calls the library through ``call`` (and ``nbytes`` for size queries), the one place that turns
+tensors into ABI arguments, picks the device and stream of a launch and reports a failed status.
 """
 import ctypes
 import os
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libsplatam_b200.so")
@@ -42,8 +46,8 @@ _SIGNATURES = {
     "sb_last_cuda_error": (ctypes.c_char_p, []),
     "sb_geometry_workspace_bytes": (_i, [_i, ctypes.POINTER(_sz)]),
     "sb_image_workspace_bytes": (_i, [_i, _i, ctypes.POINTER(_sz)]),
-    "sb_binning_workspace_bytes": (_i, [_i, _i, _i, ctypes.POINTER(_sz)]),
-    "sb_backward_workspace_bytes": (_i, [_i, ctypes.POINTER(_sz)]),
+    "sb_binning_workspace_bytes": (_i, [_i, _i, _i, _i, ctypes.POINTER(_sz)]),
+    "sb_backward_workspace_bytes": (_i, [_i, _i, ctypes.POINTER(_sz)]),
     "sb_forward_geometry": (_i, [ctypes.POINTER(SbSettings), _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz,
                                  ctypes.POINTER(_i), _vp]),
     "sb_forward": (_i, [ctypes.POINTER(SbSettings), _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _sz,
@@ -51,18 +55,11 @@ _SIGNATURES = {
     "sb_forward_async": (_i, [ctypes.POINTER(SbSettings), _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _sz,
                               _i, _vp, _sz, _vp, _vp, _vp, _vp]),
     "sb_read_counts": (_i, [_vp, _sz, _i, ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
-    "sb_forward_render": (_i, [ctypes.POINTER(SbSettings), _i, _i, _vp, _vp, _sz, _vp, _sz, _vp, _sz,
-                               _vp, _vp, _vp]),
-    "sb_binning_workspace_bytes_ex": (_i, [_i, _i, _i, _i, ctypes.POINTER(_sz)]),
-    "sb_backward_workspace_bytes_ex": (_i, [_i, _i, ctypes.POINTER(_sz)]),
-    "sb_forward_render_ex": (_i, [ctypes.POINTER(SbSettings), _i, _i, _vp, _vp, _vp, _sz, _vp, _sz, _vp, _sz,
-                                  _vp, _vp, _vp, _vp]),
-    "sb_backward_ex": (_i, [ctypes.POINTER(SbSettings), _i, _i, _vp, _vp, _vp, _vp, _vp, _vp,
-                            _vp, _sz, _vp, _sz, _vp, _sz, _vp, _sz,
-                            _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "sb_forward_render": (_i, [ctypes.POINTER(SbSettings), _i, _i, _vp, _vp, _vp, _sz, _vp, _sz, _vp, _sz,
+                               _vp, _vp, _vp, _vp]),
     "sb_backward": (_i, [ctypes.POINTER(SbSettings), _i, _i, _vp, _vp, _vp, _vp, _vp, _vp,
                          _vp, _sz, _vp, _sz, _vp, _sz, _vp, _sz,
-                         _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+                         _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "sb_mark_visible": (_i, [_i, _vp, _vp, _vp, _vp, _vp]),
     "sb_export_geometry": (_i, [_i, _vp, _sz, _vp, _vp, _vp, _vp, _vp]),
     "sb_adam_step": (_i, [_vp, _vp, _vp, _vp, _sz, ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_double), _i,
@@ -116,7 +113,7 @@ def load():
         fn = getattr(lib, name)  # AttributeError if a declared symbol is not exported
         fn.restype = restype
         fn.argtypes = argtypes
-    if lib.sb_abi_version() != 3:
+    if lib.sb_abi_version() != 4:
         raise SplatamB200Error("libsplatam_b200.so ABI version mismatch")
     _lib = lib
     return lib
@@ -128,3 +125,57 @@ def check(rc, what):
         name = lib.sb_status_string(rc).decode()
         detail = lib.sb_last_cuda_error().decode() if name == "SB_ERR_CUDA" else ""
         raise SplatamB200Error(f"{what} failed: {name} {detail}".strip())
+
+
+def ptr(a):
+    """ABI argument for `a`: a tensor's device pointer, or NULL for None or an empty tensor (the reference's "not
+    provided", X/diff_gaussian_rasterization/__init__.py:173-183); anything else (ints, floats, byref out-parameters,
+    host ctypes arrays) unchanged."""
+    if isinstance(a, torch.Tensor):
+        return a.data_ptr() if a.numel() else None
+    return a
+
+
+def stream(device):
+    return torch.cuda.current_stream(device).cuda_stream
+
+
+class on_device:
+    """torch.cuda.device(dev) only when dev is not already current (the context manager costs ~10 us)."""
+
+    def __init__(self, device):
+        self.ctx = None if torch.cuda.current_device() == device.index else torch.cuda.device(device)
+
+    def __enter__(self):
+        if self.ctx is not None:
+            self.ctx.__enter__()
+
+    def __exit__(self, *a):
+        if self.ctx is not None:
+            self.ctx.__exit__(*a)
+
+
+def call(name, *args, device=None):
+    """Calls entry point `name` with every argument passed through `ptr`; raises SplatamB200Error on a non-zero
+    status.  With `device`, that device is made current for the call and its current stream is appended as the
+    trailing `void* stream`."""
+    fn = getattr(load(), name)
+    args = [ptr(a) for a in args]
+    if device is None:
+        check(fn(*args), name)
+        return
+    with on_device(device):
+        check(fn(*args, stream(device)), name)
+
+
+def nbytes(name, *args):
+    """Size written by a `*_workspace_bytes` / `sb_compact_plan_bytes` query through its trailing size_t*."""
+    n = ctypes.c_size_t(0)
+    call(name, *args, ctypes.byref(n))
+    return n.value
+
+
+def need_cuda(what, *tensors):
+    for t in tensors:
+        if not t.is_cuda:
+            raise SplatamB200Error(f"{what} needs CUDA tensors (there is no CPU fallback)")

@@ -140,22 +140,18 @@ SB_API int sb_image_workspace_bytes(int width, int height, size_t* bytes) {
     carve_image(nullptr, width, height, bytes);
     return SB_OK;
 }
-SB_API int sb_binning_workspace_bytes_ex(int num_rendered, int width, int height, int color_sets, size_t* bytes) {
+SB_API int sb_binning_workspace_bytes(int num_rendered, int width, int height, int color_sets, size_t* bytes) {
     if (num_rendered < 0 || width <= 0 || height <= 0 || !bytes || color_sets < 1 || color_sets > 2) return SB_ERR_BAD_ARG;
     const int tiles = ((width + kTile - 1) / kTile) * ((height + kTile - 1) / kTile);
     carve_binning(nullptr, num_rendered, tiles, color_sets, bytes);
     return SB_OK;
 }
-SB_API int sb_binning_workspace_bytes(int num_rendered, int width, int height, size_t* bytes) {
-    return sb_binning_workspace_bytes_ex(num_rendered, width, height, 1, bytes);
-}
-SB_API int sb_backward_workspace_bytes_ex(int P, int color_sets, size_t* bytes) {
+SB_API int sb_backward_workspace_bytes(int P, int color_sets, size_t* bytes) {
     if (P < 0 || !bytes || color_sets < 1 || color_sets > 2) return SB_ERR_BAD_ARG;
     const int stride = color_sets > 1 ? kAccumStride2 : kAccumStride;
     *bytes = ((size_t)(P > 0 ? P : 1) * stride * sizeof(float) + kAlign - 1) / kAlign * kAlign;
     return SB_OK;
 }
-SB_API int sb_backward_workspace_bytes(int P, size_t* bytes) { return sb_backward_workspace_bytes_ex(P, 1, bytes); }
 
 SB_API int sb_forward_geometry(const sb_settings* s, int P, const float* means3D, const float* opacities,
                         const float* scales, const float* rotations, const float* cov3D_precomp,
@@ -190,11 +186,11 @@ SB_API int sb_forward(const sb_settings* s, int P, const float* means3D, const f
                                  geom_ws_bytes, num_rendered, stream);
     if (rc != SB_OK) return rc;
     size_t need = 0;
-    rc = sb_binning_workspace_bytes_ex(*num_rendered, s->image_width, s->image_height, colors2 ? 2 : 1, &need);
+    rc = sb_binning_workspace_bytes(*num_rendered, s->image_width, s->image_height, colors2 ? 2 : 1, &need);
     if (rc != SB_OK) return rc;
     if (*num_rendered > 0 && (binning_ws == nullptr || binning_ws_bytes < need)) return SB_ERR_BINNING_TOO_SMALL;
-    return sb_forward_render_ex(s, P, *num_rendered, colors, colors2, geom_ws, geom_ws_bytes, binning_ws,
-                                binning_ws_bytes, image_ws, image_ws_bytes, out_color, out_color2, out_depth, stream);
+    return sb_forward_render(s, P, *num_rendered, colors, colors2, geom_ws, geom_ws_bytes, binning_ws,
+                             binning_ws_bytes, image_ws, image_ws_bytes, out_color, out_color2, out_depth, stream);
 }
 
 SB_API int sb_forward_async(const sb_settings* s, int P, const float* means3D, const float* opacities,
@@ -240,16 +236,9 @@ SB_API int sb_read_counts(const void* geom_ws, size_t geom_ws_bytes, int P, int*
 }
 
 SB_API int sb_forward_render(const sb_settings* s, int P, int num_rendered, const float* colors,
-                      const void* geom_ws, size_t geom_ws_bytes, void* binning_ws, size_t binning_ws_bytes,
-                      void* image_ws, size_t image_ws_bytes, float* out_color, float* out_depth, void* stream) {
-    return sb_forward_render_ex(s, P, num_rendered, colors, nullptr, geom_ws, geom_ws_bytes, binning_ws,
-                                binning_ws_bytes, image_ws, image_ws_bytes, out_color, nullptr, out_depth, stream);
-}
-
-SB_API int sb_forward_render_ex(const sb_settings* s, int P, int num_rendered, const float* colors,
-                         const float* colors2, const void* geom_ws, size_t geom_ws_bytes, void* binning_ws,
-                         size_t binning_ws_bytes, void* image_ws, size_t image_ws_bytes, float* out_color,
-                         float* out_color2, float* out_depth, void* stream) {
+                      const float* colors2, const void* geom_ws, size_t geom_ws_bytes, void* binning_ws,
+                      size_t binning_ws_bytes, void* image_ws, size_t image_ws_bytes, float* out_color,
+                      float* out_color2, float* out_depth, void* stream) {
     if (!settings_ok(s) || P < 0 || num_rendered < 0 || !image_ws || !out_color || !out_depth) return SB_ERR_BAD_ARG;
     if (P > 0 && (!colors || !geom_ws)) return SB_ERR_BAD_ARG;
     if ((colors2 != nullptr) != (out_color2 != nullptr)) return SB_ERR_BAD_ARG;
@@ -272,21 +261,9 @@ SB_API int sb_backward(const sb_settings* s, int P, int num_rendered, const floa
                 const float* scales, const float* rotations, const float* cov3D_precomp, const int32_t* radii,
                 const void* geom_ws, size_t geom_ws_bytes, const void* binning_ws, size_t binning_ws_bytes,
                 const void* image_ws, size_t image_ws_bytes, void* bwd_ws, size_t bwd_ws_bytes,
-                const float* dL_dout_color, float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dcolors,
-                float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dcov3D, void* stream) {
-    return sb_backward_ex(s, P, num_rendered, means3D, colors, scales, rotations, cov3D_precomp, radii, geom_ws,
-                          geom_ws_bytes, binning_ws, binning_ws_bytes, image_ws, image_ws_bytes, bwd_ws, bwd_ws_bytes,
-                          dL_dout_color, nullptr, dL_dmeans3D, dL_dmeans2D, dL_dcolors, nullptr, dL_dopacity,
-                          dL_dscales, dL_drotations, dL_dcov3D, stream);
-}
-
-SB_API int sb_backward_ex(const sb_settings* s, int P, int num_rendered, const float* means3D, const float* colors,
-                   const float* scales, const float* rotations, const float* cov3D_precomp, const int32_t* radii,
-                   const void* geom_ws, size_t geom_ws_bytes, const void* binning_ws, size_t binning_ws_bytes,
-                   const void* image_ws, size_t image_ws_bytes, void* bwd_ws, size_t bwd_ws_bytes,
-                   const float* dL_dout_color, const float* dL_dout_color2, float* dL_dmeans3D,
-                   float* dL_dmeans2D, float* dL_dcolors, float* dL_dcolors2, float* dL_dopacity,
-                   float* dL_dscales, float* dL_drotations, float* dL_dcov3D, void* stream) {
+                const float* dL_dout_color, const float* dL_dout_color2, float* dL_dmeans3D,
+                float* dL_dmeans2D, float* dL_dcolors, float* dL_dcolors2, float* dL_dopacity,
+                float* dL_dscales, float* dL_drotations, float* dL_dcov3D, void* stream) {
     (void)geom_ws; (void)geom_ws_bytes;
     if ((dL_dout_color2 != nullptr) != (dL_dcolors2 != nullptr)) return SB_ERR_BAD_ARG;
     const int sets = dL_dout_color2 ? 2 : 1;
@@ -303,7 +280,7 @@ SB_API int sb_backward_ex(const sb_settings* s, int P, int num_rendered, const f
     if (num_rendered > 0 && binning_ws_bytes < need) return SB_ERR_WORKSPACE;
     ImageWs img = carve_image(const_cast<void*>(image_ws), s->image_width, s->image_height, &need);
     if (image_ws_bytes < need) return SB_ERR_WORKSPACE;
-    sb_backward_workspace_bytes_ex(P, sets, &need);
+    sb_backward_workspace_bytes(P, sets, &need);
     if (bwd_ws_bytes < need) return SB_ERR_WORKSPACE;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     float* accum = static_cast<float*>(bwd_ws);

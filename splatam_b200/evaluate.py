@@ -7,7 +7,6 @@ mapping and tracking (`mapping._render_pair`), one kernel pass per frame writes 
 depth sums, MS-SSIM runs on the device, and the per-frame metrics stay on the device until one read at the end.
 LPIPS is not computed (it needs pretrained AlexNet weights): the result carries ``lpips: None``.  CUDA only; no CPU
 fallback."""
-import ctypes
 import os
 
 import numpy as np
@@ -20,27 +19,13 @@ from . import mapping as M
 _PSNR, _RMSE, _L1, _NVALID, _NMASK, _SSIM = range(6)
 
 
-def _stream(device):
-    return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-
-
-def _workspace(query, *args, device):
-    n = ctypes.c_size_t(0)
-    _lib.check(query(*args, ctypes.byref(n)), query.__name__)
-    return torch.empty(max(int(n.value), 1), dtype=torch.uint8, device=device)
-
-
 def _ms_ssim_into(x, y, data_range, per_channel, mean, ws=None):
     """Enqueues sb_ms_ssim on contiguous float32 [N,C,H,W] CUDA tensors; `per_channel` / `mean`: float64 device
     tensors or None."""
-    lib = _lib.load()
     N, C, H, W = x.shape
     if ws is None:
-        ws = _workspace(lib.sb_ms_ssim_workspace_bytes, N, C, H, W, device=x.device)
-    with torch.cuda.device(x.device):
-        _lib.check(lib.sb_ms_ssim(x.data_ptr(), y.data_ptr(), N, C, H, W, float(data_range), ws.data_ptr(), ws.numel(),
-                                  None if per_channel is None else per_channel.data_ptr(),
-                                  None if mean is None else mean.data_ptr(), _stream(x.device)), "sb_ms_ssim")
+        ws = torch.empty(_lib.nbytes("sb_ms_ssim_workspace_bytes", N, C, H, W), dtype=torch.uint8, device=x.device)
+    _lib.call("sb_ms_ssim", x, y, N, C, H, W, float(data_range), ws, ws.numel(), per_channel, mean, device=x.device)
 
 
 def ms_ssim(x, y, data_range=1.0, size_average=True):
@@ -48,8 +33,7 @@ def ms_ssim(x, y, data_range=1.0, size_average=True):
     valid filtering, 5 levels with weights 0.0448, 0.2856, 0.3001, 0.2363, 0.1333), computed in double on the device.
     size_average=True returns the mean (a float64 0-d tensor); otherwise the float64 [N,C] values (pytorch_msssim
     averages those over channels).  The smaller image side must exceed 160."""
-    if not (x.is_cuda and y.is_cuda):
-        raise _lib.SplatamB200Error("ms_ssim needs CUDA tensors (there is no CPU fallback)")
+    _lib.need_cuda("ms_ssim", x, y)
     if x.dim() != 4 or x.shape != y.shape:
         raise _lib.SplatamB200Error("ms_ssim expects two [N,C,H,W] images of the same shape, got %s and %s"
                                     % (tuple(x.shape), tuple(y.shape)))
@@ -108,12 +92,10 @@ def evaluate(params, frames, cam, sil_thres, mapping_iters, add_new_gaussians, e
     depth_rmse_per_frame, depth_l1_per_frame, valid_pixels, mask_pixels.  `out_dir`: also writes psnr.txt, rmse.txt,
     l1.txt and ssim.txt as the reference does (np.savetxt, one value per evaluated frame).
     fused / render: as for mapping (`mapping._render_pair`); fused defaults to the fast path on CUDA."""
-    if not (params["means3D"].is_cuda and frames[0]["im"].is_cuda):
-        raise _lib.SplatamB200Error("evaluate needs CUDA tensors (there is no CPU fallback)")
+    _lib.need_cuda("evaluate", params["means3D"], frames[0]["im"])
     render = M.default_render if render is None else render
     if fused is None:
         fused = render is M.default_render
-    lib = _lib.load()
     dev = params["means3D"].device
     H, W = frames[0]["im"].shape[-2:]
     if min(H, W) <= 160:
@@ -123,20 +105,16 @@ def evaluate(params, frames, cam, sil_thres, mapping_iters, add_new_gaussians, e
     metrics = torch.zeros(len(ids), 6, dtype=torch.float64, device=dev)
     w_im = torch.empty(3, H, W, dtype=torch.float32, device=dev)
     w_gt = torch.empty_like(w_im)
-    ws_frame = _workspace(lib.sb_frame_metrics_workspace_bytes, H, W, device=dev)
-    ws_ssim = _workspace(lib.sb_ms_ssim_workspace_bytes, 1, 3, H, W, device=dev)
-    row_bytes = metrics.stride(0) * metrics.element_size()
+    ws_frame = torch.empty(_lib.nbytes("sb_frame_metrics_workspace_bytes", H, W), dtype=torch.uint8, device=dev)
+    ws_ssim = torch.empty(_lib.nbytes("sb_ms_ssim_workspace_bytes", 1, 3, H, W), dtype=torch.uint8, device=dev)
     with torch.no_grad(), torch.cuda.device(dev):
         for k, t in enumerate(ids):
             fr = dict(frames[t], cam=cam)
             im, depth_sil, _, _ = M._render_pair(params, fr, render, fused, camera_grad=False)
             im, depth_sil = im.float().contiguous(), depth_sil.float().contiguous()
             gt_im, gt_d = fr["im"].float().contiguous(), fr["depth"].float().contiguous()
-            row = metrics.data_ptr() + k * row_bytes
-            _lib.check(lib.sb_frame_metrics(im.data_ptr(), depth_sil.data_ptr(), gt_im.data_ptr(), gt_d.data_ptr(), H,
-                                            W, float(sil_thres), use_presence, w_im.data_ptr(), w_gt.data_ptr(),
-                                            ws_frame.data_ptr(), ws_frame.numel(), row, _stream(dev)),
-                       "sb_frame_metrics")
+            _lib.call("sb_frame_metrics", im, depth_sil, gt_im, gt_d, H, W, float(sil_thres), use_presence, w_im, w_gt,
+                      ws_frame, ws_frame.numel(), metrics[k], device=dev)
             _ms_ssim_into(w_im[None], w_gt[None], 1.0, None, metrics[k, _SSIM], ws_ssim)
     m = metrics.cpu().numpy()                    # the one device-to-host read
     out = dict(frame_ids=[int(frames[t]["id"]) for t in ids], psnr_per_frame=m[:, _PSNR], ms_ssim_per_frame=m[:, _SSIM],

@@ -14,83 +14,57 @@ from . import _lib
 GAUSSIAN_KEYS = ("means3D", "rgb_colors", "unnorm_rotations", "logit_opacities", "log_scales")
 
 
-def _stream(device):
-    return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-
-
-def _need_cuda(t, what):
-    if not t.is_cuda:
-        raise _lib.SplatamB200Error(f"{what} needs CUDA tensors (there is no CPU fallback)")
-
-
 def prune_mask(logit_opacities, log_scales, opacity_threshold, big_threshold=None):
     """bool[P] keep mask: not (sigmoid(logit) < opacity_threshold or exp(log_scales).max(1) > big_threshold)."""
-    _need_cuda(logit_opacities, "prune_mask")
-    lib = _lib.load()
+    _lib.need_cuda("prune_mask", logit_opacities)
     lo = logit_opacities.detach().contiguous().float()
     ls = log_scales.detach().contiguous().float()
     P = lo.shape[0]
     keep = torch.empty(P, dtype=torch.uint8, device=lo.device)
-    with torch.cuda.device(lo.device):
-        _lib.check(lib.sb_prune_mask(P, lo.data_ptr(), ls.data_ptr(), ls.shape[1] if ls.dim() > 1 else 1,
-                                     float(opacity_threshold), float(big_threshold) if big_threshold else 0.0,
-                                     keep.data_ptr(), _stream(lo.device)), "sb_prune_mask")
+    _lib.call("sb_prune_mask", P, lo, ls, ls.shape[1] if ls.dim() > 1 else 1, float(opacity_threshold),
+              float(big_threshold) if big_threshold else 0.0, keep, device=lo.device)
     return keep.bool()
 
 
 def compact_plan(mask):
     """Exclusive scan of a bool/uint8 mask -> (mask_u8, dst_index uint32-as-int32 tensor, count).  Synchronises."""
-    _need_cuda(mask, "compact_plan")
-    lib = _lib.load()
+    _lib.need_cuda("compact_plan", mask)
     m = mask.contiguous().view(torch.uint8) if mask.dtype == torch.bool else mask.contiguous().to(torch.uint8)
     n = m.numel()
     dst = torch.empty(max(n, 1), dtype=torch.int32, device=m.device)
-    nbytes = ctypes.c_size_t()
-    _lib.check(lib.sb_compact_plan_bytes(n, ctypes.byref(nbytes)), "sb_compact_plan_bytes")
-    temp = torch.empty(nbytes.value, dtype=torch.uint8, device=m.device)
+    temp = torch.empty(_lib.nbytes("sb_compact_plan_bytes", n), dtype=torch.uint8, device=m.device)
     count = ctypes.c_int()
-    with torch.cuda.device(m.device):
-        _lib.check(lib.sb_compact_plan(n, m.data_ptr(), dst.data_ptr(), temp.data_ptr(), temp.numel(),
-                                       ctypes.byref(count), _stream(m.device)), "sb_compact_plan")
+    _lib.call("sb_compact_plan", n, m, dst, temp, temp.numel(), ctypes.byref(count), device=m.device)
     return m, dst, count.value
 
 
 def compact_flat(flat, P, widths, mask_u8, dst_index, P_new):
     """Kept rows of a packed buffer [w0*P | w1*P | ...] -> new packed buffer with P_new rows."""
-    _need_cuda(flat, "compact_flat")
-    lib = _lib.load()
+    _lib.need_cuda("compact_flat", flat)
     assert flat.is_contiguous() and flat.dtype == torch.float32 and flat.numel() == sum(widths) * P
     out = torch.empty(sum(widths) * P_new, dtype=torch.float32, device=flat.device)
     w = (ctypes.c_int * len(widths))(*[int(x) for x in widths])
-    with torch.cuda.device(flat.device):
-        _lib.check(lib.sb_compact_flat(P, P_new, mask_u8.data_ptr(), dst_index.data_ptr(), len(widths), w,
-                                       flat.data_ptr(), out.data_ptr(), _stream(flat.device)), "sb_compact_flat")
+    _lib.call("sb_compact_flat", P, P_new, mask_u8, dst_index, len(widths), w, flat, out, device=flat.device)
     return out
 
 
 def depth_error(depth_sil, gt_depth):
     """|gt - depth| * (gt > 0) over the frame (R/scripts/splatam.py:391)."""
-    _need_cuda(depth_sil, "depth_error")
-    lib = _lib.load()
+    _lib.need_cuda("depth_error", depth_sil)
     ds, gt = depth_sil.detach().contiguous().float(), gt_depth.detach().contiguous().float()
     H, W = ds.shape[-2:]
     err = torch.empty(H, W, dtype=torch.float32, device=ds.device)
-    with torch.cuda.device(ds.device):
-        _lib.check(lib.sb_depth_error(H, W, ds.data_ptr(), gt.data_ptr(), err.data_ptr(), _stream(ds.device)),
-                   "sb_depth_error")
+    _lib.call("sb_depth_error", H, W, ds, gt, err, device=ds.device)
     return err
 
 
 def new_gaussian_mask(depth_sil, gt_depth, sil_thres, depth_err_thres):
     """bool[H*W] non-presence mask of add_new_gaussians (already AND-ed with gt_depth > 0)."""
-    _need_cuda(depth_sil, "new_gaussian_mask")
-    lib = _lib.load()
+    _lib.need_cuda("new_gaussian_mask", depth_sil)
     ds, gt = depth_sil.detach().contiguous().float(), gt_depth.detach().contiguous().float()
     H, W = ds.shape[-2:]
     mask = torch.empty(H * W, dtype=torch.uint8, device=ds.device)
-    with torch.cuda.device(ds.device):
-        _lib.check(lib.sb_new_gaussian_mask(H, W, ds.data_ptr(), gt.data_ptr(), float(sil_thres), float(depth_err_thres),
-                                            mask.data_ptr(), _stream(ds.device)), "sb_new_gaussian_mask")
+    _lib.call("sb_new_gaussian_mask", H, W, ds, gt, float(sil_thres), float(depth_err_thres), mask, device=ds.device)
     return mask.bool()
 
 
@@ -98,8 +72,7 @@ def backproject(color, depth, intrinsics, w2c, mask=None, scale_dim=1, plan=None
     """Pixels -> Gaussian rows (get_pointcloud + initialize_new_params).  intrinsics: 3x3 (tensor or nested list);
     w2c: 4x4 world-to-camera of the frame.  Returns dict(means3D, rgb_colors, unnorm_rotations, logit_opacities,
     log_scales) and mean_sq_dist, each with one row per selected pixel (row-major pixel order)."""
-    _need_cuda(color, "backproject")
-    lib = _lib.load()
+    _lib.need_cuda("backproject", color)
     dev = color.device
     color, depth = color.detach().contiguous().float(), depth.detach().contiguous().float()
     H, W = color.shape[-2:]
@@ -116,11 +89,8 @@ def backproject(color, depth, intrinsics, w2c, mask=None, scale_dim=1, plan=None
     ls = torch.empty(n, scale_dim, dtype=torch.float32, device=dev)
     msd = torch.empty(n, dtype=torch.float32, device=dev)
     if n > 0:
-        with torch.cuda.device(dev):
-            _lib.check(lib.sb_backproject(H, W, color.data_ptr(), depth.data_ptr(), fx, fy, cx, cy, c2w_host,
-                                          None if m8 is None else m8.data_ptr(), None if dst is None else dst.data_ptr(),
-                                          scale_dim, means.data_ptr(), rgb.data_ptr(), ls.data_ptr(), msd.data_ptr(),
-                                          _stream(dev)), "sb_backproject")
+        _lib.call("sb_backproject", H, W, color, depth, fx, fy, cx, cy, c2w_host, m8, dst, scale_dim, means, rgb, ls,
+                  msd, device=dev)
     rots = torch.zeros(n, 4, dtype=torch.float32, device=dev)
     rots[:, 0] = 1.0
     new = dict(means3D=means, rgb_colors=rgb, unnorm_rotations=rots,

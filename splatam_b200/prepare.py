@@ -6,21 +6,14 @@
 
 equal (to float rounding) to transform_to_frame + transformed_params2rendervar +
 transformed_params2depthplussilhouette of R/utils/slam_helpers.py.  CUDA only."""
-import ctypes
-
 import torch
 
 from . import _lib
 
 
-def _stream(device):
-    return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-
-
 class _Prepare(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, unnorm, logit, log_scales, rel_w2c, cam_rot, w2c0):
-        lib = _lib.load()
         dev = means3D.device
         P, sd = means3D.shape[0], log_scales.shape[1]
         c = lambda t: t.detach().contiguous().float()
@@ -28,11 +21,8 @@ class _Prepare(torch.autograd.Function):
         rel, cr, w0 = c(rel_w2c), c(cam_rot).reshape(4), c(w2c0)
         e = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
         means_cam, rot, opac, sc3, dcols = e(P, 3), e(P, 4), e(P, 1), e(P, 3), e(P, 3)
-        with torch.cuda.device(dev):
-            _lib.check(lib.sb_prepare_forward(P, sd, means3D.data_ptr(), unnorm.data_ptr(), logit.data_ptr(),
-                                              log_scales.data_ptr(), rel.data_ptr(), cr.data_ptr(), w0.data_ptr(),
-                                              means_cam.data_ptr(), rot.data_ptr(), opac.data_ptr(), sc3.data_ptr(),
-                                              dcols.data_ptr(), _stream(dev)), "sb_prepare_forward")
+        _lib.call("sb_prepare_forward", P, sd, means3D, unnorm, logit, log_scales, rel, cr, w0, means_cam, rot, opac,
+                  sc3, dcols, device=dev)
         ctx.save_for_backward(means3D, unnorm, rel, cr, w0, means_cam, opac, sc3)
         ctx.sd = sd
         ctx.want_pose = bool(ctx.needs_input_grad[4] or ctx.needs_input_grad[5])
@@ -41,22 +31,15 @@ class _Prepare(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_means_cam, g_rot, g_opac, g_sc3, g_dcols):
-        lib = _lib.load()
         means3D, unnorm, rel, cr, w0, means_cam, opac, sc3 = ctx.saved_tensors
         dev = means3D.device
         P = means3D.shape[0]
-        p = lambda t: None if t is None else t.contiguous().float().data_ptr()
         keep = [None if t is None else t.contiguous().float() for t in (g_means_cam, g_rot, g_opac, g_sc3, g_dcols)]
         e = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
         g_means, g_unnorm, g_logit, g_ls = e(P, 3), e(P, 4), e(*ctx.shapes[0]), e(*ctx.shapes[1])
         pose = torch.zeros(16, dtype=torch.float32, device=dev) if ctx.want_pose else None
-        with torch.cuda.device(dev):
-            _lib.check(lib.sb_prepare_backward(
-                P, ctx.sd, int(ctx.want_pose), means3D.data_ptr(), unnorm.data_ptr(), rel.data_ptr(), cr.data_ptr(),
-                w0.data_ptr(), means_cam.data_ptr(), opac.data_ptr(), sc3.data_ptr(),
-                *[None if t is None else t.data_ptr() for t in keep],
-                g_means.data_ptr(), g_unnorm.data_ptr(), g_logit.data_ptr(), g_ls.data_ptr(),
-                None if pose is None else pose.data_ptr(), _stream(dev)), "sb_prepare_backward")
+        _lib.call("sb_prepare_backward", P, ctx.sd, int(ctx.want_pose), means3D, unnorm, rel, cr, w0, means_cam, opac,
+                  sc3, *keep, g_means, g_unnorm, g_logit, g_ls, pose, device=dev)
         g_rel = g_cr = None
         if ctx.want_pose:
             g_rel = torch.zeros(4, 4, dtype=torch.float32, device=dev)
@@ -67,6 +50,5 @@ class _Prepare(torch.autograd.Function):
 
 
 def prepare_gaussians(means3D, unnorm_rotations, logit_opacities, log_scales, rel_w2c, cam_rot, w2c0):
-    if not means3D.is_cuda:
-        raise _lib.SplatamB200Error("prepare_gaussians needs CUDA tensors (there is no CPU fallback)")
+    _lib.need_cuda("prepare_gaussians", means3D)
     return _Prepare.apply(means3D, unnorm_rotations, logit_opacities, log_scales, rel_w2c, cam_rot, w2c0)

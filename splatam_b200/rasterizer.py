@@ -29,15 +29,13 @@ class GaussianRasterizationSettings(NamedTuple):
     prefiltered: bool
 
 
-def _ptr(t):
-    """Device pointer, or NULL for the reference's "not provided" empty tensor (__init__.py:173-183)."""
-    if t is None or t.numel() == 0:
-        return None
-    return t.data_ptr()
+def _given(t):
+    """False for the reference's "not provided": None or an empty tensor (__init__.py:173-183)."""
+    return t is not None and t.numel() != 0
 
 
 def _f32c(t, name):
-    if t is None or t.numel() == 0:
+    if not _given(t):
         return t
     if not t.is_cuda:
         raise _lib.SplatamB200Error(f"{name} must be a CUDA tensor (there is no CPU fallback)")
@@ -57,7 +55,7 @@ class _SettingsPack:
         self.c = _lib.SbSettings(
             int(rs.image_height), int(rs.image_width), float(rs.tanfovx), float(rs.tanfovy),
             self.bg.data_ptr(), float(rs.scale_modifier), self.view.data_ptr(), self.proj.data_ptr(),
-            int(rs.sh_degree), _ptr(self.campos), int(bool(rs.prefiltered)))
+            int(rs.sh_degree), _lib.ptr(self.campos), int(bool(rs.prefiltered)))
 
 
 _PACK_CACHE = {}
@@ -86,43 +84,25 @@ _LAST_ASYNC_STATE = {}      # device index -> state of the most recent sync-free
 _LAST_SYNC_R = [0]          # num_rendered of the most recent synchronous forward
 
 
-def _sizes(lib, P, W, H, sets):
+def _sizes(P, W, H, sets):
+    """(geometry, image, backward) workspace bytes of one problem shape."""
     key = (P, W, H, sets)
     hit = _SIZE_CACHE.get(key)
     if hit is None:
-        n = ctypes.c_size_t(0)
-        _lib.check(lib.sb_geometry_workspace_bytes(P, ctypes.byref(n)), "sb_geometry_workspace_bytes")
-        geom = n.value
-        _lib.check(lib.sb_image_workspace_bytes(W, H, ctypes.byref(n)), "sb_image_workspace_bytes")
-        img = n.value
-        _lib.check(lib.sb_backward_workspace_bytes_ex(P, sets, ctypes.byref(n)), "sb_backward_workspace_bytes_ex")
         if len(_SIZE_CACHE) > 256:
             _SIZE_CACHE.clear()
-        hit = _SIZE_CACHE[key] = (geom, img, n.value)
+        hit = _SIZE_CACHE[key] = (_lib.nbytes("sb_geometry_workspace_bytes", P),
+                                  _lib.nbytes("sb_image_workspace_bytes", W, H),
+                                  _lib.nbytes("sb_backward_workspace_bytes", P, sets))
     return hit
-
-
-class _on_device:
-    """torch.cuda.device(dev) only when dev is not already current (the context manager costs ~10 us)."""
-
-    def __init__(self, device):
-        self.ctx = None if torch.cuda.current_device() == device.index else torch.cuda.device(device)
-
-    def __enter__(self):
-        if self.ctx is not None:
-            self.ctx.__enter__()
-
-    def __exit__(self, *a):
-        if self.ctx is not None:
-            self.ctx.__exit__(*a)
 
 
 def _ws(nbytes, device):
     return torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=device)
 
 
-def _stream(device):
-    return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+def _binning_ws(num_rendered, W, H, sets, device):
+    return _ws(_lib.nbytes("sb_binning_workspace_bytes", num_rendered, W, H, sets), device)
 
 
 class _State:
@@ -136,16 +116,16 @@ class _State:
 
     def counts(self):
         """(num_rendered, overflowed) of a sync-free forward; synchronises the current stream."""
-        lib = _lib.load()
         r, o = ctypes.c_int(0), ctypes.c_int(0)
-        _lib.check(lib.sb_read_counts(self.geom.data_ptr(), self.geom.numel(), self.P, ctypes.byref(r), ctypes.byref(o),
-                                      _stream(self.geom.device)), "sb_read_counts")
+        _lib.call("sb_read_counts", self.geom, self.geom.numel(), self.P, ctypes.byref(r), ctypes.byref(o),
+                  device=self.geom.device)
         return r.value, bool(o.value)
 
 
 def _forward_impl(means3D, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
                   colors2=None, capacity=None):
-    lib = _lib.load()
+    """One or two colour sets (`colors2`) over one geometry.  Returns (color, color2 or None, radii, depth, state,
+    saved): `saved` is the tuple of inputs _backward_impl reads, None where not provided."""
     if means3D.dim() != 2 or means3D.shape[1] != 3:
         # rasterize_points.cu:56-58
         raise _lib.SplatamB200Error("means3D must have dimensions (num_points, 3)")
@@ -163,107 +143,107 @@ def _forward_impl(means3D, colors_precomp, opacities, scales, rotations, cov3Ds_
     colors2 = _f32c(colors2, "colors_extra")
     sets = 2 if colors2 is not None else 1
 
-    with _on_device(device):
-        pack = _settings_pack(raster_settings, device)
-        st = _stream(device)
-        color = torch.empty((3, H, W), dtype=torch.float32, device=device)
-        depth = torch.empty((1, H, W), dtype=torch.float32, device=device)
-        radii = torch.empty((P,), dtype=torch.int32, device=device)
-        state = _State()
-        state.settings = pack
-        state.P = P
-        n = ctypes.c_size_t(0)
-        geom_bytes, img_bytes, _ = _sizes(lib, P, W, H, sets)
-        state.geom = _ws(geom_bytes, device)
-        state.image = _ws(img_bytes, device)
-        R = ctypes.c_int(0)
-        color2 = torch.empty((3, H, W), dtype=torch.float32, device=device) if sets == 2 else None
-        if capacity is not None:
-            # sync-free mode: fixed-capacity binning workspace, num_rendered stays on the device (CUDA-graph safe)
-            capacity = int(capacity)
-            _lib.check(lib.sb_binning_workspace_bytes_ex(capacity, W, H, sets, ctypes.byref(n)),
-                       "sb_binning_workspace_bytes_ex")
-            state.binning = _ws(n.value, device)
-            _lib.check(lib.sb_forward_async(
-                ctypes.byref(pack.c), P, _ptr(means3D), _ptr(opacities), _ptr(scales), _ptr(rotations),
-                _ptr(cov3Ds_precomp), _ptr(colors_precomp), _ptr(colors2), _ptr(radii), state.geom.data_ptr(),
-                state.geom.numel(), state.binning.data_ptr(), state.binning.numel(), capacity, state.image.data_ptr(),
-                state.image.numel(), color.data_ptr(), _ptr(color2), depth.data_ptr(), st), "sb_forward_async")
-            state.num_rendered = capacity
-            _LAST_ASYNC_STATE[device.index] = state
-            saved = (means3D, colors_precomp, scales, rotations, cov3Ds_precomp)
-            if sets == 2:
-                return color, color2, radii, depth, state, saved + (colors2,)
-            return color, radii, depth, state, saved
-        # binning workspace sized from the last num_rendered seen for this problem shape (+12 % slack): the
-        # whole forward is then ONE library call and the GPU only waits for the num_rendered read-back itself
-        hint_key = (P, W, H, sets, device.index)
-        hint = _R_HINT.get(hint_key, 0)
-        if hint > 0:
-            _lib.check(lib.sb_binning_workspace_bytes_ex(int(hint * 1.125) + 4096, W, H, sets, ctypes.byref(n)),
-                       "sb_binning_workspace_bytes_ex")
-            state.binning = _ws(n.value, device)
-            bin_ptr, bin_bytes = state.binning.data_ptr(), state.binning.numel()
-        else:
-            state.binning, bin_ptr, bin_bytes = None, None, 0
-        rc = lib.sb_forward(ctypes.byref(pack.c), P, _ptr(means3D), _ptr(opacities), _ptr(scales), _ptr(rotations),
-                            _ptr(cov3Ds_precomp), _ptr(colors_precomp), _ptr(colors2), _ptr(radii),
-                            state.geom.data_ptr(), state.geom.numel(), bin_ptr, bin_bytes, state.image.data_ptr(),
-                            state.image.numel(), color.data_ptr(), _ptr(color2), depth.data_ptr(), ctypes.byref(R), st)
-        if rc == 5:      # SB_ERR_BINNING_TOO_SMALL: stage 1 is done, the guess was too small -> size exactly and finish
-            _lib.check(lib.sb_binning_workspace_bytes_ex(R.value, W, H, sets, ctypes.byref(n)),
-                       "sb_binning_workspace_bytes_ex")
-            state.binning = _ws(n.value, device)
-            _lib.check(lib.sb_forward_render_ex(
-                ctypes.byref(pack.c), P, R.value, _ptr(colors_precomp), _ptr(colors2), state.geom.data_ptr(),
-                state.geom.numel(), state.binning.data_ptr(), state.binning.numel(), state.image.data_ptr(),
-                state.image.numel(), color.data_ptr(), _ptr(color2), depth.data_ptr(), st), "sb_forward_render_ex")
-        else:
-            _lib.check(rc, "sb_forward")
-        if state.binning is None:
-            state.binning = _ws(16, device)
-        state.num_rendered = R.value
-        _LAST_SYNC_R[0] = R.value
-        _R_HINT[hint_key] = R.value
-        if len(_R_HINT) > 256:
-            _R_HINT.clear()
-    saved = (means3D, colors_precomp, scales, rotations, cov3Ds_precomp)
-    if sets == 2:
-        return color, color2, radii, depth, state, saved + (colors2,)
-    return color, radii, depth, state, saved
+    pack = _settings_pack(raster_settings, device)
+    color = torch.empty((3, H, W), dtype=torch.float32, device=device)
+    depth = torch.empty((1, H, W), dtype=torch.float32, device=device)
+    radii = torch.empty((P,), dtype=torch.int32, device=device)
+    state = _State()
+    state.settings = pack
+    state.P = P
+    geom_bytes, img_bytes, _ = _sizes(P, W, H, sets)
+    state.geom = _ws(geom_bytes, device)
+    state.image = _ws(img_bytes, device)
+    color2 = torch.empty((3, H, W), dtype=torch.float32, device=device) if sets == 2 else None
+    saved = (means3D, colors_precomp, scales, rotations, cov3Ds_precomp, colors2)
+    if capacity is not None:
+        # sync-free mode: fixed-capacity binning workspace, num_rendered stays on the device (CUDA-graph safe)
+        capacity = int(capacity)
+        state.binning = _binning_ws(capacity, W, H, sets, device)
+        _lib.call("sb_forward_async", ctypes.byref(pack.c), P, means3D, opacities, scales, rotations, cov3Ds_precomp,
+                  colors_precomp, colors2, radii, state.geom, state.geom.numel(), state.binning, state.binning.numel(),
+                  capacity, state.image, state.image.numel(), color, color2, depth, device=device)
+        state.num_rendered = capacity
+        _LAST_ASYNC_STATE[device.index] = state
+        return color, color2, radii, depth, state, saved
+    # binning workspace sized from the last num_rendered seen for this problem shape (+12 % slack): the
+    # whole forward is then ONE library call and the GPU only waits for the num_rendered read-back itself
+    hint_key = (P, W, H, sets, device.index)
+    hint = _R_HINT.get(hint_key, 0)
+    state.binning = _binning_ws(int(hint * 1.125) + 4096, W, H, sets, device) if hint > 0 else None
+    R = ctypes.c_int(0)
+    p = _lib.ptr
+    with _lib.on_device(device):
+        # called directly, not through _lib.call: SB_ERR_BINNING_TOO_SMALL is a status to act on, not a failure
+        rc = _lib.load().sb_forward(
+            ctypes.byref(pack.c), P, p(means3D), p(opacities), p(scales), p(rotations), p(cov3Ds_precomp),
+            p(colors_precomp), p(colors2), p(radii), p(state.geom), state.geom.numel(), p(state.binning),
+            0 if state.binning is None else state.binning.numel(), p(state.image), state.image.numel(), p(color),
+            p(color2), p(depth), ctypes.byref(R), _lib.stream(device))
+    if rc == 5:      # SB_ERR_BINNING_TOO_SMALL: stage 1 is done, the guess was too small -> size exactly and finish
+        state.binning = _binning_ws(R.value, W, H, sets, device)
+        _lib.call("sb_forward_render", ctypes.byref(pack.c), P, R.value, colors_precomp, colors2, state.geom,
+                  state.geom.numel(), state.binning, state.binning.numel(), state.image, state.image.numel(), color,
+                  color2, depth, device=device)
+    else:
+        _lib.check(rc, "sb_forward")
+    if state.binning is None:
+        state.binning = _ws(16, device)
+    state.num_rendered = R.value
+    _LAST_SYNC_R[0] = R.value
+    _R_HINT[hint_key] = R.value
+    if len(_R_HINT) > 256:
+        _R_HINT.clear()
+    return color, color2, radii, depth, state, saved
 
 
 def _backward_impl(state, saved, radii, grad_out_color, grad_out_color2=None):
-    lib = _lib.load()
-    means3D, colors_precomp, scales, rotations, cov3Ds_precomp = saved[:5]
-    colors2 = saved[5] if len(saved) > 5 else None
+    """Gradients (means3D, means2D, colors, colors2, opacities, scales, rotations, cov3D) of the forward that made
+    `state` and `saved`; colors2 is None for one colour set, cov3D is None unless cov3D_precomp was given, scales
+    and rotations are zeros when it was."""
+    means3D, colors_precomp, scales, rotations, cov3Ds_precomp, colors2 = saved
     sets = 2 if colors2 is not None else 1
     device = means3D.device
     P = means3D.shape[0]
     pack = state.settings
     grad_out_color = _f32c(grad_out_color, "grad_out_color")
-    with _on_device(device):
-        e = lambda *shape: torch.empty(shape, dtype=torch.float32, device=device)
-        g_means3D, g_means2D, g_colors, g_opac = e(P, 3), e(P, 3), e(P, 3), e(P, 1)
-        have_sr = scales is not None and scales.numel() != 0
-        g_scales = e(P, 3) if have_sr else torch.zeros((P, 3), dtype=torch.float32, device=device)
-        g_rot = e(P, 4) if have_sr else torch.zeros((P, 4), dtype=torch.float32, device=device)
-        g_cov3D = None if have_sr else e(P, 6)     # only the cov3D_precomp branch has a consumer for it
-        g_colors2 = e(P, 3) if sets == 2 else None
-        grad_out_color2 = _f32c(grad_out_color2, "grad_out_color2") if sets == 2 else None
-        W_, H_ = int(pack.c.image_width), int(pack.c.image_height)
-        bwd_ws = _ws(_sizes(lib, P, W_, H_, sets)[2], device)
-        _lib.check(lib.sb_backward_ex(
-            ctypes.byref(pack.c), P, state.num_rendered, _ptr(means3D), _ptr(colors_precomp), _ptr(scales),
-            _ptr(rotations), _ptr(cov3Ds_precomp), _ptr(radii),
-            state.geom.data_ptr(), state.geom.numel(), state.binning.data_ptr(), state.binning.numel(),
-            state.image.data_ptr(), state.image.numel(), bwd_ws.data_ptr(), bwd_ws.numel(),
-            _ptr(grad_out_color), _ptr(grad_out_color2), _ptr(g_means3D), _ptr(g_means2D), _ptr(g_colors),
-            _ptr(g_colors2), _ptr(g_opac), _ptr(g_scales) if have_sr else None, _ptr(g_rot) if have_sr else None,
-            _ptr(g_cov3D), _stream(device)), "sb_backward_ex")
-    if sets == 2:
-        return g_means3D, g_means2D, g_colors, g_opac, g_scales, g_rot, g_cov3D, g_colors2
-    return g_means3D, g_means2D, g_colors, g_opac, g_scales, g_rot, g_cov3D
+    grad_out_color2 = _f32c(grad_out_color2, "grad_out_color2")
+    e = lambda *shape: torch.empty(shape, dtype=torch.float32, device=device)
+    g_means3D, g_means2D, g_colors, g_opac = e(P, 3), e(P, 3), e(P, 3), e(P, 1)
+    have_sr = _given(scales)
+    g_scales = e(P, 3) if have_sr else torch.zeros((P, 3), dtype=torch.float32, device=device)
+    g_rot = e(P, 4) if have_sr else torch.zeros((P, 4), dtype=torch.float32, device=device)
+    g_cov3D = None if have_sr else e(P, 6)     # only the cov3D_precomp branch has a consumer for it
+    g_colors2 = e(P, 3) if sets == 2 else None
+    bwd_ws = _ws(_sizes(P, int(pack.c.image_width), int(pack.c.image_height), sets)[2], device)
+    _lib.call("sb_backward", ctypes.byref(pack.c), P, state.num_rendered, means3D, colors_precomp, scales, rotations,
+              cov3Ds_precomp, radii, state.geom, state.geom.numel(), state.binning, state.binning.numel(), state.image,
+              state.image.numel(), bwd_ws, bwd_ws.numel(), grad_out_color, grad_out_color2, g_means3D, g_means2D,
+              g_colors, g_colors2, g_opac, g_scales if have_sr else None, g_rot if have_sr else None, g_cov3D,
+              device=device)
+    return g_means3D, g_means2D, g_colors, g_colors2, g_opac, g_scales, g_rot, g_cov3D
+
+
+def _sh_forward(sh, means3D, raster_settings):
+    """SH colours -> rgb for the colours-precomp path (forward.cu:241-247).  Returns (rgb, what _sh_backward needs)."""
+    sh_c = _f32c(sh, "shs")
+    m_c = _f32c(means3D, "means3D")
+    P, M = sh_c.shape[0], sh_c.shape[1]
+    deg = int(raster_settings.sh_degree)
+    rgb = torch.empty((P, 3), dtype=torch.float32, device=m_c.device)
+    clamped = torch.empty((P,), dtype=torch.uint8, device=m_c.device)
+    campos = _f32c(raster_settings.campos.to(m_c.device), "campos")
+    _lib.call("sb_sh_forward", P, deg, M, m_c, campos, sh_c, rgb, clamped, device=m_c.device)
+    return rgb, (sh_c, clamped, campos, M, deg, sh.shape)
+
+
+def _sh_backward(sh_saved, means3D, radii, g_colors, g_means3D):
+    """dL/dshs from dL/drgb; adds the view-direction term to g_means3D in place."""
+    sh_c, clamped, campos, M, deg, sh_shape = sh_saved
+    P = means3D.shape[0]
+    g_sh = torch.empty((P, M, 3), dtype=torch.float32, device=means3D.device)
+    _lib.call("sb_sh_backward", P, deg, M, means3D, campos, sh_c, clamped, g_colors, radii, g_sh, g_means3D,
+              device=means3D.device)
+    return g_sh.reshape(sh_shape)
 
 
 class _RasterizeGaussians(torch.autograd.Function):
@@ -272,37 +252,23 @@ class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                 raster_settings, capacity=None):
-        if P_is_zero(means3D):
+        ctx.empty = means3D.shape[0] == 0
+        if ctx.empty:
             H, W = int(raster_settings.image_height), int(raster_settings.image_width)
             dev = means3D.device
-            ctx.empty = True
             ctx.dev = dev
             ctx.shapes = (means3D.shape, means2D.shape, colors_precomp.shape, opacities.shape, scales.shape,
                           rotations.shape)
             # rasterize_points.cu:67-75,81: P == 0 returns the zero-filled images without launching
             return (torch.zeros((3, H, W), device=dev), torch.zeros((0,), dtype=torch.int32, device=dev),
                     torch.zeros((1, H, W), device=dev))
-        use_sh = sh is not None and sh.numel() != 0
         ctx.sh = None
-        if use_sh:     # SH colours -> rgb, then the colours-precomp path (forward.cu:241-247)
-            sh_c = _f32c(sh, "shs")
-            m_c = _f32c(means3D, "means3D")
-            P, M = sh_c.shape[0], sh_c.shape[1]
-            rgb = torch.empty((P, 3), dtype=torch.float32, device=m_c.device)
-            clamped = torch.empty((P,), dtype=torch.uint8, device=m_c.device)
-            campos = _f32c(raster_settings.campos.to(m_c.device), "campos")
-            with torch.cuda.device(m_c.device):
-                _lib.check(_lib.load().sb_sh_forward(P, int(raster_settings.sh_degree), M, m_c.data_ptr(),
-                                                     campos.data_ptr(), sh_c.data_ptr(), rgb.data_ptr(),
-                                                     clamped.data_ptr(), _stream(m_c.device)), "sb_sh_forward")
-            colors_precomp = rgb
-            ctx.sh = (sh_c, clamped, campos, M, int(raster_settings.sh_degree), sh.shape)
-        color, radii, depth, state, saved = _forward_impl(
+        if _given(sh):
+            colors_precomp, ctx.sh = _sh_forward(sh, means3D, raster_settings)
+        color, _, radii, depth, ctx.state, saved = _forward_impl(
             means3D, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings, capacity=capacity)
-        ctx.empty = False
-        ctx.state = state
         ctx.opac_shape = opacities.shape
-        ctx.save_for_backward(radii, *[t if t is not None else torch.empty(0) for t in saved])
+        ctx.save_for_backward(radii, *saved)
         ctx.mark_non_differentiable(radii, depth)
         return color, radii, depth
 
@@ -313,23 +279,13 @@ class _RasterizeGaussians(torch.autograd.Function):
             z = [torch.zeros(s, device=ctx.dev) for s in ctx.shapes]
             return z[0], z[1], None, z[2], z[3], z[4], z[5], None, None, None
         radii, *saved = ctx.saved_tensors
-        g_means3D, g_means2D, g_colors, g_opac, g_scales, g_rot, g_cov3D = _backward_impl(
+        g_means3D, g_means2D, g_colors, _, g_opac, g_scales, g_rot, g_cov3D = _backward_impl(
             ctx.state, saved, radii, grad_out_color)
-        needs_cov = saved[4].numel() != 0
+        g_sh = None
         if ctx.sh is not None:
-            sh_c, clamped, campos, M, deg, sh_shape = ctx.sh
-            means3D = saved[0]
-            g_sh = torch.empty((means3D.shape[0], M, 3), dtype=torch.float32, device=means3D.device)
-            with torch.cuda.device(means3D.device):
-                _lib.check(_lib.load().sb_sh_backward(means3D.shape[0], deg, M, means3D.data_ptr(), campos.data_ptr(),
-                                                      sh_c.data_ptr(), clamped.data_ptr(), g_colors.data_ptr(),
-                                                      radii.data_ptr(), g_sh.data_ptr(), g_means3D.data_ptr(),
-                                                      _stream(means3D.device)),
-                           "sb_sh_backward")
-            return (g_means3D, g_means2D, g_sh.reshape(sh_shape), None, g_opac.reshape(ctx.opac_shape),
-                    g_scales if not needs_cov else None, g_rot if not needs_cov else None,
-                    g_cov3D if needs_cov else None, None, None)
-        return (g_means3D, g_means2D, None, g_colors, g_opac.reshape(ctx.opac_shape),
+            g_sh, g_colors = _sh_backward(ctx.sh, saved[0], radii, g_colors, g_means3D), None
+        needs_cov = _given(saved[4])
+        return (g_means3D, g_means2D, g_sh, g_colors, g_opac.reshape(ctx.opac_shape),
                 g_scales if not needs_cov else None, g_rot if not needs_cov else None,
                 g_cov3D if needs_cov else None, None, None)
 
@@ -342,15 +298,13 @@ class _RasterizeGaussiansFused(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, colors_precomp, colors_extra, opacities, scales, rotations, raster_settings,
                 capacity=None):
-        if P_is_zero(means3D):
+        if means3D.shape[0] == 0:
             raise _lib.SplatamB200Error("fused render needs at least one Gaussian")
-        empty = torch.empty(0)
-        color, color2, radii, depth, state, saved = _forward_impl(
-            means3D, colors_precomp, opacities, scales, rotations, empty, raster_settings, colors2=colors_extra,
+        color, color2, radii, depth, ctx.state, saved = _forward_impl(
+            means3D, colors_precomp, opacities, scales, rotations, None, raster_settings, colors2=colors_extra,
             capacity=capacity)
-        ctx.state = state
         ctx.opac_shape = opacities.shape
-        ctx.save_for_backward(radii, *[t if t is not None else torch.empty(0) for t in saved])
+        ctx.save_for_backward(radii, *saved)
         ctx.mark_non_differentiable(radii, depth)
         return color, color2, radii, depth
 
@@ -361,13 +315,9 @@ class _RasterizeGaussiansFused(torch.autograd.Function):
             grad_color = torch.zeros_like(grad_color2)
         if grad_color2 is None:
             grad_color2 = torch.zeros_like(grad_color)
-        g_means3D, g_means2D, g_colors, g_opac, g_scales, g_rot, _g_cov, g_colors2 = _backward_impl(
-            ctx.state, tuple(saved), radii, grad_color, grad_color2)
+        g_means3D, g_means2D, g_colors, g_colors2, g_opac, g_scales, g_rot, _ = _backward_impl(
+            ctx.state, saved, radii, grad_color, grad_color2)
         return (g_means3D, g_means2D, g_colors, g_colors2, g_opac.reshape(ctx.opac_shape), g_scales, g_rot, None, None)
-
-
-def P_is_zero(means3D):
-    return means3D.shape[0] == 0
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
@@ -400,7 +350,6 @@ class GaussianRasterizer(nn.Module):
 
     def markVisible(self, positions):
         """Boolean mask ``view_z > 0.2`` per point (reference __init__.py:152-161)."""
-        lib = _lib.load()
         with torch.no_grad():
             rs = self.raster_settings
             pos = _f32c(positions, "positions")
@@ -409,9 +358,7 @@ class GaussianRasterizer(nn.Module):
             if P:
                 view = _f32c(rs.viewmatrix.to(pos.device), "viewmatrix")
                 proj = _f32c(rs.projmatrix.to(pos.device), "projmatrix")
-                with torch.cuda.device(pos.device):
-                    _lib.check(lib.sb_mark_visible(P, pos.data_ptr(), view.data_ptr(), proj.data_ptr(),
-                                                   present.data_ptr(), _stream(pos.device)), "sb_mark_visible")
+                _lib.call("sb_mark_visible", P, pos, view, proj, present, device=pos.device)
         return present
 
     def forward_fused(self, means3D, means2D, opacities, colors_precomp, colors_extra, scales, rotations):

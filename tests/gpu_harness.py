@@ -14,7 +14,6 @@ GRADS = ["means3D", "means2D", "colors", "opacities", "scales", "rotations"]
 
 
 def run_ours(scene, dL=None, device="cuda:0", intermediates=True):
-    lib = _lib.load()
     dev = torch.device(device)
     rs = scene.settings(S.GaussianRasterizationSettings, dev)
     inp = scene.inputs(dev, requires_grad=dL is not None)
@@ -28,15 +27,11 @@ def run_ours(scene, dL=None, device="cuda:0", intermediates=True):
         tiles = ((W + 15) // 16) * ((H + 15) // 16)
         t = lambda shape, dt: torch.zeros(shape, dtype=dt, device=dev)
         depths, m2, co, tt = t(P, torch.float32), t((P, 2), torch.float32), t((P, 4), torch.float32), t(P, torch.int32)
-        cs = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        _lib.check(lib.sb_export_geometry(P, st.geom.data_ptr(), st.geom.numel(), depths.data_ptr(), m2.data_ptr(),
-                                          co.data_ptr(), tt.data_ptr(), cs), "export_geometry")
+        _lib.call("sb_export_geometry", P, st.geom, st.geom.numel(), depths, m2, co, tt, device=dev)
         keys, lst = t(max(R, 1), torch.int64), t(max(R, 1), torch.int32)
         ranges, fT, nc = t((tiles, 2), torch.int32), t((H, W), torch.float32), t((H, W), torch.int32)
-        _lib.check(lib.sb_export_binning(ctypes.byref(st.settings.c), P, R, st.geom.data_ptr(), st.geom.numel(),
-                                         st.binning.data_ptr(), st.binning.numel(), st.image.data_ptr(),
-                                         st.image.numel(), keys.data_ptr(), lst.data_ptr(), ranges.data_ptr(),
-                                         fT.data_ptr(), nc.data_ptr(), cs), "export_binning")
+        _lib.call("sb_export_binning", ctypes.byref(st.settings.c), P, R, st.geom, st.geom.numel(), st.binning,
+                  st.binning.numel(), st.image, st.image.numel(), keys, lst, ranges, fT, nc, device=dev)
         torch.cuda.synchronize(dev)
         out.update(depths=depths.cpu().numpy(), means2D=m2.cpu().numpy(), conic_opacity=co.cpu().numpy(),
                    tiles_touched=tt.cpu().numpy().view(np.uint32), keys=keys.cpu().numpy().view(np.uint64)[:R],

@@ -18,31 +18,39 @@ def _declared_symbols():
     return sorted(set(re.findall(r"SB_API\s+(?:const\s+char\*|int|size_t)\s+(sb_\w+)\s*\(", text)))
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_every_declared_symbol_of_abi_4():
     lib = _lib.load()
     declared = _declared_symbols()
     assert len(declared) >= 14
     for name in declared:
         assert hasattr(lib, name), name
     assert sorted(_lib.EXPORTED_SYMBOLS) == declared, "python binding table out of sync with the header"
-    assert lib.sb_abi_version() == 3
+    assert lib.sb_abi_version() == 4
     assert lib.sb_status_string(0) == b"SB_OK" and lib.sb_status_string(3) == b"SB_ERR_CUDA"
 
 
-def test_workspace_sizes():
+def test_workspace_sizes_per_color_set():
     lib = _lib.load()
     n = ctypes.c_size_t(0)
     assert lib.sb_geometry_workspace_bytes(1_000_000, ctypes.byref(n)) == 0
     per_gaussian = n.value / 1e6
     assert 60 <= per_gaussian <= 84, per_gaussian           # 60 B/Gaussian + 8 B ping-pong pair + sort/scan temp
-    assert lib.sb_binning_workspace_bytes(2_500_000, 1200, 680, ctypes.byref(n)) == 0
+    assert lib.sb_binning_workspace_bytes(2_500_000, 1200, 680, 1, ctypes.byref(n)) == 0
     assert 64 <= n.value / 2.5e6 <= 76                      # 48-B records + 16 B of sort arrays + 8 B ping-pong pair
+    one_set = n.value
+    assert lib.sb_binning_workspace_bytes(2_500_000, 1200, 680, 2, ctypes.byref(n)) == 0
+    assert n.value >= one_set + 16 * 2_500_000               # the second colour set adds a 16-B record per instance
     assert lib.sb_image_workspace_bytes(1200, 680, ctypes.byref(n)) == 0
     assert n.value >= 8 * 1200 * 680
-    assert lib.sb_backward_workspace_bytes(10, ctypes.byref(n)) == 0 and n.value >= 480
+    assert lib.sb_backward_workspace_bytes(10, 1, ctypes.byref(n)) == 0 and n.value >= 480
+    assert lib.sb_backward_workspace_bytes(1000, 1, ctypes.byref(n)) == 0
+    one_set = n.value
+    assert lib.sb_backward_workspace_bytes(1000, 2, ctypes.byref(n)) == 0 and n.value > one_set   # wider accumulator rows
     assert lib.sb_geometry_workspace_bytes(-1, ctypes.byref(n)) == 1      # SB_ERR_BAD_ARG
     assert lib.sb_image_workspace_bytes(0, 10, ctypes.byref(n)) == 1
     assert lib.sb_geometry_workspace_bytes(5, None) == 1
+    assert lib.sb_binning_workspace_bytes(100, 64, 64, 3, ctypes.byref(n)) == 1    # color_sets must be 1 or 2
+    assert lib.sb_backward_workspace_bytes(10, 0, ctypes.byref(n)) == 1
 
 
 def test_bad_arguments_are_rejected_before_any_launch():

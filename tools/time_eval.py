@@ -9,7 +9,6 @@ installed).  Prints the GPU name and power limit of the run and one JSON line:
   reference_metrics_ms_per_frame  the reference-style metric path for one frame (GPU PyTorch + .cpu() + CPU MS-SSIM)
 Run:  python tools/time_eval.py [--frames 200] [--reps 100] [--ref-frames 5]"""
 import argparse
-import ctypes
 import json
 import os
 import subprocess
@@ -91,7 +90,6 @@ def main():
     wall = time.perf_counter() - t0
 
     # the metric kernels alone on frame 1's renders, CUDA events over --reps calls
-    lib = _lib.load()
     H, W = sc.h, sc.w
     with torch.no_grad():
         im, ds, _, _ = M._render_pair(params, dict(frames[1], cam=cam), M.default_render, True, camera_grad=False)
@@ -99,14 +97,12 @@ def main():
     gt_im, gt_d = frames[1]["im"].contiguous(), frames[1]["depth"].contiguous()
     w_im, w_gt = torch.empty_like(im), torch.empty_like(im)
     metrics = torch.zeros(6, dtype=torch.float64, device=dev)
-    ws_f = EV._workspace(lib.sb_frame_metrics_workspace_bytes, H, W, device=dev)
-    ws_s = EV._workspace(lib.sb_ms_ssim_workspace_bytes, 1, 3, H, W, device=dev)
-    st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    ws_f = torch.empty(_lib.nbytes("sb_frame_metrics_workspace_bytes", H, W), dtype=torch.uint8, device=dev)
+    ws_s = torch.empty(_lib.nbytes("sb_ms_ssim_workspace_bytes", 1, 3, H, W), dtype=torch.uint8, device=dev)
 
     def kernels():
-        _lib.check(lib.sb_frame_metrics(im.data_ptr(), ds.data_ptr(), gt_im.data_ptr(), gt_d.data_ptr(), H, W,
-                                        args.sil_thres, 1, w_im.data_ptr(), w_gt.data_ptr(), ws_f.data_ptr(),
-                                        ws_f.numel(), metrics.data_ptr(), st), "sb_frame_metrics")
+        _lib.call("sb_frame_metrics", im, ds, gt_im, gt_d, H, W, args.sil_thres, 1, w_im, w_gt, ws_f, ws_f.numel(),
+                  metrics, device=dev)
         EV._ms_ssim_into(w_im[None], w_gt[None], 1.0, None, metrics[5], ws_s)
     for _ in range(10):
         kernels()
