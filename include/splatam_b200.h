@@ -307,6 +307,16 @@ SB_API int sb_ms_ssim_workspace_bytes(int N, int C, int H, int W, size_t* bytes)
 SB_API int sb_ms_ssim(const float* x, const float* y, int N, int C, int H, int W, double data_range, void* workspace,
                       size_t workspace_bytes, double* per_channel, double* mean, void* stream);
 
+/* ---- frame ingest (the dataset readers, splatam_b200/datasets.py; R/datasets/gradslam_datasets/basedataset.py) ---
+ * One launch: rgb uint8 [color_height, color_width, 3] (HWC) and depth uint16 [depth_height, depth_width] (device)
+ * -> color_out float32 [3, height, width] = float32(bilinear_f64(rgb)) / 255 and depth_out float32 [1, height, width]
+ * = float32(nearest(depth) / png_depth_scale), division in double: cv2.resize INTER_LINEAR / INTER_NEAREST on float64
+ * as the reference's loader calls it, including cv2's exact-2x box average and the plain copy at equal size.  The two
+ * source sizes may differ.  SB_ERR_BAD_ARG for a non-positive size or depth scale and for null pointers. */
+SB_API int sb_ingest_rgbd(const uint8_t* rgb, int color_height, int color_width, const uint16_t* depth,
+                          int depth_height, int depth_width, int height, int width, double png_depth_scale,
+                          float* color_out, float* depth_out, void* stream);
+
 /* ---- per-stage device timing (measurement only; bench.py's roofline pass) -------------------
  * Between sb_profile_begin() and sb_profile_end() every stage launch of this process is bracketed
  * by CUDA events on its stream.  sb_profile_end synchronises, writes the summed milliseconds and call

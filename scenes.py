@@ -2,7 +2,8 @@
 
 Shared by tests/, bench.py, __graft_entry__.smoke() and tests/golden/make_golden.py.  Everything is
 generated on the CPU with a seeded ``torch.Generator`` so the GPU box, this container and the golden
-fixtures all see bit-identical inputs.  No dataset access (Replica / TUM are not available offline).
+fixtures all see bit-identical inputs.  No dataset access (Replica / TUM are not available offline);
+`write_replica_sequence` renders a synthetic sequence on the GPU and writes it in Replica's on-disk layout.
 """
 import math
 
@@ -243,6 +244,38 @@ def dense_opaque(seed=7, P=4000, w=128, h=96):
     opac = 0.9 + 0.1 * _rand(g, P)
     col = _rand(g, P, 3)
     return Scene("dense", w, h, fx, fy, cx, cy, means, col, opac, s, q)
+
+
+def write_replica_sequence(dst, num_frames, device, seed=14, cam=REPLICA, png_depth_scale=6553.5, quality=95):
+    """Writes a sequence in Replica's on-disk layout (results/frame<t>.jpg, results/depth<t>.png, traj.txt of c2w
+    rows) under `dst`: the frames are rendered on `device` from a view-filling surface (`view_filling`) along
+    `slam.look_trajectory`, colour as JPEG and depth as a 16-bit PNG at `png_depth_scale`, depth as a sensor reports it
+    (alpha-normalised, 0 where the silhouette is below 0.9).  Returns the ground-truth w2c matrices [T,4,4] (CPU)."""
+    import os
+    from PIL import Image
+    import splatam_b200 as S
+    from splatam_b200 import mapping as M, slam
+    gen = view_filling(seed=seed, cam=cam, margin=48, opacity=(0.85, 0.95))
+    rs = gen.settings(S.GaussianRasterizationSettings, device)
+    gt = dict(means3D=gen.means3D, rgb_colors=gen.colors, unnorm_rotations=gen.rotations,
+              logit_opacities=torch.logit(gen.opacities.clamp(0.02, 0.98)), log_scales=torch.log(gen.scales[:, :1]))
+    gt = {k: v.to(device).contiguous() for k, v in gt.items()}
+    rots, trans = slam.look_trajectory(num_frames, device)
+    os.makedirs(os.path.join(dst, "results"), exist_ok=True)
+    w2cs, traj = [], []
+    for t in range(num_frames):
+        f = slam.render_frame(gt, rots, trans, t, rs)
+        depth = torch.where(f["sil"] > 0.9, f["depth"] / f["sil"].clamp(min=1e-6), torch.zeros_like(f["depth"]))
+        rgb = (f["im"].clamp(0, 1) * 255).round().to(torch.uint8).permute(1, 2, 0).cpu().numpy()
+        raw = (depth[0] * png_depth_scale).round().clamp(0, 65535).cpu().numpy().astype(np.uint16)
+        Image.fromarray(rgb).save(os.path.join(dst, "results", "frame%06d.jpg" % t), quality=quality)
+        Image.fromarray(raw).save(os.path.join(dst, "results", "depth%06d.png" % t))
+        w2c = M.camera_w2c(rots[..., t], trans[..., t])[0].detach().double().cpu()
+        w2cs.append(w2c)
+        traj.append(" ".join("%.17g" % v for v in torch.linalg.inv(w2c).reshape(-1).tolist()))
+    with open(os.path.join(dst, "traj.txt"), "w") as fh:
+        fh.write("\n".join(traj) + "\n")
+    return torch.stack(w2cs)
 
 
 def algorithmic_bytes(P, R, w, h):

@@ -88,6 +88,7 @@ _SIGNATURES = {
     "sb_frame_metrics": (_i, [_vp, _vp, _vp, _vp, _i, _i, ctypes.c_float, _i, _vp, _vp, _vp, _sz, _vp, _vp]),
     "sb_ms_ssim_workspace_bytes": (_i, [_i, _i, _i, _i, ctypes.POINTER(_sz)]),
     "sb_ms_ssim": (_i, [_vp, _vp, _i, _i, _i, _i, ctypes.c_double, _vp, _sz, _vp, _vp, _vp]),
+    "sb_ingest_rgbd": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, ctypes.c_double, _vp, _vp, _vp]),
     "sb_profile_begin": (_i, []),
     "sb_profile_end": (_i, [ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_int)]),
     "sb_stage_name": (ctypes.c_char_p, [_i]),

@@ -1,0 +1,116 @@
+#!/usr/bin/env python
+"""SplaTAM on a recorded sequence: reads Replica, TUM-RGBD or ScanNet from disk (splatam_b200.datasets), runs the SLAM
+loop (splatam_b200.slam.run_slam) from the back-projection of frame 0 with the shipped hyper-parameters of
+R/configs/{replica,tum,scannet}/splatam.py, then the final evaluation (splatam_b200.evaluate) against the dataset's
+ground-truth poses.  One GPU.
+
+  python tools/run_slam_dataset.py --dataset replica --basedir data/Replica --sequence room0
+  python tools/run_slam_dataset.py --dataset tum --basedir data/TUM_RGBD --sequence rgbd_dataset_freiburg1_desk
+
+--config takes a data YAML of the reference's shape (default: the shipped camera of the dataset); --start / --end /
+--stride select frames as the reference does; --frames caps the number of frames; --tracking-iters / --mapping-iters
+override the shipped iteration counts.  Prints one JSON line: ATE, PSNR, MS-SSIM, depth L1, Gaussian count, tracking
+and mapping wall times, and the load time per frame that the SLAM loop waited for (decode + upload not hidden by the
+prefetch).  --out DIR writes params.npz and the reference's psnr.txt / rmse.txt / l1.txt / ssim.txt."""
+import argparse
+import json
+import os
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+
+_PRUNE = dict(start_after=0, remove_big_after=0, stop_after=20, prune_every=20, removal_opacity_threshold=0.005,
+              final_removal_opacity_threshold=0.005, reset_opacities=False, reset_opacities_every=500)
+# R/configs/<dataset>/splatam.py: image size, iterations, keyframe / map period, window, radius ratio, eval period
+HYPER = {
+    "replica": dict(height=680, width=1200, tracking_iters=40, mapping_iters=60, keyframe_every=5, map_every=1,
+                    window=24, scene_radius_depth_ratio=3, eval_every=5),
+    "tum": dict(height=480, width=640, tracking_iters=200, mapping_iters=30, keyframe_every=5, map_every=1, window=20,
+                scene_radius_depth_ratio=2, eval_every=500),
+    "scannet": dict(height=480, width=640, tracking_iters=100, mapping_iters=30, keyframe_every=5, map_every=1,
+                    window=10, scene_radius_depth_ratio=3, eval_every=500),
+}
+SIL_THRES = 0.5          # mapping: add_new_gaussians' silhouette threshold
+
+
+class _Capped:
+    """The first n frames of a sequence (the loop and the evaluation only use len() and [t])."""
+
+    def __init__(self, seq, n):
+        self.seq, self.n = seq, min(n, len(seq)) if n else len(seq)
+
+    def __len__(self):
+        return self.n
+
+    def __getitem__(self, t):
+        if not 0 <= t < self.n:
+            raise IndexError(t)
+        return self.seq[t]
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--dataset", required=True, choices=sorted(HYPER))
+    ap.add_argument("--basedir", required=True)
+    ap.add_argument("--sequence", required=True)
+    ap.add_argument("--config", default=None, help="data YAML (camera_params); default: the shipped camera")
+    ap.add_argument("--start", type=int, default=0)
+    ap.add_argument("--end", type=int, default=-1)
+    ap.add_argument("--stride", type=int, default=1)
+    ap.add_argument("--frames", type=int, default=0, help="use only the first N selected frames (0: all)")
+    ap.add_argument("--tracking-iters", type=int, default=0)
+    ap.add_argument("--mapping-iters", type=int, default=0)
+    ap.add_argument("--prefetch", type=int, default=2)
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    from splatam_b200 import datasets, evaluate, slam
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    torch.manual_seed(0); np.random.seed(0)
+    h = dict(HYPER[a.dataset])
+    h["tracking_iters"] = a.tracking_iters or h["tracking_iters"]
+    h["mapping_iters"] = a.mapping_iters or h["mapping_iters"]
+    cfg = datasets.load_config(a.config) if a.config else None
+    seq = datasets.RGBDSequence(a.dataset, a.basedir, a.sequence, cfg, start=a.start, end=a.end, stride=a.stride,
+                                desired_height=h["height"], desired_width=h["width"], device=dev, prefetch=a.prefetch)
+    frames = _Capped(seq, a.frames)
+    T = len(frames)
+    K = seq.intrinsics.cpu()
+    init, _ = slam.initialize_map(frames[0], K)
+    radius = float(frames[0]["depth"].max()) / h["scene_radius_depth_ratio"]
+    timing = {}
+    wait0 = seq.load_wait_s
+    torch.cuda.synchronize(dev)
+    t0 = time.perf_counter()
+    out = slam.run_slam(init, frames, seq.cam, seed=0, timing=timing, tracking_iters=h["tracking_iters"],
+                        mapping_iters=h["mapping_iters"], keyframe_every=h["keyframe_every"], map_every=h["map_every"],
+                        window=h["window"], sil_thres=SIL_THRES, intrinsics=K, add_new_gaussians=True, prune_dict=_PRUNE,
+                        scene_radius=radius, select_keyframes=True, first_frame_iters=h["mapping_iters"],
+                        checkpoint_dir=None)
+    torch.cuda.synchronize(dev)
+    wall = time.perf_counter() - t0
+    load_wait = seq.load_wait_s - wait0
+    gt = [seq.files.poses[t] for t in range(T)]
+    gt_w2c = [torch.linalg.inv(p.to(dev)) for p in gt]
+    params = dict(out["gauss"], cam_unnorm_rots=out["rots"], cam_trans=out["trans"])
+    res = evaluate.evaluate(params, frames, seq.cam, SIL_THRES, h["mapping_iters"], True, eval_every=h["eval_every"],
+                            gt_w2c=gt_w2c, out_dir=a.out)
+    seq.close()
+    if a.out is not None:
+        from splatam_b200 import formats
+        formats.save_params(params, a.out)
+    print(json.dumps(dict(
+        dataset=a.dataset, sequence=a.sequence, frames=T, width=seq.width, height=seq.height, hyper=h,
+        ate_m=res["ate"], psnr_db=res["psnr"], ms_ssim=res["ms_ssim"], depth_l1_m=res["depth_l1"],
+        gaussians=int(out["counts"][-1]), wall_s=wall, tracking_s=timing["tracking_s"], mapping_s=timing["mapping_s"],
+        load_wait_ms_per_frame=1e3 * load_wait / max(T - 1, 1), evaluated_frames=len(res["frame_ids"]),
+        metric_note="ate_m = the reference's Final Average ATE RMSE (mean Horn-aligned residual); load_wait = host "
+                    "time run_slam spent in the reader for frames 1..T-1")))
+
+
+if __name__ == "__main__":
+    main()
