@@ -1,7 +1,8 @@
-"""Readers for the three datasets of SplaTAM's tables -- Replica, TUM-RGBD and ScanNet -- that turn a sequence on
-disk into the frame dicts `slam.run_slam` and `evaluate.evaluate` consume.
+"""Readers for the datasets of SplaTAM's tables -- Replica, TUM-RGBD, ScanNet, ScanNet++ and ReplicaV2 -- that turn a
+sequence on disk into the frame dicts `slam.run_slam`, `evaluate.evaluate` and `evaluate.evaluate_nvs` consume.
 
-They follow the reference's loaders (R/datasets/gradslam_datasets/basedataset.py, replica.py, tum.py, scannet.py):
+They follow the reference's loaders (R/datasets/gradslam_datasets/basedataset.py, replica.py, tum.py, scannet.py,
+scannetpp.py):
 the same files in the same (natural) order, the same `start / end / stride` subsampling, TUM's timestamp association,
 poses relative to the first retained frame, intrinsics scaled to the desired size, and pixels decoded with Pillow
 (imageio's backend for these formats).  What differs is where the per-frame work runs: the reference converts every
@@ -13,10 +14,16 @@ upload and the kernel run on a side stream that the consumer's stream waits on.
 
 Dataset configs have the reference's YAML shape (``camera_params``: image_height / image_width, fx / fy / cx / cy,
 png_depth_scale; crop_edge and distortion are accepted and unused, as in the reference); `default_config` holds the
-values of R/configs/data/{replica,TUM/*,scannet}.yaml.  CUDA only for the pixels: there is no CPU fallback."""
+values of R/configs/data/{replica,TUM/*,scannet,replica_v2}.yaml.  ScanNet++ has no YAML: its camera is read from the
+sequence's dslr/nerfstudio/transforms_undistorted.json.
+
+ScanNet++ and ReplicaV2 also have a held-out test split (``split="test"``) for novel-view evaluation: its frames
+follow the first train frame, which becomes frame 0, so every test pose is relative to it.  CUDA only for the
+pixels: there is no CPU fallback."""
 import collections
 import concurrent.futures
 import glob
+import json
 import os
 import re
 import time
@@ -28,16 +35,20 @@ import torch
 from . import _lib
 from .rasterizer import GaussianRasterizationSettings
 
-DATASETS = ("replica", "tum", "scannet")
+DATASETS = ("replica", "tum", "scannet", "scannetpp", "replicav2")
+SPLITS = ("train", "test")
+_SPLIT_DATASETS = ("scannetpp", "replicav2")         # the datasets that have a held-out test split
 
 
 def _camera_params(h, w, fx, fy, cx, cy, png_depth_scale, **extra):
     return dict(image_height=h, image_width=w, fx=fx, fy=fy, cx=cx, cy=cy, png_depth_scale=png_depth_scale, **extra)
 
 
-# R/configs/data/replica.yaml, scannet.yaml and TUM/*.yaml (the TUM cameras differ per Freiburg sensor)
+# R/configs/data/replica.yaml, scannet.yaml, replica_v2.yaml and TUM/*.yaml (the TUM cameras differ per Freiburg
+# sensor); ReplicaV2's depth PNGs are in millimetres, Replica's in 1/6553.5 m
 _CONFIGS = {
     "replica": _camera_params(680, 1200, 600.0, 600.0, 599.5, 339.5, 6553.5, crop_edge=0),
+    "replicav2": _camera_params(680, 1200, 600.0, 600.0, 599.5, 339.5, 1000.0, crop_edge=0),
     "scannet": _camera_params(968, 1296, 1169.621094, 1167.105103, 646.295044, 489.927032, 1000.0),
     "freiburg1": _camera_params(480, 640, 517.3, 516.5, 318.6, 255.3, 5000.0, crop_edge=8),
     "freiburg2": _camera_params(480, 640, 520.9, 521.0, 325.1, 249.7, 5000.0, crop_edge=8),
@@ -46,10 +57,14 @@ _CONFIGS = {
 
 
 def default_config(dataset, sequence=""):
-    """The reference's shipped data config for `dataset` ("replica", "tum", "scannet"); for TUM the camera of the
-    Freiburg sensor named in `sequence` (freiburg1 when none is named)."""
+    """The reference's shipped data config for `dataset` ("replica", "tum", "scannet", "replicav2"); for TUM the
+    camera of the Freiburg sensor named in `sequence` (freiburg1 when none is named).  ScanNet++ has none: its camera
+    comes with each sequence (`scannetpp_config`)."""
     if dataset not in DATASETS:
         raise ValueError("unknown dataset %r (expected one of %s)" % (dataset, ", ".join(DATASETS)))
+    if dataset == "scannetpp":
+        raise ValueError("scannetpp has no shipped data config: its camera is read from each sequence "
+                         "(scannetpp_config)")
     key = dataset
     if dataset == "tum":
         m = re.search(r"freiburg([123])", sequence)
@@ -80,14 +95,19 @@ def natsorted(paths):
 
 # ---- file discovery and poses (host only) -------------------------------------------------------------------------
 
+def _pose_lines(path, n):
+    """The first `n` c2w rows of a file with one row-major 4x4 matrix per line, as float32 [4,4] tensors."""
+    with open(path) as f:
+        lines = f.readlines()
+    if len(lines) < n:
+        raise ValueError("%s: %d poses for %d images" % (path, len(lines), n))
+    return [torch.from_numpy(np.array([float(v) for v in lines[i].split()]).reshape(4, 4)).float() for i in range(n)]
+
+
 def _replica_files(root):
     colors = natsorted(glob.glob(os.path.join(root, "results", "frame*.jpg")))
     depths = natsorted(glob.glob(os.path.join(root, "results", "depth*.png")))
-    with open(os.path.join(root, "traj.txt")) as f:
-        lines = f.readlines()
-    poses = [torch.from_numpy(np.array([float(v) for v in lines[i].split()]).reshape(4, 4)).float()
-             for i in range(len(colors))]
-    return colors, depths, poses
+    return colors, depths, _pose_lines(os.path.join(root, "traj.txt"), len(colors))
 
 
 def _read_list(path, skiprows=0):
@@ -142,6 +162,74 @@ def _scannet_files(root):
     return colors, depths, poses
 
 
+def _read_json(path):
+    if not os.path.isfile(path):
+        raise FileNotFoundError("%s: no such file" % path)
+    with open(path) as f:
+        return json.load(f)
+
+
+def _scannetpp_meta(root):
+    return _read_json(os.path.join(root, "dslr", "nerfstudio", "transforms_undistorted.json"))
+
+
+def scannetpp_config(root):
+    """The config of the ScanNet++ sequence at `root`, as ScannetPPDataset builds it: the undistorted DSLR camera of
+    dslr/nerfstudio/transforms_undistorted.json (fl_x, fl_y, cx, cy, w, h) and depth PNGs in millimetres."""
+    meta = _scannetpp_meta(root)
+    return dict(dataset_name="scannetpp", camera_params=_camera_params(
+        meta["h"], meta["w"], meta["fl_x"], meta["fl_y"], meta["cx"], meta["cy"], 1000.0))
+
+
+def _scannetpp_files(root, split, ignore_bad):
+    """R/datasets/gradslam_datasets/scannetpp.py: the split's image names in the order of dslr/train_test_lists.json,
+    looked up by file_path in `frames` (train) or `test_frames` (test); the test split starts with the first train
+    frame; with `ignore_bad`, the split's own frames whose metadata has is_bad set are dropped.  Poses are
+    P @ c2w @ P^T with P = diag(1, -1, -1, 1) (OpenGL -> OpenCV camera axes), in float32."""
+    lists = _read_json(os.path.join(root, "dslr", "train_test_lists.json"))
+    meta = _scannetpp_meta(root)
+    P = torch.tensor([[1, 0, 0, 0], [0, -1, 0, 0], [0, 0, -1, 0], [0, 0, 0, 1]]).float()
+
+    def lookup(frames, key, name):
+        index = {fr["file_path"]: i for i, fr in enumerate(frames)}
+        if name not in index:
+            raise ValueError("%s: image %r of the %s list is not in transforms_undistorted.json's %r"
+                             % (root, name, "train" if key == "frames" else "test", key))
+        return frames[index[name]]
+
+    def entry(name, fr):
+        c2w = torch.from_numpy(np.array(fr["transform_matrix"])).float()
+        return (os.path.join(root, "dslr", "undistorted_images", name),
+                os.path.join(root, "dslr", "undistorted_depths", name.replace(".JPG", ".png")), P @ c2w @ P.T)
+
+    key = "frames" if split == "train" else "test_frames"
+    rows = []
+    if split == "test":                               # never dropped, even when it is bad
+        first = lists["train"][0]
+        rows.append(entry(first, lookup(meta["frames"], "frames", first)))
+    for name in lists[split]:
+        fr = lookup(meta[key], key, name)
+        if ignore_bad and fr["is_bad"]:
+            continue
+        rows.append(entry(name, fr))
+    return [r[0] for r in rows], [r[1] for r in rows], [r[2] for r in rows]
+
+
+def _replicav2_files(root, split):
+    """R/datasets/gradslam_datasets/replica.py (ReplicaV2Dataset): train = imap/00, test = imap/01 after imap/00's
+    first frame; rgb/rgb_*.png and depth/depth_*.png in natural order, poses from traj_w_c.txt, one per image."""
+    train = os.path.join(root, "imap", "00")
+    folder = train if split == "train" else os.path.join(root, "imap", "01")
+    colors = natsorted(glob.glob(os.path.join(folder, "rgb", "rgb_*.png")))
+    depths = natsorted(glob.glob(os.path.join(folder, "depth", "depth_*.png")))
+    poses = _pose_lines(os.path.join(folder, "traj_w_c.txt"), len(colors))
+    if split == "test":
+        colors = [os.path.join(train, "rgb", "rgb_0.png")] + colors
+        depths = [os.path.join(train, "depth", "depth_0.png")] + depths
+        poses = _pose_lines(os.path.join(train, "traj_w_c.txt"), 1) + poses
+    return colors, depths, poses
+
+
 _FILES = {"replica": _replica_files, "tum": _tum_files, "scannet": _scannet_files}
 
 
@@ -174,11 +262,26 @@ class SequenceFiles:
     """What a sequence is before any pixel is read: colour and depth paths, relative float32 c2w poses [N,4,4], the
     retained indices into the discovered (for TUM: associated) frames, and the scaled 4x4 intrinsics.
 
-    start / end / stride select frames as the reference does: end = -1 means all, otherwise end > start."""
+    start / end / stride select frames as the reference does: end = -1 means all, otherwise end > start.  `split`:
+    "train", or for ScanNet++ and ReplicaV2 "test" (the first train frame, then the held-out views; start / end /
+    stride apply to that combined list).  `ignore_bad` (ScanNet++ only) drops the frames its metadata marks is_bad."""
 
     def __init__(self, dataset, basedir, sequence, config=None, start=0, end=-1, stride=1, desired_height=None,
-                 desired_width=None):
-        config = default_config(dataset, sequence) if config is None else config
+                 desired_width=None, split="train", ignore_bad=False):
+        if dataset not in DATASETS:
+            raise ValueError("unknown dataset %r (expected one of %s)" % (dataset, ", ".join(DATASETS)))
+        if split not in SPLITS:
+            raise ValueError("split must be one of %s, got %r" % (", ".join(SPLITS), split))
+        if split != "train" and dataset not in _SPLIT_DATASETS:
+            raise ValueError("%s has no %r split (only %s have a test split)" % (dataset, split,
+                                                                                 " and ".join(_SPLIT_DATASETS)))
+        if ignore_bad and dataset != "scannetpp":
+            raise ValueError("ignore_bad applies to scannetpp only")
+        self.root = os.path.join(basedir, sequence)
+        if not os.path.isdir(self.root):
+            raise FileNotFoundError("%s: no such sequence directory" % self.root)
+        if config is None:
+            config = scannetpp_config(self.root) if dataset == "scannetpp" else default_config(dataset, sequence)
         cam = config["camera_params"]
         if start < 0:
             raise ValueError("start must be >= 0, got %d" % start)
@@ -186,13 +289,16 @@ class SequenceFiles:
             raise ValueError("end (%d) must be -1 (all frames) or greater than start (%d)" % (end, start))
         if stride < 1:
             raise ValueError("stride must be >= 1, got %d" % stride)
-        self.dataset, self.root = dataset, os.path.join(basedir, sequence)
+        self.dataset, self.split = dataset, split
         self.height = int(cam["image_height"] if desired_height is None else desired_height)
         self.width = int(cam["image_width"] if desired_width is None else desired_width)
         self.png_depth_scale = float(cam["png_depth_scale"])
-        if not os.path.isdir(self.root):
-            raise FileNotFoundError("%s: no such sequence directory" % self.root)
-        colors, depths, poses = _FILES[dataset](self.root)
+        if dataset == "scannetpp":
+            colors, depths, poses = _scannetpp_files(self.root, split, ignore_bad)
+        elif dataset == "replicav2":
+            colors, depths, poses = _replicav2_files(self.root, split)
+        else:
+            colors, depths, poses = _FILES[dataset](self.root)
         if len(colors) != len(depths):
             raise ValueError("%s: %d colour and %d depth images" % (self.root, len(colors), len(depths)))
         if not colors:
@@ -291,7 +397,8 @@ class RGBDSequence:
 
     ``seq[t]`` is dict(id=t, cam, w2c, im [3,H,W], depth [1,H,W], intrinsics [3,3], gt_w2c [4,4]) on `device`:
     `cam` and `w2c` belong to the first frame (w2c = inv(pose_0), as SplaTAM's initialize_first_timestep computes it),
-    `gt_w2c` = inv(pose_t) of the relative pose (SplaTAM's gt_w2c), `intrinsics` the scaled 3x3 camera matrix.
+    `gt_w2c` = inv(pose_t) of the relative pose (SplaTAM's gt_w2c; on a test split, the held-out view's pose),
+    `intrinsics` the scaled 3x3 camera matrix.
     Colour and depth are fresh tensors per frame (keyframes keep them); the last `cache` frames are remembered, so
     repeated `seq[t]` returns the same tensors.
 
@@ -302,9 +409,9 @@ class RGBDSequence:
     `seq[t]` for frames that were not cached (the load time the caller sees)."""
 
     def __init__(self, dataset, basedir, sequence, config=None, start=0, end=-1, stride=1, desired_height=None,
-                 desired_width=None, device="cuda", prefetch=2, cache=4):
+                 desired_width=None, device="cuda", prefetch=2, cache=4, split="train", ignore_bad=False):
         self.files = SequenceFiles(dataset, basedir, sequence, config, start, end, stride, desired_height,
-                                   desired_width)
+                                   desired_width, split=split, ignore_bad=ignore_bad)
         self.device = torch.device(device)
         if self.device.type == "cuda" and self.device.index is None:
             self.device = torch.device("cuda", torch.cuda.current_device())

@@ -39,6 +39,29 @@ def quat_mult(q1, q2):
                         w1 * y2 - x1 * z2 + y1 * w2 + z1 * x2, w1 * z2 + x1 * y2 - y1 * x2 + z1 * w2]).T
 
 
+def matrix_to_quaternion(R):
+    """Quaternion (w,x,y,z) of a 3x3 rotation matrix, up to sign, without a host synchronisation.
+
+    For a unit quaternion, 1 + R00 + R11 + R22 = 4w^2, 1 + R00 - R11 - R22 = 4x^2, 1 - R00 + R11 - R22 = 4y^2 and
+    1 - R00 - R11 + R22 = 4z^2, and the off-diagonal sums and differences are 4wx = R21 - R12, 4wy = R02 - R20,
+    4wz = R10 - R01, 4xy = R10 + R01, 4xz = R02 + R20, 4yz = R12 + R21.  Row k of `cand` is 4 q_k q / (4 |q_k|) = +-q;
+    the row of the largest |q_k| (at least 1/2) is the well-conditioned one."""
+    m00, m01, m02, m10, m11, m12, m20, m21, m22 = R.reshape(9).unbind()
+    four_sq = torch.stack([1 + m00 + m11 + m22, 1 + m00 - m11 - m22, 1 - m00 + m11 - m22, 1 - m00 - m11 + m22])
+    cand = torch.stack([torch.stack([four_sq[0], m21 - m12, m02 - m20, m10 - m01]),
+                        torch.stack([m21 - m12, four_sq[1], m10 + m01, m02 + m20]),
+                        torch.stack([m02 - m20, m10 + m01, four_sq[2], m12 + m21]),
+                        torch.stack([m10 - m01, m02 + m20, m12 + m21, four_sq[3]])])
+    cand = cand / (2 * torch.sqrt(four_sq.clamp(min=0)))[:, None]
+    return cand.index_select(0, four_sq.argmax().reshape(1))[0]
+
+
+def gt_pose(w2c):
+    """(w2c, normalised quaternion of its rotation [1,4]): the pose argument of a render at a given w2c matrix (the
+    frames' "pose" key), as the reference's eval_nvs transforms the Gaussians by a ground-truth w2c."""
+    return w2c, F.normalize(matrix_to_quaternion(w2c[:3, :3]).unsqueeze(0))
+
+
 def camera_w2c(rot, tran):
     """(rel_w2c [4,4], normalised camera quaternion [1,4]) of an unnormalised camera quaternion [1,4] and a
     translation [1,3] (R/utils/slam_helpers.py:266-275)."""
@@ -57,9 +80,10 @@ def pose_matrices(params, time_idx, camera_grad=False):
     return camera_w2c(rot, tran)
 
 
-def transform_to_frame(params, time_idx, gaussians_grad, camera_grad):
-    """World -> camera-frame Gaussians for frame `time_idx` (R/utils/slam_helpers.py:252-304)."""
-    rel_w2c, cam_rot = pose_matrices(params, time_idx, camera_grad)
+def transform_to_frame(params, time_idx, gaussians_grad, camera_grad, pose=None):
+    """World -> camera-frame Gaussians for frame `time_idx` (R/utils/slam_helpers.py:252-304), or for the given
+    `pose` = (w2c [4,4], normalised quaternion [1,4]) instead of the frame's estimated one."""
+    rel_w2c, cam_rot = pose_matrices(params, time_idx, camera_grad) if pose is None else pose
     dev = params["means3D"].device
     pts, unnorm = params["means3D"], params["unnorm_rotations"]
     if not gaussians_grad:
@@ -170,12 +194,14 @@ def calc_ssim(img1, img2, window_size=11):
 def _render_pair(params, frame, render, fused, camera_grad, max_rendered=None):
     """The RGB and depth/silhouette renders of `frame` -> (image, depth_sil, radii, means2D of the RGB render).  Either
     the Gaussians get gradient or, with `camera_grad`, only the camera pose.  fused: one kernel builds both rendervars
-    (csrc/prepare.cu) from frame["pose"] if given, and the product rasterizer blends both colour sets in one pass (N1),
-    with a fixed instance capacity if `max_rendered`; otherwise the PyTorch glue and two `render` calls."""
+    (csrc/prepare.cu), and the product rasterizer blends both colour sets in one pass (N1), with a fixed instance
+    capacity if `max_rendered`; otherwise the PyTorch glue and two `render` calls.  Both render at frame["pose"]
+    (w2c, normalised quaternion) if given, else at the frame's pose in params."""
     if fused:
         rv_rgb, rv_depth = fused_rendervars(params, frame["id"], frame["w2c"], camera_grad, pose=frame.get("pose"))
     else:
-        tg = transform_to_frame(params, frame["id"], gaussians_grad=not camera_grad, camera_grad=camera_grad)
+        tg = transform_to_frame(params, frame["id"], gaussians_grad=not camera_grad, camera_grad=camera_grad,
+                                pose=frame.get("pose"))
         rv_rgb, rv_depth = rgb_rendervar(params, tg), depth_sil_rendervar(params, frame["w2c"], tg)
     if fused and render is default_render:
         from .rasterizer import GaussianRasterizer
@@ -233,10 +259,12 @@ def mapping_loss(params, frame, render, loss_weights=(0.5, 1.0), ignore_outlier_
     return loss_weights[0] * l_im + loss_weights[1] * l_depth, radius
 
 
-def tracking_loss(params, frame, render, sil_thres=0.99, loss_weights=(0.5, 1.0), fused=False, max_rendered=None):
+def tracking_loss(params, frame, render, sil_thres=0.99, loss_weights=(0.5, 1.0), fused=False, max_rendered=None,
+                  keep=None):
     """SplaTAM get_loss(tracking=True, use_sil_for_loss=True, use_l1=True): only the camera pose of frame
     `frame["id"]` gets gradient; L1 sums over pixels with silhouette > sil_thres and valid depth
-    (R/scripts/splatam.py:220-224,254-288; weights R/configs/replica/splatam.py:65-68)."""
+    (R/scripts/splatam.py:220-224,254-288; weights R/configs/replica/splatam.py:65-68).  `keep`: a dict that receives
+    the unweighted depth L1 sum as "depth" (the reference's losses['depth'])."""
     im, depth_sil, radius, _ = _render_pair(params, frame, render, fused, camera_grad=True, max_rendered=max_rendered)
     if fused:
         from .train_ops import masked_l1
@@ -250,13 +278,19 @@ def tracking_loss(params, frame, render, sil_thres=0.99, loss_weights=(0.5, 1.0)
         # boolean indexing, as the reference: a NaN depth under a cleared mask bit must not reach the sum
         l_depth = torch.abs(frame["depth"] - depth)[mask].sum()
         l_im = torch.abs(frame["im"] - im)[torch.tile(mask, (3, 1, 1))].sum()
+    if keep is not None:
+        keep["depth"] = l_depth
     return loss_weights[0] * l_im + loss_weights[1] * l_depth, radius
 
 
-def track_frame(params, frame, render=None, num_iters=40, lr_rot=0.0004, lr_trans=0.002, fused=None, graph=None):
+def track_frame(params, frame, render=None, num_iters=40, lr_rot=0.0004, lr_trans=0.002, fused=None, graph=None,
+                depth_loss_thres=None):
     """SplaTAM's tracking inner loop for one frame (R/scripts/splatam.py:676-744): Adam on the frame's camera
     quaternion and translation only, keeping the best-loss pose.  `params` holds detached Gaussian tensors and
     cam_unnorm_rots [1,4,T] / cam_trans [1,3,T] leaf tensors.  Returns the list of per-iteration losses.
+    depth_loss_thres: the reference's use_depth_loss_thres rule (splatam.py:727-738): when the unweighted depth L1 sum
+    of iteration `num_iters` (evaluated before its Adam step) is not below it, `num_iters` more iterations run once,
+    with the same Adam state and best-pose record; the list then has 2 * num_iters entries.
     graph: the iteration -- loss forward + backward over the sync-free rasterizer, the Adam step and the best-pose
     bookkeeping, all on the device -- is captured once and replayed, so a frame costs one host synchronisation instead of
     one per iteration (`_TrackingGraph`); None = re-use a cached graph, build one only for loops of >= 100 iterations."""
@@ -268,7 +302,8 @@ def track_frame(params, frame, render=None, num_iters=40, lr_rot=0.0004, lr_tran
         # default policy: always re-use a cached graph; BUILD one only where it pays -- long loops (TUM: 200 iterations
         # per frame) or on request (graph=True: tracking-only runs over a map that stays put).  Building costs about as
         # much as ~40 eager iterations (capacity probe, warm-up, capture into a fresh memory pool).
-        out = _track_frame_graphed(params, frame, num_iters, lr_rot, lr_trans, build=(graph is True or num_iters >= 100))
+        out = _track_frame_graphed(params, frame, num_iters, lr_rot, lr_trans, build=(graph is True or num_iters >= 100),
+                                   depth_loss_thres=depth_loss_thres)
         if out is not None:
             return out              # None: no graph, or the instance capacity overflowed mid-frame -> run eagerly
     rots, trans = params["cam_unnorm_rots"], params["cam_trans"]
@@ -276,9 +311,11 @@ def track_frame(params, frame, render=None, num_iters=40, lr_rot=0.0004, lr_tran
     opt = torch.optim.Adam([{"params": [rots], "lr": lr_rot}, {"params": [trans], "lr": lr_trans}], lr=0.0, eps=1e-15)
     t = frame["id"]
     best, best_rot, best_tran, losses = None, None, None, []
-    for _ in range(num_iters):
+    keep = None if depth_loss_thres is None else {}
+    total = num_iters
+    while len(losses) < total:
         opt.zero_grad(set_to_none=True)
-        loss, _ = tracking_loss(params, frame, render, fused=fused)
+        loss, _ = tracking_loss(params, frame, render, fused=fused, keep=keep)
         loss.backward()
         opt.step()
         with torch.no_grad():
@@ -288,6 +325,8 @@ def track_frame(params, frame, render=None, num_iters=40, lr_rot=0.0004, lr_tran
             if best is None or lv < best:
                 best, best_rot, best_tran = lv, rots[..., t].detach().clone(), trans[..., t].detach().clone()
         losses.append(lv)
+        if keep is not None and len(losses) == num_iters and not float(keep["depth"].detach()) < depth_loss_thres:
+            total = 2 * num_iters
     with torch.no_grad():
         rots[..., t] = best_rot
         trans[..., t] = best_tran
@@ -312,16 +351,23 @@ class _TrackingGraph:
     best-pose bookkeeping, all on the device) bound to ONE map (the parameter tensors' storage), camera and iteration
     count -- not to a pose column: the pose travels through two small leaf tensors.  Re-used frame after frame while the map tensors stay the same objects (tracking-only runs; SLAM phases
     without map growth): a frame then costs two small image copies, `num_iters` graph launches and one host
-    synchronisation."""
+    synchronisation.
 
-    def __init__(self, params, frame, num_iters, lr_rot, lr_trans, slack=1.5):
+    With `depth_loss_thres` the graph records the depth L1 sum too and a frame replays 2 * num_iters iterations; the
+    decision of track_frame's rule is taken on the device after iteration num_iters, and when the frame stops there
+    the remaining replays run gated: they record no loss, update no best pose and raise no overflow.  The frame
+    still costs one host synchronisation; the gated replays cost GPU time."""
+
+    def __init__(self, params, frame, num_iters, lr_rot, lr_trans, slack=1.5, depth_loss_thres=None):
         from .rasterizer import GaussianRasterizer
         dev = params["means3D"].device
         self.dev, self.t, self.num_iters = dev, frame["id"], num_iters
         t = frame["id"]
         rots, trans = params["cam_unnorm_rots"], params["cam_trans"]
         self.gp = dict({k: params[k].detach() for k in GAUSSIAN_KEYS}, cam_unnorm_rots=rots.detach(), cam_trans=trans.detach())
-        self.key = _tracking_key(params, frame, num_iters)
+        self.key = _tracking_key(params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres)
+        self.rule = rule = depth_loss_thres is not None
+        self.replays = 2 * num_iters if rule else num_iters
         gp = self.gp
         cap = _capacity(gp, [frame], slack)         # sized at the starting pose
         self.side = torch.cuda.Stream(dev)
@@ -337,29 +383,40 @@ class _TrackingGraph:
                                         eps=1e-15, capturable=True)
             self.best_loss = torch.full((), float("inf"), device=dev)
             self.best_q, self.best_tr = q.detach().clone(), tr.detach().clone()
-            self.hist = torch.zeros(num_iters, device=dev)
+            self.hist = torch.zeros(self.replays, device=dev)
             self.it = torch.zeros(1, dtype=torch.long, device=dev)
             self.bad_any = torch.zeros(1, device=dev)
+            self.live = torch.ones(1, dtype=torch.bool, device=dev)   # rule only: this replay is a real iteration
 
             def body():
                 q.grad.zero_(); tr.grad.zero_()
+                keep = {} if rule else None
                 loss, _ = tracking_loss(gp, dict(static, pose=camera_w2c(q, tr)), default_render, fused=True,
-                                        max_rendered=cap)
+                                        max_rendered=cap, keep=keep)
                 loss.backward()
                 lossd = loss.detach().reshape(1)
                 bad = (GaussianRasterizer.last_state(dev).header()[2:3] != 0) | ~torch.isfinite(lossd)
                 q.grad.copy_(torch.where(bad, torch.zeros_like(q.grad), q.grad))
                 tr.grad.copy_(torch.where(bad, torch.zeros_like(tr.grad), tr.grad))
-                self.bad_any.add_(bad.float())
+                self.bad_any.add_((bad & self.live).float() if rule else bad.float())
                 self.opt.step()
                 # the reference's rule (splatam.py:703-712): candidate = pose AFTER the step, ranked by the loss evaluated
                 # before it; the first strictly smaller loss wins
                 better = (lossd < self.best_loss) & ~bad
+                if rule:
+                    better = better & self.live
                 self.best_loss.copy_(torch.where(better, lossd, self.best_loss.reshape(1)).reshape(()))
                 self.best_q.copy_(torch.where(better, q.detach(), self.best_q))
                 self.best_tr.copy_(torch.where(better, tr.detach(), self.best_tr))
                 self.hist.scatter_(0, self.it, lossd)
-                self.it.add_(1)
+                if rule:
+                    # a gated replay overwrites slot `it` (the first unused one, num_iters) and does not advance `it`
+                    self.it.add_(self.live.long())
+                    # after the num_iters-th real iteration: continue only if its depth sum is not below the threshold
+                    stop = self.live & (self.it == num_iters) & (keep["depth"].detach().reshape(1) < depth_loss_thres)
+                    self.live.copy_(self.live & ~stop)
+                else:
+                    self.it.add_(1)
             self.body = body
             for _ in range(3):              # warm-up (initialises the capturable Adam state); undone by reset()
                 body()
@@ -376,14 +433,14 @@ class _TrackingGraph:
             for st in self.opt.state.values():
                 st["exp_avg"].zero_(); st["exp_avg_sq"].zero_(); st["step"].zero_()
             self.best_loss.fill_(float("inf")); self.best_q.copy_(self.q); self.best_tr.copy_(self.tr)
-            self.hist.zero_(); self.it.zero_(); self.bad_any.zero_()
+            self.hist.zero_(); self.it.zero_(); self.bad_any.zero_(); self.live.fill_(True)
 
     def run(self, params, frame):
         dev = self.dev
         self.side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(self.side):
             self.reset(params, frame)
-            for _ in range(self.num_iters):
+            for _ in range(self.replays):
                 self.graph.replay()
         torch.cuda.current_stream(dev).wait_stream(self.side)
         if float(self.bad_any) != 0.0:                                   # the one host synchronisation of the frame
@@ -391,29 +448,31 @@ class _TrackingGraph:
         with torch.no_grad():
             params["cam_unnorm_rots"][..., frame["id"]] = self.best_q
             params["cam_trans"][..., frame["id"]] = self.best_tr
-        return self.hist.tolist()
+        hist = self.hist.tolist()
+        return hist[:int(self.it)] if self.rule else hist
 
 
 _TRACK_GRAPHS = {}
 
 
-def _tracking_key(params, frame, num_iters):
+def _tracking_key(params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres):
     return (params["means3D"].data_ptr(), tuple(params["means3D"].shape), params["log_scales"].shape[1],
-            id(frame["cam"]), tuple(frame["im"].shape), num_iters)
+            id(frame["cam"]), tuple(frame["im"].shape), num_iters, lr_rot, lr_trans, depth_loss_thres)
 
 
-def _track_frame_graphed(params, frame, num_iters, lr_rot, lr_trans, build=True):
+def _track_frame_graphed(params, frame, num_iters, lr_rot, lr_trans, build=True, depth_loss_thres=None):
     """Graph-replayed tracking of one frame, or None when no graph is available / an iteration overflowed the instance
     capacity (the caller then runs the frame eagerly).  Graphs are cached per (map storage, camera, pose column,
     iteration count); `build` creates one on a miss (worth it for long loops or when the map stays put)."""
-    key = _tracking_key(params, frame, num_iters)
+    key = _tracking_key(params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres)
     tg = _TRACK_GRAPHS.get(key)
     if tg is None:
         if not build:
             return None
         if len(_TRACK_GRAPHS) >= 2:
             _TRACK_GRAPHS.clear()
-        tg = _TRACK_GRAPHS[key] = _TrackingGraph(params, frame, num_iters, lr_rot, lr_trans)
+        tg = _TRACK_GRAPHS[key] = _TrackingGraph(params, frame, num_iters, lr_rot, lr_trans,
+                                                 depth_loss_thres=depth_loss_thres)
     return tg.run(params, frame)
 
 

@@ -62,7 +62,7 @@ def _curr_w2c(rots, trans, t):
 def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_iters=8, keyframe_every=2,
              window=4, fused=None, seed=0, intrinsics=None, add_new_gaussians=False, sil_thres=0.5, prune_dict=None,
              scene_radius=None, select_keyframes=False, checkpoint_dir=None, first_frame_iters=0, map_every=None,
-             graph=False, timing=None, densify_dict=None):
+             graph=False, timing=None, densify_dict=None, tracking_lrs=(0.0004, 0.002), depth_loss_thres=None):
     """Tracks every frame and maps on keyframes.  gauss_init: dict of the five Gaussian tensors (the map's
     starting point); frames: list of dict(id, cam, w2c, im, depth).  Returns dict(rots, trans, psnr, gauss).
 
@@ -76,8 +76,10 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     the keyframe list, as the reference's two config keys do (splatam.py:777,912).  `graph`: each mapping phase is
     captured into a CUDA graph over the sync-free rasterizer (fused path only).  `densify_dict`: gradient-based
     densification inside the mapping iterations (the reference's `use_gaussian_splatting_densification` branch,
-    splatam.py:863-864; eager steps only -- the map size changes).  `timing`: dict that receives the
-    accumulated wall seconds of tracking / mapping (synchronised) and the mapping iteration count."""
+    splatam.py:863-864; eager steps only -- the map size changes).  `tracking_lrs`: the tracking learning rates of
+    (cam_unnorm_rots, cam_trans); the default is Replica's.  `depth_loss_thres`: track_frame's rule that doubles a
+    frame's tracking iterations while the depth loss stays high (ScanNet++: 20000).  `timing`: dict that receives the
+    accumulated wall seconds of tracking / mapping (synchronised) and the tracking and mapping iteration counts."""
     import time
     map_every = keyframe_every if map_every is None else map_every
     timing = {} if timing is None else timing
@@ -106,10 +108,11 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
         params = dict({k: v.detach() for k, v in mapper.g.params.items()}, cam_unnorm_rots=rots, cam_trans=trans)
         torch.cuda.synchronize(dev) if dev.type == "cuda" else None
         t0 = time.perf_counter()
-        M.track_frame(params, frames[t], render=render, num_iters=tracking_iters, fused=fused)
+        losses = M.track_frame(params, frames[t], render=render, num_iters=tracking_iters, lr_rot=tracking_lrs[0],
+                               lr_trans=tracking_lrs[1], fused=fused, depth_loss_thres=depth_loss_thres)
         torch.cuda.synchronize(dev) if dev.type == "cuda" else None
         timing["tracking_s"] += time.perf_counter() - t0
-        timing["tracking_iters"] += tracking_iters
+        timing["tracking_iters"] += len(losses)
         rots, trans = params["cam_unnorm_rots"].detach(), params["cam_trans"].detach()
         mapper.cam = dict(cam_unnorm_rots=rots, cam_trans=trans)
         cam_now = mapper.sync_camera()            # multi-rank runs: rank 0's tracking result is the pose of record

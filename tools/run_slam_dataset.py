@@ -1,11 +1,14 @@
 #!/usr/bin/env python
-"""SplaTAM on a recorded sequence: reads Replica, TUM-RGBD or ScanNet from disk (splatam_b200.datasets), runs the SLAM
-loop (splatam_b200.slam.run_slam) from the back-projection of frame 0 with the shipped hyper-parameters of
-R/configs/{replica,tum,scannet}/splatam.py, then the final evaluation (splatam_b200.evaluate) against the dataset's
-ground-truth poses.  One GPU.
+"""SplaTAM on a recorded sequence: reads Replica, TUM-RGBD, ScanNet, ScanNet++ or ReplicaV2 from disk
+(splatam_b200.datasets), runs the SLAM loop (splatam_b200.slam.run_slam) from the back-projection of frame 0 with the
+shipped hyper-parameters of R/configs/{replica,tum,scannet,scannetpp,replica_v2}/splatam.py, then the final evaluation
+(splatam_b200.evaluate) against the dataset's ground-truth poses.  ScanNet++ and ReplicaV2 run on their train split;
+with --nvs the test split is read too and the novel-view evaluation (evaluate.evaluate_nvs) is reported as well.
+One GPU.
 
   python tools/run_slam_dataset.py --dataset replica --basedir data/Replica --sequence room0
   python tools/run_slam_dataset.py --dataset tum --basedir data/TUM_RGBD --sequence rgbd_dataset_freiburg1_desk
+  python tools/run_slam_dataset.py --dataset scannetpp --basedir data/ScanNet++/data --sequence 8b5caf3398 --nvs
 
 --config takes a data YAML of the reference's shape (default: the shipped camera of the dataset); --start / --end /
 --stride select frames as the reference does; --frames caps the number of frames; --tracking-iters / --mapping-iters
@@ -33,7 +36,15 @@ HYPER = {
                 scene_radius_depth_ratio=2, eval_every=500),
     "scannet": dict(height=480, width=640, tracking_iters=100, mapping_iters=30, keyframe_every=5, map_every=1,
                     window=10, scene_radius_depth_ratio=3, eval_every=500),
+    "scannetpp": dict(height=584, width=876, tracking_iters=200, mapping_iters=60, keyframe_every=5, map_every=1,
+                      window=24, scene_radius_depth_ratio=3, eval_every=1, tracking_lrs=(0.001, 0.004),
+                      depth_loss_thres=20000),
+    "replicav2": dict(height=680, width=1200, tracking_iters=40, mapping_iters=60, keyframe_every=5, map_every=1,
+                      window=24, scene_radius_depth_ratio=3, eval_every=5),
 }
+# rows without these keys track with Replica's rates and without the depth-loss rule
+# (follow-up: the shipped TUM and ScanNet configs have their own tracking rates)
+_TRACKING_DEFAULTS = dict(tracking_lrs=(0.0004, 0.002), depth_loss_thres=None)
 SIL_THRES = 0.5          # mapping: add_new_gaussians' silhouette threshold
 
 
@@ -66,12 +77,16 @@ def main():
     ap.add_argument("--mapping-iters", type=int, default=0)
     ap.add_argument("--prefetch", type=int, default=2)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--nvs", action="store_true", help="also evaluate novel views on the test split "
+                                                       "(scannetpp, replicav2)")
     a = ap.parse_args()
+    if a.nvs and a.dataset not in ("scannetpp", "replicav2"):
+        ap.error("--nvs needs a dataset with a test split (scannetpp, replicav2)")
     from splatam_b200 import datasets, evaluate, slam
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
     torch.manual_seed(0); np.random.seed(0)
-    h = dict(HYPER[a.dataset])
+    h = dict(_TRACKING_DEFAULTS, **HYPER[a.dataset])
     h["tracking_iters"] = a.tracking_iters or h["tracking_iters"]
     h["mapping_iters"] = a.mapping_iters or h["mapping_iters"]
     cfg = datasets.load_config(a.config) if a.config else None
@@ -90,7 +105,7 @@ def main():
                         mapping_iters=h["mapping_iters"], keyframe_every=h["keyframe_every"], map_every=h["map_every"],
                         window=h["window"], sil_thres=SIL_THRES, intrinsics=K, add_new_gaussians=True, prune_dict=_PRUNE,
                         scene_radius=radius, select_keyframes=True, first_frame_iters=h["mapping_iters"],
-                        checkpoint_dir=None)
+                        checkpoint_dir=None, tracking_lrs=h["tracking_lrs"], depth_loss_thres=h["depth_loss_thres"])
     torch.cuda.synchronize(dev)
     wall = time.perf_counter() - t0
     load_wait = seq.load_wait_s - wait0
@@ -100,6 +115,16 @@ def main():
     res = evaluate.evaluate(params, frames, seq.cam, SIL_THRES, h["mapping_iters"], True, eval_every=h["eval_every"],
                             gt_w2c=gt_w2c, out_dir=a.out)
     seq.close()
+    nvs = {}
+    if a.nvs:
+        with datasets.RGBDSequence(a.dataset, a.basedir, a.sequence, cfg, desired_height=h["height"],
+                                   desired_width=h["width"], device=dev, prefetch=a.prefetch, split="test") as test:
+            r = evaluate.evaluate_nvs(out["gauss"], test, test.cam, SIL_THRES, h["mapping_iters"], True,
+                                      eval_every=h["eval_every"],
+                                      out_dir=None if a.out is None else os.path.join(a.out, "eval_nvs"))
+        nvs = dict(nvs_psnr_db=r["psnr"], nvs_ms_ssim=r["ms_ssim"], nvs_depth_rmse_m=r["depth_rmse"],
+                   nvs_depth_l1_m=r["depth_l1"], nvs_evaluated_frames=len(r["frame_ids"]),
+                   nvs_valid_frames=int(r["valid_nvs_frames"].sum()))
     if a.out is not None:
         from splatam_b200 import formats
         formats.save_params(params, a.out)
@@ -108,6 +133,7 @@ def main():
         ate_m=res["ate"], psnr_db=res["psnr"], ms_ssim=res["ms_ssim"], depth_l1_m=res["depth_l1"],
         gaussians=int(out["counts"][-1]), wall_s=wall, tracking_s=timing["tracking_s"], mapping_s=timing["mapping_s"],
         load_wait_ms_per_frame=1e3 * load_wait / max(T - 1, 1), evaluated_frames=len(res["frame_ids"]),
+        tracking_iters=timing["tracking_iters"], **nvs,
         metric_note="ate_m = the reference's Final Average ATE RMSE (mean Horn-aligned residual); load_wait = host "
                     "time run_slam spent in the reader for frames 1..T-1")))
 

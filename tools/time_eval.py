@@ -7,7 +7,10 @@ installed).  Prints the GPU name and power limit of the run and one JSON line:
   evaluate_frames_per_s      whole evaluate() (two renders + metrics per frame, one read-back at the end)
   metric_kernels_ms_per_frame  sb_frame_metrics + sb_ms_ssim on one frame, CUDA events over --reps calls
   reference_metrics_ms_per_frame  the reference-style metric path for one frame (GPU PyTorch + .cpu() + CPU MS-SSIM)
-Run:  python tools/time_eval.py [--frames 200] [--reps 100] [--ref-frames 5]"""
+--nvs instead times evaluate.evaluate_nvs (renders at the ground-truth poses, the unmasked branch with its extra hole
+count) over --frames held-out views of a view-filling map at ScanNet++'s 876x584 and ReplicaV2's 1200x680, and
+prints nvs_frames_per_s per size.
+Run:  python tools/time_eval.py [--frames 200] [--reps 100] [--ref-frames 5] [--nvs]"""
 import argparse
 import json
 import os
@@ -51,14 +54,48 @@ def reference_metrics(im, depth_sil, gt_im, gt_depth, sil_thres, use_presence):
     return psnr.cpu(), ssim, rmse.cpu(), l1.cpu()
 
 
+def time_nvs(frames_n, sil_thres):
+    """{"WxH": evaluate_nvs frames/s} over a view-filling map seen from `frames_n` poses along slam.look_trajectory."""
+    import splatam_b200 as S
+    from splatam_b200 import evaluate as EV, slam
+    from splatam_b200 import mapping as M
+    dev = torch.device("cuda:0")
+    out = {}
+    for w, h in ((876, 584), (1200, 680)):
+        cam_d = dict(w=w, h=h, fx=w / 2.0, fy=w / 2.0, cx=(w - 1) / 2.0, cy=(h - 1) / 2.0)
+        sc = scenes.view_filling(margin=100, cam=cam_d)
+        cam = sc.settings(S.GaussianRasterizationSettings, dev)
+        gt = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
+                  logit_opacities=torch.logit(sc.opacities.reshape(-1, 1)), log_scales=torch.log(sc.scales[:, :1]))
+        gt = {k: v.to(dev).contiguous() for k, v in gt.items()}
+        rots, trans = slam.look_trajectory(frames_n, dev, step=(0.002, -0.001, 0.001), rot_step=(0.0005, -0.0004, 0.0003))
+        frames = [slam.render_frame(gt, rots, trans, t, cam) for t in range(frames_n)]
+        for t, fr in enumerate(frames):
+            fr["gt_w2c"] = M.camera_w2c(rots[..., t], trans[..., t])[0]
+        EV.evaluate_nvs(gt, frames[:4], cam, sil_thres, 60, True)                 # warm-up
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        res = EV.evaluate_nvs(gt, frames, cam, sil_thres, 60, True)
+        torch.cuda.synchronize()
+        wall = time.perf_counter() - t0
+        out["%dx%d" % (w, h)] = dict(nvs_frames_per_s=round(len(res["frame_ids"]) / wall, 2), gaussians=sc.P,
+                                     evaluated=len(res["frame_ids"]), valid=int(res["valid_nvs_frames"].sum()),
+                                     psnr=round(res["psnr"], 3))
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=200)
     ap.add_argument("--reps", type=int, default=100)
     ap.add_argument("--ref-frames", type=int, default=5)
     ap.add_argument("--sil-thres", type=float, default=0.5)
+    ap.add_argument("--nvs", action="store_true", help="time evaluate_nvs at 876x584 and 1200x680 instead")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "time_eval.py measures on a CUDA device"
+    if args.nvs:
+        print(json.dumps(dict(gpu=gpu_info(), frames=args.frames, **time_nvs(args.frames, args.sil_thres))))
+        return
     import splatam_b200 as S
     from splatam_b200 import _lib, evaluate as EV, slam
     from splatam_b200 import mapping as M
