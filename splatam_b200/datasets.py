@@ -10,7 +10,8 @@ frame to float64 on the host, resizes it with cv2, divides the depth and uploads
 from pageable memory, synchronously.  Here the raw uint8 colour and uint16 depth (5 B per pixel) are uploaded from pinned memory and one
 CUDA kernel (csrc/ingest.cu, `ingest_rgbd`) resizes, scales and lays them out exactly as the reference's float path
 does.  With `prefetch` > 0 a host thread decodes the next frames while the GPU works on the current one, and the
-upload and the kernel run on a side stream that the consumer's stream waits on.
+upload and the kernel run on a side stream that the consumer's stream waits on.  With a separate densification size
+(SplaTAM-S) a second launch of the same kernel turns the already uploaded pixels into the frame at that size.
 
 Dataset configs have the reference's YAML shape (``camera_params``: image_height / image_width, fx / fy / cx / cy,
 png_depth_scale; crop_edge and distortion are accepted and unused, as in the reference); `default_config` holds the
@@ -24,6 +25,7 @@ import collections
 import concurrent.futures
 import glob
 import json
+import numbers
 import os
 import re
 import time
@@ -260,7 +262,8 @@ def scaled_intrinsics(cam, height, width):
 
 class SequenceFiles:
     """What a sequence is before any pixel is read: colour and depth paths, relative float32 c2w poses [N,4,4], the
-    retained indices into the discovered (for TUM: associated) frames, and the scaled 4x4 intrinsics.
+    retained indices into the discovered (for TUM: associated) frames, the native camera (`camera_params`) and the
+    scaled 4x4 intrinsics.
 
     start / end / stride select frames as the reference does: end = -1 means all, otherwise end > start.  `split`:
     "train", or for ScanNet++ and ReplicaV2 "test" (the first train frame, then the held-out views; start / end /
@@ -290,6 +293,7 @@ class SequenceFiles:
         if stride < 1:
             raise ValueError("stride must be >= 1, got %d" % stride)
         self.dataset, self.split = dataset, split
+        self.camera_params = dict(cam)
         self.height = int(cam["image_height"] if desired_height is None else desired_height)
         self.width = int(cam["image_width"] if desired_width is None else desired_width)
         self.png_depth_scale = float(cam["png_depth_scale"])
@@ -402,14 +406,28 @@ class RGBDSequence:
     Colour and depth are fresh tensors per frame (keyframes keep them); the last `cache` frames are remembered, so
     repeated `seq[t]` returns the same tensors.
 
+    densify_height / densify_width (both or neither): the densification resolution of SplaTAM-S
+    (R/scripts/splatam.py:498-507,781-794).  When it differs from the desired size, every frame dict also carries
+    ``densify`` = dict(id, cam, w2c, im [3,h,w], depth [1,h,w], intrinsics [3,3]) at that size: `intrinsics` scaled
+    to it (`densify_intrinsics`), `cam` = `densify_cam` (that size, the first frame's w2c), and the pixels from a
+    second ingest launch on the same uploaded frame, so each file is decoded and uploaded once.  `run_slam` grows the
+    map from it.  At the desired size, or when not given, there is no ``densify`` entry and both attributes are None.
+
     prefetch = k > 0: while frame t is consumed, a host thread decodes frames t+1 .. t+k into a ring of k pinned
-    staging slots and enqueues their upload and the ingest kernel on a side stream; `seq[t]` makes the caller's
+    staging slots and enqueues their upload and the ingest kernel(s) on a side stream; `seq[t]` makes the caller's
     current stream wait on frame t's event and blocks the host only while frame t is still being decoded.
     prefetch = 0 reads synchronously on the current stream.  `load_wait_s` accumulates the host time spent in
     `seq[t]` for frames that were not cached (the load time the caller sees)."""
 
     def __init__(self, dataset, basedir, sequence, config=None, start=0, end=-1, stride=1, desired_height=None,
-                 desired_width=None, device="cuda", prefetch=2, cache=4, split="train", ignore_bad=False):
+                 desired_width=None, device="cuda", prefetch=2, cache=4, split="train", ignore_bad=False,
+                 densify_height=None, densify_width=None):
+        if (densify_height is None) != (densify_width is None):
+            raise ValueError("give both densify_height and densify_width or neither, got %r and %r"
+                             % (densify_height, densify_width))
+        for name, v in (("densify_height", densify_height), ("densify_width", densify_width)):
+            if v is not None and (isinstance(v, bool) or not isinstance(v, numbers.Integral) or v <= 0):
+                raise ValueError("%s must be a positive integer, got %r" % (name, v))
         self.files = SequenceFiles(dataset, basedir, sequence, config, start, end, stride, desired_height,
                                    desired_width, split=split, ignore_bad=ignore_bad)
         self.device = torch.device(device)
@@ -420,6 +438,13 @@ class RGBDSequence:
         self.w2c = torch.linalg.inv(self.files.poses[0].to(self.device))
         self.cam = setup_camera(self.width, self.height, self.intrinsics.cpu().numpy(), self.w2c.cpu().numpy(),
                                 self.device)
+        self.densify_height = self.densify_width = self.densify_intrinsics = self.densify_cam = None
+        if densify_height is not None and (int(densify_height), int(densify_width)) != (self.height, self.width):
+            self.densify_height, self.densify_width = int(densify_height), int(densify_width)
+            K_d = scaled_intrinsics(self.files.camera_params, self.densify_height, self.densify_width)
+            self.densify_intrinsics = K_d[:3, :3].to(self.device)
+            self.densify_cam = setup_camera(self.densify_width, self.densify_height,
+                                            self.densify_intrinsics.cpu().numpy(), self.w2c.cpu().numpy(), self.device)
         self.prefetch = int(prefetch)
         self._cache = collections.OrderedDict()
         self._cache_size = max(int(cache), 1)
@@ -451,10 +476,19 @@ class RGBDSequence:
     def _decode(self, t):
         return decode_color(self.files.color_paths[t]), decode_depth(self.files.depth_paths[t])
 
+    def _ingest(self, rgb, depth):
+        """The ingest launch(es) on the current stream for one uploaded frame: (colour, depth) at the desired size and
+        the (colour, depth) pair at the densification size, or None when there is none."""
+        scale = self.files.png_depth_scale
+        color, depth_out = ingest_rgbd(rgb, depth, self.height, self.width, scale)
+        dens = None
+        if self.densify_height is not None:
+            dens = ingest_rgbd(rgb, depth, self.densify_height, self.densify_width, scale)
+        return color, depth_out, dens
+
     def _load_sync(self, t):
         rgb, depth = self._decode(t)
-        return ingest_rgbd(torch.from_numpy(rgb).to(self.device), torch.from_numpy(depth).to(self.device),
-                           self.height, self.width, self.files.png_depth_scale) + (None,)
+        return self._ingest(torch.from_numpy(rgb).to(self.device), torch.from_numpy(depth).to(self.device)) + (None,)
 
     def _load_async(self, t, slot):
         """Worker thread: decode into the slot's pinned arrays, then enqueue upload + ingest on the side stream."""
@@ -467,10 +501,10 @@ class RGBDSequence:
             dd = pd.to(self.device, non_blocking=True)
             slot.copied = torch.cuda.Event()
             slot.copied.record(self._side)
-            color, depth_out = ingest_rgbd(dr, dd, self.height, self.width, self.files.png_depth_scale)
+            out = self._ingest(dr, dd)
             ready = torch.cuda.Event()
             ready.record(self._side)
-        return color, depth_out, ready
+        return out + (ready,)
 
     def _submit(self, t):
         if t in self._pending or t in self._cache or not 0 <= t < len(self):
@@ -482,7 +516,7 @@ class RGBDSequence:
     def _frame(self, t):
         t0 = time.perf_counter()
         if self._pool is None:
-            color, depth, _ = self._load_sync(t)
+            color, depth, dens, _ = self._load_sync(t)
         else:
             self._submit(t)
             for j in range(t + 1, t + 1 + self.prefetch):
@@ -490,14 +524,18 @@ class RGBDSequence:
             fut = self._pending.pop(t)
             for j in [j for j in self._pending if j < t or j > t + self.prefetch]:
                 self._pending.pop(j)                  # stale look-ahead after a jump: its results are dropped
-            color, depth, ready = fut.result()
+            color, depth, dens, ready = fut.result()
             consumer = torch.cuda.current_stream(self.device)
             consumer.wait_event(ready)
-            color.record_stream(consumer)             # allocated on the side stream, used and freed on the consumer's
-            depth.record_stream(consumer)
+            for x in (color, depth) + (dens or ()):
+                x.record_stream(consumer)             # allocated on the side stream, used and freed on the consumer's
         self.load_wait_s += time.perf_counter() - t0
-        return dict(id=t, cam=self.cam, w2c=self.w2c, im=color, depth=depth, intrinsics=self.intrinsics,
-                    gt_w2c=self._gt_w2c(t))
+        fr = dict(id=t, cam=self.cam, w2c=self.w2c, im=color, depth=depth, intrinsics=self.intrinsics,
+                  gt_w2c=self._gt_w2c(t))
+        if dens is not None:
+            fr["densify"] = dict(id=t, cam=self.densify_cam, w2c=self.w2c, im=dens[0], depth=dens[1],
+                                 intrinsics=self.densify_intrinsics)
+        return fr
 
     def __getitem__(self, t):
         if isinstance(t, slice):

@@ -59,6 +59,12 @@ def _curr_w2c(rots, trans, t):
     return M.camera_w2c(rots[..., t], trans[..., t])[0]
 
 
+def _without_densify(frame):
+    """The frame dict without its densification-size copy: keyframes are kept for the whole run, and only the frame
+    being mapped needs the second resolution."""
+    return {k: v for k, v in frame.items() if k != "densify"}
+
+
 def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_iters=8, keyframe_every=2,
              window=4, fused=None, seed=0, intrinsics=None, add_new_gaussians=False, sil_thres=0.5, prune_dict=None,
              scene_radius=None, select_keyframes=False, checkpoint_dir=None, first_frame_iters=0, map_every=None,
@@ -67,7 +73,9 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     starting point); frames: list of dict(id, cam, w2c, im, depth).  Returns dict(rots, trans, psnr, gauss).
 
     The optional stages follow the reference's main loop (R/scripts/splatam.py:776-925): `add_new_gaussians` grows
-    the map from each mapped frame's silhouette holes before mapping, `prune_dict` prunes inside the mapping
+    the map from each mapped frame's silhouette holes before mapping -- from the frame's ``densify`` entry, with that
+    entry's camera and intrinsics, when it has one (SplaTAM-S's densification resolution, splatam.py:781-794; see
+    datasets.RGBDSequence; keyframes are stored without it) --, `prune_dict` prunes inside the mapping
     iterations (prune_gaussians' schedule keys), `select_keyframes` picks the mapping window by re-projection
     overlap (window-2 selected + the last keyframe + the current frame) instead of the last `window` keyframes,
     `checkpoint_dir` writes params<t>.npz per mapped frame and params.npz at the end; `first_frame_iters` mapping
@@ -90,7 +98,7 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     trans = torch.zeros(1, 3, T, device=dev)
     kw = {} if render is None else {"render": render}
     mapper = M.ShardedMapper(gauss_init, rots, trans, seed=seed, fused=fused, track_means2D=densify_dict is not None, **kw)
-    keyframes = [dict(frames[0], est_w2c=torch.eye(4, device=dev))]
+    keyframes = [dict(_without_densify(frames[0]), est_w2c=torch.eye(4, device=dev))]
     counts = [mapper.g.shapes["means3D"][0]]
     for it in range(first_frame_iters):       # the reference maps frame 0 before it tracks frame 1 (splatam.py:777)
         mapper.step([keyframes[0]])
@@ -117,10 +125,14 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
         mapper.cam = dict(cam_unnorm_rots=rots, cam_trans=trans)
         cam_now = mapper.sync_camera()            # multi-rank runs: rank 0's tracking result is the pose of record
         rots, trans = cam_now["cam_unnorm_rots"], cam_now["cam_trans"]
-        cur = dict(frames[t], est_w2c=_curr_w2c(rots, trans, t))
+        frame = frames[t]
+        cur = dict(_without_densify(frame), est_w2c=_curr_w2c(rots, trans, t))
         if t % map_every == 0:
             if add_new_gaussians:
-                mapper.add_new_gaussians(frames[t], t, intrinsics, sil_thres)
+                if "densify" in frame:            # SplaTAM-S: grow the map from the densification-size frame
+                    mapper.add_new_gaussians(frame["densify"], t, frame["densify"]["intrinsics"], sil_thres)
+                else:
+                    mapper.add_new_gaussians(frame, t, intrinsics, sil_thres)
             if select_keyframes:
                 from .keyframes import keyframe_selection_overlap
                 if mapper.world > 1:      # the selection draws from the global RNGs: every rank must draw the same

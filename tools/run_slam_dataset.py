@@ -4,15 +4,19 @@
 shipped hyper-parameters of R/configs/{replica,tum,scannet,scannetpp,replica_v2}/splatam.py, then the final evaluation
 (splatam_b200.evaluate) against the dataset's ground-truth poses.  ScanNet++ and ReplicaV2 run on their train split;
 with --nvs the test split is read too and the novel-view evaluation (evaluate.evaluate_nvs) is reported as well.
+--variant splatam_s runs SplaTAM-S (R/configs/replica/splatam_s.py, Replica only): 10 tracking and 15 mapping
+iterations, a window of 32, and new Gaussians -- the initial map included -- from each frame read at 340x600.
 One GPU.
 
   python tools/run_slam_dataset.py --dataset replica --basedir data/Replica --sequence room0
+  python tools/run_slam_dataset.py --dataset replica --basedir data/Replica --sequence room0 --variant splatam_s
   python tools/run_slam_dataset.py --dataset tum --basedir data/TUM_RGBD --sequence rgbd_dataset_freiburg1_desk
   python tools/run_slam_dataset.py --dataset scannetpp --basedir data/ScanNet++/data --sequence 8b5caf3398 --nvs
 
 --config takes a data YAML of the reference's shape (default: the shipped camera of the dataset); --start / --end /
 --stride select frames as the reference does; --frames caps the number of frames; --tracking-iters / --mapping-iters
-override the shipped iteration counts.  Prints one JSON line: ATE, PSNR, MS-SSIM, depth L1, Gaussian count, tracking
+override the shipped iteration counts.  Prints one JSON line: ATE, PSNR, MS-SSIM, depth L1, initial and final
+Gaussian counts, tracking
 and mapping wall times, and the load time per frame that the SLAM loop waited for (decode + upload not hidden by the
 prefetch).  --out DIR writes params.npz and the reference's psnr.txt / rmse.txt / l1.txt / ssim.txt."""
 import argparse
@@ -41,6 +45,14 @@ HYPER = {
                       depth_loss_thres=20000),
     "replicav2": dict(height=680, width=1200, tracking_iters=40, mapping_iters=60, keyframe_every=5, map_every=1,
                       window=24, scene_radius_depth_ratio=3, eval_every=5),
+}
+# R/configs/replica/splatam_s.py: SplaTAM-S, the fast variant; new Gaussians come from the frame read at the
+# densification size (340x600) while tracking and mapping use 680x1200
+VARIANTS = ("splatam", "splatam_s")
+HYPER_S = {
+    "replica": dict(height=680, width=1200, densify_height=340, densify_width=600, tracking_iters=10,
+                    mapping_iters=15, keyframe_every=5, map_every=1, window=32, scene_radius_depth_ratio=3,
+                    eval_every=5),
 }
 # rows without these keys track with Replica's rates and without the depth-loss rule
 # (follow-up: the shipped TUM and ScanNet configs have their own tracking rates)
@@ -79,24 +91,33 @@ def main():
     ap.add_argument("--out", default=None)
     ap.add_argument("--nvs", action="store_true", help="also evaluate novel views on the test split "
                                                        "(scannetpp, replicav2)")
+    ap.add_argument("--variant", default="splatam", choices=VARIANTS,
+                    help="splatam_s: SplaTAM-S, the fast variant (replica only)")
     a = ap.parse_args()
     if a.nvs and a.dataset not in ("scannetpp", "replicav2"):
         ap.error("--nvs needs a dataset with a test split (scannetpp, replicav2)")
+    if a.variant == "splatam_s" and a.dataset not in HYPER_S:
+        ap.error("--variant splatam_s has a shipped config for %s only" % ", ".join(sorted(HYPER_S)))
     from splatam_b200 import datasets, evaluate, slam
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
     torch.manual_seed(0); np.random.seed(0)
-    h = dict(_TRACKING_DEFAULTS, **HYPER[a.dataset])
+    h = dict(_TRACKING_DEFAULTS, **(HYPER_S if a.variant == "splatam_s" else HYPER)[a.dataset])
     h["tracking_iters"] = a.tracking_iters or h["tracking_iters"]
     h["mapping_iters"] = a.mapping_iters or h["mapping_iters"]
     cfg = datasets.load_config(a.config) if a.config else None
     seq = datasets.RGBDSequence(a.dataset, a.basedir, a.sequence, cfg, start=a.start, end=a.end, stride=a.stride,
-                                desired_height=h["height"], desired_width=h["width"], device=dev, prefetch=a.prefetch)
+                                desired_height=h["height"], desired_width=h["width"], device=dev, prefetch=a.prefetch,
+                                densify_height=h.get("densify_height"), densify_width=h.get("densify_width"))
     frames = _Capped(seq, a.frames)
     T = len(frames)
     K = seq.intrinsics.cpu()
-    init, _ = slam.initialize_map(frames[0], K)
-    radius = float(frames[0]["depth"].max()) / h["scene_radius_depth_ratio"]
+    # the initial map and the scene radius come from the densification-size frame 0 when there is one
+    # (splatam.py:185-206): its max depth can be below the full-size one
+    first = frames[0].get("densify", frames[0])
+    init, _ = slam.initialize_map(first, first["intrinsics"].cpu())
+    initial_gaussians = int(init["means3D"].shape[0])
+    radius = float(first["depth"].max()) / h["scene_radius_depth_ratio"]
     timing = {}
     wait0 = seq.load_wait_s
     torch.cuda.synchronize(dev)
@@ -129,7 +150,9 @@ def main():
         from splatam_b200 import formats
         formats.save_params(params, a.out)
     print(json.dumps(dict(
-        dataset=a.dataset, sequence=a.sequence, frames=T, width=seq.width, height=seq.height, hyper=h,
+        dataset=a.dataset, sequence=a.sequence, variant=a.variant, frames=T, width=seq.width, height=seq.height,
+        densify_height=seq.densify_height, densify_width=seq.densify_width, hyper=h,
+        initial_gaussians=initial_gaussians,
         ate_m=res["ate"], psnr_db=res["psnr"], ms_ssim=res["ms_ssim"], depth_l1_m=res["depth_l1"],
         gaussians=int(out["counts"][-1]), wall_s=wall, tracking_s=timing["tracking_s"], mapping_s=timing["mapping_s"],
         load_wait_ms_per_frame=1e3 * load_wait / max(T - 1, 1), evaluated_frames=len(res["frame_ids"]),
