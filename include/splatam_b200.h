@@ -307,6 +307,26 @@ SB_API int sb_ms_ssim_workspace_bytes(int N, int C, int H, int W, size_t* bytes)
 SB_API int sb_ms_ssim(const float* x, const float* y, int N, int C, int H, int W, double data_range, void* workspace,
                       size_t workspace_bytes, double* per_channel, double* mean, void* stream);
 
+/* ---- LPIPS (AlexNet, v0.1) of the final evaluation (R/utils/eval_helpers.py:484-485, 730-731) ----------------------
+ * torchmetrics' LearnedPerceptualImagePatchSimilarity(net_type='alex', normalize=True) applied to clamp(x, 0, 1) and
+ * clamp(y, 0, 1), forward only, deterministic FP32 (no atomics, no split-K; per-block partials reduced in a fixed
+ * order), no host synchronisation.  x, y: [N,3,H,W] contiguous float; per_image [N] and/or mean (device doubles, either
+ * may be NULL, not both).  Per pair: inputs 2x - 1, then (x - shift) / scale with shift = (-0.030, -0.088, -0.188),
+ * scale = (0.458, 0.448, 0.450); torchvision AlexNet features f1..f5 = relu(conv1..conv5) (3x3 stride-2 max-pools
+ * after f1 and f2); per layer and pixel d = sum_c lin_c (fx / sqrt(1e-8 + |fx|^2) - fy / sqrt(1e-8 + |fy|^2))^2;
+ * LPIPS = sum over the five layers of the mean of d over the layer's pixels.  H and W must be >= 31.
+ * weights: sb_lpips_weights_floats() device floats, packed as
+ *   for l = 0..4: conv_l weight as [K_l][Cout_l], k = (ci * ks + ky) * ks + kx (the transpose of torchvision's
+ *                 features.{0,3,6,8,10}.weight viewed as [Cout_l, K_l]), then conv_l bias [Cout_l];
+ *   then lin_0 .. lin_4 [Cout_l] (lpips' lin{l}.model.1.weight),
+ * with (Cin, Cout, ks) = (3, 64, 11), (64, 192, 5), (192, 384, 3), (384, 256, 3), (256, 256, 3).
+ * workspace: sb_lpips_workspace_bytes(N, H, W) device bytes (any content; ~39 MB per image at 1200x680, and
+ * the 2N images of x and y all run). */
+SB_API int sb_lpips_weights_floats(size_t* n);
+SB_API int sb_lpips_workspace_bytes(int N, int H, int W, size_t* bytes);
+SB_API int sb_lpips(const float* x, const float* y, int N, int H, int W, const float* weights, void* workspace,
+                    size_t workspace_bytes, double* per_image, double* mean, void* stream);
+
 /* ---- frame ingest (the dataset readers, splatam_b200/datasets.py; R/datasets/gradslam_datasets/basedataset.py) ---
  * One launch: rgb uint8 [color_height, color_width, 3] (HWC) and depth uint16 [depth_height, depth_width] (device)
  * -> color_out float32 [3, height, width] = float32(bilinear_f64(rgb)) / 255 and depth_out float32 [1, height, width]

@@ -137,6 +137,22 @@ int launch_mark_visible(int P, const float* means3D, const float* viewmatrix, ui
                         cudaStream_t st);
 
 // ---- device helpers ------------------------------------------------------------------------
+// Sum of one double per thread over a block of NT threads, in a fixed order (deterministic); `red` holds NT / 32
+// doubles of shared memory.  The result is valid in thread tid == 0 only.
+template <int NT>
+__device__ __forceinline__ double block_sum(double v, double* red, int tid) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+    const int lane = tid & 31, warp = tid >> 5;
+    __syncthreads();                      // red may still be read by the previous call
+    if (lane == 0) red[warp] = v;
+    __syncthreads();
+    double s = 0.0;
+    if (tid == 0)
+        for (int w = 0; w < NT / 32; ++w) s += red[w];
+    return s;
+}
+
 // Row k of a reference 4x4 matrix applied to a point, with the exact operation order nvcc emits
 // for `m[k]*p.x + m[k+4]*p.y + m[k+8]*p.z + m[k+12]` (auxiliary.h:58-77):
 //   fadd(fma(p.z, m[k+8], fma(p.x, m[k], fmul(p.y, m[k+4]))), m[k+12])

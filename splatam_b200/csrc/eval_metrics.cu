@@ -24,20 +24,6 @@ constexpr int kFrameMaxBlocks = 528;    // 132 SMs x 4
 int frame_blocks(int HW) { return (HW + kFrameThreads - 1) / kFrameThreads < kFrameMaxBlocks
                                       ? (HW + kFrameThreads - 1) / kFrameThreads : kFrameMaxBlocks; }
 
-template <int NT>
-__device__ __forceinline__ double block_sum(double v, double* red, int tid) {
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-    const int lane = tid & 31, warp = tid >> 5;
-    __syncthreads();                      // red may still be read by the previous call
-    if (lane == 0) red[warp] = v;
-    __syncthreads();
-    double s = 0.0;
-    if (tid == 0)
-        for (int w = 0; w < NT / 32; ++w) s += red[w];
-    return s;                             // valid in thread tid == 0 only
-}
-
 __global__ void __launch_bounds__(kFrameThreads)
 frame_metrics_kernel(const float* __restrict__ im, const float* __restrict__ depth_sil, const float* __restrict__ gt_im,
                      const float* __restrict__ gt_depth, int HW, float sil_thres, int use_presence,

@@ -7,8 +7,9 @@ mapping and tracking (`mapping._render_pair`), one kernel pass per frame writes 
 depth sums, MS-SSIM runs on the device, and the per-frame metrics stay on the device until one read at the end.
 `evaluate_nvs` is the reference's novel-view evaluation (eval_helpers.py:626-841, `eval_nvs`) over a test split: the
 same metrics on held-out views rendered at their ground-truth poses, averaged over the views the map covers.
-LPIPS is not computed (it needs pretrained AlexNet weights): the result carries ``lpips: None``.  CUDA only; no CPU
-fallback."""
+LPIPS (AlexNet, v0.1, csrc/lpips.cu) is opt-in: pass ``lpips=LpipsAlex.load(alexnet_path, lin_path, device)`` with the
+two weight files already on disk (nothing is downloaded); without it the result carries ``lpips: None``.  CUDA only;
+no CPU fallback."""
 import os
 
 import numpy as np
@@ -17,8 +18,8 @@ import torch
 from . import _lib
 from . import mapping as M
 
-# columns of the per-frame metric rows: the five that sb_frame_metrics writes, then MS-SSIM
-_PSNR, _RMSE, _L1, _NVALID, _NMASK, _SSIM = range(6)
+# columns of the per-frame metric rows: the five that sb_frame_metrics writes, then MS-SSIM and LPIPS
+_PSNR, _RMSE, _L1, _NVALID, _NMASK, _SSIM, _LPIPS = range(7)
 
 
 def _ms_ssim_into(x, y, data_range, per_channel, mean, ws=None):
@@ -52,6 +53,88 @@ def ms_ssim(x, y, data_range=1.0, size_average=True):
     return out
 
 
+# (features index, Cin, Cout, kernel) of torchvision's five AlexNet convolutions, in sb_lpips' packing order
+_ALEX_CONVS = ((0, 3, 64, 11), (3, 64, 192, 5), (6, 192, 384, 3), (8, 384, 256, 3), (10, 256, 256, 3))
+
+
+class LpipsAlex:
+    """The weights of LPIPS v0.1 with the AlexNet backbone (torchmetrics' net_type='alex'), packed on one device in
+    the layout sb_lpips reads (include/splatam_b200.h): `weights`, a float32 device tensor."""
+
+    def __init__(self, weights):
+        self.weights = weights
+
+    @classmethod
+    def load(cls, alexnet_path, lin_path, device):
+        """Reads torchvision's ImageNet AlexNet state dict (alexnet-owt-7be5be79.pth; features.{0,3,6,8,10}.{weight,
+        bias}, classifier keys ignored) and LPIPS v0.1's alex.pth (lin{0..4}.model.1.weight, [1,C,1,1]) with
+        torch.load(weights_only=True).  Nothing is downloaded; a missing key or a wrong shape raises
+        SplatamB200Error naming the key."""
+        load = lambda p: torch.load(p, map_location="cpu", weights_only=True)
+        return cls.from_state_dicts(load(alexnet_path), load(lin_path), device)
+
+    @classmethod
+    def from_state_dicts(cls, alexnet, lin, device):
+        """As `load`, from the two state dicts already in memory."""
+        def get(sd, key, shape):
+            if key not in sd:
+                raise _lib.SplatamB200Error("LPIPS weights: missing key %r" % key)
+            t = sd[key]
+            if not isinstance(t, torch.Tensor) or tuple(t.shape) != shape:
+                raise _lib.SplatamB200Error("LPIPS weights: %r has shape %s, expected %s"
+                                            % (key, tuple(getattr(t, "shape", ())), shape))
+            return t.detach().to("cpu", torch.float32)
+        parts = []
+        for idx, cin, cout, k in _ALEX_CONVS:
+            w = get(alexnet, "features.%d.weight" % idx, (cout, cin, k, k))
+            parts += [w.reshape(cout, -1).t().reshape(-1), get(alexnet, "features.%d.bias" % idx, (cout,))]
+        for l, (_, _, cout, _) in enumerate(_ALEX_CONVS):
+            parts.append(get(lin, "lin%d.model.1.weight" % l, (1, cout, 1, 1)).reshape(-1))
+        packed = torch.cat(parts)
+        n = _lib.nbytes("sb_lpips_weights_floats")
+        if packed.numel() != n:
+            raise _lib.SplatamB200Error("LPIPS weights: packed %d floats, sb_lpips reads %d" % (packed.numel(), n))
+        return cls(packed.to(device))
+
+
+def _lpips_into(x, y, net, per_image, mean, ws=None):
+    """Enqueues sb_lpips on contiguous float32 [N,3,H,W] CUDA tensors; `per_image` / `mean`: float64 device tensors or
+    None."""
+    N, _, H, W = x.shape
+    if ws is None:
+        ws = torch.empty(_lib.nbytes("sb_lpips_workspace_bytes", N, H, W), dtype=torch.uint8, device=x.device)
+    _lib.call("sb_lpips", x, y, N, H, W, net.weights, ws, ws.numel(), per_image, mean, device=x.device)
+
+
+def _check_lpips_net(net, device):
+    if not isinstance(net, LpipsAlex):
+        raise _lib.SplatamB200Error("lpips expects an evaluate.LpipsAlex, got %s" % type(net).__name__)
+    if net.weights.device != device:
+        raise _lib.SplatamB200Error("LPIPS weights are on %s, the images on %s" % (net.weights.device, device))
+
+
+def lpips(x, y, net, size_average=True):
+    """LPIPS (AlexNet, v0.1) of two [N,3,H,W] CUDA images as torchmetrics' LearnedPerceptualImagePatchSimilarity(
+    net_type='alex', normalize=True) defines it, on clamp(x, 0, 1) and clamp(y, 0, 1); `net`: an LpipsAlex on the
+    images' device.  FP32 convolutions, deterministic.  size_average=True returns the mean (a float64 0-d tensor);
+    otherwise the float64 [N] values.  H and W must be >= 31."""
+    _lib.need_cuda("lpips", x, y)
+    if x.dim() != 4 or x.shape[1] != 3 or x.shape != y.shape:
+        raise _lib.SplatamB200Error("lpips expects two [N,3,H,W] images of the same shape, got %s and %s"
+                                    % (tuple(x.shape), tuple(y.shape)))
+    if min(x.shape[-2:]) < 31:
+        raise _lib.SplatamB200Error("lpips needs H and W >= 31, got %s" % (tuple(x.shape),))
+    _check_lpips_net(net, x.device)
+    x, y = x.detach().float().contiguous(), y.detach().float().contiguous()
+    if size_average:
+        mean = torch.empty((), dtype=torch.float64, device=x.device)
+        _lpips_into(x, y, net, None, mean)
+        return mean
+    out = torch.empty(x.shape[0], dtype=torch.float64, device=x.device)
+    _lpips_into(x, y, net, out, None)
+    return out
+
+
 def select_frames(num_frames, eval_every=1):
     """Indices the reference evaluates: frame 0, then every frame with (t + 1) % eval_every == 0
     (eval_helpers.py:447-448)."""
@@ -74,31 +157,36 @@ def trajectory_ate(params, first_w2c, gt_w2c):
     return ate_horn(ref, est)
 
 
-def _check_inputs(name, params, frames):
+def _check_inputs(name, params, frames, lpips):
     _lib.need_cuda(name, params["means3D"], frames[0]["im"])
     H, W = frames[0]["im"].shape[-2:]
     if min(H, W) <= 160:
         raise _lib.SplatamB200Error("%s: MS-SSIM needs a smaller image side > 160, got %dx%d" % (name, W, H))
+    if lpips is not None:
+        _check_lpips_net(lpips, params["means3D"].device)
     return H, W
 
 
 def _score_frames(params, frames, ids, cam, sil_thres, use_presence, render, fused, at_gt_pose=False,
-                  count_holes=False):
-    """Renders frames[t] for t in `ids` and scores each with sb_frame_metrics and MS-SSIM: float64 device rows
-    [len(ids), 6] (columns _PSNR .. _SSIM).  at_gt_pose: render at the frame's gt_w2c instead of its estimated pose.
-    count_holes: also returns [len(ids), 6] rows of a presence-masked sb_frame_metrics call into scratch images, whose
+                  count_holes=False, lpips=None):
+    """Renders frames[t] for t in `ids` and scores each with sb_frame_metrics and MS-SSIM, and with sb_lpips on the
+    same weighted images when `lpips` (an LpipsAlex) is given: float64 device rows [len(ids), 7] (columns _PSNR ..
+    _LPIPS; _LPIPS stays 0 without `lpips`).  at_gt_pose: render at the frame's gt_w2c instead of its estimated pose.
+    count_holes: also returns [len(ids), 7] rows of a presence-masked sb_frame_metrics call into scratch images, whose
     _NVALID - _NMASK is the number of valid-depth pixels the silhouette leaves uncovered (None otherwise)."""
     render = M.default_render if render is None else render
     if fused is None:
         fused = render is M.default_render
     dev = params["means3D"].device
     H, W = frames[0]["im"].shape[-2:]
-    metrics = torch.zeros(len(ids), 6, dtype=torch.float64, device=dev)
+    metrics = torch.zeros(len(ids), 7, dtype=torch.float64, device=dev)
     presence = torch.zeros_like(metrics) if count_holes else None
     w_im = torch.empty(3, H, W, dtype=torch.float32, device=dev)
     w_gt = torch.empty_like(w_im)
     ws_frame = torch.empty(_lib.nbytes("sb_frame_metrics_workspace_bytes", H, W), dtype=torch.uint8, device=dev)
     ws_ssim = torch.empty(_lib.nbytes("sb_ms_ssim_workspace_bytes", 1, 3, H, W), dtype=torch.uint8, device=dev)
+    if lpips is not None:
+        ws_lpips = torch.empty(_lib.nbytes("sb_lpips_workspace_bytes", 1, H, W), dtype=torch.uint8, device=dev)
     with torch.no_grad(), torch.cuda.device(dev):
         for k, t in enumerate(ids):
             fr = dict(frames[t], cam=cam)
@@ -110,6 +198,8 @@ def _score_frames(params, frames, ids, cam, sil_thres, use_presence, render, fus
             _lib.call("sb_frame_metrics", im, depth_sil, gt_im, gt_d, H, W, float(sil_thres), use_presence, w_im, w_gt,
                       ws_frame, ws_frame.numel(), metrics[k], device=dev)
             _ms_ssim_into(w_im[None], w_gt[None], 1.0, None, metrics[k, _SSIM], ws_ssim)
+            if lpips is not None:                # sb_lpips clamps the weighted images to [0, 1] as it loads them
+                _lpips_into(w_im[None], w_gt[None], lpips, None, metrics[k, _LPIPS], ws_lpips)
             if count_holes:
                 if use_presence:
                     presence[k].copy_(metrics[k])
@@ -119,21 +209,25 @@ def _score_frames(params, frames, ids, cam, sil_thres, use_presence, render, fus
     return metrics, presence
 
 
-def _per_frame(m):
-    return dict(psnr_per_frame=m[:, _PSNR], ms_ssim_per_frame=m[:, _SSIM], depth_rmse_per_frame=m[:, _RMSE],
-                depth_l1_per_frame=m[:, _L1], valid_pixels=m[:, _NVALID].astype(np.int64),
-                mask_pixels=m[:, _NMASK].astype(np.int64))
+def _per_frame(m, lpips):
+    out = dict(psnr_per_frame=m[:, _PSNR], ms_ssim_per_frame=m[:, _SSIM], depth_rmse_per_frame=m[:, _RMSE],
+               depth_l1_per_frame=m[:, _L1], valid_pixels=m[:, _NVALID].astype(np.int64),
+               mask_pixels=m[:, _NMASK].astype(np.int64))
+    if lpips is not None:
+        out["lpips_per_frame"] = m[:, _LPIPS]
+    return out
 
 
 def _write_lists(out_dir, out):
     os.makedirs(out_dir, exist_ok=True)
     for name, key in (("psnr", "psnr_per_frame"), ("rmse", "depth_rmse_per_frame"), ("l1", "depth_l1_per_frame"),
-                      ("ssim", "ms_ssim_per_frame")):
-        np.savetxt(os.path.join(out_dir, name + ".txt"), out[key])
+                      ("ssim", "ms_ssim_per_frame"), ("lpips", "lpips_per_frame")):
+        if key in out:
+            np.savetxt(os.path.join(out_dir, name + ".txt"), out[key])
 
 
 def evaluate(params, frames, cam, sil_thres, mapping_iters, add_new_gaussians, eval_every=1, gt_w2c=None, fused=None,
-             render=None, out_dir=None):
+             render=None, out_dir=None, lpips=None):
     """The reference's final `eval` over this repo's frame dicts (id, im [3,H,W] in [0,1], depth [1,H,W], w2c = the
     first frame's w2c, as slam.render_frame builds them).  `params`: the final Gaussians plus cam_unnorm_rots /
     cam_trans [.., T]; `cam`: the raster settings; frames are evaluated as `select_frames` picks them.
@@ -147,19 +241,22 @@ def evaluate(params, frames, cam, sil_thres, mapping_iters, add_new_gaussians, e
                   masked mean absolute error; it is reported as the reference defines it
       depth_l1    sum(|e| * valid) / sum(valid)
       ate         `trajectory_ate` against gt_w2c (a list of T ground-truth w2c matrices), None without it
-      lpips       None (not computed)
+      lpips       with `lpips` (an LpipsAlex on the map's device, `LpipsAlex.load`): LPIPS of the weighted images clamped
+                  to [0, 1] (`lpips`), else None
     Returns those averages plus frame_ids and the per-frame arrays psnr_per_frame, ms_ssim_per_frame,
-    depth_rmse_per_frame, depth_l1_per_frame, valid_pixels, mask_pixels.  `out_dir`: also writes psnr.txt, rmse.txt,
-    l1.txt and ssim.txt as the reference does (np.savetxt, one value per evaluated frame).
+    depth_rmse_per_frame, depth_l1_per_frame, valid_pixels, mask_pixels and, with `lpips`, lpips_per_frame.
+    `out_dir`: also writes psnr.txt, rmse.txt, l1.txt, ssim.txt and, with `lpips`, lpips.txt as the reference does
+    (np.savetxt, one value per evaluated frame).
     fused / render: as for mapping (`mapping._render_pair`); fused defaults to the fast path on CUDA."""
-    _check_inputs("evaluate", params, frames)
+    _check_inputs("evaluate", params, frames, lpips)
     ids = select_frames(len(frames), eval_every)
     use_presence = int(mapping_iters == 0 and not add_new_gaussians)
-    metrics, _ = _score_frames(params, frames, ids, cam, sil_thres, use_presence, render, fused)
+    metrics, _ = _score_frames(params, frames, ids, cam, sil_thres, use_presence, render, fused, lpips=lpips)
     m = metrics.cpu().numpy()                    # the one device-to-host read
-    out = dict(frame_ids=[int(frames[t]["id"]) for t in ids], **_per_frame(m))
+    out = dict(frame_ids=[int(frames[t]["id"]) for t in ids], **_per_frame(m, lpips))
     out.update(psnr=float(m[:, _PSNR].mean()), ms_ssim=float(m[:, _SSIM].mean()),
-               depth_rmse=float(m[:, _RMSE].mean()), depth_l1=float(m[:, _L1].mean()), lpips=None,
+               depth_rmse=float(m[:, _RMSE].mean()), depth_l1=float(m[:, _L1].mean()),
+               lpips=None if lpips is None else float(m[:, _LPIPS].mean()),
                ate=None if gt_w2c is None else trajectory_ate(params, frames[0]["w2c"], gt_w2c))
     if out_dir is not None:
         _write_lists(out_dir, out)
@@ -173,7 +270,7 @@ def select_nvs_frames(num_frames, eval_every=1):
 
 
 def evaluate_nvs(params, frames, cam, sil_thres, mapping_iters, add_new_gaussians, eval_every=1, fused=None,
-                 render=None, out_dir=None):
+                 render=None, out_dir=None, lpips=None):
     """The reference's novel-view evaluation `eval_nvs` over a test split (datasets.RGBDSequence(..., split="test"):
     frame 0 is the first train frame, frames 1.. the held-out views, each with its ground-truth `gt_w2c`).  Frames are
     picked by `select_nvs_frames` and rendered at gt_w2c -- the means transformed by it, anisotropic rotations
@@ -182,21 +279,23 @@ def evaluate_nvs(params, frames, cam, sil_thres, mapping_iters, add_new_gaussian
     Masks and per-frame metrics are those of `evaluate`.  A view is valid unless its holes -- pixels with gt depth > 0
     and silhouette <= sil_thres -- exceed 0.1 % of the image (holes * 1000 > H * W; the reference's float32 percentage
     test agrees at the datasets' image sizes).  Returns the averages psnr, ms_ssim, depth_rmse and depth_l1 over the
-    valid views (NaN when none is valid), lpips None, frame_ids (indices into `frames`), the per-frame arrays of
-    `evaluate` over every evaluated view, hole_pixels and valid_nvs_frames (bool).  `out_dir`: also writes psnr.txt,
-    rmse.txt, l1.txt and ssim.txt over every evaluated view and valid_nvs_frames.npy, as the reference does."""
-    H, W = _check_inputs("evaluate_nvs", params, frames)
+    valid views (NaN when none is valid), lpips (the same average with `lpips`, an LpipsAlex, else None), frame_ids
+    (indices into `frames`), the per-frame arrays of `evaluate` over every evaluated view, hole_pixels and
+    valid_nvs_frames (bool).  `out_dir`: also writes psnr.txt, rmse.txt, l1.txt, ssim.txt (and lpips.txt with `lpips`)
+    over every evaluated view and valid_nvs_frames.npy, as the reference does."""
+    H, W = _check_inputs("evaluate_nvs", params, frames, lpips)
     ids = select_nvs_frames(len(frames), eval_every)
     use_presence = int(mapping_iters == 0 and not add_new_gaussians)
     metrics, presence = _score_frames(params, frames, ids, cam, sil_thres, use_presence, render, fused,
-                                      at_gt_pose=True, count_holes=True)
+                                      at_gt_pose=True, count_holes=True, lpips=lpips)
     m, p = torch.stack([metrics, presence]).cpu().numpy()          # the one device-to-host read
     holes = (p[:, _NVALID] - p[:, _NMASK]).astype(np.int64)
     valid = holes * 1000 <= H * W
     out = dict(frame_ids=[int(frames[t]["id"]) for t in ids], hole_pixels=holes, valid_nvs_frames=valid,
-               **_per_frame(m))
+               **_per_frame(m, lpips))
     avg = lambda c: float(m[valid, c].mean()) if valid.any() else float("nan")
-    out.update(psnr=avg(_PSNR), ms_ssim=avg(_SSIM), depth_rmse=avg(_RMSE), depth_l1=avg(_L1), lpips=None)
+    out.update(psnr=avg(_PSNR), ms_ssim=avg(_SSIM), depth_rmse=avg(_RMSE), depth_l1=avg(_L1),
+               lpips=None if lpips is None else avg(_LPIPS))
     if out_dir is not None:
         _write_lists(out_dir, out)
         np.save(os.path.join(out_dir, "valid_nvs_frames.npy"), valid)

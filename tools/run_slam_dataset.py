@@ -18,7 +18,10 @@ One GPU.
 override the shipped iteration counts.  Prints one JSON line: ATE, PSNR, MS-SSIM, depth L1, initial and final
 Gaussian counts, tracking
 and mapping wall times, and the load time per frame that the SLAM loop waited for (decode + upload not hidden by the
-prefetch).  --out DIR writes params.npz and the reference's psnr.txt / rmse.txt / l1.txt / ssim.txt."""
+prefetch).  --out DIR writes params.npz and the reference's psnr.txt / rmse.txt / l1.txt / ssim.txt.
+--lpips-alexnet PATH --lpips-lin PATH (both or neither: torchvision's alexnet-owt-7be5be79.pth and LPIPS v0.1's
+alex.pth, read from disk, never downloaded) add LPIPS to the evaluation: `lpips` (and `nvs_lpips` with --nvs) in the
+JSON line and lpips.txt under --out."""
 import argparse
 import json
 import os
@@ -93,7 +96,11 @@ def main():
                                                        "(scannetpp, replicav2)")
     ap.add_argument("--variant", default="splatam", choices=VARIANTS,
                     help="splatam_s: SplaTAM-S, the fast variant (replica only)")
+    ap.add_argument("--lpips-alexnet", default=None, help="torchvision AlexNet weights (alexnet-owt-7be5be79.pth)")
+    ap.add_argument("--lpips-lin", default=None, help="LPIPS v0.1 linear heads (alex.pth)")
     a = ap.parse_args()
+    if (a.lpips_alexnet is None) != (a.lpips_lin is None):
+        ap.error("--lpips-alexnet and --lpips-lin go together")
     if a.nvs and a.dataset not in ("scannetpp", "replicav2"):
         ap.error("--nvs needs a dataset with a test split (scannetpp, replicav2)")
     if a.variant == "splatam_s" and a.dataset not in HYPER_S:
@@ -106,6 +113,7 @@ def main():
     h["tracking_iters"] = a.tracking_iters or h["tracking_iters"]
     h["mapping_iters"] = a.mapping_iters or h["mapping_iters"]
     cfg = datasets.load_config(a.config) if a.config else None
+    net = None if a.lpips_alexnet is None else evaluate.LpipsAlex.load(a.lpips_alexnet, a.lpips_lin, dev)
     seq = datasets.RGBDSequence(a.dataset, a.basedir, a.sequence, cfg, start=a.start, end=a.end, stride=a.stride,
                                 desired_height=h["height"], desired_width=h["width"], device=dev, prefetch=a.prefetch,
                                 densify_height=h.get("densify_height"), densify_width=h.get("densify_width"))
@@ -134,7 +142,7 @@ def main():
     gt_w2c = [torch.linalg.inv(p.to(dev)) for p in gt]
     params = dict(out["gauss"], cam_unnorm_rots=out["rots"], cam_trans=out["trans"])
     res = evaluate.evaluate(params, frames, seq.cam, SIL_THRES, h["mapping_iters"], True, eval_every=h["eval_every"],
-                            gt_w2c=gt_w2c, out_dir=a.out)
+                            gt_w2c=gt_w2c, out_dir=a.out, lpips=net)
     seq.close()
     nvs = {}
     if a.nvs:
@@ -142,10 +150,12 @@ def main():
                                    desired_width=h["width"], device=dev, prefetch=a.prefetch, split="test") as test:
             r = evaluate.evaluate_nvs(out["gauss"], test, test.cam, SIL_THRES, h["mapping_iters"], True,
                                       eval_every=h["eval_every"],
-                                      out_dir=None if a.out is None else os.path.join(a.out, "eval_nvs"))
+                                      out_dir=None if a.out is None else os.path.join(a.out, "eval_nvs"), lpips=net)
         nvs = dict(nvs_psnr_db=r["psnr"], nvs_ms_ssim=r["ms_ssim"], nvs_depth_rmse_m=r["depth_rmse"],
                    nvs_depth_l1_m=r["depth_l1"], nvs_evaluated_frames=len(r["frame_ids"]),
                    nvs_valid_frames=int(r["valid_nvs_frames"].sum()))
+        if net is not None:
+            nvs["nvs_lpips"] = r["lpips"]
     if a.out is not None:
         from splatam_b200 import formats
         formats.save_params(params, a.out)
@@ -156,7 +166,7 @@ def main():
         ate_m=res["ate"], psnr_db=res["psnr"], ms_ssim=res["ms_ssim"], depth_l1_m=res["depth_l1"],
         gaussians=int(out["counts"][-1]), wall_s=wall, tracking_s=timing["tracking_s"], mapping_s=timing["mapping_s"],
         load_wait_ms_per_frame=1e3 * load_wait / max(T - 1, 1), evaluated_frames=len(res["frame_ids"]),
-        tracking_iters=timing["tracking_iters"], **nvs,
+        tracking_iters=timing["tracking_iters"], **({} if net is None else dict(lpips=res["lpips"])), **nvs,
         metric_note="ate_m = the reference's Final Average ATE RMSE (mean Horn-aligned residual); load_wait = host "
                     "time run_slam spent in the reader for frames 1..T-1")))
 

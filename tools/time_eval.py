@@ -10,7 +10,12 @@ installed).  Prints the GPU name and power limit of the run and one JSON line:
 --nvs instead times evaluate.evaluate_nvs (renders at the ground-truth poses, the unmasked branch with its extra hole
 count) over --frames held-out views of a view-filling map at ScanNet++'s 876x584 and ReplicaV2's 1200x680, and
 prints nvs_frames_per_s per size.
-Run:  python tools/time_eval.py [--frames 200] [--reps 100] [--ref-frames 5] [--nvs]"""
+--lpips instead times sb_lpips (csrc/lpips.cu) on one image pair at 1200x680 and 876x584 with seeded random weights (a
+dense convolution's time does not depend on the weight values): the time per call from CUDA events over --reps calls,
+each launch's time from a torch.profiler pass, GFLOP/s against the 67 TFLOP/s FP32 data-sheet rate, the same network
+through torch.nn.functional on the GPU as the reference-style path, and evaluate() frames/s without and with LPIPS
+over --frames frames at 1200x680.
+Run:  python tools/time_eval.py [--frames 200] [--reps 100] [--ref-frames 5] [--nvs | --lpips]"""
 import argparse
 import json
 import os
@@ -84,6 +89,111 @@ def time_nvs(frames_n, sil_thres):
     return out
 
 
+# sb_lpips' launches in order, for the per-layer times of the profiled calls
+_LPIPS_KERNELS = ("conv1", "pool1", "conv2", "pool2", "conv3", "conv4", "conv5", "head1", "head2", "head3", "head4",
+                  "head5", "finalize")
+
+
+def _lpips_gflop(N, H, W):
+    """{conv1..conv5: GFLOP (2 x MAC)} of one sb_lpips call on N pairs (2N images)."""
+    from oracle import lpips_torch as OL
+    x = torch.empty(2 * N, 3, H, W, device="meta")
+    alex, _ = OL.random_state_dicts(0)
+    fs = OL.features(x, alex, dtype=torch.float32)
+    return {"conv%d" % (l + 1): 2.0 * f.numel() * cin * k * k / 1e9
+            for l, (f, (_, cin, _, k, _, _)) in enumerate(zip(fs, OL.ALEX_CONVS))}
+
+
+def time_lpips(frames_n, reps, sil_thres):
+    """sb_lpips at 1200x680 and 876x584 (one pair, seeded random weights): time per call from CUDA events over `reps`
+    calls, the time of each launch from a torch.profiler pass, GFLOP/s against the 67 TFLOP/s FP32 data-sheet rate,
+    the same network through torch.nn.functional on the GPU (cuDNN with PyTorch's default TF32 setting), and
+    evaluate() frames/s without and with LPIPS over `frames_n` frames of a view-filling map."""
+    import tempfile
+    import splatam_b200 as S
+    from oracle import lpips_torch as OL
+    from splatam_b200 import _lib, evaluate as EV, slam
+    dev = torch.device("cuda:0")
+    alex, lin = OL.random_state_dicts(seed=0)
+    net = EV.LpipsAlex.from_state_dicts(alex, lin, dev)
+    wdev = {k: v.to(dev) for k, v in dict(alex, **lin).items()}
+    out = {}
+    for w, h in ((1200, 680), (876, 584)):
+        g = torch.Generator().manual_seed(w)
+        x = torch.rand(1, 3, h, w, generator=g).to(dev)
+        y = (x + 0.1 * torch.randn(x.shape, generator=g).to(dev)).clamp(0, 1)
+        mean = torch.empty((), dtype=torch.float64, device=dev)
+        ws = torch.empty(_lib.nbytes("sb_lpips_workspace_bytes", 1, h, w), dtype=torch.uint8, device=dev)
+        call = lambda: EV._lpips_into(x, y, net, None, mean, ws)
+        for _ in range(10):
+            call()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            call()
+        e1.record()
+        torch.cuda.synchronize()
+        ms = e0.elapsed_time(e1) / reps
+        # per-launch times: one profiled pass, kernels matched to _LPIPS_KERNELS by launch order
+        prof_calls = 20
+        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+            for _ in range(prof_calls):
+                call()
+            torch.cuda.synchronize()
+        with tempfile.TemporaryDirectory() as tmp:
+            path = os.path.join(tmp, "trace.json")
+            prof.export_chrome_trace(path)
+            events = json.load(open(path))["traceEvents"]
+        kernels = sorted((e for e in events if e.get("cat") == "kernel"), key=lambda e: e["ts"])
+        assert len(kernels) == prof_calls * len(_LPIPS_KERNELS), len(kernels)
+        per = {k: 0.0 for k in _LPIPS_KERNELS}
+        for i, e in enumerate(kernels):
+            per[_LPIPS_KERNELS[i % len(_LPIPS_KERNELS)]] += e["dur"] / 1e3 / prof_calls
+        gflop = _lpips_gflop(1, h, w)
+        total_gflop = sum(gflop.values())
+        # the reference-style path: the same network through torch.nn.functional on the GPU
+        ref = lambda: OL.lpips(x, y, wdev, dtype=torch.float32)
+        for _ in range(5):
+            ref()
+        e0.record()
+        for _ in range(20):
+            r = ref()
+        e1.record()
+        torch.cuda.synchronize()
+        ref_ms = e0.elapsed_time(e1) / 20
+        out["%dx%d" % (w, h)] = dict(
+            lpips_ms_per_call=round(ms, 4), layer_ms={k: round(v, 4) for k, v in per.items()},
+            gflop_per_call=round(total_gflop, 2), gflop_per_s=round(total_gflop / ms * 1e3, 1),
+            share_of_67_tflops=round(total_gflop / ms * 1e3 / 67e3, 3),
+            conv_gflop_per_s={k: round(gflop[k] / per[k] * 1e3, 1) for k in gflop},
+            functional_ms_per_call=round(ref_ms, 3), functional_cudnn_tf32=torch.backends.cudnn.allow_tf32,
+            lpips=[mean.item(), float(r[0])])
+    # evaluate() with and without LPIPS on a 1200x680 view-filling map, run alternately
+    sc = scenes.view_filling(margin=100)
+    cam = sc.settings(S.GaussianRasterizationSettings, dev)
+    gt = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
+              logit_opacities=torch.logit(sc.opacities.reshape(-1, 1)), log_scales=torch.log(sc.scales[:, :1]))
+    gt = {k: v.to(dev).contiguous() for k, v in gt.items()}
+    rots, trans = slam.look_trajectory(frames_n, dev, step=(0.002, -0.001, 0.001), rot_step=(0.0005, -0.0004, 0.0003))
+    frames = [slam.render_frame(gt, rots, trans, t, cam) for t in range(frames_n)]
+    params = dict(gt, cam_unnorm_rots=rots, cam_trans=trans)
+    g = torch.Generator().manual_seed(1)
+    params["rgb_colors"] = (gt["rgb_colors"] + 0.05 * torch.randn(gt["rgb_colors"].shape, generator=g).to(dev)).clamp(0, 1)
+    fps = {"without": [], "with": []}
+    for lp in (None, net):
+        EV.evaluate(params, frames[:4], cam, sil_thres, 0, False, lpips=lp)           # warm-up
+    for _ in range(2):
+        for key, lp in (("without", None), ("with", net)):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            res = EV.evaluate(params, frames, cam, sil_thres, 0, False, lpips=lp)
+            torch.cuda.synchronize()
+            fps[key].append(round(frames_n / (time.perf_counter() - t0), 2))
+    out["evaluate_1200x680"] = dict(frames=frames_n, frames_per_s_without_lpips=fps["without"],
+                                    frames_per_s_with_lpips=fps["with"], lpips=round(res["lpips"], 6))
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=200)
@@ -91,8 +201,12 @@ def main():
     ap.add_argument("--ref-frames", type=int, default=5)
     ap.add_argument("--sil-thres", type=float, default=0.5)
     ap.add_argument("--nvs", action="store_true", help="time evaluate_nvs at 876x584 and 1200x680 instead")
+    ap.add_argument("--lpips", action="store_true", help="time sb_lpips and evaluate() with LPIPS instead")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "time_eval.py measures on a CUDA device"
+    if args.lpips:
+        print(json.dumps(dict(gpu=gpu_info(), **time_lpips(args.frames, args.reps, args.sil_thres))))
+        return
     if args.nvs:
         print(json.dumps(dict(gpu=gpu_info(), frames=args.frames, **time_nvs(args.frames, args.sil_thres))))
         return
