@@ -526,15 +526,25 @@ class ShardedMapper:
                        log_scales=0.001)
 
     def __init__(self, gaussians, cam_unnorm_rots, cam_trans, lrs=None, render=default_render, group=None, seed=0,
-                 fused=None, track_means2D=False):
+                 fused=None, track_means2D=False, timestep=None):
         """track_means2D: keep d loss / d means2D of every eager step's RGB render and which Gaussians it saw (the
-        statistic of `densify`)."""
+        statistic of `densify`).  timestep: the frame that created each Gaussian ([P], e.g. from a checkpoint); default
+        zeros, as the reference starts its initial map (R/scripts/splatam.py:155)."""
         import torch.distributed as dist
         self.dist = dist if (dist.is_available() and dist.is_initialized()) else None
         self.group = group
         self.rank = self.dist.get_rank(group) if self.dist else 0
         self.world = self.dist.get_world_size(group) if self.dist else 1
         self.g = FlatGaussians(gaussians)
+        P, dev = self.g.shapes["means3D"][0], self.g.flat.device
+        # per-Gaussian creation frame: kept beside the flat buffer, outside the gradient / Adam / all-reduce layout, and
+        # edited with the same masks as the parameters, so every replica holds the same one
+        if timestep is None:
+            self.timestep = torch.zeros(P, dtype=torch.float32, device=dev)
+        else:
+            self.timestep = torch.as_tensor(timestep).detach().to(dev, torch.float32).reshape(-1).clone()
+            if self.timestep.shape[0] != P:
+                raise ValueError("timestep has %d entries for a map of %d Gaussians" % (self.timestep.shape[0], P))
         self.cam = dict(cam_unnorm_rots=cam_unnorm_rots.detach(), cam_trans=cam_trans.detach())
         lrs = dict(self.DEFAULT_LRS, **(lrs or {}))
         self.lrs = lrs
@@ -626,7 +636,7 @@ class ShardedMapper:
         self._graph = None                      # shapes changed: a captured graph is stale
 
     def remove_points(self, to_remove):
-        """Drop the rows where `to_remove` is set from the parameters and both Adam moments
+        """Drop the rows where `to_remove` is set from the parameters, both Adam moments and `timestep`
         (remove_points, R/utils/slam_external.py:144-167).  Returns the number of Gaussians kept."""
         P = self.g.shapes["means3D"][0]
         keep = ~to_remove.reshape(-1).bool()
@@ -634,12 +644,15 @@ class ShardedMapper:
             from . import map_ops
             m8, dst, P_new = map_ops.compact_plan(keep)
             compact = lambda buf: map_ops.compact_flat(buf, P, self._widths(), m8, dst, P_new)
+            compact_ts = lambda ts: map_ops.compact_flat(ts, P, [1], m8, dst, P_new)
         else:
             P_new = int(keep.sum())
             compact = lambda buf: torch.cat([x[keep].reshape(-1) for x in self.g.views(buf).values()])
+            compact_ts = lambda ts: ts[keep]
         if P_new == P:
             return P
         self._rebuild(compact(self.g.flat), P_new, compact(self.exp_avg), compact(self.exp_avg_sq), self._adam_steps())
+        self.timestep = compact_ts(self.timestep.contiguous())
         return P_new
 
     def _reset_opacities(self):
@@ -674,25 +687,31 @@ class ShardedMapper:
             self._reset_opacities()
         return P
 
-    def add_gaussians(self, new):
+    def add_gaussians(self, new, timestep=0):
         """Append rows (dict of the five tensors) to the map; Adam moments of the new rows start at zero
-        (cat_params_to_optimizer, R/utils/slam_external.py:121-141).  Returns the new Gaussian count."""
+        (cat_params_to_optimizer, R/utils/slam_external.py:121-141).  `timestep`: the new rows' creation frame, one
+        value for all of them or one per row.  Returns the new Gaussian count."""
         P, n_new = self.g.shapes["means3D"][0], new["means3D"].shape[0]
         if n_new == 0:
             return P
         dev = self.g.flat.device
+        ts = torch.as_tensor(timestep).detach().to(dev, torch.float32)
+        ts = ts.expand(n_new) if ts.dim() == 0 else ts.reshape(-1)
+        if ts.shape[0] != n_new:
+            raise ValueError("timestep has %d entries for %d new Gaussians" % (ts.shape[0], n_new))
 
         def grown(buf, rows):
             return torch.cat([torch.cat([x, rows[k]], 0).reshape(-1) for k, x in self.g.views(buf).items()])
         zeros = {k: torch.zeros(n_new, w, device=dev) for k, w in zip(GAUSSIAN_KEYS, self._widths())}
         flat = grown(self.g.flat, {k: new[k].to(dev).float().reshape(n_new, -1) for k in GAUSSIAN_KEYS})
         self._rebuild(flat, P + n_new, grown(self.exp_avg, zeros), grown(self.exp_avg_sq, zeros), self._adam_steps())
+        self.timestep = torch.cat([self.timestep, ts])
         return P + n_new
 
     def add_new_gaussians(self, frame, time_idx, intrinsics, sil_thres):
         """add_new_gaussians of the reference (R/scripts/splatam.py:378-420): one depth/silhouette render of the
         current map at the frame's estimated pose, non-presence mask, back-projection of the selected pixels,
-        append.  CUDA only.  Returns the number of Gaussians added."""
+        append with `timestep` = time_idx (splatam.py:417-418).  CUDA only.  Returns the number of Gaussians added."""
         from . import map_ops
         p = self.params()
         with torch.no_grad():
@@ -702,7 +721,7 @@ class ShardedMapper:
         new, n = map_ops.new_gaussians_from_frame(depth_sil, frame, intrinsics, curr_w2c, sil_thres,
                                                   scale_dim=self._widths()[4])
         if n:
-            self.add_gaussians(new)
+            self.add_gaussians(new, timestep=time_idx)
         return n
 
     # ---- CUDA-graph mode -----------------------------------------------------------------------------------
@@ -832,7 +851,9 @@ class ShardedMapper:
         remove_big_after, reset_opacities, reset_opacities_every): accumulates |d loss / d means2D| of the seen
         Gaussians, clones the small high-gradient ones, splits the large ones into num_to_split_into samples of
         their own distribution, drops transparent / oversized ones and optionally resets opacities.  Parameters and both
-        Adam moments follow (new rows start with zero moments).  Every rank must call it with the same all-reduced
+        Adam moments follow (new rows start with zero moments).  Clones and split samples inherit their parent's
+        `timestep`, as R/utils/gs_external.py:202-222 does: the SLAM densify of slam_external.py does not grow it at all
+        (DESIGN.md section 9).  Every rank must call it with the same all-reduced
         statistics; `generator` (default: the mapper's shared-seed generator when distributed, else torch's global
         RNG, as the reference) draws the split samples.  Returns the Gaussian count afterwards."""
         P = self.g.shapes["means3D"][0]
@@ -863,7 +884,7 @@ class ShardedMapper:
         cur = lambda: {k: self.g.params[k].detach() for k in GAUSSIAN_KEYS}
         big = lambda: torch.max(torch.exp(self.g.params["log_scales"].detach()), dim=1).values
         to_clone = torch.logical_and(grads >= thr, big() <= 0.01 * scene_radius)
-        self.add_gaussians({k: v[to_clone] for k, v in cur().items()})
+        self.add_gaussians({k: v[to_clone] for k, v in cur().items()}, timestep=self.timestep[to_clone])
         num = self.g.shapes["means3D"][0]
         padded = torch.zeros(num, device=dev)
         padded[:grads.shape[0]] = grads
@@ -878,7 +899,7 @@ class ShardedMapper:
         rots = build_rotation(p["unnorm_rotations"][to_split]).repeat(n, 1, 1)
         new["means3D"] = new["means3D"] + torch.bmm(rots, samples.unsqueeze(-1)).squeeze(-1)
         new["log_scales"] = torch.log(torch.exp(new["log_scales"]) / (0.8 * n))
-        self.add_gaussians(new)
+        self.add_gaussians(new, timestep=self.timestep[to_split].repeat(n))
         self.remove_points(torch.cat((to_split, torch.zeros(n * int(to_split.sum()), dtype=torch.bool, device=dev))))
         rthr = (densify_dict["final_removal_opacity_threshold"] if iter == densify_dict["stop_after"]
                 else densify_dict["removal_opacity_threshold"])

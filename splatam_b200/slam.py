@@ -65,12 +65,89 @@ def _without_densify(frame):
     return {k: v for k, v in frame.items() if k != "densify"}
 
 
+def keyframes_from_checkpoint(frames, ckpt):
+    """The keyframe list of a checkpoint (formats.load_checkpoint): frames[k] for every stored id k, with est_w2c
+    rebuilt from the stored camera column k (F.normalize + build_rotation, as R/scripts/splatam.py:619-638 does)."""
+    rots, trans = ckpt["cam_unnorm_rots"], ckpt["cam_trans"]
+    return [dict(_without_densify(frames[k]), est_w2c=_curr_w2c(rots, trans, k)) for k in ckpt["keyframe_time_indices"]]
+
+
+def _run_state(mapper, counts):
+    """The sidecar of a checkpoint (formats.save_checkpoint's `run_state`): what continues a run exactly and the
+    reference's params{t}.npz cannot carry -- the Gaussians' `timestep`, torch's CPU RNG and the CUDA RNG of the map's
+    device (keyframe selection and densification draw from the global generators), NumPy's global RNG
+    (keyframe_selection_overlap's permutation), the mapper's schedule generator and its device generator if it has
+    one, the densification statistic if there is one, and the Gaussian counts so far.  Numeric arrays only."""
+    import numpy as np
+    dev = mapper.g.flat.device
+    _, keys, pos, has_gauss, cached = np.random.get_state()
+    st = dict(timestep=mapper.timestep.detach().cpu().numpy(), torch_rng=torch.get_rng_state().numpy(),
+              numpy_rng_keys=np.asarray(keys, dtype=np.uint32), numpy_rng_pos=np.array(pos, dtype=np.int64),
+              numpy_rng_has_gauss=np.array(has_gauss, dtype=np.int64),
+              numpy_rng_cached_gaussian=np.array(cached, dtype=np.float64),
+              mapper_gen=mapper.gen.get_state().numpy(), counts=np.array(counts, dtype=np.int64))
+    if dev.type == "cuda":
+        st["cuda_rng"] = torch.cuda.get_rng_state(dev).numpy()
+    if mapper._dev_gen is not None:
+        st["mapper_dev_gen"] = mapper._dev_gen.get_state().numpy()
+    if mapper._dens is not None:
+        st["dens_accum"] = mapper._dens["accum"].detach().cpu().numpy()
+        st["dens_denom"] = mapper._dens["denom"].detach().cpu().numpy()
+    return st
+
+
+def _restore_run_state(mapper, st):
+    """Inverse of _run_state on a mapper built from the checkpoint's map; returns the Gaussian counts so far."""
+    import numpy as np
+    dev = mapper.g.flat.device
+    P = mapper.g.shapes["means3D"][0]
+    if st["timestep"].shape != (P,):
+        raise ValueError("the checkpoint's run state holds %d timesteps for a map of %d Gaussians"
+                         % (st["timestep"].shape[0], P))
+    mapper.timestep = torch.from_numpy(np.array(st["timestep"], dtype=np.float32)).to(dev)
+    torch.set_rng_state(torch.from_numpy(np.array(st["torch_rng"], dtype=np.uint8)))
+    np.random.set_state(("MT19937", np.array(st["numpy_rng_keys"], dtype=np.uint32), int(st["numpy_rng_pos"]),
+                         int(st["numpy_rng_has_gauss"]), float(st["numpy_rng_cached_gaussian"])))
+    mapper.gen.set_state(torch.from_numpy(np.array(st["mapper_gen"], dtype=np.uint8)))
+    if dev.type == "cuda" and "cuda_rng" in st:
+        torch.cuda.set_rng_state(torch.from_numpy(np.array(st["cuda_rng"], dtype=np.uint8)), dev)
+    if "mapper_dev_gen" in st:
+        mapper._device_generator().set_state(torch.from_numpy(np.array(st["mapper_dev_gen"], dtype=np.uint8)))
+    if "dens_accum" in st:
+        mapper._dens = dict(accum=torch.from_numpy(np.array(st["dens_accum"], dtype=np.float32)).to(dev),
+                            denom=torch.from_numpy(np.array(st["dens_denom"], dtype=np.float32)).to(dev))
+    return [int(c) for c in st["counts"]]
+
+
+def _check_resume(gauss_init, resume, T, checkpoint_every, checkpoint_dir):
+    import numbers
+    if checkpoint_every is not None:
+        if (isinstance(checkpoint_every, bool) or not isinstance(checkpoint_every, numbers.Integral)
+                or checkpoint_every <= 0):
+            raise ValueError("checkpoint_every must be a positive integer, got %r" % (checkpoint_every,))
+        if checkpoint_dir is None:
+            raise ValueError("checkpoint_every needs a checkpoint_dir")
+    if resume is None:
+        if gauss_init is None:
+            raise ValueError("run_slam needs gauss_init or resume")
+        return
+    if gauss_init is not None:
+        raise ValueError("give gauss_init or resume, not both")
+    n = resume["cam_unnorm_rots"].shape[-1]
+    if n != T or resume["cam_trans"].shape[-1] != T:
+        raise ValueError("the checkpoint's cameras cover %d frames, the sequence has %d" % (n, T))
+    if not 0 <= int(resume["time_idx"]) <= T - 1:
+        raise ValueError("checkpoint frame %d is outside [0, %d]" % (int(resume["time_idx"]), T - 1))
+
+
 def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_iters=8, keyframe_every=2,
              window=4, fused=None, seed=0, intrinsics=None, add_new_gaussians=False, sil_thres=0.5, prune_dict=None,
              scene_radius=None, select_keyframes=False, checkpoint_dir=None, first_frame_iters=0, map_every=None,
-             graph=False, timing=None, densify_dict=None, tracking_lrs=(0.0004, 0.002), depth_loss_thres=None):
+             graph=False, timing=None, densify_dict=None, tracking_lrs=(0.0004, 0.002), depth_loss_thres=None,
+             checkpoint_every=None, resume=None):
     """Tracks every frame and maps on keyframes.  gauss_init: dict of the five Gaussian tensors (the map's
-    starting point); frames: list of dict(id, cam, w2c, im, depth).  Returns dict(rots, trans, psnr, gauss).
+    starting point); frames: list of dict(id, cam, w2c, im, depth).  Returns dict(rots, trans, psnr, gauss, counts,
+    timestep, keyframe_time_indices): `timestep` is the frame that created each Gaussian of the final map.
 
     The optional stages follow the reference's main loop (R/scripts/splatam.py:776-925): `add_new_gaussians` grows
     the map from each mapped frame's silhouette holes before mapping -- from the frame's ``densify`` entry, with that
@@ -87,24 +164,68 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     splatam.py:863-864; eager steps only -- the map size changes).  `tracking_lrs`: the tracking learning rates of
     (cam_unnorm_rots, cam_trans); the default is Replica's.  `depth_loss_thres`: track_frame's rule that doubles a
     frame's tracking iterations while the depth loss stays high (ScanNet++: 20000).  `timing`: dict that receives the
-    accumulated wall seconds of tracking / mapping (synchronised) and the tracking and mapping iteration counts."""
+    accumulated wall seconds of tracking / mapping (synchronised), the tracking and mapping iteration counts, and
+    `setup_s`, the wall seconds from the call to the start of the frame loop.
+
+    Checkpoints and resume (R/scripts/splatam.py:604-643,927-931).  With `checkpoint_dir` and `checkpoint_every` = N,
+    after frame t's mapping and keyframe step, for every t % N == 0 (frame 0 included, after `first_frame_iters`),
+    rank 0 writes formats.save_checkpoint's three files: the reference's params{t}.npz and keyframe_time_indices{t}.npy,
+    and the run_state{t}.npz sidecar (`_run_state`); the per-keyframe params<t>.npz are then not written, and the final
+    params.npz is written by rank 0 only.  Without `checkpoint_every`, `checkpoint_dir` writes params<t>.npz per
+    keyframe and params.npz at the end.
+    `resume` = formats.load_checkpoint(dir, t, device), with gauss_init None: the map, the cameras and the keyframe list
+    come from the checkpoint (keyframe k is frames[k] with est_w2c rebuilt from the stored camera column, as
+    splatam.py:619-638 does); with a sidecar every RNG, the schedule generator, the densification statistic, `timestep`
+    and `counts` are restored, without one (a checkpoint the reference wrote) `timestep` is zeros, `counts` starts at
+    the loaded map and the RNGs are left as they are.  `first_frame_iters` does not run.  The loop continues at frame
+    t + 1, unlike the reference, which restarts at t: it tracks and maps frame t a second time and appends it to its
+    keyframe list twice.  Continuing at t + 1 is what makes a resumed run equal the uninterrupted one."""
     import time
+    t_setup = time.perf_counter()
     map_every = keyframe_every if map_every is None else map_every
     timing = {} if timing is None else timing
-    timing.update(tracking_s=0.0, mapping_s=0.0, mapping_iters=0, tracking_iters=0)
-    dev = gauss_init["means3D"].device
+    timing.update(tracking_s=0.0, mapping_s=0.0, mapping_iters=0, tracking_iters=0, setup_s=0.0)
     T = len(frames)
-    rots = torch.zeros(1, 4, T, device=dev); rots[:, 0] = 1.0
-    trans = torch.zeros(1, 3, T, device=dev)
+    _check_resume(gauss_init, resume, T, checkpoint_every, checkpoint_dir)
     kw = {} if render is None else {"render": render}
-    mapper = M.ShardedMapper(gauss_init, rots, trans, seed=seed, fused=fused, track_means2D=densify_dict is not None, **kw)
-    keyframes = [dict(_without_densify(frames[0]), est_w2c=torch.eye(4, device=dev))]
-    counts = [mapper.g.shapes["means3D"][0]]
+    track_m2d = densify_dict is not None
+    if resume is None:
+        dev = gauss_init["means3D"].device
+        rots = torch.zeros(1, 4, T, device=dev); rots[:, 0] = 1.0
+        trans = torch.zeros(1, 3, T, device=dev)
+        mapper = M.ShardedMapper(gauss_init, rots, trans, seed=seed, fused=fused, track_means2D=track_m2d, **kw)
+        keyframes = [dict(_without_densify(frames[0]), est_w2c=torch.eye(4, device=dev))]
+        counts = [mapper.g.shapes["means3D"][0]]
+        start = 1
+    else:
+        dev = resume["gauss"]["means3D"].device
+        rots = resume["cam_unnorm_rots"].detach().clone().to(dev)
+        trans = resume["cam_trans"].detach().clone().to(dev)
+        mapper = M.ShardedMapper(resume["gauss"], rots, trans, seed=seed, fused=fused, track_means2D=track_m2d, **kw)
+        keyframes = keyframes_from_checkpoint(frames, dict(resume, cam_unnorm_rots=rots, cam_trans=trans))
+        if resume["state"] is not None:
+            counts = _restore_run_state(mapper, resume["state"])
+        else:
+            counts = [mapper.g.shapes["means3D"][0]]
+        start = int(resume["time_idx"]) + 1
+        first_frame_iters = 0
+
+    def checkpoint(t):
+        if checkpoint_every is None or t % checkpoint_every != 0 or mapper.rank != 0:
+            return
+        from . import formats
+        formats.save_checkpoint(checkpoint_dir, t, dict(mapper.g.params, cam_unnorm_rots=rots, cam_trans=trans),
+                                [kf["id"] for kf in keyframes], _run_state(mapper, counts))
+
     for it in range(first_frame_iters):       # the reference maps frame 0 before it tracks frame 1 (splatam.py:777)
         mapper.step([keyframes[0]])
         if prune_dict is not None:
             mapper.prune_gaussians(it, prune_dict, scene_radius)
-    for t in range(1, T):
+    if resume is None:
+        checkpoint(0)
+    torch.cuda.synchronize(dev) if dev.type == "cuda" else None
+    timing["setup_s"] = time.perf_counter() - t_setup
+    for t in range(start, T):
         with torch.no_grad():           # constant-velocity initialisation (splatam.py:423-444)
             if t > 1:
                 r1, r2 = F.normalize(rots[0, :, t - 1], dim=0), F.normalize(rots[0, :, t - 2], dim=0)
@@ -161,19 +282,21 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
             counts.append(mapper.g.shapes["means3D"][0])
         if t % keyframe_every == 0:
             keyframes.append(cur)
-            if checkpoint_dir is not None:
+            if checkpoint_dir is not None and checkpoint_every is None:
                 from . import formats
                 formats.save_params_ckpt(dict(mapper.g.params, cam_unnorm_rots=rots, cam_trans=trans), checkpoint_dir, t)
+        checkpoint(t)
     # PSNR of the keyframes re-rendered from the final map at the estimated poses
     final = {k: v.detach() for k, v in mapper.g.params.items()}
     vals = []
     for fr in keyframes:
         est = render_frame(final, rots, trans, fr["id"], cam, render)
         vals.append(psnr(est["im"].clamp(0, 1), fr["im"].clamp(0, 1)))
-    if checkpoint_dir is not None:
+    if checkpoint_dir is not None and (checkpoint_every is None or mapper.rank == 0):
         from . import formats
         formats.save_params(dict(final, cam_unnorm_rots=rots, cam_trans=trans), checkpoint_dir)
-    return dict(rots=rots, trans=trans, psnr=sum(vals) / len(vals), gauss=final, counts=counts)
+    return dict(rots=rots, trans=trans, psnr=sum(vals) / len(vals), gauss=final, counts=counts,
+                timestep=mapper.timestep.detach().clone(), keyframe_time_indices=[int(kf["id"]) for kf in keyframes])
 
 
 def w2c_list(rots, trans):

@@ -18,10 +18,20 @@ One GPU.
 override the shipped iteration counts.  Prints one JSON line: ATE, PSNR, MS-SSIM, depth L1, initial and final
 Gaussian counts, tracking
 and mapping wall times, and the load time per frame that the SLAM loop waited for (decode + upload not hidden by the
-prefetch).  --out DIR writes params.npz and the reference's psnr.txt / rmse.txt / l1.txt / ssim.txt.
+prefetch).  --out DIR writes the reference's psnr.txt / rmse.txt / l1.txt / ssim.txt and its full params.npz record
+(formats.save_run_record: the Gaussians, the cameras, `timestep`, `intrinsics`, `w2c`, `org_width` / `org_height`,
+`gt_w2c_all_frames` and `keyframe_time_indices`), which the reference's viewers and post_splatam_opt.py open.
 --lpips-alexnet PATH --lpips-lin PATH (both or neither: torchvision's alexnet-owt-7be5be79.pth and LPIPS v0.1's
 alex.pth, read from disk, never downloaded) add LPIPS to the evaluation: `lpips` (and `nvs_lpips` with --nvs) in the
-JSON line and lpips.txt under --out."""
+JSON line and lpips.txt under --out.
+--checkpoint-every N writes the reference's params{t}.npz / keyframe_time_indices{t}.npy, and a run_state{t}.npz
+sidecar, under --out every N frames; --resume T continues the run from the checkpoint of frame T under --out (one
+written here, or the reference's own, which then continues without the sidecar's RNG states):
+
+  python tools/run_slam_dataset.py --dataset replica --basedir data/Replica --sequence room0 --out runs/room0 \\
+      --checkpoint-every 100
+  python tools/run_slam_dataset.py --dataset replica --basedir data/Replica --sequence room0 --out runs/room0 \\
+      --checkpoint-every 100 --resume 1500"""
 import argparse
 import json
 import os
@@ -98,9 +108,18 @@ def main():
                     help="splatam_s: SplaTAM-S, the fast variant (replica only)")
     ap.add_argument("--lpips-alexnet", default=None, help="torchvision AlexNet weights (alexnet-owt-7be5be79.pth)")
     ap.add_argument("--lpips-lin", default=None, help="LPIPS v0.1 linear heads (alex.pth)")
+    ap.add_argument("--checkpoint-every", type=int, default=0,
+                    help="write a checkpoint under --out every N frames (0: off); the reference's shipped "
+                         "checkpoint_interval is 100 for Replica, TUM, ScanNet and ReplicaV2 and 5 for ScanNet++")
+    ap.add_argument("--resume", type=int, default=None, metavar="T",
+                    help="continue from the checkpoint of frame T under --out")
     a = ap.parse_args()
     if (a.lpips_alexnet is None) != (a.lpips_lin is None):
         ap.error("--lpips-alexnet and --lpips-lin go together")
+    if a.checkpoint_every < 0:
+        ap.error("--checkpoint-every must be 0 (off) or positive")
+    if (a.checkpoint_every or a.resume is not None) and a.out is None:
+        ap.error("--checkpoint-every and --resume need --out")
     if a.nvs and a.dataset not in ("scannetpp", "replicav2"):
         ap.error("--nvs needs a dataset with a test split (scannetpp, replicav2)")
     if a.variant == "splatam_s" and a.dataset not in HYPER_S:
@@ -120,12 +139,19 @@ def main():
     frames = _Capped(seq, a.frames)
     T = len(frames)
     K = seq.intrinsics.cpu()
+    from splatam_b200 import formats
+    t_resume = time.perf_counter()
     # the initial map and the scene radius come from the densification-size frame 0 when there is one
-    # (splatam.py:185-206): its max depth can be below the full-size one
+    # (splatam.py:185-206): its max depth can be below the full-size one; a resumed run reads frame 0 for the radius
+    # only, as the reference still computes it there
     first = frames[0].get("densify", frames[0])
-    init, _ = slam.initialize_map(first, first["intrinsics"].cpu())
-    initial_gaussians = int(init["means3D"].shape[0])
     radius = float(first["depth"].max()) / h["scene_radius_depth_ratio"]
+    if a.resume is None:
+        init, _ = slam.initialize_map(first, first["intrinsics"].cpu())
+        ckpt = None
+    else:
+        init, ckpt = None, formats.load_checkpoint(a.out, a.resume, dev)
+    initial_gaussians = int((init if ckpt is None else ckpt["gauss"])["means3D"].shape[0])
     timing = {}
     wait0 = seq.load_wait_s
     torch.cuda.synchronize(dev)
@@ -134,12 +160,17 @@ def main():
                         mapping_iters=h["mapping_iters"], keyframe_every=h["keyframe_every"], map_every=h["map_every"],
                         window=h["window"], sil_thres=SIL_THRES, intrinsics=K, add_new_gaussians=True, prune_dict=_PRUNE,
                         scene_radius=radius, select_keyframes=True, first_frame_iters=h["mapping_iters"],
-                        checkpoint_dir=None, tracking_lrs=h["tracking_lrs"], depth_loss_thres=h["depth_loss_thres"])
+                        checkpoint_dir=a.out if a.checkpoint_every else None,
+                        checkpoint_every=a.checkpoint_every or None, resume=ckpt,
+                        tracking_lrs=h["tracking_lrs"], depth_loss_thres=h["depth_loss_thres"])
     torch.cuda.synchronize(dev)
     wall = time.perf_counter() - t0
+    # --resume: wall time from reading the checkpoint to the first tracked frame (frame-0 read, load, keyframe rebuild)
+    resume_s = None if ckpt is None else t0 - t_resume + timing["setup_s"]
     load_wait = seq.load_wait_s - wait0
     gt = [seq.files.poses[t] for t in range(T)]
     gt_w2c = [torch.linalg.inv(p.to(dev)) for p in gt]
+    gt_w2c_all = seq.gt_w2c[:T]                  # the record's gt_w2c_all_frames: NaN where a pose is invalid
     params = dict(out["gauss"], cam_unnorm_rots=out["rots"], cam_trans=out["trans"])
     res = evaluate.evaluate(params, frames, seq.cam, SIL_THRES, h["mapping_iters"], True, eval_every=h["eval_every"],
                             gt_w2c=gt_w2c, out_dir=a.out, lpips=net)
@@ -157,12 +188,12 @@ def main():
         if net is not None:
             nvs["nvs_lpips"] = r["lpips"]
     if a.out is not None:
-        from splatam_b200 import formats
-        formats.save_params(params, a.out)
+        formats.save_run_record(a.out, out["gauss"], out["rots"], out["trans"], out["timestep"], K, seq.w2c, seq.width,
+                                seq.height, gt_w2c_all, out["keyframe_time_indices"])
     print(json.dumps(dict(
         dataset=a.dataset, sequence=a.sequence, variant=a.variant, frames=T, width=seq.width, height=seq.height,
         densify_height=seq.densify_height, densify_width=seq.densify_width, hyper=h,
-        initial_gaussians=initial_gaussians,
+        initial_gaussians=initial_gaussians, resumed_from=a.resume, resume_s=resume_s,
         ate_m=res["ate"], psnr_db=res["psnr"], ms_ssim=res["ms_ssim"], depth_l1_m=res["depth_l1"],
         gaussians=int(out["counts"][-1]), wall_s=wall, tracking_s=timing["tracking_s"], mapping_s=timing["mapping_s"],
         load_wait_ms_per_frame=1e3 * load_wait / max(T - 1, 1), evaluated_frames=len(res["frame_ids"]),
