@@ -272,7 +272,10 @@ SB_API int sb_masked_l1_backward(const float* depth_sil, const float* gt_depth, 
  * sb_backproject: pixels (all, or those with mask != 0 written to row dst_index[pixel]) -> new Gaussian rows:
  * means3D = c2w * ((x-cx)/fx*z, (y-cy)/fy*z, z, 1), rgb = colour of the pixel, log_scales = log(sqrt((z /
  * ((fx+fy)/2))^2)) repeated scale_dim times, optional mean_sq_dist (get_pointcloud, R/scripts/splatam.py:67-118;
- * initialize_new_params, :348-375).  c2w_host: 12+ floats, row-major 3x4 (or 4x4), HOST memory. */
+ * initialize_new_params, :348-375).  c2w_host: 12+ floats, row-major 3x4 (or 4x4), HOST memory.
+ * sb_densify_accumulate: the densification statistic (accumulate_mean2d_gradient, R/utils/slam_external.py:200-204):
+ * for every i < P with seen[i] != 0, accum[i] += sqrt(g0^2 + g1^2) and denom[i] += 1, where g = means2D_grad + i *
+ * grad_stride (>= 2 floats per row); one pass, no host synchronisation, bit-equal to the torch statement. */
 SB_API int sb_prune_mask(int P, const float* logit_opacities, const float* log_scales, int scale_dim,
                          float opacity_threshold, float big_threshold, uint8_t* keep, void* stream);
 SB_API int sb_compact_plan_bytes(int n, size_t* bytes);
@@ -280,6 +283,8 @@ SB_API int sb_compact_plan(int n, const uint8_t* keep, uint32_t* dst_index, void
                            int* count_host, void* stream);
 SB_API int sb_compact_flat(int P, int P_new, const uint8_t* keep, const uint32_t* dst_index, int num_segments,
                            const int* widths, const float* src, float* dst, void* stream);
+SB_API int sb_densify_accumulate(int P, const float* means2D_grad, int grad_stride, const uint8_t* seen, float* accum,
+                                 float* denom, void* stream);
 SB_API int sb_depth_error(int H, int W, const float* depth_sil, const float* gt_depth, float* err, void* stream);
 SB_API int sb_new_gaussian_mask(int H, int W, const float* depth_sil, const float* gt_depth, float sil_thres,
                                 float depth_err_thres, uint8_t* mask, void* stream);

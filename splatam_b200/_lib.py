@@ -80,6 +80,7 @@ _SIGNATURES = {
     "sb_compact_plan_bytes": (_i, [_i, ctypes.POINTER(ctypes.c_size_t)]),
     "sb_compact_plan": (_i, [_i, _vp, _vp, _vp, _sz, ctypes.POINTER(ctypes.c_int), _vp]),
     "sb_compact_flat": (_i, [_i, _i, _vp, _vp, _i, ctypes.POINTER(ctypes.c_int), _vp, _vp, _vp]),
+    "sb_densify_accumulate": (_i, [_i, _vp, _i, _vp, _vp, _vp, _vp]),
     "sb_depth_error": (_i, [_i, _i, _vp, _vp, _vp, _vp]),
     "sb_new_gaussian_mask": (_i, [_i, _i, _vp, _vp, ctypes.c_float, ctypes.c_float, _vp, _vp]),
     "sb_backproject": (_i, [_i, _i, _vp, _vp, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float,

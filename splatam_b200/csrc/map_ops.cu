@@ -82,6 +82,20 @@ new_gaussian_mask_kernel(int HW, const float* __restrict__ depth_sil, const floa
     mask[i] = ((no_sil || in_front) && gt > 0.f) ? 1 : 0;                // :394, :404-405
 }
 
+// accumulate_mean2d_gradient of densify (R/utils/slam_external.py:200-204) without the boolean-mask gathers and the
+// nonzero they synchronise on: each seen row gets accum += |g[:2]| and denom += 1, each element one addition, so the
+// result is the torch statement's bit for bit.  The norm is sqrt(round(gx^2) + round(gy^2)), the rounding of torch's
+// two-element NormTwoOps reduction: explicit _rn intrinsics keep nvcc from contracting it into an FMA.
+__global__ void __launch_bounds__(256)
+densify_accumulate_kernel(int P, const float* __restrict__ means2D_grad, int grad_stride,
+                          const uint8_t* __restrict__ seen, float* __restrict__ accum, float* __restrict__ denom) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P || !seen[i]) return;
+    const float gx = means2D_grad[(size_t)i * grad_stride], gy = means2D_grad[(size_t)i * grad_stride + 1];
+    accum[i] = __fadd_rn(accum[i], sqrtf(__fadd_rn(__fmul_rn(gx, gx), __fmul_rn(gy, gy))));
+    denom[i] = __fadd_rn(denom[i], 1.0f);
+}
+
 struct Mat34 { float m[12]; };
 
 __global__ void __launch_bounds__(256)
@@ -178,6 +192,17 @@ SB_API int sb_compact_flat(int P, int P_new, const uint8_t* keep, const uint32_t
     compact_flat_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(n, (uint32_t)P, (uint32_t)P_new, keep,
                                                                            dst_index, segs, src, dst);
     SB_LAUNCH_CHECK("compact_flat_kernel");
+    return SB_OK;
+}
+
+SB_API int sb_densify_accumulate(int P, const float* means2D_grad, int grad_stride, const uint8_t* seen, float* accum,
+                                 float* denom, void* stream) {
+    if (P < 0 || grad_stride < 2) return SB_ERR_BAD_ARG;
+    if (P == 0) return SB_OK;
+    if (!means2D_grad || !seen || !accum || !denom) return SB_ERR_BAD_ARG;
+    densify_accumulate_kernel<<<(P + 255) / 256, 256, 0, (cudaStream_t)stream>>>(P, means2D_grad, grad_stride, seen,
+                                                                                 accum, denom);
+    SB_LAUNCH_CHECK("densify_accumulate_kernel");
     return SB_OK;
 }
 

@@ -227,7 +227,7 @@ def _write_lists(out_dir, out):
 
 
 def evaluate(params, frames, cam, sil_thres, mapping_iters, add_new_gaussians, eval_every=1, gt_w2c=None, fused=None,
-             render=None, out_dir=None, lpips=None):
+             render=None, out_dir=None, lpips=None, at_gt_pose=False):
     """The reference's final `eval` over this repo's frame dicts (id, im [3,H,W] in [0,1], depth [1,H,W], w2c = the
     first frame's w2c, as slam.render_frame builds them).  `params`: the final Gaussians plus cam_unnorm_rots /
     cam_trans [.., T]; `cam`: the raster settings; frames are evaluated as `select_frames` picks them.
@@ -247,11 +247,14 @@ def evaluate(params, frames, cam, sil_thres, mapping_iters, add_new_gaussians, e
     depth_rmse_per_frame, depth_l1_per_frame, valid_pixels, mask_pixels and, with `lpips`, lpips_per_frame.
     `out_dir`: also writes psnr.txt, rmse.txt, l1.txt, ssim.txt and, with `lpips`, lpips.txt as the reference does
     (np.savetxt, one value per evaluated frame).
-    fused / render: as for mapping (`mapping._render_pair`); fused defaults to the fast path on CUDA."""
+    fused / render: as for mapping (`mapping._render_pair`); fused defaults to the fast path on CUDA.
+    at_gt_pose: render every frame at its `gt_w2c` instead of its estimated pose, as the offline drivers' `eval` does
+    (R/utils/gs_helpers.py:463-510); `params` then needs no camera tensors."""
     _check_inputs("evaluate", params, frames, lpips)
     ids = select_frames(len(frames), eval_every)
     use_presence = int(mapping_iters == 0 and not add_new_gaussians)
-    metrics, _ = _score_frames(params, frames, ids, cam, sil_thres, use_presence, render, fused, lpips=lpips)
+    metrics, _ = _score_frames(params, frames, ids, cam, sil_thres, use_presence, render, fused, at_gt_pose=at_gt_pose,
+                               lpips=lpips)
     m = metrics.cpu().numpy()                    # the one device-to-host read
     out = dict(frame_ids=[int(frames[t]["id"]) for t in ids], **_per_frame(m, lpips))
     out.update(psnr=float(m[:, _PSNR].mean()), ms_ssim=float(m[:, _SSIM].mean()),

@@ -120,7 +120,8 @@ def save_run_record(out_dir, gauss, rots, trans, timestep, intrinsics, first_w2c
     the five Gaussian tensors, cam_unnorm_rots / cam_trans, `timestep` [P], `intrinsics` [3,3], `w2c` (the first
     frame's) [4,4], all float32; `org_width` / `org_height` as 0-d int64; `gt_w2c_all_frames` [T,4,4] float32 (NaN where
     the pose is invalid); `keyframe_time_indices` int64.  `gt_w2c`: a [T,4,4] tensor / array or a list of [4,4].
-    Returns the path."""
+    keyframe_time_indices=None writes the 13 keys without it, as the offline drivers save their record
+    (R/scripts/post_splatam_opt.py:372-383).  Returns the path."""
     f32 = lambda a: np.ascontiguousarray(np.asarray(a.detach().cpu().numpy() if hasattr(a, "detach") else a,
                                                     dtype=np.float32))
     rec = {k: f32(gauss[k]) for k in GAUSSIAN_KEYS}
@@ -128,14 +129,15 @@ def save_run_record(out_dir, gauss, rots, trans, timestep, intrinsics, first_w2c
                intrinsics=f32(intrinsics)[:3, :3], w2c=f32(first_w2c).reshape(4, 4),
                org_width=np.array(int(width), dtype=np.int64), org_height=np.array(int(height), dtype=np.int64),
                gt_w2c_all_frames=(np.stack([f32(m).reshape(4, 4) for m in gt_w2c]) if len(gt_w2c)
-                                  else np.zeros((0, 4, 4), np.float32)),
-               keyframe_time_indices=np.array([int(i) for i in keyframe_time_indices], dtype=np.int64))
+                                  else np.zeros((0, 4, 4), np.float32)))
+    if keyframe_time_indices is not None:
+        rec["keyframe_time_indices"] = np.array([int(i) for i in keyframe_time_indices], dtype=np.int64)
     if rec["timestep"].shape[0] != rec["means3D"].shape[0]:
         raise ValueError("timestep has %d entries for %d Gaussians" % (rec["timestep"].shape[0],
                                                                      rec["means3D"].shape[0]))
     os.makedirs(out_dir, exist_ok=True)
     path = os.path.join(out_dir, "params.npz")
-    np.savez(path, **{k: rec[k] for k in RECORD_KEYS})
+    np.savez(path, **{k: rec[k] for k in RECORD_KEYS if k in rec})
     return path
 
 

@@ -48,6 +48,24 @@ def compact_flat(flat, P, widths, mask_u8, dst_index, P_new):
     return out
 
 
+def densify_accumulate(means2D_grad, seen, accum, denom):
+    """accum[seen] += norm(means2D_grad[seen, :2], dim=-1); denom[seen] += 1, in place and in one launch with no host
+    synchronisation (densify's statistic, R/utils/slam_external.py:200-204).  means2D_grad: contiguous float32 [P, >=2];
+    seen: bool [P]; accum, denom: contiguous float32 [P]."""
+    _lib.need_cuda("densify_accumulate", means2D_grad, seen, accum, denom)
+    P = accum.shape[0]
+    g = means2D_grad.detach()
+    if not (g.is_contiguous() and g.dtype == torch.float32 and g.dim() == 2 and g.shape[0] == P and g.shape[1] >= 2):
+        raise _lib.SplatamB200Error("densify_accumulate expects a contiguous float32 [%d, >=2] gradient, got %s %s"
+                                    % (P, g.dtype, tuple(g.shape)))
+    if seen.dtype != torch.bool or seen.numel() != P or not seen.is_contiguous():
+        raise _lib.SplatamB200Error("densify_accumulate expects a contiguous bool [%d] seen mask" % P)
+    for t in (accum, denom):
+        if t.dtype != torch.float32 or t.numel() != P or not t.is_contiguous():
+            raise _lib.SplatamB200Error("densify_accumulate expects contiguous float32 [%d] accum and denom" % P)
+    _lib.call("sb_densify_accumulate", P, g, g.shape[1], seen.view(torch.uint8), accum, denom, device=accum.device)
+
+
 def depth_error(depth_sil, gt_depth):
     """|gt - depth| * (gt > 0) over the frame (R/scripts/splatam.py:391)."""
     _lib.need_cuda("depth_error", depth_sil)

@@ -514,6 +514,13 @@ class FlatGaussians:
         self.bucket.zero_()
 
 
+def densify_due(iter, densify_dict):
+    """Whether `densify` edits the map at iteration `iter` (R/utils/slam_external.py:205): it then replaces every
+    Gaussian tensor, so in the reference's loops the optimizer step that follows finds no gradient."""
+    return (densify_dict["start_after"] <= iter <= densify_dict["stop_after"]
+            and iter % densify_dict["densify_every"] == 0)
+
+
 def default_render(settings, **rendervar):
     from .rasterizer import GaussianRasterizer
     return GaussianRasterizer(raster_settings=settings)(**rendervar)
@@ -615,6 +622,16 @@ class ShardedMapper:
         if self.fused:
             return self.opt.applied_steps()[0]
         return int(self.opt.state[self.g.params["means3D"]]["step"])
+
+    def set_lr(self, key, lr):
+        """Learning rate of Gaussian tensor `key` from the next Adam step on, and for the optimizers a map edit
+        rebuilds (update_learning_rate, R/utils/gs_external.py:260-266)."""
+        self.lrs[key] = float(lr)
+        i = GAUSSIAN_KEYS.index(key)
+        if self.fused:
+            self.opt.set_lr(i, lr)
+        else:
+            self.opt.param_groups[i]["lr"] = float(lr)
 
     def reset_optimizer(self):
         """Fresh Adam state, as the reference re-creates its optimizer at the start of every frame's mapping
@@ -873,10 +890,13 @@ class ShardedMapper:
             self.dist.all_reduce(st, op=self.dist.ReduceOp.SUM, group=self.group)
             self._dens["accum"] += st[0]
             self._dens["denom"] += st[1]
+        elif self.fused:            # one launch, no nonzero() synchronisation (csrc/map_ops.cu)
+            from . import map_ops
+            map_ops.densify_accumulate(means2D_grad, seen, self._dens["accum"], self._dens["denom"])
         else:
             self._dens["accum"][seen] += torch.norm(means2D_grad[seen, :2], dim=-1)      # accumulate_mean2d_gradient
             self._dens["denom"][seen] += 1
-        if not (iter >= densify_dict["start_after"] and iter % densify_dict["densify_every"] == 0):
+        if not densify_due(iter, densify_dict):
             return P
         grads = self._dens["accum"] / self._dens["denom"]
         grads[grads.isnan()] = 0.0

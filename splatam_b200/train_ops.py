@@ -30,6 +30,13 @@ class FusedAdam:
         self.betas, self.eps, self.t = betas, eps, int(step)
         self.clock = None           # device-side step clock of the guarded mode (created on first use)
 
+    def set_lr(self, segment, lr):
+        """Learning rate of segment `segment` from the next step on: a host-side write into the array each launch
+        reads (no reallocation, no synchronisation)."""
+        if not 0 <= int(segment) < self.n:
+            raise IndexError("segment %d out of range for %d segments" % (segment, self.n))
+        self.seg_lr[int(segment)] = float(lr)
+
     def _clock(self):
         if self.clock is None:
             nints = (int(_lib.load().sb_adam_clock_bytes()) + 3) // 4
