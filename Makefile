@@ -6,7 +6,8 @@ NVFLAGS := -O3 -std=c++17 $(ARCH) -lineinfo -Xcompiler -fPIC -Xcompiler -fvisibi
 CSRC := splatam_b200/csrc
 OBJS := $(CSRC)/abi.o $(CSRC)/radix_sort.o $(CSRC)/project.o $(CSRC)/binning.o $(CSRC)/blend_forward.o \
         $(CSRC)/blend_backward.o $(CSRC)/geometry_backward.o $(CSRC)/train_ops.o $(CSRC)/prepare.o $(CSRC)/sh.o \
-        $(CSRC)/map_ops.o $(CSRC)/eval_metrics.o $(CSRC)/ingest.o $(CSRC)/lpips.o
+        $(CSRC)/map_ops.o $(CSRC)/eval_metrics.o $(CSRC)/ingest.o $(CSRC)/lpips.o \
+        $(CSRC)/eval_frames.o
 LIB := splatam_b200/libsplatam_b200.so
 
 all: $(LIB) oracle

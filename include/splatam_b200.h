@@ -332,6 +332,16 @@ SB_API int sb_lpips_workspace_bytes(int N, int H, int W, size_t* bytes);
 SB_API int sb_lpips(const float* x, const float* y, int N, int H, int W, const float* weights, void* workspace,
                     size_t workspace_bytes, double* per_image, double* mean, void* stream);
 
+/* ---- saved evaluation frames (R/utils/eval_helpers.py:509-528, 755-774, save_frames=True) ---------------------------
+ * One launch per frame, no host synchronisation.  im, gt_im [3,H,W], depth_sil [3,H,W] (channel 0 is read),
+ * gt_depth [1,H,W], contiguous float; lut: 256 x RGB uint8 (device), the colormap; out: uint8 [4,H,W,3] (device) =
+ * {rendered RGB, rendered depth, ground-truth RGB, ground-truth depth}, HWC RGB.
+ *   RGB:   u8 = round_half_even(clamp(x, 0, 1) * 255f), NaN -> 0 (cv2.imwrite of a float32 image)
+ *   depth: lut[trunc(clip(d / 6f, 0, 1) * 255f)], an IEEE float32 division, NaN -> index 0
+ * SB_ERR_BAD_ARG for null pointers and non-positive sizes. */
+SB_API int sb_eval_frames_u8(const float* im, const float* depth_sil, const float* gt_im, const float* gt_depth, int H,
+                             int W, const uint8_t* lut, uint8_t* out, void* stream);
+
 /* ---- frame ingest (the dataset readers, splatam_b200/datasets.py; R/datasets/gradslam_datasets/basedataset.py) ---
  * One launch: rgb uint8 [color_height, color_width, 3] (HWC) and depth uint16 [depth_height, depth_width] (device)
  * -> color_out float32 [3, height, width] = float32(bilinear_f64(rgb)) / 255 and depth_out float32 [1, height, width]

@@ -92,6 +92,7 @@ _SIGNATURES = {
     "sb_lpips_weights_floats": (_i, [ctypes.POINTER(_sz)]),
     "sb_lpips_workspace_bytes": (_i, [_i, _i, _i, ctypes.POINTER(_sz)]),
     "sb_lpips": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, _vp, _vp, _vp]),
+    "sb_eval_frames_u8": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     "sb_ingest_rgbd": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, ctypes.c_double, _vp, _vp, _vp]),
     "sb_profile_begin": (_i, []),
     "sb_profile_end": (_i, [ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_int)]),

@@ -8,9 +8,12 @@ depth sums, MS-SSIM runs on the device, and the per-frame metrics stay on the de
 `evaluate_nvs` is the reference's novel-view evaluation (eval_helpers.py:626-841, `eval_nvs`) over a test split: the
 same metrics on held-out views rendered at their ground-truth poses, averaged over the views the map covers.
 LPIPS (AlexNet, v0.1, csrc/lpips.cu) is opt-in: pass ``lpips=LpipsAlex.load(alexnet_path, lin_path, device)`` with the
-two weight files already on disk (nothing is downloaded); without it the result carries ``lpips: None``.  CUDA only;
-no CPU fallback."""
+two weight files already on disk (nothing is downloaded); without it the result carries ``lpips: None``.
+``save_frames=True`` also writes the reference's four PNGs per evaluated frame (rendered and ground-truth colour and
+depth, csrc/eval_frames.cu), encoded by writer threads while the evaluation goes on.  CUDA only; no CPU fallback."""
 import os
+import queue
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
@@ -20,6 +23,39 @@ from . import mapping as M
 
 # columns of the per-frame metric rows: the five that sb_frame_metrics writes, then MS-SSIM and LPIPS
 _PSNR, _RMSE, _L1, _NVALID, _NMASK, _SSIM, _LPIPS = range(7)
+
+# cv2.COLORMAP_JET as 256 RGB entries, the table the reference's saved depth images go through:
+#   cv2.applyColorMap(np.arange(256, dtype=np.uint8)[:, None], cv2.COLORMAP_JET)[:, 0, ::-1].tobytes().hex()
+# No closed form was found that reproduces it: the usual clip(1.5 - |4x - c|, 0, 1) is one off at some entries, and
+# the integer ramps that match the rest give 2 where cv2 has 1 (blue, entry 159).
+JET_RGB = np.frombuffer(bytes.fromhex(
+    "00008000008400008800008c00009000009400009800009c0000a00000a40000a80000ac0000b00000b40000b80000bc"
+    "0000c00000c40000c80000cc0000d00000d40000d80000dc0000e00000e40000e80000ec0000f00000f40000f80000fc"
+    "0000ff0004ff0008ff000cff0010ff0014ff0018ff001cff0020ff0024ff0028ff002cff0030ff0034ff0038ff003cff"
+    "0040ff0044ff0048ff004cff0050ff0054ff0058ff005cff0060ff0064ff0068ff006cff0070ff0074ff0078ff007cff"
+    "0080ff0084ff0088ff008cff0090ff0094ff0098ff009cff00a0ff00a4ff00a8ff00acff00b0ff00b4ff00b8ff00bcff"
+    "00c0ff00c4ff00c8ff00ccff00d0ff00d4ff00d8ff00dcff00e0ff00e4ff00e8ff00ecff00f0ff00f4ff00f8ff00fcff"
+    "02fffe06fffa0afff60efff212ffee16ffea1affe61effe222ffde26ffda2affd62effd232ffce36ffca3affc63effc2"
+    "42ffbe46ffba4affb64effb252ffae56ffaa5affa65effa262ff9e66ff9a6aff966eff9272ff8e76ff8a7aff867eff82"
+    "82ff7e86ff7a8aff768eff7292ff6e96ff6a9aff669eff62a2ff5ea6ff5aaaff56aeff52b2ff4eb6ff4abaff46beff42"
+    "c2ff3ec6ff3acaff36ceff32d2ff2ed6ff2adaff26deff22e2ff1ee6ff1aeaff16eeff12f2ff0ef6ff0afaff06feff01"
+    "fffc00fff800fff400fff000ffec00ffe800ffe400ffe000ffdc00ffd800ffd400ffd000ffcc00ffc800ffc400ffc000"
+    "ffbc00ffb800ffb400ffb000ffac00ffa800ffa400ffa000ff9c00ff9800ff9400ff9000ff8c00ff8800ff8400ff8000"
+    "ff7c00ff7800ff7400ff7000ff6c00ff6800ff6400ff6000ff5c00ff5800ff5400ff5000ff4c00ff4800ff4400ff4000"
+    "ff3c00ff3800ff3400ff3000ff2c00ff2800ff2400ff2000ff1c00ff1800ff1400ff1000ff0c00ff0800ff0400ff0000"
+    "fc0000f80000f40000f00000ec0000e80000e40000e00000dc0000d80000d40000d00000cc0000c80000c40000c00000"
+    "bc0000b80000b40000b00000ac0000a80000a40000a000009c00009800009400009000008c0000880000840000800000"),
+    dtype=np.uint8).reshape(256, 3)
+
+# the reference's frame directories, in the order of sb_eval_frames_u8's four images
+FRAME_DIRS = ("rendered_rgb", "rendered_depth", "rgb", "depth")
+# threads that encode the saved frames; the evaluation loop waits only when all FRAME_WRITER_THREADS + 2 pinned host
+# slots hold frames not yet written.  Saving is bound by PNG encoding on the host, which scales with the threads
+# (tools/time_eval_frames.py: 3.3, 6.3, 13.1 and 25.4 frames/s at 1, 2, 4 and 8 threads, 1200x680, one H100 80GB HBM3
+# at 700 W with 16 host CPUs)
+FRAME_WRITER_THREADS = min(8, os.cpu_count() or 1)
+# zlib level of the saved PNGs: the contract is the decoded pixels, not the file bytes, so the fastest level is used
+PNG_COMPRESS_LEVEL = 1
 
 
 def _ms_ssim_into(x, y, data_range, per_channel, mean, ws=None):
@@ -135,6 +171,95 @@ def lpips(x, y, net, size_average=True):
     return out
 
 
+def jet_lut(device):
+    """JET_RGB as a contiguous uint8 [256, 3] tensor on `device`, the colormap sb_eval_frames_u8 reads."""
+    return torch.from_numpy(JET_RGB.copy()).to(device)
+
+
+def eval_frames_u8(im, depth_sil, gt_im, gt_depth, lut=None, out=None):
+    """The four images the reference saves for an evaluated frame (eval_helpers.py:509-528), as uint8 HWC RGB in one
+    [4, H, W, 3] CUDA tensor: the rendered colour `im` [3,H,W] and ground-truth colour `gt_im` [3,H,W] as
+    round_half_even(clamp(x, 0, 1) * 255) (NaN -> 0), the rendered depth (channel 0 of `depth_sil` [3,H,W], unmasked)
+    and `gt_depth` [1,H,W] through `lut` (default: JET_RGB) at trunc(clip(d / 6, 0, 1) * 255) (NaN -> 0), all in
+    float32 as numpy and cv2 compute them.  `out`: a contiguous uint8 [4,H,W,3] tensor to write into.  One launch on
+    the current stream, no synchronisation."""
+    _lib.need_cuda("eval_frames_u8", im, depth_sil, gt_im, gt_depth)
+    H, W = im.shape[-2:]
+    if im.shape != (3, H, W) or depth_sil.shape != (3, H, W) or gt_im.shape != (3, H, W) or \
+            gt_depth.shape != (1, H, W):
+        raise _lib.SplatamB200Error("eval_frames_u8 expects im, depth_sil, gt_im [3,H,W] and gt_depth [1,H,W], got "
+                                    "%s" % ([tuple(t.shape) for t in (im, depth_sil, gt_im, gt_depth)],))
+    dev = im.device
+    lut = jet_lut(dev) if lut is None else lut
+    if out is None:
+        out = torch.empty(4, H, W, 3, dtype=torch.uint8, device=dev)
+    if lut.dtype != torch.uint8 or lut.shape != (256, 3) or not lut.is_contiguous() or \
+            out.dtype != torch.uint8 or out.shape != (4, H, W, 3) or not out.is_contiguous():
+        raise _lib.SplatamB200Error("eval_frames_u8 needs a contiguous uint8 [256,3] lut and [4,H,W,3] out")
+    c = lambda t: t.detach().float().contiguous()
+    _lib.call("sb_eval_frames_u8", c(im), c(depth_sil), c(gt_im), c(gt_depth), H, W, lut, out, device=dev)
+    return out
+
+
+class _FrameWriter:
+    """Saves the four images of each evaluated frame under out_dir/{FRAME_DIRS} without holding up the evaluation:
+    sb_eval_frames_u8 writes one device staging buffer, an async copy moves it to a free pinned host slot, and a writer
+    thread waits for that copy's event, encodes the four PNGs with Pillow and frees the slot.  The next frame's kernel
+    may reuse the staging buffer at once, since it runs after the copy on the same stream.  `put` blocks only when every
+    host slot is busy.  `close` waits for every file and re-raises the first writer error; no thread outlives it.
+    File names: <render_prefix>_{i:04d}.png for the renders and gt_{i:04d}.png for the ground truth, with
+    i = t + index_offset for frame t."""
+
+    def __init__(self, out_dir, render_prefix, index_offset, H, W, device, threads=None):
+        threads = FRAME_WRITER_THREADS if threads is None else threads
+        self.dirs = [os.path.join(out_dir, d) for d in FRAME_DIRS]
+        for d in self.dirs:
+            os.makedirs(d, exist_ok=True)
+        self.prefixes = (render_prefix, render_prefix, "gt", "gt")
+        self.offset, self.H, self.W, self.device = index_offset, H, W, device
+        self.lut = jet_lut(device)
+        self.staging = torch.empty(4, H, W, 3, dtype=torch.uint8, device=device)
+        n = threads + 2
+        self.host = [torch.empty(4, H, W, 3, dtype=torch.uint8).pin_memory() for _ in range(n)]
+        self.events = [torch.cuda.Event() for _ in range(n)]
+        self.free = queue.SimpleQueue()
+        for s in range(n):
+            self.free.put(s)
+        self.pool = ThreadPoolExecutor(threads, thread_name_prefix="eval-frames")
+        self.jobs = []
+
+    def put(self, t, im, depth_sil, gt_im, gt_depth):
+        """Enqueues frame t's four images on the current stream (im, depth_sil, gt_im, gt_depth: contiguous float32)."""
+        s = self.free.get()
+        _lib.call("sb_eval_frames_u8", im, depth_sil, gt_im, gt_depth, self.H, self.W, self.lut, self.staging,
+                  device=self.device)
+        self.host[s].copy_(self.staging, non_blocking=True)
+        self.events[s].record()
+        i = t + self.offset
+        paths = [os.path.join(d, "%s_%04d.png" % (p, i)) for d, p in zip(self.dirs, self.prefixes)]
+        self.jobs.append(self.pool.submit(self._write, s, paths))
+
+    def _write(self, s, paths):
+        from PIL import Image
+        try:
+            self.events[s].synchronize()
+            px = self.host[s].numpy()
+            for k, path in enumerate(paths):
+                Image.fromarray(px[k]).save(path, compress_level=PNG_COMPRESS_LEVEL)
+        finally:
+            self.free.put(s)
+
+    def close(self):
+        self.pool.shutdown(wait=True)
+        for job in self.jobs:
+            job.result()
+
+
+def _check_save_frames(name, save_frames, out_dir):
+    if save_frames and out_dir is None:
+        raise ValueError("%s: save_frames=True needs out_dir" % name)
+
+
 def select_frames(num_frames, eval_every=1):
     """Indices the reference evaluates: frame 0, then every frame with (t + 1) % eval_every == 0
     (eval_helpers.py:447-448)."""
@@ -168,12 +293,13 @@ def _check_inputs(name, params, frames, lpips):
 
 
 def _score_frames(params, frames, ids, cam, sil_thres, use_presence, render, fused, at_gt_pose=False,
-                  count_holes=False, lpips=None):
+                  count_holes=False, lpips=None, writer=None):
     """Renders frames[t] for t in `ids` and scores each with sb_frame_metrics and MS-SSIM, and with sb_lpips on the
     same weighted images when `lpips` (an LpipsAlex) is given: float64 device rows [len(ids), 7] (columns _PSNR ..
     _LPIPS; _LPIPS stays 0 without `lpips`).  at_gt_pose: render at the frame's gt_w2c instead of its estimated pose.
     count_holes: also returns [len(ids), 7] rows of a presence-masked sb_frame_metrics call into scratch images, whose
-    _NVALID - _NMASK is the number of valid-depth pixels the silhouette leaves uncovered (None otherwise)."""
+    _NVALID - _NMASK is the number of valid-depth pixels the silhouette leaves uncovered (None otherwise).
+    writer: a _FrameWriter that is handed each frame's unmasked renders and ground truth."""
     render = M.default_render if render is None else render
     if fused is None:
         fused = render is M.default_render
@@ -198,6 +324,8 @@ def _score_frames(params, frames, ids, cam, sil_thres, use_presence, render, fus
             _lib.call("sb_frame_metrics", im, depth_sil, gt_im, gt_d, H, W, float(sil_thres), use_presence, w_im, w_gt,
                       ws_frame, ws_frame.numel(), metrics[k], device=dev)
             _ms_ssim_into(w_im[None], w_gt[None], 1.0, None, metrics[k, _SSIM], ws_ssim)
+            if writer is not None:
+                writer.put(t, im, depth_sil, gt_im, gt_d)
             if lpips is not None:                # sb_lpips clamps the weighted images to [0, 1] as it loads them
                 _lpips_into(w_im[None], w_gt[None], lpips, None, metrics[k, _LPIPS], ws_lpips)
             if count_holes:
@@ -227,7 +355,7 @@ def _write_lists(out_dir, out):
 
 
 def evaluate(params, frames, cam, sil_thres, mapping_iters, add_new_gaussians, eval_every=1, gt_w2c=None, fused=None,
-             render=None, out_dir=None, lpips=None, at_gt_pose=False):
+             render=None, out_dir=None, lpips=None, at_gt_pose=False, save_frames=False):
     """The reference's final `eval` over this repo's frame dicts (id, im [3,H,W] in [0,1], depth [1,H,W], w2c = the
     first frame's w2c, as slam.render_frame builds them).  `params`: the final Gaussians plus cam_unnorm_rots /
     cam_trans [.., T]; `cam`: the raster settings; frames are evaluated as `select_frames` picks them.
@@ -249,12 +377,22 @@ def evaluate(params, frames, cam, sil_thres, mapping_iters, add_new_gaussians, e
     (np.savetxt, one value per evaluated frame).
     fused / render: as for mapping (`mapping._render_pair`); fused defaults to the fast path on CUDA.
     at_gt_pose: render every frame at its `gt_w2c` instead of its estimated pose, as the offline drivers' `eval` does
-    (R/utils/gs_helpers.py:463-510); `params` then needs no camera tensors."""
-    _check_inputs("evaluate", params, frames, lpips)
+    (R/utils/gs_helpers.py:463-510); `params` then needs no camera tensors.
+    save_frames: also writes, for each evaluated frame t (its position in `frames`), the reference's four PNGs
+    (`eval_frames_u8` of the unmasked renders): out_dir/rendered_rgb/gs_{t:04d}.png, rendered_depth/gs_{t:04d}.png,
+    rgb/gt_{t:04d}.png and depth/gt_{t:04d}.png.  Needs `out_dir` (ValueError otherwise); returns once every file is
+    written and re-raises a writer's error."""
+    _check_save_frames("evaluate", save_frames, out_dir)
+    H, W = _check_inputs("evaluate", params, frames, lpips)
     ids = select_frames(len(frames), eval_every)
     use_presence = int(mapping_iters == 0 and not add_new_gaussians)
-    metrics, _ = _score_frames(params, frames, ids, cam, sil_thres, use_presence, render, fused, at_gt_pose=at_gt_pose,
-                               lpips=lpips)
+    writer = _FrameWriter(out_dir, "gs", 0, H, W, params["means3D"].device) if save_frames else None
+    try:
+        metrics, _ = _score_frames(params, frames, ids, cam, sil_thres, use_presence, render, fused,
+                                   at_gt_pose=at_gt_pose, lpips=lpips, writer=writer)
+    finally:
+        if writer is not None:
+            writer.close()
     m = metrics.cpu().numpy()                    # the one device-to-host read
     out = dict(frame_ids=[int(frames[t]["id"]) for t in ids], **_per_frame(m, lpips))
     out.update(psnr=float(m[:, _PSNR].mean()), ms_ssim=float(m[:, _SSIM].mean()),
@@ -273,7 +411,7 @@ def select_nvs_frames(num_frames, eval_every=1):
 
 
 def evaluate_nvs(params, frames, cam, sil_thres, mapping_iters, add_new_gaussians, eval_every=1, fused=None,
-                 render=None, out_dir=None, lpips=None):
+                 render=None, out_dir=None, lpips=None, save_frames=False):
     """The reference's novel-view evaluation `eval_nvs` over a test split (datasets.RGBDSequence(..., split="test"):
     frame 0 is the first train frame, frames 1.. the held-out views, each with its ground-truth `gt_w2c`).  Frames are
     picked by `select_nvs_frames` and rendered at gt_w2c -- the means transformed by it, anisotropic rotations
@@ -285,12 +423,21 @@ def evaluate_nvs(params, frames, cam, sil_thres, mapping_iters, add_new_gaussian
     valid views (NaN when none is valid), lpips (the same average with `lpips`, an LpipsAlex, else None), frame_ids
     (indices into `frames`), the per-frame arrays of `evaluate` over every evaluated view, hole_pixels and
     valid_nvs_frames (bool).  `out_dir`: also writes psnr.txt, rmse.txt, l1.txt, ssim.txt (and lpips.txt with `lpips`)
-    over every evaluated view and valid_nvs_frames.npy, as the reference does."""
+    over every evaluated view and valid_nvs_frames.npy, as the reference does.
+    save_frames: the four PNGs of `evaluate` for every evaluated view, valid or not, named by the test-view index
+    k = t - 1: rendered_rgb/splatam_{k:04d}.png, rendered_depth/splatam_{k:04d}.png, rgb/gt_{k:04d}.png and
+    depth/gt_{k:04d}.png.  Needs `out_dir` (ValueError otherwise)."""
+    _check_save_frames("evaluate_nvs", save_frames, out_dir)
     H, W = _check_inputs("evaluate_nvs", params, frames, lpips)
     ids = select_nvs_frames(len(frames), eval_every)
     use_presence = int(mapping_iters == 0 and not add_new_gaussians)
-    metrics, presence = _score_frames(params, frames, ids, cam, sil_thres, use_presence, render, fused,
-                                      at_gt_pose=True, count_holes=True, lpips=lpips)
+    writer = _FrameWriter(out_dir, "splatam", -1, H, W, params["means3D"].device) if save_frames else None
+    try:
+        metrics, presence = _score_frames(params, frames, ids, cam, sil_thres, use_presence, render, fused,
+                                          at_gt_pose=True, count_holes=True, lpips=lpips, writer=writer)
+    finally:
+        if writer is not None:
+            writer.close()
     m, p = torch.stack([metrics, presence]).cpu().numpy()          # the one device-to-host read
     holes = (p[:, _NVALID] - p[:, _NMASK]).astype(np.int64)
     valid = holes * 1000 <= H * W

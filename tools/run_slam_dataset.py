@@ -24,6 +24,8 @@ prefetch).  --out DIR writes the reference's psnr.txt / rmse.txt / l1.txt / ssim
 --lpips-alexnet PATH --lpips-lin PATH (both or neither: torchvision's alexnet-owt-7be5be79.pth and LPIPS v0.1's
 alex.pth, read from disk, never downloaded) add LPIPS to the evaluation: `lpips` (and `nvs_lpips` with --nvs) in the
 JSON line and lpips.txt under --out.
+--save-frames (needs --out) also saves the final evaluation's rendered and ground-truth colour and depth PNGs under
+--out (rendered_rgb/, rendered_depth/, rgb/, depth/), and with --nvs those of the novel views under --out/eval_nvs.
 --checkpoint-every N writes the reference's params{t}.npz / keyframe_time_indices{t}.npy, and a run_state{t}.npz
 sidecar, under --out every N frames; --resume T continues the run from the checkpoint of frame T under --out (one
 written here, or the reference's own, which then continues without the sidecar's RNG states):
@@ -113,6 +115,8 @@ def main():
                          "checkpoint_interval is 100 for Replica, TUM, ScanNet and ReplicaV2 and 5 for ScanNet++")
     ap.add_argument("--resume", type=int, default=None, metavar="T",
                     help="continue from the checkpoint of frame T under --out")
+    ap.add_argument("--save-frames", action="store_true",
+                    help="save the evaluation's rendered and ground-truth frames under --out")
     a = ap.parse_args()
     if (a.lpips_alexnet is None) != (a.lpips_lin is None):
         ap.error("--lpips-alexnet and --lpips-lin go together")
@@ -120,6 +124,8 @@ def main():
         ap.error("--checkpoint-every must be 0 (off) or positive")
     if (a.checkpoint_every or a.resume is not None) and a.out is None:
         ap.error("--checkpoint-every and --resume need --out")
+    if a.save_frames and a.out is None:
+        ap.error("--save-frames needs --out")
     if a.nvs and a.dataset not in ("scannetpp", "replicav2"):
         ap.error("--nvs needs a dataset with a test split (scannetpp, replicav2)")
     if a.variant == "splatam_s" and a.dataset not in HYPER_S:
@@ -173,7 +179,7 @@ def main():
     gt_w2c_all = seq.gt_w2c[:T]                  # the record's gt_w2c_all_frames: NaN where a pose is invalid
     params = dict(out["gauss"], cam_unnorm_rots=out["rots"], cam_trans=out["trans"])
     res = evaluate.evaluate(params, frames, seq.cam, SIL_THRES, h["mapping_iters"], True, eval_every=h["eval_every"],
-                            gt_w2c=gt_w2c, out_dir=a.out, lpips=net)
+                            gt_w2c=gt_w2c, out_dir=a.out, lpips=net, save_frames=a.save_frames)
     seq.close()
     nvs = {}
     if a.nvs:
@@ -181,7 +187,8 @@ def main():
                                    desired_width=h["width"], device=dev, prefetch=a.prefetch, split="test") as test:
             r = evaluate.evaluate_nvs(out["gauss"], test, test.cam, SIL_THRES, h["mapping_iters"], True,
                                       eval_every=h["eval_every"],
-                                      out_dir=None if a.out is None else os.path.join(a.out, "eval_nvs"), lpips=net)
+                                      out_dir=None if a.out is None else os.path.join(a.out, "eval_nvs"), lpips=net,
+                                      save_frames=a.save_frames)
         nvs = dict(nvs_psnr_db=r["psnr"], nvs_ms_ssim=r["ms_ssim"], nvs_depth_rmse_m=r["depth_rmse"],
                    nvs_depth_l1_m=r["depth_l1"], nvs_evaluated_frames=len(r["frame_ids"]),
                    nvs_valid_frames=int(r["valid_nvs_frames"].sum()))
