@@ -28,8 +28,13 @@ def _quat_to_rot(q):
 
 
 def render(means3D, colors, opacities, scales, rotations, *, width, height, tanfovx, tanfovy, bg,
-           viewmatrix, projmatrix, scale_modifier=1.0, means2D=None, dtype=torch.float64, rows=None):
+           viewmatrix, projmatrix, scale_modifier=1.0, means2D=None, dtype=torch.float64, rows=None,
+           frozen_clamp=False):
     """Returns dict(color [3,H,W], depth [1,H,W], final_T [H,W], n_contrib [H,W], radii [P]).
+
+    frozen_clamp=True: the backward of a Gaussian outside the 1.3 x tanfov frustum is the reference's (the clamped
+    coordinate is a constant); by default autograd differentiates through the clamp, as the CPU loop fixtures
+    (tests/golden/offline) were recorded.  The forward is the same either way.
 
     rows=(r0, r1): composite only image rows [r0, r1) (pixels are independent), returning images of height
     r1-r0 -- lets a caller walk a large image in bands with bounded memory (bench.py's brute-force timing).
@@ -63,6 +68,13 @@ def render(means3D, colors, opacities, scales, rotations, *, width, height, tanf
     tz = t[:, 2]
     txc = torch.clamp(t[:, 0] / tz, -limx, limx) * tz
     tyc = torch.clamp(t[:, 1] / tz, -limy, limy) * tz
+    if frozen_clamp:
+        # a coordinate clamped to the 1.3 x tanfov frustum is a constant to the reference's backward: no gradient to
+        # it (x_grad_mul = 0) and none through its clamped value to tz (dL/dtz differentiates J with t.x held fixed),
+        # backward.cu computeCov2DCUDA
+        txz, tyz = (t[:, 0] / tz).detach(), (t[:, 1] / tz).detach()
+        txc = torch.where((txz < -limx) | (txz > limx), txc.detach(), t[:, 0])
+        tyc = torch.where((tyz < -limy) | (tyz > limy), tyc.detach(), t[:, 1])
     zero = torch.zeros_like(tz)
     # J (GLM columns): J[0] = (fx/tz, 0, -fx tx/tz^2), J[1] = (0, fy/tz, -fy ty/tz^2), J[2] = 0
     J = torch.stack([torch.stack([fx / tz, zero, -(fx * txc) / (tz * tz)], -1),

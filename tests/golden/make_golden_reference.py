@@ -4,11 +4,14 @@ an H100 with oracle/_ref built:
 
     python tests/golden/make_golden_reference.py OUT_DIR
 
-then copy OUT_DIR/* into tests/golden/reference/.  The inputs are the tests' own seeded problems (imported from the
+then copy OUT_DIR/* into tests/golden/reference/.  `--only adversarial` writes only the parity_adv_*.npz records of
+the adversarial scenes (scenes.adversarial), leaving the other records -- and the atomics noise sampled into them --
+as they are.  The inputs are the tests' own seeded problems (imported from the
 test modules), so a fixture and the test that reads it always see the same data.  Large outputs are stored as
 SHA-256 digests of their bytes (for the bit-exact comparisons) and as a fixed, seeded sample of the Gaussians (for
 the gradient tolerances), which keeps every file far below 1 MB.
 """
+import argparse
 import json
 import os
 import sys
@@ -26,25 +29,40 @@ import test_ref_glue_gpu as TG  # noqa: E402
 import test_slam_gpu as TS  # noqa: E402
 import test_tracking_gpu as TT  # noqa: E402
 from gpu_harness import GRADS, random_dL, run_ref  # noqa: E402
-from util import digest, exact_arrays, l2_rel, reference_extension, sample_rows  # noqa: E402
+from util import REL, digest, exact_arrays, l2_rel, oracle_outputs, reference_extension, rel_err, sample_rows  # noqa: E402,E501
 
 
-def parity(name, make, out):
-    """test_cuda_vs_reference_extension: digests of every exact output, two runs' gradient noise, sampled gradients."""
+def parity(name, make, out, tails=False):
+    """test_cuda_vs_reference_extension: digests of every exact output, two runs' gradient noise (overall and per
+    gradient), sampled gradients; with `tails`, the fraction of all entries by which the reference misses the
+    double-accumulating C oracle at 10 x its tolerance (util.reference_tail)."""
     sc = make()
     dL = random_dL(sc)
     r1, r2 = run_ref(sc, dL), run_ref(sc, dL)
     idx = sample_rows(r1["radii"] > 0, 128)
     d = dict(num_rendered=r1["num_rendered"], index=idx,
              noise=max(l2_rel(r2["grad_" + k], r1["grad_" + k]) for k in GRADS),
+             **{"noise_" + k: l2_rel(r2["grad_" + k], r1["grad_" + k]) for k in GRADS},
              max_grad_rotations=np.abs(r1["grad_rotations"]).max(), max_grad_scales=np.abs(r1["grad_scales"]).max())
     for k, a in exact_arrays(r1).items():
         d["digest_" + k] = digest(a)
+    og = oracle_outputs(sc, dL) if tails else None
     for k in GRADS:
         g = r1["grad_" + k].reshape(sc.P, -1)
         d["grad_" + k] = g[idx]
         d["absmax_grad_" + k] = np.abs(g).max()
+        if tails:
+            # the reference's own element-wise miss of the double oracle over every entry, at the tests' threshold
+            tol = max(REL, 4 * d["noise_" + k])
+            d["tail_" + k] = float((rel_err(g, og["grad_" + k].reshape(sc.P, -1), 1e-3) > 10 * tol).mean())
     np.savez_compressed(os.path.join(out, "parity_%s.npz" % name), **d)
+
+
+def adversarial(out):
+    """test_raster_adversarial_gpu.test_adversarial_vs_reference_extension: one parity record per adversarial scene."""
+    for name, make in sorted(scenes.adversarial().items()):
+        parity("adv_" + name, make, out, tails=True)
+        print("parity adv_" + name, flush=True)
 
 
 def gradient_stats(out):
@@ -107,14 +125,23 @@ def loops(ref, out):
 
 
 if __name__ == "__main__":
-    out = sys.argv[1]
+    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
+    ap.add_argument("out", help="directory the records are written to")
+    ap.add_argument("--only", choices=["adversarial"], help="write only this group of records")
+    args = ap.parse_args()
+    out = args.out
     os.makedirs(out, exist_ok=True)
     ref = reference_extension()
     assert ref is not None and refsrc.available(), "oracle/_ref is not built (oracle/reference.py)"
+    if args.only == "adversarial":
+        adversarial(out)
+        print("adversarial records written to", out)
+        sys.exit(0)
     for name, make in TP.BIG:
         parity(name, make, out)
         print("parity", name, flush=True)
     branches(ref, out)
     loops(ref, out)
     gradient_stats(out)
+    adversarial(out)
     print("golden written to", out)

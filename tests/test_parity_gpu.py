@@ -14,55 +14,16 @@ import pytest
 import torch
 
 import scenes
-from util import GOLDEN, digest, exact_arrays, l2_rel, rel_err
+from util import GOLDEN, GRADS, REL, bits, check_against, check_against_reference, digest, l2_rel, \
+    oracle_outputs, rel_err
 
 pytestmark = pytest.mark.gpu
 
-GRADS = ["means3D", "means2D", "colors", "opacities", "scales", "rotations"]
-REL = 1e-4
 REF_GOLDEN = os.path.join(GOLDEN, "reference")      # written by tests/golden/make_golden_reference.py
 
 
 def _golden(name):
     return np.load(os.path.join(REF_GOLDEN, name))
-
-
-def _bits(a):
-    return np.ascontiguousarray(a).view(np.uint32)
-
-
-def _check_against(ours, ref, exact_images, tag, grad_tol=REL):
-    vis = ref["radii"] > 0
-    assert np.array_equal(ours["radii"], ref["radii"]), tag
-    assert np.array_equal(ours["tiles_touched"], ref["tiles_touched"]), tag
-    assert np.array_equal(_bits(ours["depths"][vis]), _bits(ref["depths"][vis])), tag
-    assert np.array_equal(_bits(ours["means2D"][vis]), _bits(ref["means2D"][vis])), tag
-    assert np.array_equal(_bits(ours["conic_opacity"][vis]), _bits(ref["conic_opacity"][vis])), tag
-    assert ours["num_rendered"] == len(ref["keys"]), tag
-    assert np.array_equal(ours["keys"], ref["keys"]), tag + ": sorted (tile|depth) keys must be bit-identical"
-    assert np.array_equal(ours["point_list"], ref["point_list"]), tag
-    assert np.array_equal(ours["ranges"], ref["ranges"]), tag
-    if exact_images:
-        assert np.array_equal(ours["n_contrib"], ref["n_contrib"]), tag
-        assert np.array_equal(_bits(ours["final_T"]), _bits(ref["final_T"])), tag
-        assert np.array_equal(_bits(ours["color"]), _bits(ref["color"])), tag
-        assert np.array_equal(_bits(ours["depth"]), _bits(ref["depth"])), tag
-    else:  # CPU expf differs from libdevice expf by an ulp or two
-        assert (ours["n_contrib"] != ref["n_contrib"]).mean() < 1e-3, tag
-        assert (rel_err(ours["color"], ref["color"], 1e-3) > REL).mean() < 1e-3, tag
-        assert (rel_err(ours["final_T"], ref["final_T"], 1e-3) > REL).mean() < 1e-3, tag
-    for k in GRADS:
-        a, b = ours["grad_" + k].reshape(-1), ref["grad_" + k].reshape(-1)
-        if k == "rotations" and np.abs(b).max() < 1e-6 * np.abs(ref["grad_scales"]).max():
-            # isotropic scene: the quaternion gradient is mathematically zero and pure cancellation noise (~1e-10) in
-            # every implementation (the reference's two runs differ by ~100 % here); only its smallness is meaningful
-            assert np.abs(a).max() < 1e-6 * np.abs(ref["grad_scales"]).max(), (tag, k)
-            continue
-        assert l2_rel(a, b) < grad_tol, (tag, k, l2_rel(a, b))
-        # element-wise: entries that are sums with heavy cancellation carry float32 summation-order noise
-        # (the reference's own atomics are order-nondeterministic), so floor at 1e-3 of the largest entry
-        frac = (rel_err(a, b, 1e-3) > 10 * grad_tol).mean()
-        assert frac <= max(2e-3, 2.0 / a.size), (tag, k, frac)
 
 
 SMALL = [scenes.config1, scenes.edge_cases, lambda: scenes.dense_opaque(P=600, w=64, h=48),
@@ -75,14 +36,7 @@ def test_cuda_vs_oracle(make, cuda_device):
     sc = make()
     dL = random_dL(sc)
     ours = run_ours(sc, dL)
-    o = sc.oracle()
-    geo, b, r = o.geometry(), o.binning(), o.render()
-    g = o.backward(dL)
-    ref = dict(radii=geo["radii"], tiles_touched=geo["tiles_touched"], depths=geo["depths"], means2D=geo["means2D"],
-               conic_opacity=geo["conic_opacity"], keys=b["keys"], point_list=b["point_list"], ranges=b["ranges"],
-               n_contrib=r["n_contrib"], final_T=r["final_T"], color=r["color"], depth=r["depth"])
-    ref.update({"grad_" + k: g[k] for k in GRADS})
-    _check_against(ours, ref, exact_images=False, tag=sc.name + " vs oracle")
+    check_against(ours, oracle_outputs(sc, dL), exact_images=False, tag=sc.name + " vs oracle")
 
 
 @pytest.mark.parametrize("path", sorted(glob.glob(os.path.join(GOLDEN, "*.npz"))) or [None])
@@ -97,7 +51,7 @@ def test_cuda_vs_golden(path, cuda_device):
                       w2c=torch.from_numpy(z["w2c"]), bg=tuple(z["bg"].tolist()))
     ours = run_ours(sc, z["dL_dcolor"])
     ref = {k[4:]: z[k] for k in z.files if k.startswith("ref_")}
-    _check_against(ours, ref, exact_images=True, tag=os.path.basename(path))
+    check_against(ours, ref, exact_images=True, tag=os.path.basename(path))
 
 
 BIG = [("config1", scenes.config1), ("edge", scenes.edge_cases), ("dense", lambda: scenes.dense_opaque()),
@@ -111,28 +65,11 @@ BIG = [("config1", scenes.config1), ("edge", scenes.edge_cases), ("dense", lambd
 @pytest.mark.parametrize("name,make", BIG)
 def test_cuda_vs_reference_extension(name, make, cuda_device):
     """Same inputs as the unmodified reference extension was given (tests/golden/reference/parity_<name>.npz): every
-    output of _check_against's exact branch bit for bit (as SHA-256 digests), the gradients on a seeded sample of the
+    output of check_against's exact branch bit for bit (as SHA-256 digests), the gradients on a seeded sample of the
     visible Gaussians within max(1e-4, 4 x the reference's own run-to-run atomics noise)."""
     from gpu_harness import random_dL, run_ours
-    z = _golden("parity_%s.npz" % name)
     sc = make()
-    ours = run_ours(sc, random_dL(sc))
-    assert ours["num_rendered"] == int(z["num_rendered"]), name
-    for k, a in exact_arrays(ours).items():
-        assert digest(a) == str(z["digest_" + k]), (name, k, "must be bit-identical to the reference")
-    grad_tol = max(REL, 4 * float(z["noise"]))
-    scale = float(z["max_grad_scales"])
-    for k in GRADS:
-        g = ours["grad_" + k].reshape(sc.P, -1)
-        if k == "rotations" and float(z["max_grad_rotations"]) < 1e-6 * scale:
-            # isotropic scene: the quaternion gradient is mathematically zero (see _check_against)
-            assert np.abs(g).max() < 1e-6 * scale, (name, k)
-            continue
-        a, b = g[z["index"]].reshape(-1), z["grad_" + k].reshape(-1)
-        assert l2_rel(a, b) < grad_tol, (name, k, l2_rel(a, b))
-        e = np.abs(a - b) / np.maximum(np.abs(b), 1e-3 * float(z["absmax_grad_" + k]))
-        frac = (e > 10 * grad_tol).mean()
-        assert frac <= max(2e-3, 2.0 / a.size), (name, k, frac)
+    check_against_reference(run_ours(sc, random_dL(sc)), _golden("parity_%s.npz" % name), sc.P, name)
 
 
 def _err_stats(a, b):
@@ -179,11 +116,11 @@ def test_full_size_properties(cuda_device):
     same = keys[1:] == keys[:-1]
     assert np.all(lst[1:][same] > lst[:-1][same])
     assert int(a["tiles_touched"].sum()) == a["num_rendered"] == int((a["ranges"][:, 1] - a["ranges"][:, 0]).sum())
-    assert np.array_equal((keys & 0xFFFFFFFF).astype(np.uint32), _bits(a["depths"])[lst])
+    assert np.array_equal((keys & 0xFFFFFFFF).astype(np.uint32), bits(a["depths"])[lst])
     # forward is deterministic; backward is linear in dL/dcolor
     b = run_ours(sc, dL2, intermediates=False)
     c = run_ours(sc, dL1 + dL2, intermediates=False)
-    assert np.array_equal(_bits(a["color"]), _bits(b["color"]))
+    assert np.array_equal(bits(a["color"]), bits(b["color"]))
     for k in GRADS:
         if k == "rotations":   # isotropic scene: the quaternion gradient is pure cancellation noise (~1e-12)
             assert np.abs(c["grad_" + k]).max() < 1e-6 * np.abs(c["grad_scales"]).max()
