@@ -19,6 +19,8 @@ import math
 import torch
 import torch.nn.functional as F
 
+from .rasterizer import GaussianRasterizer
+
 GAUSSIAN_KEYS = ("means3D", "rgb_colors", "unnorm_rotations", "logit_opacities", "log_scales")
 
 
@@ -204,7 +206,6 @@ def _render_pair(params, frame, render, fused, camera_grad, max_rendered=None):
                                 pose=frame.get("pose"))
         rv_rgb, rv_depth = rgb_rendervar(params, tg), depth_sil_rendervar(params, frame["w2c"], tg)
     if fused and render is default_render:
-        from .rasterizer import GaussianRasterizer
         im, depth_sil, radius, _ = GaussianRasterizer(raster_settings=frame["cam"], max_rendered=max_rendered).forward_fused(
             means3D=rv_rgb["means3D"], means2D=rv_rgb["means2D"], opacities=rv_rgb["opacities"],
             colors_precomp=rv_rgb["colors_precomp"], colors_extra=rv_depth["colors_precomp"],
@@ -213,19 +214,6 @@ def _render_pair(params, frame, render, fused, camera_grad, max_rendered=None):
         im, radius, _ = render(frame["cam"], **rv_rgb)
         depth_sil, _, _ = render(frame["cam"], **rv_depth)
     return im, depth_sil, radius, rv_rgb["means2D"]
-
-
-def _capacity(params, frames, slack):
-    """Instance capacity of the sync-free rasterizer for renders like those of `frames`: one synchronous forward per
-    frame, slack x the largest num_rendered, plus 4096."""
-    from . import rasterizer
-    worst = 0
-    for fr in frames:
-        with torch.no_grad():
-            rgb, _ = fused_rendervars(params, fr["id"], fr["w2c"], camera_grad=False)
-            rasterizer.GaussianRasterizer(fr["cam"])(**rgb)
-        worst = max(worst, rasterizer._LAST_SYNC_R[0])
-    return int(worst * slack) + 4096
 
 
 def mapping_loss(params, frame, render, loss_weights=(0.5, 1.0), ignore_outlier_depth_loss=False, fused_loss=False,
@@ -333,48 +321,75 @@ def track_frame(params, frame, render=None, num_iters=40, lr_rot=0.0004, lr_tran
     return losses
 
 
-def _capture(body):
-    """Captures body() on the CURRENT (non-default) stream into a CUDA graph.  capture_begin / capture_end directly: the
-    torch.cuda.graph context manager also runs gc.collect() and torch.cuda.empty_cache(), which costs tens of
-    milliseconds and throws the allocator's cached blocks away."""
-    g = torch.cuda.CUDAGraph()
-    g.capture_begin()
-    try:
-        body()
-    finally:
-        g.capture_end()
-    return g
+class _CapturedStep:
+    """One step over the sync-free rasterizer, captured into a CUDA graph on a side stream and replayed: its instance
+    capacity `cap`, the static frame buffers it renders (`frame`: id, cam, w2c, im, depth; `load` refills them) and
+    the overflow flag of its render.  `cap` is `capacity`, or slack x the largest instance count of the `probe`
+    frames at their poses in `params`, plus 4096."""
+
+    def __init__(self, params, frame, probe, slack, capacity=None):
+        self.dev = params["means3D"].device
+        if capacity is None:
+            worst = 0
+            for fr in probe:
+                with torch.no_grad():
+                    rgb, _ = fused_rendervars(params, fr["id"], fr["w2c"], camera_grad=False)
+                worst = max(worst, GaussianRasterizer(fr["cam"]).num_rendered(rgb["means3D"], rgb["opacities"],
+                                                                              rgb["scales"], rgb["rotations"]))
+            capacity = int(worst * slack) + 4096
+        self.cap = int(capacity)
+        self.frame = dict(id=frame["id"], cam=frame["cam"], w2c=frame["w2c"].clone(), im=frame["im"].clone(),
+                          depth=frame["depth"].clone())
+        self.side = torch.cuda.Stream(self.dev)
+        self.side.wait_stream(torch.cuda.current_stream(self.dev))      # for state a caller creates on it before capture
+
+    def load(self, frame):
+        for k in ("im", "depth", "w2c"):
+            self.frame[k].copy_(frame[k], non_blocking=True)
+
+    def overflow(self):
+        """int32 [1] device view of the overflow flag of the latest sync-free render: inside the step, its own."""
+        return GaussianRasterizer.last_state(self.dev).header()[2:3]
+
+    def capture(self, body):
+        """Runs body() three times (warm-up: kernels load, lazily created state such as capturable Adam's exists),
+        then captures it into `graph`, all on the side stream after the work enqueued so far on the current one.
+        capture_begin / capture_end directly: the torch.cuda.graph context manager also runs gc.collect() and
+        torch.cuda.empty_cache(), which costs tens of milliseconds and throws the allocator's cached blocks away."""
+        self.side.wait_stream(torch.cuda.current_stream(self.dev))
+        with torch.cuda.stream(self.side):
+            for _ in range(3):
+                body()
+            self.graph = torch.cuda.CUDAGraph()
+            self.graph.capture_begin()
+            try:
+                body()
+            finally:
+                self.graph.capture_end()
+        torch.cuda.current_stream(self.dev).wait_stream(self.side)
 
 
 class _TrackingGraph:
     """One captured tracking iteration (loss forward + backward over the sync-free rasterizer, capturable Adam step,
-    best-pose bookkeeping, all on the device) bound to ONE map (the parameter tensors' storage), camera and iteration
-    count -- not to a pose column: the pose travels through two small leaf tensors.  Re-used frame after frame while the map tensors stay the same objects (tracking-only runs; SLAM phases
-    without map growth): a frame then costs two small image copies, `num_iters` graph launches and one host
-    synchronisation.
+    best-pose bookkeeping, all on the device) bound to ONE map (the Gaussian tensors' storage), camera and iteration
+    count -- not to a pose column: the pose travels through two small leaf tensors.  Re-used frame after frame while
+    the map tensors stay the same objects (tracking-only runs; SLAM phases without map growth): a frame then costs two
+    small image copies, `num_iters` graph launches and one host synchronisation.
 
     With `depth_loss_thres` the graph records the depth L1 sum too and a frame replays 2 * num_iters iterations; the
     decision of track_frame's rule is taken on the device after iteration num_iters, and when the frame stops there
     the remaining replays run gated: they record no loss, update no best pose and raise no overflow.  The frame
     still costs one host synchronisation; the gated replays cost GPU time."""
 
-    def __init__(self, params, frame, num_iters, lr_rot, lr_trans, slack=1.5, depth_loss_thres=None):
-        from .rasterizer import GaussianRasterizer
-        dev = params["means3D"].device
-        self.dev, self.t, self.num_iters = dev, frame["id"], num_iters
+    def __init__(self, params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres=None):
         t = frame["id"]
         rots, trans = params["cam_unnorm_rots"], params["cam_trans"]
-        self.gp = dict({k: params[k].detach() for k in GAUSSIAN_KEYS}, cam_unnorm_rots=rots.detach(), cam_trans=trans.detach())
-        self.key = _tracking_key(params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres)
+        self.gp = gp = {k: params[k].detach() for k in GAUSSIAN_KEYS}        # keeps the storage the graph reads alive
         self.rule = rule = depth_loss_thres is not None
         self.replays = 2 * num_iters if rule else num_iters
-        gp = self.gp
-        cap = _capacity(gp, [frame], slack)         # sized at the starting pose
-        self.side = torch.cuda.Stream(dev)
-        self.side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(self.side):
-            self.im, self.depth, self.w2c = frame["im"].clone(), frame["depth"].clone(), frame["w2c"].clone()
-            static = dict(id=t, cam=frame["cam"], w2c=self.w2c, im=self.im, depth=self.depth)
+        self.step = step = _CapturedStep(params, frame, [frame], slack=1.5)     # sized at the starting pose
+        dev = step.dev
+        with torch.cuda.stream(step.side):
             self.q = rots[..., t].detach().clone().requires_grad_(True)      # [1,4], [1,3]: leaves born on the capture stream
             self.tr = trans[..., t].detach().clone().requires_grad_(True)
             q, tr = self.q, self.tr
@@ -388,47 +403,43 @@ class _TrackingGraph:
             self.bad_any = torch.zeros(1, device=dev)
             self.live = torch.ones(1, dtype=torch.bool, device=dev)   # rule only: this replay is a real iteration
 
-            def body():
-                q.grad.zero_(); tr.grad.zero_()
-                keep = {} if rule else None
-                loss, _ = tracking_loss(gp, dict(static, pose=camera_w2c(q, tr)), default_render, fused=True,
-                                        max_rendered=cap, keep=keep)
-                loss.backward()
-                lossd = loss.detach().reshape(1)
-                bad = (GaussianRasterizer.last_state(dev).header()[2:3] != 0) | ~torch.isfinite(lossd)
-                q.grad.copy_(torch.where(bad, torch.zeros_like(q.grad), q.grad))
-                tr.grad.copy_(torch.where(bad, torch.zeros_like(tr.grad), tr.grad))
-                self.bad_any.add_((bad & self.live).float() if rule else bad.float())
-                self.opt.step()
-                # the reference's rule (splatam.py:703-712): candidate = pose AFTER the step, ranked by the loss evaluated
-                # before it; the first strictly smaller loss wins
-                better = (lossd < self.best_loss) & ~bad
-                if rule:
-                    better = better & self.live
-                self.best_loss.copy_(torch.where(better, lossd, self.best_loss.reshape(1)).reshape(()))
-                self.best_q.copy_(torch.where(better, q.detach(), self.best_q))
-                self.best_tr.copy_(torch.where(better, tr.detach(), self.best_tr))
-                self.hist.scatter_(0, self.it, lossd)
-                if rule:
-                    # a gated replay overwrites slot `it` (the first unused one, num_iters) and does not advance `it`
-                    self.it.add_(self.live.long())
-                    # after the num_iters-th real iteration: continue only if its depth sum is not below the threshold
-                    stop = self.live & (self.it == num_iters) & (keep["depth"].detach().reshape(1) < depth_loss_thres)
-                    self.live.copy_(self.live & ~stop)
-                else:
-                    self.it.add_(1)
-            self.body = body
-            for _ in range(3):              # warm-up (initialises the capturable Adam state); undone by reset()
-                body()
-            self.graph = _capture(body)
-        torch.cuda.current_stream(dev).wait_stream(self.side)
+        def body():
+            q.grad.zero_(); tr.grad.zero_()
+            keep = {} if rule else None
+            loss, _ = tracking_loss(gp, dict(step.frame, pose=camera_w2c(q, tr)), default_render, fused=True,
+                                    max_rendered=step.cap, keep=keep)
+            loss.backward()
+            lossd = loss.detach().reshape(1)
+            bad = (step.overflow() != 0) | ~torch.isfinite(lossd)
+            q.grad.copy_(torch.where(bad, torch.zeros_like(q.grad), q.grad))
+            tr.grad.copy_(torch.where(bad, torch.zeros_like(tr.grad), tr.grad))
+            self.bad_any.add_((bad & self.live).float() if rule else bad.float())
+            self.opt.step()
+            # the reference's rule (splatam.py:703-712): candidate = pose AFTER the step, ranked by the loss evaluated
+            # before it; the first strictly smaller loss wins
+            better = (lossd < self.best_loss) & ~bad
+            if rule:
+                better = better & self.live
+            self.best_loss.copy_(torch.where(better, lossd, self.best_loss.reshape(1)).reshape(()))
+            self.best_q.copy_(torch.where(better, q.detach(), self.best_q))
+            self.best_tr.copy_(torch.where(better, tr.detach(), self.best_tr))
+            self.hist.scatter_(0, self.it, lossd)
+            if rule:
+                # a gated replay overwrites slot `it` (the first unused one, num_iters) and does not advance `it`
+                self.it.add_(self.live.long())
+                # after the num_iters-th real iteration: continue only if its depth sum is not below the threshold
+                stop = self.live & (self.it == num_iters) & (keep["depth"].detach().reshape(1) < depth_loss_thres)
+                self.live.copy_(self.live & ~stop)
+            else:
+                self.it.add_(1)
+        step.capture(body)              # the warm-up's optimizer steps and records are undone by reset()
 
     def reset(self, params, frame):
         """Loads a frame: images, starting pose, fresh optimizer state (the reference builds a new Adam per frame,
         splatam.py:680), empty best-pose record."""
         t = frame["id"]
         with torch.no_grad():
-            self.im.copy_(frame["im"]); self.depth.copy_(frame["depth"]); self.w2c.copy_(frame["w2c"])
+            self.step.load(frame)
             self.q.copy_(params["cam_unnorm_rots"][..., t]); self.tr.copy_(params["cam_trans"][..., t])
             for st in self.opt.state.values():
                 st["exp_avg"].zero_(); st["exp_avg_sq"].zero_(); st["step"].zero_()
@@ -436,13 +447,13 @@ class _TrackingGraph:
             self.hist.zero_(); self.it.zero_(); self.bad_any.zero_(); self.live.fill_(True)
 
     def run(self, params, frame):
-        dev = self.dev
-        self.side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(self.side):
+        side, cur = self.step.side, torch.cuda.current_stream(self.step.dev)
+        side.wait_stream(cur)
+        with torch.cuda.stream(side):
             self.reset(params, frame)
             for _ in range(self.replays):
-                self.graph.replay()
-        torch.cuda.current_stream(dev).wait_stream(self.side)
+                self.step.graph.replay()
+        cur.wait_stream(side)
         if float(self.bad_any) != 0.0:                                   # the one host synchronisation of the frame
             return None
         with torch.no_grad():
@@ -456,14 +467,16 @@ _TRACK_GRAPHS = {}
 
 
 def _tracking_key(params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres):
-    return (params["means3D"].data_ptr(), tuple(params["means3D"].shape), params["log_scales"].shape[1],
-            id(frame["cam"]), tuple(frame["im"].shape), num_iters, lr_rot, lr_trans, depth_loss_thres)
+    """What a captured tracking iteration is bound to: the storage (pointer and shape) of each Gaussian tensor it
+    reads, the camera, the image shape, the iteration count, the learning rates and the depth-loss rule."""
+    return (tuple((params[k].data_ptr(), tuple(params[k].shape)) for k in GAUSSIAN_KEYS), id(frame["cam"]),
+            tuple(frame["im"].shape), num_iters, lr_rot, lr_trans, depth_loss_thres)
 
 
 def _track_frame_graphed(params, frame, num_iters, lr_rot, lr_trans, build=True, depth_loss_thres=None):
     """Graph-replayed tracking of one frame, or None when no graph is available / an iteration overflowed the instance
-    capacity (the caller then runs the frame eagerly).  Graphs are cached per (map storage, camera, pose column,
-    iteration count); `build` creates one on a miss (worth it for long loops or when the map stays put)."""
+    capacity (the caller then runs the frame eagerly).  Graphs are cached per `_tracking_key`; `build` creates one on
+    a miss (worth it for long loops or when the map stays put)."""
     key = _tracking_key(params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres)
     tg = _TRACK_GRAPHS.get(key)
     if tg is None:
@@ -522,7 +535,6 @@ def densify_due(iter, densify_dict):
 
 
 def default_render(settings, **rendervar):
-    from .rasterizer import GaussianRasterizer
     return GaussianRasterizer(raster_settings=settings)(**rendervar)
 
 
@@ -566,10 +578,7 @@ class ShardedMapper:
         self.last_means2D_grad = self.last_seen_local = None
         self._dens = None                   # densification statistic: dict(accum, denom) per Gaussian
         self._dev_gen = None                # shared-seed device generator of the split samples (world > 1)
-        # CUDA-graph mode (enable_graph): captured step, its static frame buffers, instance capacity, in-flight polls
-        self._graph = self._static = None
-        self._cap, self._slack = 0, 1.3
-        self._polls, self._pin = [], []
+        self._graph = None                  # CUDA-graph mode: the captured step (enable_graph)
         self.overflow_events = 0
 
     def params(self):
@@ -754,52 +763,28 @@ class ShardedMapper:
         polls the flag with a one-step lag, never blocking on the step in flight -- re-captures with a larger
         capacity.  An overflowed step therefore costs time, never correctness."""
         assert self.fused and self.g.flat.is_cuda and self.render is default_render
-        from .rasterizer import GaussianRasterizer
-        dev = self.g.flat.device
-        f0 = window[0]
-        if capacity is None:
-            # a few synchronous forwards size the capacity (an overflow later is safe: it skips the step and
-            # re-captures, see the docstring)
-            probe = window if len(window) <= 3 else [window[0], window[len(window) // 2], window[-1]]
-            capacity = _capacity(self.params(), probe, slack)
-        self._cap = int(capacity)
+        # a geometry pass per probed frame sizes the capacity (an overflow later is safe: it skips the step and
+        # re-captures, see the docstring)
+        probe = window if len(window) <= 3 else [window[0], window[len(window) // 2], window[-1]]
+        step = _CapturedStep(self.params(), window[0], probe, slack, capacity)
+        step.frame["pose"] = tuple(t.clone() for t in fused_pose_cached(self.params(), window[0]["id"]))
         self._slack = slack
         self._polls = []                 # (event, pinned copy of the overflow slot) of steps in flight
         self._pin = [torch.empty(1, dtype=torch.float32, pin_memory=True) for _ in range(8)]
-        self._static = dict(id=f0["id"], cam=f0["cam"], w2c=f0["w2c"].clone(), im=f0["im"].clone(), depth=f0["depth"].clone(),
-                            pose=tuple(t.clone() for t in pose_matrices(self.params(), f0["id"])))
-        side = torch.cuda.Stream(dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):
-            for _ in range(3):
-                self.g.zero_grad()
-                loss, radius = mapping_loss(self.params(), self._static, self.render, fused_loss=True, max_rendered=self._cap)
-                loss.backward()
+
         def body():
             self.g.bucket.zero_()
-            loss, radius = mapping_loss(self.params(), self._static, self.render, fused_loss=True, max_rendered=self._cap)
+            loss, radius = mapping_loss(self.params(), step.frame, self.render, fused_loss=True, max_rendered=step.cap)
             loss.backward()
             self.g.seen_f.copy_(radius > 0)
             self.g.loss_slot.copy_(loss.detach().reshape(1))
-            self.g.overflow_slot.copy_(GaussianRasterizer.last_state(dev).header()[2:3])     # int32 0/1 -> float
-        with torch.cuda.stream(side):
-            self._graph = _capture(body)
-        torch.cuda.current_stream(dev).wait_stream(side)
-        return self._cap
-
-    def _replay(self, frame):
-        st = self._static
-        st["im"].copy_(frame["im"], non_blocking=True)
-        st["depth"].copy_(frame["depth"], non_blocking=True)
-        st["w2c"].copy_(frame["w2c"], non_blocking=True)
-        rel, cr = fused_pose_cached(self.params(), frame["id"])
-        st["pose"][0].copy_(rel, non_blocking=True)
-        st["pose"][1].copy_(cr, non_blocking=True)
-        self._graph.replay()
+            self.g.overflow_slot.copy_(step.overflow())     # int32 0/1 -> float
+        step.capture(body)
+        self._graph = step
+        return step.cap
 
     def check_capacity(self):
         """(num_rendered, overflowed) of the last graph replay; synchronises."""
-        from .rasterizer import GaussianRasterizer
         return GaussianRasterizer.last_counts(self.g.flat.device)
 
     def effective_steps(self):
@@ -822,7 +807,7 @@ class ShardedMapper:
             self._polls = []
             n_r, _ = self.check_capacity()
             self.overflow_events += 1
-            self.enable_graph(window, slack=self._slack, capacity=max(int(n_r * self._slack), int(self._cap * 1.5)) + 4096)
+            self.enable_graph(window, slack=self._slack, capacity=max(int(n_r * self._slack), int(self._graph.cap * 1.5)) + 4096)
         return hit
 
     def timing_breakdown(self, window, reps=10):
@@ -938,13 +923,45 @@ class ShardedMapper:
             self._dev_gen.manual_seed(12345)
         return self._dev_gen
 
+    def run_state(self):
+        """The mapper's part of a checkpoint's run state (slam._run_state), as numpy arrays: `timestep`, the schedule
+        generator, the device generator if it has one and the densification statistic if there is one."""
+        st = dict(timestep=self.timestep.detach().cpu().numpy(), mapper_gen=self.gen.get_state().numpy())
+        if self._dev_gen is not None:
+            st["mapper_dev_gen"] = self._dev_gen.get_state().numpy()
+        if self._dens is not None:
+            st["dens_accum"] = self._dens["accum"].detach().cpu().numpy()
+            st["dens_denom"] = self._dens["denom"].detach().cpu().numpy()
+        return st
+
+    def load_run_state(self, st):
+        """Inverse of run_state on a mapper built from the checkpoint's map; changes nothing if `timestep` does not
+        fit the map."""
+        import numpy as np
+        dev = self.g.flat.device
+        P = self.g.shapes["means3D"][0]
+        if st["timestep"].shape != (P,):
+            raise ValueError("the checkpoint's run state holds %d timesteps for a map of %d Gaussians"
+                             % (st["timestep"].shape[0], P))
+        self.timestep = torch.from_numpy(np.array(st["timestep"], dtype=np.float32)).to(dev)
+        self.gen.set_state(torch.from_numpy(np.array(st["mapper_gen"], dtype=np.uint8)))
+        if "mapper_dev_gen" in st:
+            self._device_generator().set_state(torch.from_numpy(np.array(st["mapper_dev_gen"], dtype=np.uint8)))
+        if "dens_accum" in st:
+            self._dens = dict(accum=torch.from_numpy(np.array(st["dens_accum"], dtype=np.float32)).to(dev),
+                              denom=torch.from_numpy(np.array(st["dens_denom"], dtype=np.float32)).to(dev))
+
     def step(self, window):
         """One sharded mapping step over `window` (list of keyframe dicts).  Returns the mean loss."""
         picks = self.schedule(len(window))
         graphed = self._graph is not None
         if graphed:
             self.poll_overflow(window)
-            self._replay(window[picks[self.rank]])
+            step, frame = self._graph, window[picks[self.rank]]
+            step.load(frame)
+            for static, v in zip(step.frame["pose"], fused_pose_cached(self.params(), frame["id"])):
+                static.copy_(v, non_blocking=True)
+            step.graph.replay()
         else:
             self.g.zero_grad()
             loss, radius = self.accumulate(window[picks[self.rank]])

@@ -81,7 +81,6 @@ def _settings_pack(rs, device):
 _SIZE_CACHE = {}
 _R_HINT = {}
 _LAST_ASYNC_STATE = {}      # device index -> state of the most recent sync-free forward on that device
-_LAST_SYNC_R = [0]          # num_rendered of the most recent synchronous forward
 
 
 def _sizes(P, W, H, sets):
@@ -189,7 +188,6 @@ def _forward_impl(means3D, colors_precomp, opacities, scales, rotations, cov3Ds_
     if state.binning is None:
         state.binning = _ws(16, device)
     state.num_rendered = R.value
-    _LAST_SYNC_R[0] = R.value
     _R_HINT[hint_key] = R.value
     if len(_R_HINT) > 256:
         _R_HINT.clear()
@@ -347,6 +345,18 @@ class GaussianRasterizer(nn.Module):
         device); synchronises.  On overflow the images of that forward are NaN."""
         st = GaussianRasterizer.last_state(device)
         return None if st is None else st.counts()
+
+    def num_rendered(self, means3D, opacities, scales, rotations):
+        """Tile instances a render of these Gaussians bins, from the forward's first stage alone (sb_forward_geometry:
+        projection and depth ordering, the count a synchronous forward renders with); synchronises."""
+        dev, P = means3D.device, means3D.shape[0]
+        pack = _settings_pack(self.raster_settings, dev)
+        geom = _ws(_lib.nbytes("sb_geometry_workspace_bytes", P), dev)
+        R = ctypes.c_int(0)
+        _lib.call("sb_forward_geometry", ctypes.byref(pack.c), P, _f32c(means3D, "means3D"), _f32c(opacities, "opacities"),
+                  _f32c(scales, "scales"), _f32c(rotations, "rotations"), None,
+                  torch.empty((P,), dtype=torch.int32, device=dev), geom, geom.numel(), ctypes.byref(R), device=dev)
+        return R.value
 
     def markVisible(self, positions):
         """Boolean mask ``view_z > 0.2`` per point (reference __init__.py:152-161)."""

@@ -74,48 +74,32 @@ def keyframes_from_checkpoint(frames, ckpt):
 
 def _run_state(mapper, counts):
     """The sidecar of a checkpoint (formats.save_checkpoint's `run_state`): what continues a run exactly and the
-    reference's params{t}.npz cannot carry -- the Gaussians' `timestep`, torch's CPU RNG and the CUDA RNG of the map's
-    device (keyframe selection and densification draw from the global generators), NumPy's global RNG
-    (keyframe_selection_overlap's permutation), the mapper's schedule generator and its device generator if it has
-    one, the densification statistic if there is one, and the Gaussian counts so far.  Numeric arrays only."""
+    reference's params{t}.npz cannot carry -- the mapper's own state (ShardedMapper.run_state: the Gaussians'
+    `timestep`, its schedule and device generators, the densification statistic), torch's CPU RNG and the CUDA RNG of
+    the map's device (keyframe selection and densification draw from the global generators), NumPy's global RNG
+    (keyframe_selection_overlap's permutation) and the Gaussian counts so far.  Numeric arrays only."""
     import numpy as np
     dev = mapper.g.flat.device
     _, keys, pos, has_gauss, cached = np.random.get_state()
-    st = dict(timestep=mapper.timestep.detach().cpu().numpy(), torch_rng=torch.get_rng_state().numpy(),
+    st = dict(mapper.run_state(), torch_rng=torch.get_rng_state().numpy(),
               numpy_rng_keys=np.asarray(keys, dtype=np.uint32), numpy_rng_pos=np.array(pos, dtype=np.int64),
               numpy_rng_has_gauss=np.array(has_gauss, dtype=np.int64),
-              numpy_rng_cached_gaussian=np.array(cached, dtype=np.float64),
-              mapper_gen=mapper.gen.get_state().numpy(), counts=np.array(counts, dtype=np.int64))
+              numpy_rng_cached_gaussian=np.array(cached, dtype=np.float64), counts=np.array(counts, dtype=np.int64))
     if dev.type == "cuda":
         st["cuda_rng"] = torch.cuda.get_rng_state(dev).numpy()
-    if mapper._dev_gen is not None:
-        st["mapper_dev_gen"] = mapper._dev_gen.get_state().numpy()
-    if mapper._dens is not None:
-        st["dens_accum"] = mapper._dens["accum"].detach().cpu().numpy()
-        st["dens_denom"] = mapper._dens["denom"].detach().cpu().numpy()
     return st
 
 
 def _restore_run_state(mapper, st):
     """Inverse of _run_state on a mapper built from the checkpoint's map; returns the Gaussian counts so far."""
     import numpy as np
+    mapper.load_run_state(st)
     dev = mapper.g.flat.device
-    P = mapper.g.shapes["means3D"][0]
-    if st["timestep"].shape != (P,):
-        raise ValueError("the checkpoint's run state holds %d timesteps for a map of %d Gaussians"
-                         % (st["timestep"].shape[0], P))
-    mapper.timestep = torch.from_numpy(np.array(st["timestep"], dtype=np.float32)).to(dev)
     torch.set_rng_state(torch.from_numpy(np.array(st["torch_rng"], dtype=np.uint8)))
     np.random.set_state(("MT19937", np.array(st["numpy_rng_keys"], dtype=np.uint32), int(st["numpy_rng_pos"]),
                          int(st["numpy_rng_has_gauss"]), float(st["numpy_rng_cached_gaussian"])))
-    mapper.gen.set_state(torch.from_numpy(np.array(st["mapper_gen"], dtype=np.uint8)))
     if dev.type == "cuda" and "cuda_rng" in st:
         torch.cuda.set_rng_state(torch.from_numpy(np.array(st["cuda_rng"], dtype=np.uint8)), dev)
-    if "mapper_dev_gen" in st:
-        mapper._device_generator().set_state(torch.from_numpy(np.array(st["mapper_dev_gen"], dtype=np.uint8)))
-    if "dens_accum" in st:
-        mapper._dens = dict(accum=torch.from_numpy(np.array(st["dens_accum"], dtype=np.float32)).to(dev),
-                            denom=torch.from_numpy(np.array(st["dens_denom"], dtype=np.float32)).to(dev))
     return [int(c) for c in st["counts"]]
 
 

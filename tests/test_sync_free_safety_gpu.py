@@ -23,6 +23,8 @@ def test_overflow_poisons_images_and_is_reported(cuda_device):
     c2, _, _ = small(**inp)
     n_r, overflow = small.last_counts(dev)
     assert overflow and n_r > 64 and (R is None or n_r == R)
+    # the capacity probe of the CUDA-graph paths: the forward's first stage alone counts the same instances
+    assert S.GaussianRasterizer(rs).num_rendered(inp["means3D"], inp["opacities"], inp["scales"], inp["rotations"]) == n_r
     assert torch.isnan(c2).all(), "a truncated render must be poisoned"
     big = S.GaussianRasterizer(rs, max_rendered=n_r + 10)
     c3, _, _ = big(**inp)
