@@ -342,6 +342,41 @@ SB_API int sb_lpips(const float* x, const float* y, int N, int H, int W, const f
 SB_API int sb_eval_frames_u8(const float* im, const float* depth_sil, const float* gt_im, const float* gt_depth, int H,
                              int W, const uint8_t* lut, uint8_t* out, void* stream);
 
+/* ---- headless viewer (R/viz_scripts/final_recon.py, online_recon.py; splatam_b200/viewer.py) ----------------------
+ * Frames are uint8 HWC RGB [H, W, 3] at H = h * s, W = w * s (s = view_scale >= 1), with a float32 depth buffer
+ * zbuf [H, W] (camera z, +inf where nothing is drawn).  Background: white at infinite depth.  Colours:
+ * round_half_even(clamp(x, 0, 1) * 255f), NaN -> 0.  No host synchronisation; every pass is enqueued on `stream`.
+ * w2c: row-major float32 4x4 on the device (rows 0..2 are read).  fx, fy, cx, cy: the intrinsics at output size.
+ *
+ * sb_viewer_compose: color [3,h,w], depth [h,w], sil [h,w] (contiguous float) -> out, zbuf.  Output pixel (X, Y)
+ *   shows render pixel (X / s, Y / s); a pixel with depth <= 0 or NaN is background.  mode 0: the colour; mode 1:
+ *   lut[i] (256 x RGB uint8, matplotlib's jet), i = trunc(float32(d / vmax) * 256f) with 256 -> 255 and i = 0 when
+ *   vmax == 0, vmax = max of d over pixels with 0 < d < 15 (device, `vmax_bits`: one scratch uint), d >= 15 white;
+ *   mode 2: round_half_even(clamp(1 - sil, 0, 1) * 255f) in all three channels.  Only the inputs the mode reads
+ *   need be non-NULL.
+ * sb_viewer_points: P centres means [P,3] with colors [P,3]; with `timestep` [P] (may be NULL) only those with
+ *   timestep <= t_max.  Camera z = ((r0 x + r1 y) + r2 z) + t per row, float32; points with !(near < z < far) or a
+ *   non-finite u = fx x / z + cx, v = fy y / z + cy are skipped.  Each covers the s x s square whose top-left pixel is
+ *   (floor(u + 0.5), floor(v + 0.5)); per pixel the key (float bits of z) << 32 | index is kept by atomicMin (nearest
+ *   first, ties to the lower index).  keys: [H*W] uint64 scratch.  Writes every pixel of out and zbuf.
+ * sb_viewer_lines: S segments [S,6] (two world points each) with colors [S,3] uint8, drawn over out.  Endpoints are
+ *   clipped to z >= near (segments wholly at z <= near are dropped) and projected; a DDA along the major screen axis
+ *   visits each pixel centre c + 0.5 within the span, a = (c + 0.5 - p0) / (p1 - p0), minor = floor(q0 + a dq), depth
+ *   1 / ((1 - a) / z0 + a / z1).  A pixel is drawn when that depth is below zbuf; overlaps resolve by the (depth bits,
+ *   segment index) atomicMin in keys ([H*W] uint64 scratch).  zbuf is read, not written.
+ * SB_ERR_BAD_ARG for null pointers the call reads, non-positive sizes, view_scale < 1, near < 0 (points), near <= 0
+ * (lines) or far <= near. */
+SB_API int sb_viewer_compose(const float* color, const float* depth, const float* sil, int h, int w, int mode,
+                             int view_scale, const uint8_t* lut, unsigned int* vmax_bits, uint8_t* out, float* zbuf,
+                             void* stream);
+SB_API int sb_viewer_points(int P, const float* means, const float* colors, const float* timestep, float t_max,
+                            const float* w2c, float fx, float fy, float cx, float cy, int width, int height,
+                            int view_scale, float near, float far, unsigned long long* keys, uint8_t* out, float* zbuf,
+                            void* stream);
+SB_API int sb_viewer_lines(int S, const float* segments, const uint8_t* colors, const float* w2c, float fx, float fy,
+                           float cx, float cy, int width, int height, float near, const float* zbuf,
+                           unsigned long long* keys, uint8_t* out, void* stream);
+
 /* ---- frame ingest (the dataset readers, splatam_b200/datasets.py; R/datasets/gradslam_datasets/basedataset.py) ---
  * One launch: rgb uint8 [color_height, color_width, 3] (HWC) and depth uint16 [depth_height, depth_width] (device)
  * -> color_out float32 [3, height, width] = float32(bilinear_f64(rgb)) / 255 and depth_out float32 [1, height, width]

@@ -38,7 +38,7 @@ class SplatamB200Error(RuntimeError):
     pass
 
 
-_vp, _sz, _i = ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int
+_vp, _sz, _i, _f = ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_float
 _SIGNATURES = {
     # name: (restype, argtypes)  -- must list every symbol include/splatam_b200.h declares
     "sb_abi_version": (_i, []),
@@ -93,6 +93,9 @@ _SIGNATURES = {
     "sb_lpips_workspace_bytes": (_i, [_i, _i, _i, ctypes.POINTER(_sz)]),
     "sb_lpips": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, _vp, _vp, _vp]),
     "sb_eval_frames_u8": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "sb_viewer_compose": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "sb_viewer_points": (_i, [_i, _vp, _vp, _vp, _f, _vp, _f, _f, _f, _f, _i, _i, _i, _f, _f, _vp, _vp, _vp, _vp]),
+    "sb_viewer_lines": (_i, [_i, _vp, _vp, _vp, _f, _f, _f, _f, _i, _i, _f, _vp, _vp, _vp, _vp]),
     "sb_ingest_rgbd": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, ctypes.c_double, _vp, _vp, _vp]),
     "sb_profile_begin": (_i, []),
     "sb_profile_end": (_i, [ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_int)]),

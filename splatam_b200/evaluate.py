@@ -201,51 +201,46 @@ def eval_frames_u8(im, depth_sil, gt_im, gt_depth, lut=None, out=None):
     return out
 
 
-class _FrameWriter:
-    """Saves the four images of each evaluated frame under out_dir/{FRAME_DIRS} without holding up the evaluation:
-    sb_eval_frames_u8 writes one device staging buffer, an async copy moves it to a free pinned host slot, and a writer
-    thread waits for that copy's event, encodes the four PNGs with Pillow and frees the slot.  The next frame's kernel
-    may reuse the staging buffer at once, since it runs after the copy on the same stream.  `put` blocks only when every
-    host slot is busy.  `close` waits for every file and re-raises the first writer error; no thread outlives it.
-    File names: <render_prefix>_{i:04d}.png for the renders and gt_{i:04d}.png for the ground truth, with
-    i = t + index_offset for frame t."""
+def save_png(px, path):
+    """Pillow PNG of one uint8 HWC RGB image at PNG_COMPRESS_LEVEL."""
+    from PIL import Image
+    Image.fromarray(px).save(path, compress_level=PNG_COMPRESS_LEVEL)
 
-    def __init__(self, out_dir, render_prefix, index_offset, H, W, device, threads=None):
+
+class HostWriter:
+    """Moves uint8 images made on the GPU to files without holding up the stream that makes them: `put` lets the
+    caller write one device staging buffer, an async copy moves it to a free pinned host slot, and a writer thread
+    waits for that copy's event, runs the caller's `write(px)` on the slot's numpy array and frees the slot.  The next
+    `put` may reuse the staging buffer at once, since its kernels run after the copy on the same stream.  `put` blocks
+    only when every one of the threads + 2 host slots is busy.  With threads=1 the writes run in `put` order.  `close`
+    waits for every write and re-raises the first writer error; no thread outlives it."""
+
+    def __init__(self, shape, device, threads=None, name="frame-writer"):
         threads = FRAME_WRITER_THREADS if threads is None else threads
-        self.dirs = [os.path.join(out_dir, d) for d in FRAME_DIRS]
-        for d in self.dirs:
-            os.makedirs(d, exist_ok=True)
-        self.prefixes = (render_prefix, render_prefix, "gt", "gt")
-        self.offset, self.H, self.W, self.device = index_offset, H, W, device
-        self.lut = jet_lut(device)
-        self.staging = torch.empty(4, H, W, 3, dtype=torch.uint8, device=device)
+        self.device = device
+        self.staging = torch.empty(shape, dtype=torch.uint8, device=device)
         n = threads + 2
-        self.host = [torch.empty(4, H, W, 3, dtype=torch.uint8).pin_memory() for _ in range(n)]
+        self.host = [torch.empty(shape, dtype=torch.uint8).pin_memory() for _ in range(n)]
         self.events = [torch.cuda.Event() for _ in range(n)]
         self.free = queue.SimpleQueue()
         for s in range(n):
             self.free.put(s)
-        self.pool = ThreadPoolExecutor(threads, thread_name_prefix="eval-frames")
+        self.pool = ThreadPoolExecutor(threads, thread_name_prefix=name)
         self.jobs = []
 
-    def put(self, t, im, depth_sil, gt_im, gt_depth):
-        """Enqueues frame t's four images on the current stream (im, depth_sil, gt_im, gt_depth: contiguous float32)."""
+    def put(self, fill, write):
+        """fill(staging) enqueues the kernels that write the staging buffer on the current stream; write(px) then runs
+        on a writer thread with the copied pixels (a numpy view of the host slot, valid during the call)."""
         s = self.free.get()
-        _lib.call("sb_eval_frames_u8", im, depth_sil, gt_im, gt_depth, self.H, self.W, self.lut, self.staging,
-                  device=self.device)
+        fill(self.staging)
         self.host[s].copy_(self.staging, non_blocking=True)
         self.events[s].record()
-        i = t + self.offset
-        paths = [os.path.join(d, "%s_%04d.png" % (p, i)) for d, p in zip(self.dirs, self.prefixes)]
-        self.jobs.append(self.pool.submit(self._write, s, paths))
+        self.jobs.append(self.pool.submit(self._write, s, write))
 
-    def _write(self, s, paths):
-        from PIL import Image
+    def _write(self, s, write):
         try:
             self.events[s].synchronize()
-            px = self.host[s].numpy()
-            for k, path in enumerate(paths):
-                Image.fromarray(px[k]).save(path, compress_level=PNG_COMPRESS_LEVEL)
+            write(self.host[s].numpy())
         finally:
             self.free.put(s)
 
@@ -253,6 +248,33 @@ class _FrameWriter:
         self.pool.shutdown(wait=True)
         for job in self.jobs:
             job.result()
+
+
+class _FrameWriter:
+    """Saves the four images of each evaluated frame under out_dir/{FRAME_DIRS} through a HostWriter: sb_eval_frames_u8
+    fills the staging buffer and a writer thread encodes the four PNGs with Pillow.  `close` waits for every file and
+    re-raises the first writer error.  File names: <render_prefix>_{i:04d}.png for the renders and gt_{i:04d}.png for
+    the ground truth, with i = t + index_offset for frame t."""
+
+    def __init__(self, out_dir, render_prefix, index_offset, H, W, device, threads=None):
+        self.dirs = [os.path.join(out_dir, d) for d in FRAME_DIRS]
+        for d in self.dirs:
+            os.makedirs(d, exist_ok=True)
+        self.prefixes = (render_prefix, render_prefix, "gt", "gt")
+        self.offset, self.H, self.W, self.device = index_offset, H, W, device
+        self.lut = jet_lut(device)
+        self.writer = HostWriter((4, H, W, 3), device, threads, name="eval-frames")
+
+    def put(self, t, im, depth_sil, gt_im, gt_depth):
+        """Enqueues frame t's four images on the current stream (im, depth_sil, gt_im, gt_depth: contiguous float32)."""
+        fill = lambda staging: _lib.call("sb_eval_frames_u8", im, depth_sil, gt_im, gt_depth, self.H, self.W,
+                                         self.lut, staging, device=self.device)
+        i = t + self.offset
+        paths = [os.path.join(d, "%s_%04d.png" % (p, i)) for d, p in zip(self.dirs, self.prefixes)]
+        self.writer.put(fill, lambda px: [save_png(px[k], path) for k, path in enumerate(paths)])
+
+    def close(self):
+        self.writer.close()
 
 
 def _check_save_frames(name, save_frames, out_dir):
