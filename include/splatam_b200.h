@@ -387,6 +387,21 @@ SB_API int sb_ingest_rgbd(const uint8_t* rgb, int color_height, int color_width,
                           int depth_height, int depth_width, int height, int width, double png_depth_scale,
                           float* color_out, float* depth_out, void* stream);
 
+/* ---- live capture packets (splatam_b200/capture.py; R/scripts/iphone_demo.py, nerfcapture2dataset.py) -----------
+ * sb_ingest_capture: one packet's rgb uint8 [color_height, color_width, 3] and float32 depth in metres
+ * [depth_height, depth_width] (device) -> color_out float32 [3, height, width] = cv2.resize(uint8, INTER_LINEAR) / 255
+ * (cv2's fixed-point uint8 path; its 2x2 INTER_AREA at an exact 2x downscale; a copy at equal size) and depth_out
+ * float32 [1, height, width] = cv2.resize(float32, INTER_NEAREST), every value passed through bit for bit.
+ * sb_capture_depth_u16: out uint16 [height, width] = cv2.resize(uint16(depth * 65535 / depth_scale), INTER_NEAREST),
+ * float32 arithmetic, the cast as numpy's on x86-64 (truncation to int32, low 16 bits; NaN, +-inf and values past
+ * int32 give 0).  Both return SB_ERR_BAD_ARG, before any launch, for null pointers, non-positive sizes, sizes whose
+ * element count passes INT_MAX, and (sb_capture_depth_u16) a depth scale that is not finite and positive. */
+SB_API int sb_ingest_capture(const uint8_t* rgb, int color_height, int color_width, const float* depth,
+                             int depth_height, int depth_width, int height, int width, float* color_out,
+                             float* depth_out, void* stream);
+SB_API int sb_capture_depth_u16(const float* depth, int depth_height, int depth_width, float depth_scale, int height,
+                                int width, uint16_t* out, void* stream);
+
 /* ---- per-stage device timing (measurement only; bench.py's roofline pass) -------------------
  * Between sb_profile_begin() and sb_profile_end() every stage launch of this process is bracketed
  * by CUDA events on its stream.  sb_profile_end synchronises, writes the summed milliseconds and call

@@ -16,7 +16,8 @@ upload and the kernel run on a side stream that the consumer's stream waits on. 
 Dataset configs have the reference's YAML shape (``camera_params``: image_height / image_width, fx / fy / cx / cy,
 png_depth_scale; crop_edge and distortion are accepted and unused, as in the reference); `default_config` holds the
 values of R/configs/data/{replica,TUM/*,scannet,replica_v2}.yaml.  ScanNet++ has no YAML: its camera is read from the
-sequence's dslr/nerfstudio/transforms_undistorted.json.
+sequence's dslr/nerfstudio/transforms_undistorted.json.  Neither has a NeRFCapture capture (an iPhone recording,
+written by capture.CaptureWriter or the reference's nerfcapture2dataset.py): its camera is transforms.json's.
 
 ScanNet++ and ReplicaV2 also have a held-out test split (``split="test"``) for novel-view evaluation: its frames
 follow the first train frame, which becomes frame 0, so every test pose is relative to it.  CUDA only for the
@@ -37,7 +38,7 @@ import torch
 from . import _lib
 from .rasterizer import GaussianRasterizationSettings
 
-DATASETS = ("replica", "tum", "scannet", "scannetpp", "replicav2")
+DATASETS = ("replica", "tum", "scannet", "scannetpp", "replicav2", "nerfcapture")
 SPLITS = ("train", "test")
 _SPLIT_DATASETS = ("scannetpp", "replicav2")         # the datasets that have a held-out test split
 
@@ -64,9 +65,9 @@ def default_config(dataset, sequence=""):
     comes with each sequence (`scannetpp_config`)."""
     if dataset not in DATASETS:
         raise ValueError("unknown dataset %r (expected one of %s)" % (dataset, ", ".join(DATASETS)))
-    if dataset == "scannetpp":
-        raise ValueError("scannetpp has no shipped data config: its camera is read from each sequence "
-                         "(scannetpp_config)")
+    if dataset in ("scannetpp", "nerfcapture"):
+        raise ValueError("%s has no shipped data config: its camera is read from each sequence (%s_config)"
+                         % (dataset, dataset))
     key = dataset
     if dataset == "tum":
         m = re.search(r"freiburg([123])", sequence)
@@ -232,6 +233,45 @@ def _replicav2_files(root, split):
     return colors, depths, poses
 
 
+NERFCAPTURE_DEPTH_SCALE = 10.0          # metres at uint16 65535: R/configs/iphone/*.py's depth_scale
+NERFCAPTURE_PNG_DEPTH_SCALE = 6553.5    # what NeRFCaptureDataset divides by, right for that depth_scale only
+_OPENGL_TO_OPENCV = ((1, 0, 0, 0), (0, -1, 0, 0), (0, 0, -1, 0), (0, 0, 0, 1))
+
+
+def nerfcapture_config(root):
+    """The config of the NeRFCapture capture at `root`, as NeRFCaptureDataset builds it: the camera of
+    transforms.json's top-level fl_x, fl_y, cx, cy, w, h (per-frame intrinsics are ignored) and depth PNGs at
+    png_depth_scale 6553.5.  A capture whose integer_depth_scale is not 10 / 65535 was written with another depth
+    scale; it is read as the reference reads it, with a warning that its depth is then off by that ratio."""
+    meta = _read_json(os.path.join(root, "transforms.json"))
+    ids = meta.get("integer_depth_scale")
+    if ids is not None and ids != NERFCAPTURE_DEPTH_SCALE / 65535.0:
+        warnings.warn("%s: integer_depth_scale is %r, not 10/65535; its depth is read at png_depth_scale %g as the "
+                      "reference reads it, so metric depth is off by a factor of %g"
+                      % (root, ids, NERFCAPTURE_PNG_DEPTH_SCALE, ids * 65535.0 / NERFCAPTURE_DEPTH_SCALE))
+    return dict(dataset_name="nerfcapture", camera_params=_camera_params(
+        meta["h"], meta["w"], meta["fl_x"], meta["fl_y"], meta["cx"], meta["cy"], NERFCAPTURE_PNG_DEPTH_SCALE))
+
+
+def _nerfcapture_files(root):
+    """R/datasets/gradslam_datasets/nerfcapture.py: rgb/ in natural order, each rgb/<name> looked up by file_path in
+    transforms.json's frames; the depth path is the name with every 'rgb' replaced by 'depth'; poses are
+    P @ c2w @ P^T with P = diag(1, -1, -1, 1) (ARKit's OpenGL camera axes -> OpenCV's), in float32."""
+    meta = _read_json(os.path.join(root, "transforms.json"))
+    index = {fr["file_path"]: i for i, fr in enumerate(meta["frames"])}
+    P = torch.tensor(_OPENGL_TO_OPENCV).float()
+    colors, depths, poses = [], [], []
+    for name in natsorted(os.listdir(os.path.join(root, "rgb"))):
+        name = "rgb/" + name
+        if name not in index:
+            raise ValueError("%s: image %r has no entry in transforms.json's frames" % (root, name))
+        c2w = torch.from_numpy(np.array(meta["frames"][index[name]]["transform_matrix"])).float()
+        colors.append(os.path.join(root, name))
+        depths.append(os.path.join(root, name.replace("rgb", "depth")))
+        poses.append(P @ c2w @ P.T)
+    return colors, depths, poses
+
+
 _FILES = {"replica": _replica_files, "tum": _tum_files, "scannet": _scannet_files}
 
 
@@ -284,7 +324,8 @@ class SequenceFiles:
         if not os.path.isdir(self.root):
             raise FileNotFoundError("%s: no such sequence directory" % self.root)
         if config is None:
-            config = scannetpp_config(self.root) if dataset == "scannetpp" else default_config(dataset, sequence)
+            config = (scannetpp_config(self.root) if dataset == "scannetpp" else
+                      nerfcapture_config(self.root) if dataset == "nerfcapture" else default_config(dataset, sequence))
         cam = config["camera_params"]
         if start < 0:
             raise ValueError("start must be >= 0, got %d" % start)
@@ -301,6 +342,8 @@ class SequenceFiles:
             colors, depths, poses = _scannetpp_files(self.root, split, ignore_bad)
         elif dataset == "replicav2":
             colors, depths, poses = _replicav2_files(self.root, split)
+        elif dataset == "nerfcapture":
+            colors, depths, poses = _nerfcapture_files(self.root)
         else:
             colors, depths, poses = _FILES[dataset](self.root)
         if len(colors) != len(depths):

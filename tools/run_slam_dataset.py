@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""SplaTAM on a recorded sequence: reads Replica, TUM-RGBD, ScanNet, ScanNet++ or ReplicaV2 from disk
+"""SplaTAM on a recorded sequence: reads Replica, TUM-RGBD, ScanNet, ScanNet++, ReplicaV2 or a NeRFCapture iPhone
+capture (rgb/, depth/, transforms.json; --dataset nerfcapture, evaluated against its ARKit poses) from disk
 (splatam_b200.datasets), runs the SLAM loop (splatam_b200.slam.run_slam) from the back-projection of frame 0 with the
 shipped hyper-parameters of R/configs/{replica,tum,scannet,scannetpp,replica_v2}/splatam.py, then the final evaluation
 (splatam_b200.evaluate) against the dataset's ground-truth poses.  ScanNet++ and ReplicaV2 run on their train split;
@@ -60,6 +61,11 @@ HYPER = {
                       depth_loss_thres=20000),
     "replicav2": dict(height=680, width=1200, tracking_iters=40, mapping_iters=60, keyframe_every=5, map_every=1,
                       window=24, scene_radius_depth_ratio=3, eval_every=5),
+    # R/configs/iphone/splatam.py: half the phone's 1920x1440, new Gaussians from the quarter-size frame;
+    # keyframe_every depends on the frame count (nerfcapture_keyframe_every)
+    "nerfcapture": dict(height=720, width=960, densify_height=360, densify_width=480, tracking_iters=60,
+                        mapping_iters=60, keyframe_every=None, map_every=1, window=32, scene_radius_depth_ratio=3,
+                        eval_every=1, tracking_lrs=(0.001, 0.004), depth_loss_thres=20000),
 }
 # R/configs/replica/splatam_s.py: SplaTAM-S, the fast variant; new Gaussians come from the frame read at the
 # densification size (340x600) while tracking and mapping use 680x1200
@@ -73,6 +79,14 @@ HYPER_S = {
 # (follow-up: the shipped TUM and ScanNet configs have their own tracking rates)
 _TRACKING_DEFAULTS = dict(tracking_lrs=(0.0004, 0.002), depth_loss_thres=None)
 SIL_THRES = 0.5          # mapping: add_new_gaussians' silhouette threshold
+
+
+def nerfcapture_keyframe_every(frames):
+    """R/configs/iphone/*.py: frames // 5 below 25 frames, else 5; fewer than 5 frames would make it 0 (the reference
+    then divides by zero), so they are rejected."""
+    if frames < 5:
+        raise ValueError("a NeRFCapture run needs at least 5 frames, got %d" % frames)
+    return frames // 5 if frames < 25 else 5
 
 
 class _Capped:
@@ -144,6 +158,11 @@ def main():
                                 densify_height=h.get("densify_height"), densify_width=h.get("densify_width"))
     frames = _Capped(seq, a.frames)
     T = len(frames)
+    if a.dataset == "nerfcapture":
+        try:
+            h["keyframe_every"] = nerfcapture_keyframe_every(T)
+        except ValueError as e:
+            ap.error(str(e))
     K = seq.intrinsics.cpu()
     from splatam_b200 import formats
     t_resume = time.perf_counter()
