@@ -234,7 +234,8 @@ SB_API int sb_image_loss_backward(const float* x, const float* y, int C, int H, 
  * R/utils/slam_helpers.py:124-139,196-304).  scale_dim = 1 (isotropic log_scales [P,1]) or 3.
  * rel_w2c, w2c0: row-major 4x4; cam_rot: the normalised camera quaternion (w,x,y,z).
  * sb_prepare_backward: gradients of the six outputs (any may be NULL = zero) -> gradients of the raw
- * parameters; if want_pose, g_pose16 receives d/d rel_w2c[0:3,0:4] (12) then d/d cam_rot (4). */
+ * parameters; if want_pose, g_pose16 (16 device doubles, zeroed here) receives d/d rel_w2c[0:3,0:4] (12) then
+ * d/d cam_rot (4), accumulated in double. */
 SB_API int sb_prepare_forward(int P, int scale_dim, const float* means3D, const float* unnorm_rotations,
                               const float* logit_opacities, const float* log_scales, const float* rel_w2c,
                               const float* cam_rot, const float* w2c0, float* means_cam, float* rotations,
@@ -245,7 +246,7 @@ SB_API int sb_prepare_backward(int P, int scale_dim, int want_pose, const float*
                                const float* scales3, const float* g_means_cam, const float* g_rotations,
                                const float* g_opacities, const float* g_scales3, const float* g_depth_sil_colors,
                                float* g_means3D, float* g_unnorm_rotations, float* g_logit_opacities,
-                               float* g_log_scales, float* g_pose16, void* stream);
+                               float* g_log_scales, double* g_pose16, void* stream);
 
 /* Masked L1 terms of SplaTAM's get_loss (R/scripts/splatam.py:254-288): mask = (gt_depth > 0) & !isnan(depth)
  * & !isnan(depth_sq - depth^2) [& silhouette > sil_thres when use_sil]; depth_sil is the [3,H,W] depth /

@@ -7,8 +7,9 @@
 //           frame's rel_w2c  ->  the five operator inputs (camera-frame means, normalised rotations,
 //           sigmoid opacities, exp scales tiled x3) and the depth/silhouette colours [z, 1, z^2].
 // backward: gradients of those six tensors -> gradients of the raw parameters, plus the 3x4 gradient
-//           of rel_w2c and the gradient of the (normalised) camera quaternion, block-reduced and added
-//           with 16 atomics per CTA (camera-pose gradients for tracking).
+//           of rel_w2c and the gradient of the (normalised) camera quaternion, block-reduced in double and
+//           added with 16 double atomics per CTA (camera-pose gradients for tracking: at SplaTAM's map sizes
+//           these are sums of ~1M products that cancel most of each other once tracking has converged).
 #include "common.cuh"
 
 namespace sb {
@@ -21,15 +22,19 @@ __device__ __forceinline__ Quat qmul(const Quat& a, const Quat& b) {   // Hamilt
     return {a.w * b.w - a.x * b.x - a.y * b.y - a.z * b.z, a.w * b.x + a.x * b.w + a.y * b.z - a.z * b.y,
             a.w * b.y - a.x * b.z + a.y * b.w + a.z * b.x, a.w * b.z + a.x * b.y - a.y * b.x + a.z * b.w};
 }
-__device__ __forceinline__ Quat qnormalize(const Quat& q, float* inv_norm) {   // F.normalize: x / max(|x|, 1e-12)
-    const float n = fmaxf(sqrtf(q.w * q.w + q.x * q.x + q.y * q.y + q.z * q.z), 1e-12f);
-    *inv_norm = 1.f / n;
-    return {q.w * *inv_norm, q.x * *inv_norm, q.y * *inv_norm, q.z * *inv_norm};
+// F.normalize: x / max(|x|, 1e-12).  The returned inverse norm is negative when the clamp is active (|x| < 1e-12):
+// the divisor is then the constant 1e-12 and the backward must not project out the radial component.
+__device__ __forceinline__ Quat qnormalize(const Quat& q, float* inv_norm) {
+    const float r = sqrtf(q.w * q.w + q.x * q.x + q.y * q.y + q.z * q.z);
+    const float inv = 1.f / fmaxf(r, 1e-12f);
+    *inv_norm = r < 1e-12f ? -inv : inv;
+    return {q.w * inv, q.x * inv, q.y * inv, q.z * inv};
 }
-// backward of y = x/|x| : g_x = (g_y - y (y.g_y)) / |x|
+// backward of y = x/|x| : g_x = (g_y - y (y.g_y)) / |x| ; of the clamped branch y = x/1e-12 : g_x = g_y / 1e-12
 __device__ __forceinline__ Quat qnormalize_bwd(const Quat& y, float inv_norm, const Quat& g) {
-    const float d = y.w * g.w + y.x * g.x + y.y * g.y + y.z * g.z;
-    return {(g.w - y.w * d) * inv_norm, (g.x - y.x * d) * inv_norm, (g.y - y.y * d) * inv_norm, (g.z - y.z * d) * inv_norm};
+    const float d = inv_norm < 0.f ? 0.f : y.w * g.w + y.x * g.x + y.y * g.y + y.z * g.z;
+    const float inv = fabsf(inv_norm);
+    return {(g.w - y.w * d) * inv, (g.x - y.x * d) * inv, (g.y - y.y * d) * inv, (g.z - y.z * d) * inv};
 }
 
 __global__ void __launch_bounds__(256)
@@ -76,8 +81,8 @@ prepare_backward_kernel(int P, int scale_dim, int want_pose, const float* __rest
                         const float* __restrict__ g_opac, const float* __restrict__ g_scales3,
                         const float* __restrict__ g_dcols,
                         float* __restrict__ g_means, float* __restrict__ g_unnorm, float* __restrict__ g_logit,
-                        float* __restrict__ g_log_scales, float* __restrict__ g_pose /* [16]: 12 rel + 4 cam_rot */) {
-    __shared__ float red[16][8];
+                        float* __restrict__ g_log_scales, double* __restrict__ g_pose /* [16]: 12 rel + 4 cam_rot */) {
+    __shared__ double red[16][8];
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     float pose[16];
 #pragma unroll
@@ -132,18 +137,18 @@ prepare_backward_kernel(int P, int scale_dim, int want_pose, const float* __rest
         g_unnorm[i4] = gu.w; g_unnorm[i4 + 1] = gu.x; g_unnorm[i4 + 2] = gu.y; g_unnorm[i4 + 3] = gu.z;
     }
     if (!want_pose) return;
-    // CTA reduction of the 16 pose sums: warp shuffle, then 8 warp partials in shared memory
+    // CTA reduction of the 16 pose sums in double: warp shuffle, then 8 warp partials in shared memory
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
     for (int k = 0; k < 16; ++k) {
-        float v = pose[k];
+        double v = pose[k];
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
         if (lane == 0) red[k][warp] = v;
     }
     __syncthreads();
     if (threadIdx.x < 16) {
-        float v = 0.f;
+        double v = 0.0;
 #pragma unroll
         for (int w = 0; w < 8; ++w) v += red[threadIdx.x][w];
         atomicAdd(g_pose + threadIdx.x, v);
@@ -180,14 +185,14 @@ SB_API int sb_prepare_backward(int P, int scale_dim, int want_pose, const float*
                                const float* scales3, const float* g_means_cam, const float* g_rotations,
                                const float* g_opacities, const float* g_scales3, const float* g_depth_sil_colors,
                                float* g_means3D, float* g_unnorm_rotations, float* g_logit_opacities,
-                               float* g_log_scales, float* g_pose16, void* stream) {
+                               float* g_log_scales, double* g_pose16, void* stream) {
     if (P < 0 || (scale_dim != 1 && scale_dim != 3)) return SB_ERR_BAD_ARG;
     if (P == 0) return SB_OK;
     if (!means3D || !unnorm_rotations || !rel_w2c || !cam_rot || !w2c0 || !means_cam || !opacities || !scales3 ||
         !g_means3D || !g_unnorm_rotations || !g_logit_opacities || !g_log_scales || (want_pose && !g_pose16))
         return SB_ERR_BAD_ARG;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (want_pose) SB_CUDA_CHECK(cudaMemsetAsync(g_pose16, 0, 16 * sizeof(float), st));
+    if (want_pose) SB_CUDA_CHECK(cudaMemsetAsync(g_pose16, 0, 16 * sizeof(double), st));
     prepare_backward_kernel<<<(P + 255) / 256, 256, 0, st>>>(
         P, scale_dim, want_pose, means3D, unnorm_rotations, rel_w2c, cam_rot, w2c0, means_cam, opacities, scales3,
         g_means_cam, g_rotations, g_opacities, g_scales3, g_depth_sil_colors, g_means3D, g_unnorm_rotations,

@@ -336,12 +336,15 @@ SB_API int sb_masked_l1_backward(const float* depth_sil, const float* gt_depth, 
     return SB_OK;
 }
 
-// slam_external.gaussian(): float32 exp values divided by their float32 sum (R/utils/slam_external.py:54-57)
+// slam_external.gaussian(): float32 exp values divided by their float32 sum (R/utils/slam_external.py:54-57).  The
+// sum is accumulated in double and rounded once: that is the value torch's float32 sum gives for these 11 weights,
+// where a left-to-right float sum lands one ulp lower and would filter with a slightly different window.
 static GaussWin gauss_window() {
     GaussWin g;
     for (int i = 0; i < kWin; ++i) g.w[i] = (float)exp(-(double)((i - kWin / 2) * (i - kWin / 2)) / (2.0 * 1.5 * 1.5));
-    float fs = 0.f;
-    for (int i = 0; i < kWin; ++i) fs += g.w[i];
+    double ds = 0.0;
+    for (int i = 0; i < kWin; ++i) ds += g.w[i];
+    const float fs = (float)ds;
     for (int i = 0; i < kWin; ++i) g.w[i] = g.w[i] / fs;
     return g;
 }

@@ -37,7 +37,7 @@ class _Prepare(torch.autograd.Function):
         keep = [None if t is None else t.contiguous().float() for t in (g_means_cam, g_rot, g_opac, g_sc3, g_dcols)]
         e = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
         g_means, g_unnorm, g_logit, g_ls = e(P, 3), e(P, 4), e(*ctx.shapes[0]), e(*ctx.shapes[1])
-        pose = torch.zeros(16, dtype=torch.float32, device=dev) if ctx.want_pose else None
+        pose = torch.empty(16, dtype=torch.float64, device=dev) if ctx.want_pose else None     # zeroed by the call
         _lib.call("sb_prepare_backward", P, ctx.sd, int(ctx.want_pose), means3D, unnorm, rel, cr, w0, means_cam, opac,
                   sc3, *keep, g_means, g_unnorm, g_logit, g_ls, pose, device=dev)
         g_rel = g_cr = None
@@ -45,7 +45,7 @@ class _Prepare(torch.autograd.Function):
             g_rel = torch.zeros(4, 4, dtype=torch.float32, device=dev)
             g_rel[:3, :] = pose[:12].view(3, 4)
             g_rel = g_rel.reshape(ctx.shapes[2])
-            g_cr = pose[12:].reshape(ctx.shapes[3])
+            g_cr = pose[12:].float().reshape(ctx.shapes[3])
         return g_means, g_unnorm, g_logit, g_ls, g_rel, g_cr, None
 
 

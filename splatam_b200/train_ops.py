@@ -23,7 +23,9 @@ class FusedAdam:
         for n in seg_sizes:
             acc += int(n)
             ends.append(acc)
-        assert acc == flat.numel() and len(ends) == len(seg_lrs) <= 16
+        if acc != flat.numel() or len(ends) != len(seg_lrs) or len(ends) > 16:
+            raise ValueError("FusedAdam: %d segments of %d elements with %d learning rates for %d parameters "
+                             "(at most 16 segments)" % (len(ends), acc, len(seg_lrs), flat.numel()))
         self.n = len(ends)
         self.seg_end = (ctypes.c_uint32 * self.n)(*ends)
         self.seg_lr = (ctypes.c_double * self.n)(*[float(x) for x in seg_lrs])
