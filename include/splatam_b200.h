@@ -403,6 +403,38 @@ SB_API int sb_ingest_capture(const uint8_t* rgb, int color_height, int color_wid
 SB_API int sb_capture_depth_u16(const float* depth, int depth_height, int depth_width, float depth_scale, int height,
                                 int width, uint16_t* out, void* stream);
 
+/* ---- mesh extraction: TSDF fusion and marching cubes (splatam_b200/mesh.py, csrc/mesh.cu) ------------------------
+ * A volume of nz x ny x nx samples (x fastest) at p = origin + voxel * (i, j, k) holds tsdf, weight [nz,ny,nx] and
+ * color [nz,ny,nx,3], float32 on the device; a fresh volume is T = 1, W = 0, C = 0.  Float32, each operation rounded
+ * as written.  No host synchronisation except where the caller reads sb_mc_count's totals.
+ * sb_tsdf_integrate: fuses B frames in order -- depth [B,H,W] (0 = no measurement), rgb [B,3,H,W], w2c [B,4,4]
+ *   row-major (rows 0..2 read), one pinhole camera fx, fy, cx, cy -- into the volume; B frames give exactly what B
+ *   single-frame calls give.  Per voxel and frame: (x, y, z) = ((r0 px + r1 py) + r2 pz) + t; z > 0; pixel
+ *   (floor(((fx x) / z) + cx + 0.5), floor(((fy y) / z) + cy + 0.5)) inside the image; d = depth there, 0 < d <=
+ *   depth_max (+inf: no limit); sdf = d - z >= -trunc; f = min(1, sdf / trunc); W' = W + 1, T' = (T W + f) / W',
+ *   C' = (C W + rgb) / W'.
+ * sb_mc_count / sb_mc_emit: the indexed mesh of the volume.  A cell is live iff its 8 samples have W >= min_weight,
+ *   a sample is inside iff T < 0.  One vertex per crossed grid edge (id 3 * sample index + axis) that a live cell
+ *   touches, at p_a + t * voxel along the axis, t = T_a / (T_a - T_b), colour C_a + t * (C_b - C_a), in ascending
+ *   edge id; faces int32 [F,3] in ascending cell index, then the order of the generated table (csrc/mc_table.h),
+ *   facing increasing T.  sb_mc_count writes totals (device int[2]) = {V, F}, -1 for a count past INT_MAX / 3;
+ *   sb_mc_emit then fills vertices [V,3], colors [V,3] and faces [F,3] from the same workspace
+ *   (sb_mc_workspace_bytes) and the same tsdf / color.
+ * SB_ERR_BAD_ARG, before any launch, for null pointers the call reads, a non-positive size, a grid of 2^31 or more
+ * samples (marching cubes: 2^32 / 5 or more, so the packed
+ * per-sample counts cannot wrap in the scan), a non-finite origin, voxel, truncation, camera or min_weight, a
+ * non-positive voxel, truncation or depth_max; SB_ERR_WORKSPACE for a short workspace. */
+SB_API int sb_tsdf_integrate(int nx, int ny, int nz, float ox, float oy, float oz, float voxel, float trunc, int B,
+                             int height, int width, const float* depth, const float* rgb, const float* w2c, float fx,
+                             float fy, float cx, float cy, float depth_max, float* tsdf, float* weight, float* color,
+                             void* stream);
+SB_API int sb_mc_workspace_bytes(int nx, int ny, int nz, size_t* bytes);
+SB_API int sb_mc_count(int nx, int ny, int nz, const float* tsdf, const float* weight, float min_weight,
+                       void* workspace, size_t workspace_bytes, int* totals, void* stream);
+SB_API int sb_mc_emit(int nx, int ny, int nz, float ox, float oy, float oz, float voxel, const float* tsdf,
+                      const float* color, void* workspace, size_t workspace_bytes, float* vertices, float* colors,
+                      int* faces, void* stream);
+
 /* ---- per-stage device timing (measurement only; bench.py's roofline pass) -------------------
  * Between sb_profile_begin() and sb_profile_end() every stage launch of this process is bracketed
  * by CUDA events on its stream.  sb_profile_end synchronises, writes the summed milliseconds and call

@@ -99,6 +99,11 @@ _SIGNATURES = {
     "sb_ingest_rgbd": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, ctypes.c_double, _vp, _vp, _vp]),
     "sb_ingest_capture": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "sb_capture_depth_u16": (_i, [_vp, _i, _i, _f, _i, _i, _vp, _vp]),
+    "sb_tsdf_integrate": (_i, [_i, _i, _i, _f, _f, _f, _f, _f, _i, _i, _i, _vp, _vp, _vp, _f, _f, _f, _f, _f,
+                               _vp, _vp, _vp, _vp]),
+    "sb_mc_workspace_bytes": (_i, [_i, _i, _i, ctypes.POINTER(_sz)]),
+    "sb_mc_count": (_i, [_i, _i, _i, _vp, _vp, _f, _vp, _sz, _vp, _vp]),
+    "sb_mc_emit": (_i, [_i, _i, _i, _f, _f, _f, _f, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
     "sb_profile_begin": (_i, []),
     "sb_profile_end": (_i, [ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_int)]),
     "sb_stage_name": (ctypes.c_char_p, [_i]),

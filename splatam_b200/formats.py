@@ -10,6 +10,8 @@ and the 3DGS-viewer PLY export, byte-compatible with what the reference writes.
 * ``save_ply`` / ``load_ply`` / ``export_ply``               R/scripts/export_ply.py:20-77 (binary little-endian PLY,
   one `vertex` element of 17 float32 properties; the reference writes it through the `plyfile` package, which is
   not a dependency here: the header and the packed records are produced directly)
+* ``save_mesh_ply`` / ``load_mesh_ply``                      a coloured triangle mesh (splatam_b200/mesh.py) as a
+  binary little-endian PLY that MeshLab and Blender open
 """
 import os
 
@@ -199,3 +201,67 @@ def export_ply(params_path, ply_path=None):
     p = dict(np.load(params_path, allow_pickle=True))
     ply_path = ply_path or os.path.join(os.path.dirname(params_path), "splat.ply")
     return save_ply(ply_path, p["means3D"], p["log_scales"], p["unnorm_rotations"], p["rgb_colors"], p["logit_opacities"])
+
+
+MESH_VERTEX_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("red", "u1"), ("green", "u1"),
+                              ("blue", "u1")])
+MESH_FACE_DTYPE = np.dtype([("n", "u1"), ("v", "<i4", (3,))])
+
+
+def _mesh_ply_header(nv, nf):
+    lines = ["ply", "format binary_little_endian 1.0", f"element vertex {nv}", "property float x", "property float y",
+             "property float z", "property uchar red", "property uchar green", "property uchar blue",
+             f"element face {nf}", "property list uchar int vertex_indices", "end_header", ""]
+    return "\n".join(lines).encode("ascii")
+
+
+def _host(a):
+    return a.detach().cpu().numpy() if hasattr(a, "detach") else np.asarray(a)
+
+
+def save_mesh_ply(path, vertices, colors, faces):
+    """Writes vertices [V,3] (float32), colors [V,3] in [0, 1] and faces [F,3] (vertex indices) as a binary
+    little-endian PLY: `element vertex V` with float x, y, z and uchar red, green, blue, `element face F` with
+    `property list uchar int vertex_indices`.  Colours become rint(clip(c, 0, 1) * 255), NaN -> 0.  Accepts numpy
+    arrays or tensors on any device.  Returns the path."""
+    v = np.asarray(_host(vertices), np.float32).reshape(-1, 3)
+    c = np.nan_to_num(np.asarray(_host(colors), np.float64).reshape(-1, 3), nan=0.0)
+    f = np.asarray(_host(faces)).reshape(-1, 3)
+    if c.shape[0] != v.shape[0]:
+        raise ValueError("%d colours for %d vertices" % (c.shape[0], v.shape[0]))
+    if f.size and (f.min() < 0 or f.max() >= v.shape[0]):
+        raise ValueError("face indices must lie in [0, %d)" % v.shape[0])
+    vert = np.empty(v.shape[0], MESH_VERTEX_DTYPE)
+    vert["x"], vert["y"], vert["z"] = v[:, 0], v[:, 1], v[:, 2]
+    u8 = np.rint(np.clip(c, 0.0, 1.0) * 255).astype(np.uint8)
+    vert["red"], vert["green"], vert["blue"] = u8[:, 0], u8[:, 1], u8[:, 2]
+    face = np.empty(f.shape[0], MESH_FACE_DTYPE)
+    face["n"] = 3
+    face["v"] = f.astype(np.int32)
+    with open(path, "wb") as out:
+        out.write(_mesh_ply_header(v.shape[0], f.shape[0]))
+        out.write(vert.tobytes())
+        out.write(face.tobytes())
+    return path
+
+
+def load_mesh_ply(path):
+    """Inverse of save_mesh_ply: (vertices [V,3] float32, colors [V,3] uint8, faces [F,3] int32).  Reads only the
+    layout save_mesh_ply writes (triangles, the properties in its order)."""
+    with open(path, "rb") as f:
+        blob = f.read()
+    end = blob.index(b"end_header\n") + len(b"end_header\n")
+    header = blob[:end].decode("ascii").split("\n")
+    if header[0] != "ply" or header[1] != "format binary_little_endian 1.0":
+        raise ValueError("%s is not a binary little-endian PLY" % path)
+    nv = int([h for h in header if h.startswith("element vertex")][0].split()[-1])
+    nf = int([h for h in header if h.startswith("element face")][0].split()[-1])
+    if blob[:end] != _mesh_ply_header(nv, nf):
+        raise ValueError("%s does not have save_mesh_ply's layout" % path)
+    vert = np.frombuffer(blob, MESH_VERTEX_DTYPE, count=nv, offset=end)
+    face = np.frombuffer(blob, MESH_FACE_DTYPE, count=nf, offset=end + nv * MESH_VERTEX_DTYPE.itemsize)
+    if nf and not np.all(face["n"] == 3):
+        raise ValueError("%s has faces that are not triangles" % path)
+    verts = np.stack([vert["x"], vert["y"], vert["z"]], 1).astype(np.float32)
+    cols = np.stack([vert["red"], vert["green"], vert["blue"]], 1)
+    return verts, cols, np.ascontiguousarray(face["v"]).astype(np.int32)

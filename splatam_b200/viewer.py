@@ -202,22 +202,8 @@ def load_record(path, device, viz=None, camera=None):
     settings early; each view takes its own config.  A missing key raises ValueError naming it, as does a
     cam_unnorm_rots / cam_trans pair whose camera counts differ.  Without `timestep` only the final view renders."""
     _as_cfg(viz)
-    raw = dict(np.load(path, allow_pickle=True))
-    raw.update(camera or {})
-    missing = [k for k in _GAUSS_KEYS + ("cam_unnorm_rots", "cam_trans") + _CAMERA_KEYS if k not in raw]
-    if missing:
-        hint = " (a checkpoint holds no camera: pass camera=dict(intrinsics=, w2c=, org_width=, org_height=))" \
-            if set(missing) <= set(_CAMERA_KEYS) else ""
-        raise ValueError("%s lacks %s%s" % (path, ", ".join(missing), hint))
+    raw = read_record(path, camera)
     rots, trans = np.asarray(raw["cam_unnorm_rots"]), np.asarray(raw["cam_trans"])
-    if rots.ndim != 3 or rots.shape[:2] != (1, 4) or trans.ndim != 3 or trans.shape[:2] != (1, 3) or \
-            rots.shape[-1] != trans.shape[-1] or rots.shape[-1] < 1:
-        raise ValueError("camera count mismatch: cam_unnorm_rots %s and cam_trans %s must be [1,4,T] and [1,3,T] with "
-                         "one T >= 1" % (rots.shape, trans.shape))
-    P = np.asarray(raw["means3D"]).shape[0]
-    for k in _GAUSS_KEYS + (("timestep",) if "timestep" in raw else ()):
-        if np.asarray(raw[k]).shape[0] != P:
-            raise ValueError("%s has %d rows for %d Gaussians" % (k, np.asarray(raw[k]).shape[0], P))
     dev = torch.device(device)
     t = lambda k: torch.from_numpy(np.ascontiguousarray(np.asarray(raw[k], np.float32))).to(dev)
     log_scales = t("log_scales")
@@ -235,6 +221,28 @@ def load_record(path, device, viz=None, camera=None):
         opacities=torch.sigmoid(t("logit_opacities")), scales=torch.exp(log_scales),
         timestep=None if ts is None else torch.from_numpy(ts).to(dev), timestep_host=ts, monotone=monotone,
         counts=counts)
+
+
+def read_record(path, camera=None):
+    """The arrays of a run record on the host, checked as load_record checks them: dict of the file's entries with
+    `camera` (dict(intrinsics=, w2c=, org_width=, org_height=), any subset) applied over them."""
+    raw = dict(np.load(path, allow_pickle=True))
+    raw.update(camera or {})
+    missing = [k for k in _GAUSS_KEYS + ("cam_unnorm_rots", "cam_trans") + _CAMERA_KEYS if k not in raw]
+    if missing:
+        hint = " (a checkpoint holds no camera: pass camera=dict(intrinsics=, w2c=, org_width=, org_height=))" \
+            if set(missing) <= set(_CAMERA_KEYS) else ""
+        raise ValueError("%s lacks %s%s" % (path, ", ".join(missing), hint))
+    rots, trans = np.asarray(raw["cam_unnorm_rots"]), np.asarray(raw["cam_trans"])
+    if rots.ndim != 3 or rots.shape[:2] != (1, 4) or trans.ndim != 3 or trans.shape[:2] != (1, 3) or \
+            rots.shape[-1] != trans.shape[-1] or rots.shape[-1] < 1:
+        raise ValueError("camera count mismatch: cam_unnorm_rots %s and cam_trans %s must be [1,4,T] and [1,3,T] with "
+                         "one T >= 1" % (rots.shape, trans.shape))
+    P = np.asarray(raw["means3D"]).shape[0]
+    for k in _GAUSS_KEYS + (("timestep",) if "timestep" in raw else ()):
+        if np.asarray(raw[k]).shape[0] != P:
+            raise ValueError("%s has %d rows for %d Gaussians" % (k, np.asarray(raw[k]).shape[0], P))
+    return raw
 
 
 def select_mask(record, t):
