@@ -7,6 +7,8 @@ and the 3DGS-viewer PLY export, byte-compatible with what the reference writes.
   `keyframe_time_indices{t}.npy`, plus a `run_state{t}.npz` sidecar that only this project reads)
 * ``save_run_record``                                        R/scripts/splatam.py:973-986 (the final `params.npz` with
   the reference's 14 keys)
+* ``read_record`` / ``check_camera_columns`` / ``record_tensors``   the one checked reader of a run record (this
+  project's or the reference's `params.npz`, the 13-key offline record, a checkpoint's `params{t}.npz`)
 * ``save_ply`` / ``load_ply`` / ``export_ply``               R/scripts/export_ply.py:20-77 (binary little-endian PLY,
   one `vertex` element of 17 float32 properties; the reference writes it through the `plyfile` package, which is
   not a dependency here: the header and the packed records are produced directly)
@@ -22,6 +24,8 @@ CHECKPOINT_KEYS = GAUSSIAN_KEYS + ("cam_unnorm_rots", "cam_trans")
 # the keys save_params writes at the end of the reference's run, in its order (splatam.py:973-983)
 RECORD_KEYS = CHECKPOINT_KEYS + ("timestep", "intrinsics", "w2c", "org_width", "org_height", "gt_w2c_all_frames",
                                  "keyframe_time_indices")
+# the record keys the reference's loaders leave out of the Gaussian parameters; a checkpoint holds none of them
+CAMERA_KEYS = ("intrinsics", "w2c", "org_width", "org_height")
 
 C0 = 0.28209479177387814            # SH band-0 constant (export_ply.py:9)
 
@@ -58,14 +62,49 @@ def load_params(path, device=None):
     raw = dict(np.load(path, allow_pickle=True))
     if device is None:
         return raw
+    floats = [k for k, v in raw.items() if isinstance(v, np.ndarray) and v.dtype.kind == "f"]
+    return dict(raw, **record_tensors(raw, floats, device))
+
+
+def record_tensors(rec, keys, device):
+    """{k: rec[k] as a contiguous float32 tensor on `device`} for each of `keys`."""
     import torch
-    out = {}
-    for k, v in raw.items():
-        if isinstance(v, np.ndarray) and v.dtype.kind == "f":
-            out[k] = torch.from_numpy(np.ascontiguousarray(v)).to(device).float()
-        else:
-            out[k] = v
-    return out
+    return {k: torch.from_numpy(np.ascontiguousarray(rec[k], dtype=np.float32)).to(device) for k in keys}
+
+
+def read_record(path, need, camera=None):
+    """The entries of a run record on the host, as dict(np.load(path, allow_pickle=True)) gives them, with `camera`
+    (dict(intrinsics=, w2c=, org_width=, org_height=), any subset) applied over them.  ValueError when a key of `need`
+    is missing; when `need` holds cam_unnorm_rots and cam_trans, unless they are [1,4,T] and [1,3,T] with one T >= 1;
+    and when a Gaussian tensor or `timestep` has another row count than means3D."""
+    with np.load(path, allow_pickle=True) as z:
+        rec = dict(z)
+    rec.update(camera or {})
+    missing = [k for k in need if k not in rec]
+    if missing:
+        hint = " (a checkpoint holds no camera: pass camera=dict(intrinsics=, w2c=, org_width=, org_height=))" \
+            if set(missing) <= set(CAMERA_KEYS) else ""
+        raise ValueError("%s lacks %s%s" % (path, ", ".join(missing), hint))
+    if {"cam_unnorm_rots", "cam_trans"} <= set(need):
+        rots, trans = np.shape(rec["cam_unnorm_rots"]), np.shape(rec["cam_trans"])
+        if len(rots) != 3 or rots[:2] != (1, 4) or len(trans) != 3 or trans[:2] != (1, 3) or rots[-1] != trans[-1] \
+                or rots[-1] < 1:
+            raise ValueError("camera count mismatch: cam_unnorm_rots %s and cam_trans %s must be [1,4,T] and [1,3,T] "
+                             "with one T >= 1" % (rots, trans))
+    if "means3D" in rec:
+        P = np.shape(rec["means3D"])[0]
+        for k in GAUSSIAN_KEYS + ("timestep",):
+            if k in rec and np.shape(rec[k])[0] != P:
+                raise ValueError("%s has %d rows for %d Gaussians" % (k, np.shape(rec[k])[0], P))
+    return rec
+
+
+def check_camera_columns(path, rec, indices):
+    """ValueError naming the first of the frame `indices` outside [0, T), T the camera count of the record `rec`."""
+    T = np.shape(rec["cam_unnorm_rots"])[-1]
+    bad = [k for k in indices if not 0 <= k < T]
+    if bad:
+        raise ValueError("%s has %d camera columns; frame index %d has none" % (path, T, bad[0]))
 
 
 def _ckpt_paths(directory, time_idx):
@@ -96,7 +135,6 @@ def load_checkpoint(directory, time_idx, device):
     cam_trans (float32 tensors on `device`), keyframe_time_indices (list of int), state = the `run_state{t}.npz`
     sidecar as a dict of numpy arrays, or None when there is none, e.g. for a checkpoint the reference wrote).  A
     missing `params{t}.npz` or `keyframe_time_indices{t}.npy` raises FileNotFoundError naming the path."""
-    import torch
     p_path, k_path, s_path = _ckpt_paths(directory, time_idx)
     for path in (p_path, k_path):
         if not os.path.isfile(path):
@@ -105,14 +143,13 @@ def load_checkpoint(directory, time_idx, device):
         missing = [k for k in CHECKPOINT_KEYS if k not in z.files]
         if missing:
             raise ValueError("%s lacks %s" % (p_path, ", ".join(missing)))
-        raw = {k: z[k] for k in CHECKPOINT_KEYS}
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(device).float()
+        t = record_tensors(z, CHECKPOINT_KEYS, device)
     state = None
     if os.path.isfile(s_path):
         with np.load(s_path) as z:
             state = {k: z[k] for k in z.files}
-    return dict(time_idx=int(time_idx), gauss={k: t(raw[k]) for k in GAUSSIAN_KEYS},
-                cam_unnorm_rots=t(raw["cam_unnorm_rots"]), cam_trans=t(raw["cam_trans"]),
+    return dict(time_idx=int(time_idx), gauss={k: t[k] for k in GAUSSIAN_KEYS},
+                cam_unnorm_rots=t["cam_unnorm_rots"], cam_trans=t["cam_trans"],
                 keyframe_time_indices=[int(i) for i in np.load(k_path).reshape(-1).tolist()], state=state)
 
 

@@ -11,8 +11,6 @@ import torch
 
 from . import _lib
 
-GAUSSIAN_KEYS = ("means3D", "rgb_colors", "unnorm_rotations", "logit_opacities", "log_scales")
-
 
 def prune_mask(logit_opacities, log_scales, opacity_threshold, big_threshold=None):
     """bool[P] keep mask: not (sigmoid(logit) < opacity_threshold or exp(log_scales).max(1) > big_threshold)."""

@@ -19,9 +19,8 @@ import math
 import torch
 import torch.nn.functional as F
 
+from .formats import GAUSSIAN_KEYS
 from .rasterizer import GaussianRasterizer
-
-GAUSSIAN_KEYS = ("means3D", "rgb_colors", "unnorm_rotations", "logit_opacities", "log_scales")
 
 
 def build_rotation(q):

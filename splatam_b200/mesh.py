@@ -12,9 +12,9 @@ import torch
 
 from . import _lib
 from . import datasets as D
+from . import formats
 from . import mapping as M
 from . import mc_table
-from . import viewer as V
 
 MAX_VOXELS = 500_000_000
 # marching cubes packs each sample's triangle count (<= MAX_TRIANGLES) and vertex count (<= 3) into the two 32-bit
@@ -155,7 +155,7 @@ class _Timer:
 
 class RecordFusion:
     """The fusion of one run record (mesh_record's loop), set up once: the record, read and checked as
-    viewer.load_record reads it (viewer.read_record), its Gaussians and cameras on `device`, the poses of the frames
+    viewer.load_record reads it (formats.read_record), its Gaussians and cameras on `device`, the poses of the frames
     t = 0, every, 2 every, ... and the batch buffers.  ``fuse(vol)`` renders or reads those frames and integrates them
     into `vol`, with no host synchronisation.  `source`, when given, must hold exactly one frame per camera of the
     record (frame t is fused at the record's pose t): ValueError otherwise."""
@@ -170,7 +170,7 @@ class RecordFusion:
         if dev.type == "cuda" and dev.index is None:
             dev = torch.device("cuda", torch.cuda.current_device())
         self.device, self.sil_thres, self.depth_max, self.source = dev, float(sil_thres), depth_max, source
-        raw = V.read_record(path, camera)
+        raw = formats.read_record(path, formats.CHECKPOINT_KEYS + formats.CAMERA_KEYS, camera)
         T = np.asarray(raw["cam_unnorm_rots"]).shape[-1]
         if source is not None and len(source) != T:
             raise ValueError("%s has %d cameras but the source has %d frames: frame t is fused at the record's pose "
@@ -182,9 +182,7 @@ class RecordFusion:
         first_w2c = np.array(raw["w2c"], np.float32).reshape(4, 4)
         self.ids = list(range(0, T, int(every)))
         with torch.cuda.device(dev), torch.no_grad():
-            t32 = lambda k: torch.from_numpy(np.ascontiguousarray(np.asarray(raw[k], np.float32))).to(dev)
-            self.params = {k: t32(k) for k in ("means3D", "rgb_colors", "unnorm_rotations", "logit_opacities",
-                                               "log_scales", "cam_unnorm_rots", "cam_trans")}
+            self.params = formats.record_tensors(raw, formats.CHECKPOINT_KEYS, dev)
             self.cam = D.setup_camera(w, h, self.K, first_w2c, dev)
             self.w2c0 = torch.from_numpy(first_w2c).to(dev)
             self.poses = [M.pose_matrices(self.params, t) for t in self.ids]

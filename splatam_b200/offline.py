@@ -104,24 +104,18 @@ def from_record(path, frames, frame_indices, device, lrs=LRS, render=M.default_r
     frame_indices[t]: the original index of frames[t] in the SLAM run's sequence (start + stride * t for a reader with
     that start and stride, when the SLAM run read every frame from 0).  The reference indexes the camera tensor by loop
     position t instead, which is the same thing only at stride 1 (DESIGN.md, "Offline map optimisation").  A record
-    whose camera tensor has no column for some frame raises ValueError.
+    that formats.read_record rejects, or whose camera tensor has no column for some frame, raises ValueError.
     Returns (mapper, training frames = the frame dicts with "pose", scene_radius = max depth of frames[0] / 2, the
-    record as loaded by formats.load_params)."""
-    rec = formats.load_params(path)
-    missing = [k for k in formats.CHECKPOINT_KEYS + ("timestep",) if k not in rec]
-    if missing:
-        raise ValueError("%s lacks %s" % (path, ", ".join(missing)))
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).to(device)
-    rots, trans = t(rec["cam_unnorm_rots"]), t(rec["cam_trans"])
+    record as formats.read_record returns it)."""
+    rec = formats.read_record(path, formats.CHECKPOINT_KEYS + ("timestep",))
     idx = [int(i) for i in frame_indices]
     if len(idx) != len(frames):
         raise ValueError("%d frame indices for %d frames" % (len(idx), len(frames)))
-    n_cam = rots.shape[-1]
-    bad = [k for k in idx if not 0 <= k < n_cam]
-    if bad:
-        raise ValueError("%s has %d camera columns; frame index %d has none" % (path, n_cam, bad[0]))
+    formats.check_camera_columns(path, rec, idx)
+    t = formats.record_tensors(rec, formats.CHECKPOINT_KEYS, device)
+    rots, trans = t["cam_unnorm_rots"], t["cam_trans"]
     train = [dict(frames[i], pose=M.camera_w2c(rots[..., k], trans[..., k])) for i, k in enumerate(idx)]
-    mapper = M.ShardedMapper({k: t(rec[k]) for k in formats.GAUSSIAN_KEYS}, rots, trans, lrs=lrs, render=render,
+    mapper = M.ShardedMapper({k: t[k] for k in formats.GAUSSIAN_KEYS}, rots, trans, lrs=lrs, render=render,
                              fused=fused, timestep=rec["timestep"])
     return mapper, train, float(frames[0]["depth"].max()) / 2.0, rec
 

@@ -25,6 +25,7 @@ import torch.nn.functional as F
 
 from . import _lib
 from . import evaluate as EV
+from . import formats
 from . import map_ops
 from . import mapping as M
 from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer
@@ -41,10 +42,6 @@ JET_DATA = {"red": ((0.00, 0, 0), (0.35, 0, 0), (0.66, 1, 1), (0.89, 1, 1), (1.0
             "blue": ((0.00, 0.5, 0.5), (0.11, 1, 1), (0.34, 1, 1), (0.65, 0, 0), (1.00, 0, 0))}
 COOL_DATA = {"red": ((0., 0., 0.), (1.0, 1.0, 1.0)), "green": ((0., 1., 1.), (1.0, 0., 0.)),
              "blue": ((0., 1., 1.), (1.0, 1., 1.))}
-
-# the record keys the reference's loaders leave out of the Gaussian parameters
-_CAMERA_KEYS = ("intrinsics", "w2c", "org_width", "org_height")
-_GAUSS_KEYS = ("means3D", "rgb_colors", "unnorm_rotations", "logit_opacities", "log_scales")
 
 
 def segment_lut(data, N=256):
@@ -200,13 +197,14 @@ def load_record(path, device, viz=None, camera=None):
     checkpoint `params{t}.npz`; a checkpoint holds no camera, so pass ``camera=dict(intrinsics=, w2c=, org_width=,
     org_height=)`` (any of these also overrides the record's).  `viz` (a ViewerConfig or `viz` dict) only checks the
     settings early; each view takes its own config.  A missing key raises ValueError naming it, as does a
-    cam_unnorm_rots / cam_trans pair whose camera counts differ.  Without `timestep` only the final view renders."""
+    cam_unnorm_rots / cam_trans pair whose camera counts differ (formats.read_record).  Without `timestep` only the
+    final view renders."""
     _as_cfg(viz)
-    raw = read_record(path, camera)
+    raw = formats.read_record(path, formats.CHECKPOINT_KEYS + formats.CAMERA_KEYS, camera)
     rots, trans = np.asarray(raw["cam_unnorm_rots"]), np.asarray(raw["cam_trans"])
     dev = torch.device(device)
-    t = lambda k: torch.from_numpy(np.ascontiguousarray(np.asarray(raw[k], np.float32))).to(dev)
-    log_scales = t("log_scales")
+    g = formats.record_tensors(raw, formats.GAUSSIAN_KEYS, dev)
+    log_scales = g["log_scales"]
     if log_scales.shape[-1] == 1:
         log_scales = torch.tile(log_scales, (1, 3))
     ts = None if "timestep" not in raw else np.ascontiguousarray(np.asarray(raw["timestep"], np.float32).reshape(-1))
@@ -217,32 +215,10 @@ def load_record(path, device, viz=None, camera=None):
         path=path, device=dev, intrinsics=np.array(raw["intrinsics"], np.float32)[:3, :3],
         first_w2c=np.array(raw["w2c"], np.float32).reshape(4, 4), org_width=np.asarray(raw["org_width"]),
         org_height=np.asarray(raw["org_height"]), all_w2cs=trajectory_w2cs(rots, trans),
-        means3D=t("means3D"), colors=t("rgb_colors"), rotations=F.normalize(t("unnorm_rotations")),
-        opacities=torch.sigmoid(t("logit_opacities")), scales=torch.exp(log_scales),
+        means3D=g["means3D"], colors=g["rgb_colors"], rotations=F.normalize(g["unnorm_rotations"]),
+        opacities=torch.sigmoid(g["logit_opacities"]), scales=torch.exp(log_scales),
         timestep=None if ts is None else torch.from_numpy(ts).to(dev), timestep_host=ts, monotone=monotone,
         counts=counts)
-
-
-def read_record(path, camera=None):
-    """The arrays of a run record on the host, checked as load_record checks them: dict of the file's entries with
-    `camera` (dict(intrinsics=, w2c=, org_width=, org_height=), any subset) applied over them."""
-    raw = dict(np.load(path, allow_pickle=True))
-    raw.update(camera or {})
-    missing = [k for k in _GAUSS_KEYS + ("cam_unnorm_rots", "cam_trans") + _CAMERA_KEYS if k not in raw]
-    if missing:
-        hint = " (a checkpoint holds no camera: pass camera=dict(intrinsics=, w2c=, org_width=, org_height=))" \
-            if set(missing) <= set(_CAMERA_KEYS) else ""
-        raise ValueError("%s lacks %s%s" % (path, ", ".join(missing), hint))
-    rots, trans = np.asarray(raw["cam_unnorm_rots"]), np.asarray(raw["cam_trans"])
-    if rots.ndim != 3 or rots.shape[:2] != (1, 4) or trans.ndim != 3 or trans.shape[:2] != (1, 3) or \
-            rots.shape[-1] != trans.shape[-1] or rots.shape[-1] < 1:
-        raise ValueError("camera count mismatch: cam_unnorm_rots %s and cam_trans %s must be [1,4,T] and [1,3,T] with "
-                         "one T >= 1" % (rots.shape, trans.shape))
-    P = np.asarray(raw["means3D"]).shape[0]
-    for k in _GAUSS_KEYS + (("timestep",) if "timestep" in raw else ()):
-        if np.asarray(raw[k]).shape[0] != P:
-            raise ValueError("%s has %d rows for %d Gaussians" % (k, np.asarray(raw[k]).shape[0], P))
-    return raw
 
 
 def select_mask(record, t):

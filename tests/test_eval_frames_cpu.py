@@ -162,18 +162,22 @@ def test_eval_record_argument_errors(tool, tmp_path, capsys):
     assert a.out == os.path.join(str(tmp_path / "run"), "eval_nvs")
 
 
-def test_eval_record_names_the_first_frame_without_a_camera_column(tool, tmp_path):
+def test_eval_record_checks_its_record_with_the_formats_reader(tool, tmp_path):
+    """tools/eval_record.py reads the record with formats.read_record (the Gaussians, and the cameras on the train
+    split) and names the first evaluated frame without a camera column (formats.check_camera_columns)."""
     _replica_layout(str(tmp_path), 12)
     rec = _record(str(tmp_path / "run"), 9)
     base = ["--dataset", "replica", "--basedir", str(tmp_path), "--sequence", "room0", "--record", rec]
     # Replica evaluates every 5th frame: 0, 4, 9 of 12 frames; the record has columns 0 .. 8
     with pytest.raises(ValueError, match="has 9 camera columns; frame index 9 has none"):
         tool.main(base)
+    train = formats.read_record(rec, formats.CHECKPOINT_KEYS)
     with pytest.raises(ValueError, match="has 9 camera columns; frame index 9 has none"):
-        tool.load_record(rec, "train", 10, 5)
-    assert tool.load_record(rec, "train", 9, 5)["cam_trans"].shape[-1] == 9
-    assert tool.load_record(rec, "test", 100, 1)["means3D"].shape == (5, 3)
+        formats.check_camera_columns(rec, train, EV.select_frames(10, 5))
+    formats.check_camera_columns(rec, train, EV.select_frames(9, 5))
+    assert train["cam_trans"].shape[-1] == 9
+    assert formats.read_record(rec, formats.GAUSSIAN_KEYS)["means3D"].shape == (5, 3)
     partial = str(tmp_path / "partial.npz")
     np.savez(partial, **{k: v for k, v in np.load(rec).items() if k != "cam_trans"})
     with pytest.raises(ValueError, match="lacks cam_trans"):
-        tool.load_record(partial, "train", 1, 5)
+        tool.main(base[:-1] + [partial])

@@ -27,7 +27,6 @@ import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 
@@ -67,24 +66,6 @@ def parse_args(argv=None):
     return a
 
 
-def load_record(path, split, num_frames, eval_every):
-    """The record's arrays (formats.load_params).  Checks that it has the five Gaussian tensors and, for the train
-    split, a camera column for every frame evaluate.select_frames picks among `num_frames`: ValueError naming the first
-    frame index without one."""
-    from splatam_b200 import evaluate, formats
-    rec = formats.load_params(path)
-    need = formats.GAUSSIAN_KEYS + (("cam_unnorm_rots", "cam_trans") if split == "train" else ())
-    missing = [k for k in need if k not in rec]
-    if missing:
-        raise ValueError("%s lacks %s" % (path, ", ".join(missing)))
-    if split == "train":
-        n_cam = min(rec["cam_unnorm_rots"].shape[-1], rec["cam_trans"].shape[-1])
-        bad = [t for t in evaluate.select_frames(num_frames, eval_every) if t >= n_cam]
-        if bad:
-            raise ValueError("%s has %d camera columns; frame index %d has none" % (path, n_cam, bad[0]))
-    return rec
-
-
 def main(argv=None):
     a = parse_args(argv)
     from splatam_b200 import datasets, evaluate, formats
@@ -92,12 +73,14 @@ def main(argv=None):
     files = datasets.SequenceFiles(a.dataset, a.basedir, a.sequence, desired_height=h["height"],
                                    desired_width=h["width"], split=a.split)
     T = min(a.frames, len(files)) if a.frames else len(files)
-    rec = load_record(a.record, a.split, T, h["eval_every"])
+    # the train split renders every evaluated frame at the record's camera column for it
+    rec = formats.read_record(a.record, formats.CHECKPOINT_KEYS if a.split == "train" else formats.GAUSSIAN_KEYS)
+    if a.split == "train":
+        formats.check_camera_columns(a.record, rec, evaluate.select_frames(T, h["eval_every"]))
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
     net = None if a.lpips_alexnet is None else evaluate.LpipsAlex.load(a.lpips_alexnet, a.lpips_lin, dev)
-    t32 = lambda k: torch.from_numpy(np.ascontiguousarray(rec[k], dtype=np.float32)).to(dev)
-    gauss = {k: t32(k) for k in formats.GAUSSIAN_KEYS}
+    gauss = formats.record_tensors(rec, formats.GAUSSIAN_KEYS, dev)
     save = not a.no_frames
     with datasets.RGBDSequence(a.dataset, a.basedir, a.sequence, desired_height=h["height"], desired_width=h["width"],
                                device=dev, split=a.split) as seq:
@@ -105,7 +88,8 @@ def main(argv=None):
         torch.cuda.synchronize(dev)
         t0 = time.perf_counter()
         if a.split == "train":
-            params = dict(gauss, cam_unnorm_rots=t32("cam_unnorm_rots")[..., :T], cam_trans=t32("cam_trans")[..., :T])
+            cams = formats.record_tensors(rec, ("cam_unnorm_rots", "cam_trans"), dev)
+            params = dict(gauss, **{k: v[..., :T] for k, v in cams.items()})
             gt_w2c = [torch.linalg.inv(seq.files.poses[t].to(dev)) for t in range(T)]
             res = evaluate.evaluate(params, frames, seq.cam, RSD.SIL_THRES, h["mapping_iters"], True,
                                     eval_every=h["eval_every"], gt_w2c=gt_w2c, out_dir=a.out, lpips=net,

@@ -69,9 +69,9 @@ def open_input(a, record, device):
     """--source input: the run's frames as run_slam_dataset.py selects them -- datasets.RGBDSequence with the same
     config, start, end and stride, capped at --frames -- read at the record's image size.  Returns (sequence, frames);
     ValueError, with the sequence closed, when the selected frame count differs from the record's camera count."""
-    from splatam_b200 import datasets, viewer
+    from splatam_b200 import datasets, formats
     rsd = _run_slam_dataset()
-    raw = viewer.read_record(record)
+    raw = formats.read_record(record, formats.CHECKPOINT_KEYS + formats.CAMERA_KEYS)
     T = raw["cam_unnorm_rots"].shape[-1]
     height, width = int(raw["org_height"]), int(raw["org_width"])
     cfg = datasets.load_config(a.config) if a.config else None

@@ -18,7 +18,6 @@ import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 
@@ -45,14 +44,14 @@ def parse(argv=None):
 
 def main(argv=None):
     a = parse(argv)
-    from splatam_b200 import viewer as V
+    from splatam_b200 import formats, viewer as V
     cfg = V.ViewerConfig(render_mode=a.render_mode, show_sil=a.show_sil, visualize_cams=not a.no_cams,
                          offset_first_viz_cam=not a.no_offset, viz_w=a.viz_w, viz_h=a.viz_h, viz_near=a.viz_near,
                          viz_far=a.viz_far, view_scale=a.view_scale)
     camera = None
     if a.camera_from:
-        with np.load(a.camera_from) as z:
-            camera = {k: z[k] for k in ("intrinsics", "w2c", "org_width", "org_height")}
+        src = formats.read_record(a.camera_from, formats.CAMERA_KEYS)
+        camera = {k: src[k] for k in formats.CAMERA_KEYS}
     rec = V.load_record(a.record, torch.device(a.device), cfg, camera=camera)
     t0 = time.perf_counter()
     paths = V.render_record(rec, cfg, a.out, a.view, every=a.every, raw=a.raw)
