@@ -435,6 +435,31 @@ SB_API int sb_mc_emit(int nx, int ny, int nz, float ox, float oy, float oz, floa
                       const float* color, void* workspace, size_t workspace_bytes, float* vertices, float* colors,
                       int* faces, void* stream);
 
+/* ---- mesh evaluation: visibility culling and exact nearest neighbours (splatam_b200/mesh_eval.py,
+ * csrc/mesh_eval.cu) ---------------------------------------------------------------------------------------------
+ * Float32, each operation rounded as written.  No host synchronisation.
+ * sb_points_visible: points [N,3]; depth [B,H,W] and w2c [B,4,4] row-major (rows 0..2 read); mask uint8 [N] is read
+ *   once and set to 1 where some frame of the launch sees the point: sb_tsdf_integrate's projection -- (x, y, z) =
+ *   ((r0 px + r1 py) + r2 pz) + t; z > 0; pixel (floor(((fx x) / z) + cx + 0.5), floor(((fy y) / z) + cy + 0.5))
+ *   inside the image -- and the depth d there has d > 0 and z <= d + occlusion_eps.  A frame with a non-finite pose
+ *   marks nothing.  B frames give exactly what B single-frame calls give.
+ * sb_nn_grid_build: bins N >= 1 reference points [N,3] into the gx x gy x gz grid of cubic cells of edge `cell` from
+ *   origin o (cell (floor((p - o) / cell)) per axis, clamped into the grid), at most 2^28 cells, and keeps in the
+ *   workspace (sb_nn_grid_workspace_bytes) the points in cell order and the per-cell start offsets.
+ * sb_nn_query: d2 [M] float32 = min over the N reference points of (dx dx + dy dy) + dz dz, dx = qx - px, ...: equal
+ *   to the brute-force minimum bit for bit (NaN for a non-finite query).  The same grid arguments as the build.
+ * SB_ERR_BAD_ARG, before any launch, for null pointers the call reads, negative counts, an empty reference set, a
+ * non-positive image or grid size, more than 2^28 cells, a non-finite origin, cell, camera or occlusion_eps, a
+ * non-positive cell or a negative occlusion_eps; SB_ERR_WORKSPACE for a short workspace. */
+SB_API int sb_points_visible(int n, const float* points, int B, int height, int width, const float* depth,
+                             const float* w2c, float fx, float fy, float cx, float cy, float occlusion_eps,
+                             uint8_t* mask, void* stream);
+SB_API int sb_nn_grid_workspace_bytes(int n, int gx, int gy, int gz, size_t* bytes);
+SB_API int sb_nn_grid_build(int n, const float* points, float ox, float oy, float oz, float cell, int gx, int gy,
+                            int gz, void* workspace, size_t workspace_bytes, void* stream);
+SB_API int sb_nn_query(int m, const float* queries, int n, float ox, float oy, float oz, float cell, int gx, int gy,
+                       int gz, const void* workspace, size_t workspace_bytes, float* d2, void* stream);
+
 /* ---- per-stage device timing (measurement only; bench.py's roofline pass) -------------------
  * Between sb_profile_begin() and sb_profile_end() every stage launch of this process is bracketed
  * by CUDA events on its stream.  sb_profile_end synchronises, writes the summed milliseconds and call

@@ -273,6 +273,8 @@ def _nerfcapture_files(root):
 
 
 _FILES = {"replica": _replica_files, "tum": _tum_files, "scannet": _scannet_files}
+# readers whose poses are P c2w P^T: their map frame sees the native world through P as well (world_to_map)
+_AXIS_CHANGE_DATASETS = ("scannetpp", "nerfcapture")
 
 
 def relative_poses(poses):
@@ -357,9 +359,24 @@ class SequenceFiles:
         raw = torch.stack(poses[start:end:stride])
         self.poses = relative_poses(raw).float()
         self.intrinsics = scaled_intrinsics(cam, self.height, self.width)
+        self._raw_pose0 = raw[0].double().numpy()
+        self._world_axes = np.array(_OPENGL_TO_OPENCV if dataset in _AXIS_CHANGE_DATASETS else np.eye(4), np.float64)
 
     def __len__(self):
         return len(self.color_paths)
+
+    @property
+    def world_to_map(self):
+        """float64 [4,4] taking a point of the dataset's native world frame (that of its pose files and its
+        ground-truth mesh) into the SLAM map's frame, whose origin and axes are the first retained camera's:
+        inv(raw_pose_0) @ A.  raw_pose_0 is that camera's c2w as the reader builds it, before `relative_poses`; A is
+        the world-side axis change the reader applied, diag(1, -1, -1, 1) for ScanNet++ and NeRFCapture (whose poses
+        are P c2w P^T) and the identity otherwise.  Depends on `start`, not on `stride`.  ValueError when that pose is
+        not finite (ScanNet's invalid frames)."""
+        if not np.all(np.isfinite(self._raw_pose0)):
+            raise ValueError("%s: the first retained frame's pose is not finite, so it cannot define the map's frame; "
+                             "choose another --start" % self.root)
+        return np.linalg.inv(self._raw_pose0) @ self._world_axes
 
 
 # ---- decoding and the ingest kernel --------------------------------------------------------------------------------

@@ -13,7 +13,8 @@ and the 3DGS-viewer PLY export, byte-compatible with what the reference writes.
   one `vertex` element of 17 float32 properties; the reference writes it through the `plyfile` package, which is
   not a dependency here: the header and the packed records are produced directly)
 * ``save_mesh_ply`` / ``load_mesh_ply``                      a coloured triangle mesh (splatam_b200/mesh.py) as a
-  binary little-endian PLY that MeshLab and Blender open
+  binary little-endian PLY that MeshLab and Blender open; ``load_mesh_ply`` also reads the ground-truth meshes of the
+  datasets (ASCII or binary, extra properties, same-count polygons)
 """
 import os
 
@@ -282,23 +283,145 @@ def save_mesh_ply(path, vertices, colors, faces):
     return path
 
 
+_PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "i2", "int16": "i2",
+              "ushort": "u2", "uint16": "u2", "int": "i4", "int32": "i4", "uint": "u4", "uint32": "u4",
+              "float": "f4", "float32": "f4", "double": "f8", "float64": "f8"}
+
+
+def _parse_ply_header(path, blob):
+    """(format, [(element name, count, [(property, dtype) or (property, count dtype, index dtype)])], data offset)."""
+    end = blob.find(b"end_header")
+    nl = blob.find(b"\n", end)
+    if not blob.startswith(b"ply") or end < 0 or nl < 0:
+        raise ValueError("%s is not a PLY file" % path)
+    fmt, elements = None, []
+    for line in blob[:end].decode("ascii", "replace").splitlines()[1:]:
+        t = line.split()
+        if not t or t[0] in ("comment", "obj_info"):
+            continue
+        if t[0] == "format":
+            fmt = t[1] if len(t) > 1 else None
+        elif t[0] == "element" and len(t) == 3:
+            elements.append((t[1], int(t[2]), []))
+        elif t[0] == "property" and elements and len(t) == 3 and t[1] in _PLY_TYPES:
+            elements[-1][2].append((t[2], _PLY_TYPES[t[1]]))
+        elif (t[0] == "property" and elements and len(t) == 5 and t[1] == "list" and t[2] in _PLY_TYPES
+              and t[3] in _PLY_TYPES):
+            elements[-1][2].append((t[4], _PLY_TYPES[t[2]], _PLY_TYPES[t[3]]))
+        else:
+            raise ValueError("%s: unsupported PLY header line %r" % (path, line))
+    if fmt == "binary_big_endian":
+        raise ValueError("%s is a big-endian PLY, which is not supported" % path)
+    if fmt not in ("binary_little_endian", "ascii"):
+        raise ValueError("%s: unsupported PLY format %r" % (path, fmt))
+    return fmt, elements, nl + 1
+
+
+def _face_layout(path, props):
+    """(index of the vertex list among the face properties, count dtype, index dtype)."""
+    lists = [k for k, p in enumerate(props) if len(p) == 3]
+    if len(lists) != 1 or props[lists[0]][0] not in ("vertex_indices", "vertex_index"):
+        raise ValueError("%s: the face element needs one list property vertex_indices or vertex_index" % path)
+    k = lists[0]
+    if np.dtype(props[k][1]).kind not in "ui" or np.dtype(props[k][2]).kind not in "ui":
+        raise ValueError("%s: the face list must have integer counts and indices" % path)
+    return k, props[k][1], props[k][2]
+
+
+def _read_binary(path, blob, offset, elements):
+    """{element name: structured array}; faces are read with one dtype for the count of their first face."""
+    out = {}
+    for name, count, props in elements:
+        if any(len(p) == 3 for p in props):
+            if name != "face":
+                raise ValueError("%s: list properties are supported on the face element only" % path)
+            k, ct, it = _face_layout(path, props)
+            n = 0
+            if count:
+                head = np.dtype([(p[0], "<" + p[1]) for p in props[:k]])
+                n = int(np.frombuffer(blob, "<" + ct, count=1, offset=offset + head.itemsize)[0])
+            fields = [(p[0], "<" + p[1]) if len(p) == 2 else ("n", "<" + ct) for p in props]
+            fields[k] = ("n", "<" + ct)
+            fields.insert(k + 1, ("v", "<" + it, (n,)))
+            dt = np.dtype(fields)
+        else:
+            dt = np.dtype([(p[0], "<" + p[1]) for p in props])
+        if offset + count * dt.itemsize > len(blob):
+            raise ValueError("%s is truncated in its %s element%s" % (
+                path, name, " or mixes polygons of different vertex counts" if name == "face" else ""))
+        out[name] = np.frombuffer(blob, dt, count=count, offset=offset)
+        if name == "face" and count and not np.all(out[name]["n"] == n):
+            raise ValueError("%s mixes polygons of different vertex counts" % path)
+        offset += count * dt.itemsize
+    return out
+
+
+def _read_ascii(path, blob, offset, elements):
+    lines = blob[offset:].decode("ascii", "replace").split("\n")
+    out, row = {}, 0
+    for name, count, props in elements:
+        block = [ln.split() for ln in lines[row:row + count]]
+        row += count
+        if len(block) != count:
+            raise ValueError("%s is truncated in its %s element" % (path, name))
+        widths = {len(b) for b in block}
+        if len(widths) > 1:
+            raise ValueError("%s mixes polygons of different vertex counts" % path if name == "face" else
+                             "%s: rows of its %s element differ in length" % (path, name))
+        vals = np.array(block, dtype=np.float64).reshape(count, -1) if count else np.zeros((0, 0))
+        if any(len(p) == 3 for p in props):
+            if name != "face":
+                raise ValueError("%s: list properties are supported on the face element only" % path)
+            k, _, it = _face_layout(path, props)
+            n = int(vals[0, k]) if count else 0
+            if count and (vals.shape[1] != len(props) + n or not np.all(vals[:, k] == n)):
+                raise ValueError("%s mixes polygons of different vertex counts" % path)
+            out[name] = dict(n=np.full(count, n), v=vals[:, k + 1:k + 1 + n].astype(np.int64))
+        else:
+            if count and vals.shape[1] != len(props):
+                raise ValueError("%s: its %s rows do not have %d values" % (path, name, len(props)))
+            out[name] = {p[0]: vals[:, j].astype(p[1]) for j, p in enumerate(props)}
+    return out
+
+
 def load_mesh_ply(path):
-    """Inverse of save_mesh_ply: (vertices [V,3] float32, colors [V,3] uint8, faces [F,3] int32).  Reads only the
-    layout save_mesh_ply writes (triangles, the properties in its order)."""
+    """A triangle mesh from a PLY: (vertices [V,3] float32, colors [V,3] uint8, faces [F,3] int32).  Reads binary
+    little-endian and ASCII files with a `vertex` element holding x, y, z and any other scalar properties (skipped;
+    red, green, blue are the colours when present, clipped into uint8, zeros otherwise) and a `face` element whose
+    list property vertex_indices or vertex_index has an integer count and index type.  Every face must have the
+    same vertex count n >= 3; n-gons are fanned into n - 2 triangles (v0, vk, vk+1).  ValueError, naming the path,
+    for big-endian files, mixed polygon counts, indices outside [0, V) and non-finite vertices that a face uses.
+    Reads what save_mesh_ply writes exactly as written."""
     with open(path, "rb") as f:
         blob = f.read()
-    end = blob.index(b"end_header\n") + len(b"end_header\n")
-    header = blob[:end].decode("ascii").split("\n")
-    if header[0] != "ply" or header[1] != "format binary_little_endian 1.0":
-        raise ValueError("%s is not a binary little-endian PLY" % path)
-    nv = int([h for h in header if h.startswith("element vertex")][0].split()[-1])
-    nf = int([h for h in header if h.startswith("element face")][0].split()[-1])
-    if blob[:end] != _mesh_ply_header(nv, nf):
-        raise ValueError("%s does not have save_mesh_ply's layout" % path)
-    vert = np.frombuffer(blob, MESH_VERTEX_DTYPE, count=nv, offset=end)
-    face = np.frombuffer(blob, MESH_FACE_DTYPE, count=nf, offset=end + nv * MESH_VERTEX_DTYPE.itemsize)
-    if nf and not np.all(face["n"] == 3):
-        raise ValueError("%s has faces that are not triangles" % path)
-    verts = np.stack([vert["x"], vert["y"], vert["z"]], 1).astype(np.float32)
-    cols = np.stack([vert["red"], vert["green"], vert["blue"]], 1)
-    return verts, cols, np.ascontiguousarray(face["v"]).astype(np.int32)
+    fmt, elements, offset = _parse_ply_header(path, blob)
+    names = [e[0] for e in elements]
+    if "vertex" not in names:
+        raise ValueError("%s has no vertex element" % path)
+    data = (_read_binary if fmt == "binary_little_endian" else _read_ascii)(path, blob, offset, elements)
+    vert = data["vertex"]
+    vprops = [p[0] for p in elements[names.index("vertex")][2]]
+    if not {"x", "y", "z"} <= set(vprops):
+        raise ValueError("%s: the vertex element lacks x, y or z" % path)
+    verts = np.stack([np.asarray(vert[k]) for k in ("x", "y", "z")], 1).astype(np.float32)
+    if {"red", "green", "blue"} <= set(vprops):
+        cols = np.stack([np.clip(np.asarray(vert[k]), 0, 255) for k in ("red", "green", "blue")], 1).astype(np.uint8)
+    else:
+        cols = np.zeros((len(verts), 3), np.uint8)
+    if "face" not in data or len(data["face"]["n"]) == 0:
+        return verts, cols, np.zeros((0, 3), np.int32)
+    poly = np.asarray(data["face"]["v"]).astype(np.int64)
+    n = poly.shape[1]
+    if n < 3:
+        raise ValueError("%s has faces of %d vertices" % (path, n))
+    if poly.min() < 0 or poly.max() >= len(verts):
+        raise ValueError("%s has face indices outside [0, %d)" % (path, len(verts)))
+    used = np.zeros(len(verts), bool)
+    used[poly.reshape(-1)] = True
+    if not np.all(np.isfinite(verts[used])):
+        raise ValueError("%s has non-finite vertices that faces use" % path)
+    if n == 3:
+        return verts, cols, np.ascontiguousarray(poly).astype(np.int32)
+    k = np.arange(1, n - 1)
+    tris = np.stack([np.broadcast_to(poly[:, :1], (len(poly), n - 2)), poly[:, k], poly[:, k + 1]], -1)
+    return verts, cols, tris.reshape(-1, 3).astype(np.int32)
