@@ -460,6 +460,34 @@ SB_API int sb_nn_grid_build(int n, const float* points, float ox, float oy, floa
 SB_API int sb_nn_query(int m, const float* queries, int n, float ox, float oy, float oz, float cell, int gx, int gy,
                        int gz, const void* workspace, size_t workspace_bytes, float* d2, void* stream);
 
+/* ---- mesh depth rendering: a z-buffer triangle rasterizer (splatam_b200/mesh_eval.py, csrc/mesh_render.cu) -------
+ * sb_mesh_depth: depth [B,H,W] float32 and face_id [B,H,W] int32 of the mesh vertices [V,3], faces int32 [F,3] seen
+ *   by B cameras w2c [B,4,4] row-major (rows 0..2 read) with one pinhole fx, fy, cx, cy.  Float32, each operation
+ *   rounded as written.  Per view and face:
+ *   1. (x, y, z) = ((r0 px + r1 py) + r2 pz) + t per vertex (sb_tsdf_integrate's transform).
+ *   2. The face is dropped when an index lies outside [0, V) or any camera coordinate is non-finite.
+ *   3. Near clipping, z >= near inside: all three inside, the face as it is; none, dropped; otherwise the polygon of
+ *      3 or 4 vertices the edges (v0,v1), (v1,v2), (v2,v0) give in order (each inside vertex, then the crossing
+ *      point of a crossing edge), fanned from its first vertex.  A crossing edge with P inside and Q outside crosses
+ *      at s = (near - zP) / (zQ - zP), x = xP + s (xQ - xP), y likewise, z = near exactly.  Pieces keep the face index.
+ *   4. u = ((fx x) / z) + cx, v = ((fy y) / z) + cy; pixel (c, r) has its centre at (u, v) = (c, r).
+ *   5. The pixels tested are c in [ceil(min u), floor(max u)], r in [ceil(min v), floor(max v)], clamped to the image.
+ *   6. Edge function of P -> Q: e = ((u1 - u0)(r - v0)) - ((v1 - v0)(c - u0)) with (u0, v0), (u1, v1) the endpoints
+ *      in lexicographic (u, v) order, negated when that swapped them.  ea = e(b -> c), eb = e(c -> a), ec = e(a -> b).
+ *      Covered: all three >= 0 or all three <= 0, and s = (ea + eb) + ec != 0.  No back-face culling.
+ *   7. iz = (((ea / za) + (eb / zb)) + (ec / zc)) / s, z = 1 / iz, drawn when z is finite and > 0.
+ *   8. Z-buffer: atomicMin of the key (uint64(bits(z)) << 32) | face, so the nearest wins and, at equal depth, the
+ *      lower face index; the result does not depend on the order of the writes.  depth = z and face_id = face where
+ *      some face drew, 0 and -1 elsewhere.
+ *   B views give exactly what B single-view calls give.  No host synchronisation.
+ * SB_ERR_BAD_ARG, before any launch, for null pointers, V or F < 1, B, H or W < 1, B H W >= 2^31, B F >= 2^31 - 1,
+ * a non-finite camera, fx or fy <= 0 and near <= 0 or non-finite; SB_ERR_WORKSPACE for a workspace smaller than
+ * sb_mesh_depth_workspace_bytes gives. */
+SB_API int sb_mesh_depth_workspace_bytes(int f, int B, int height, int width, size_t* bytes);
+SB_API int sb_mesh_depth(int v, const float* vertices, int f, const int* faces, int B, int height, int width,
+                         const float* w2c, float fx, float fy, float cx, float cy, float near, void* workspace,
+                         size_t workspace_bytes, float* depth, int* face_id, void* stream);
+
 /* ---- per-stage device timing (measurement only; bench.py's roofline pass) -------------------
  * Between sb_profile_begin() and sb_profile_end() every stage launch of this process is bracketed
  * by CUDA events on its stream.  sb_profile_end synchronises, writes the summed milliseconds and call

@@ -10,6 +10,10 @@ Both meshes are sampled by area; the ground-truth samples are culled to what the
 (``visible_mask``, csrc/mesh_eval.cu: sb_points_visible); distances are exact nearest-neighbour distances between the
 two sample sets (``NearestGrid``: sb_nn_grid_build / sb_nn_query, bit-equal to a brute-force minimum).  Both meshes
 must already be in the map's frame: ``datasets.SequenceFiles.world_to_map`` moves a dataset's ground-truth mesh there.
+
+``depth_l1`` adds the rendered-depth column of the same table: both meshes are drawn from random viewpoints
+(``MeshDepth``: sb_mesh_depth, a z-buffer triangle rasterizer bit-equal to oracle/mesh_render_numpy.py) and their depth
+maps compared, which sees floaters in front of the surface and holes that the sample distances miss.
 CUDA only; no CPU fallback for the kernels."""
 import itertools
 
@@ -198,7 +202,7 @@ def _first_intrinsics(frames):
 
 
 def evaluate_mesh(pred, gt, frames=None, K=None, samples=200_000, threshold=0.05, occlusion_eps=0.03, seed=0,
-                  device="cuda", batch=8, cell=None):
+                  device="cuda", batch=8, cell=None, depth_views=0):
     """Scores the reconstruction `pred` against the ground truth `gt`, both (vertices [V,3], faces [F,3]) in the
     map's frame.  `samples` points are drawn on each mesh by area (``sample_surface``, one torch.Generator seeded
     with `seed`: the prediction first, then the ground truth).
@@ -211,14 +215,23 @@ def evaluate_mesh(pred, gt, frames=None, K=None, samples=200_000, threshold=0.05
     truth that is already culled.
 
     Returns a dict: accuracy, completion (metres), precision, recall (the completion ratio), fscore (``scores``),
-    pred_samples, gt_samples, gt_samples_kept, and the device times cull_ms, grid_ms and query_ms."""
+    pred_samples, gt_samples, gt_samples_kept, and the device times cull_ms, grid_ms and query_ms.
+
+    With depth_views > 0 it also scores rendered depth (``depth_l1`` with views=depth_views and the same frames, K,
+    seed and occlusion_eps; the view centres are drawn in the box of the kept ground-truth samples) and adds
+    depth_l1, depth_l1_surface (metres), hole_ratio, depth_views_used, depth_views_drawn and the device times
+    depth_render_ms and depth_cull_ms.  The frames' depth is then held on the device (``_FrameStack``)."""
     dev = _device(device)
     if dev.type != "cuda":
         raise _lib.SplatamB200Error("evaluate_mesh needs a CUDA device (there is no CPU fallback)")
     if not (np.isfinite(threshold) and threshold > 0):
         raise ValueError("threshold must be finite and positive, got %r" % (threshold,))
+    if int(depth_views) != depth_views or depth_views < 0:
+        raise ValueError("depth_views must be a non-negative integer, got %r" % (depth_views,))
     if frames is not None and K is None:
         K, frames = _first_intrinsics(frames)
+    if depth_views and frames is not None:
+        frames = _FrameStack(frames, dev)
     t_cull, t_grid, t_query = _Timer(), _Timer(), _Timer()
     with torch.cuda.device(dev):
         gen = torch.Generator(dev).manual_seed(int(seed))
@@ -226,7 +239,10 @@ def evaluate_mesh(pred, gt, frames=None, K=None, samples=200_000, threshold=0.05
         g_pts, _ = sample_surface(*gt, samples, gen, dev)
         if frames is not None:
             t_cull.start()
-            mask = visible_mask(g_pts, frames, K, occlusion_eps, batch)
+            if isinstance(frames, _FrameStack):
+                mask = frames.cull(g_pts, K, occlusion_eps)
+            else:
+                mask = visible_mask(g_pts, frames, K, occlusion_eps, batch)
             t_cull.stop()
             g_kept = g_pts[mask.bool()]
             if g_kept.shape[0] == 0:
@@ -250,4 +266,253 @@ def evaluate_mesh(pred, gt, frames=None, K=None, samples=200_000, threshold=0.05
         torch.cuda.synchronize(dev)
     out.update(pred_samples=int(p_pts.shape[0]), gt_samples=int(g_pts.shape[0]), gt_samples_kept=int(g_kept.shape[0]),
                cull_ms=t_cull.ms() if t_cull.pairs else 0.0, grid_ms=t_grid.ms(), query_ms=t_query.ms())
+    if depth_views:
+        d = depth_l1(pred, gt, frames, K, views=depth_views, seed=seed, occlusion_eps=occlusion_eps, gt_kept=g_kept,
+                     device=dev)
+        out.update(depth_l1=d["depth_l1"], depth_l1_surface=d["depth_l1_surface"], hole_ratio=d["hole_ratio"],
+                   depth_views_used=d["views_used"], depth_views_drawn=d["views_drawn"],
+                   depth_render_ms=d["render_ms"], depth_cull_ms=d["cull_ms"])
+    return out
+
+
+# ---- rendered depth ----------------------------------------------------------------------------------------------
+# The random-view protocol (the NICE-SLAM image and intrinsics; the views themselves are this project's own draw).
+DEPTH_VIEW_HW = (500, 500)
+DEPTH_VIEW_K = np.array([[300.0, 0.0, 249.5], [0.0, 300.0, 249.5], [0.0, 0.0, 1.0]])
+DEPTH_VIEW_NEAR = 0.01
+CULL_FRAMES_PER_LAUNCH = 32
+
+
+class MeshDepth:
+    """A triangle mesh (vertices [V,3], faces [F,3]) uploaded once to `device` and checked once on the host: face
+    indices in [0, V), the vertices that faces use finite in float32, V < 2^31 and F < 2^31 - 1 (ValueError
+    otherwise).  ``render(w2c, K, height, width, near)`` draws it from the cameras w2c [B,4,4] (a CUDA tensor; K a
+    3x3 on the host) with sb_mesh_depth and returns (depth [B,H,W] float32, 0 where nothing drew, face_id [B,H,W]
+    int32, -1 there).  It issues no host synchronisation; the workspace is kept between calls.  CUDA only."""
+
+    def __init__(self, vertices, faces, device="cuda"):
+        dev = _device(device)
+        if dev.type != "cuda":
+            raise _lib.SplatamB200Error("MeshDepth needs a CUDA device (there is no CPU fallback)")
+        v = np.asarray(torch.as_tensor(vertices).detach().cpu()).reshape(-1, 3).astype(np.float32)
+        f = np.asarray(torch.as_tensor(faces).detach().cpu()).reshape(-1, 3)
+        if len(v) == 0 or len(f) == 0:
+            raise ValueError("the mesh is empty (%d vertices, %d faces)" % (len(v), len(f)))
+        if not np.issubdtype(f.dtype, np.integer):
+            raise ValueError("face indices must be integers, got %s" % f.dtype)
+        if len(v) >= 1 << 31 or len(f) >= (1 << 31) - 1:
+            raise ValueError("MeshDepth takes fewer than 2^31 vertices and 2^31 - 1 faces, got %d and %d"
+                             % (len(v), len(f)))
+        if f.min() < 0 or f.max() >= len(v):
+            raise ValueError("face indices must lie in [0, %d), got [%d, %d]" % (len(v), f.min(), f.max()))
+        used = np.zeros(len(v), bool)
+        used[f.ravel()] = True
+        if not np.all(np.isfinite(v[used])):
+            raise ValueError("the vertices that faces use must be finite")
+        self.device = dev
+        self.vertices = torch.from_numpy(v).to(dev)
+        self.faces = torch.from_numpy(f.astype(np.int32)).to(dev)
+        self.ws = torch.empty(0, dtype=torch.uint8, device=dev)
+
+    def render(self, w2c, K, height, width, near=DEPTH_VIEW_NEAR, out=None):
+        w = torch.as_tensor(w2c)
+        _lib.need_cuda("MeshDepth.render", w)
+        w = w.to(self.device, torch.float32).reshape(-1, 4, 4).contiguous()
+        B, H, W = w.shape[0], int(height), int(width)
+        K = np.asarray(K, np.float64)
+        V, F = self.vertices.shape[0], self.faces.shape[0]
+        with _lib.on_device(self.device):
+            nb = _lib.nbytes("sb_mesh_depth_workspace_bytes", F, B, H, W)
+        if self.ws.numel() < nb:
+            self.ws = torch.empty(nb, dtype=torch.uint8, device=self.device)
+        if out is None:
+            out = (torch.empty(B, H, W, dtype=torch.float32, device=self.device),
+                   torch.empty(B, H, W, dtype=torch.int32, device=self.device))
+        depth, face_id = out
+        for t, dt in ((depth, torch.float32), (face_id, torch.int32)):
+            if t.shape != (B, H, W) or t.dtype != dt or t.device != self.device or not t.is_contiguous():
+                raise ValueError("out must be contiguous (float32, int32) tensors [%d,%d,%d] on %s"
+                                 % (B, H, W, self.device))
+        _lib.call("sb_mesh_depth", V, self.vertices, F, self.faces, B, H, W, w, float(K[0, 0]), float(K[1, 1]),
+                  float(K[0, 2]), float(K[1, 2]), float(near), self.ws, self.ws.numel(), depth, face_id,
+                  device=self.device)
+        return depth, face_id
+
+
+def depth_views(gt_kept, n, seed=0):
+    """n random cameras w2c [n,4,4] float32 (numpy) for ``depth_l1``, one view at a time from one
+    numpy.random.Generator(seed) in float64, so the first k of n views do not depend on n:
+
+    * centre: uniform in the axis-aligned box of the points gt_kept [N,3] (the kept ground-truth samples)
+    * direction (the camera's +z): uniform on the sphere, drawn again while it lies within 0.99 of +-y
+    * no roll: the camera's x axis is y_map x z_cam, normalised (perpendicular to the map's y axis, the first
+      camera's "down"), and its y axis z_cam x x_cam"""
+    p = torch.as_tensor(gt_kept).reshape(-1, 3)
+    if p.shape[0] == 0:
+        raise ValueError("depth_views needs at least one point to bound the view centres")
+    lo, hi = torch.stack(p.double().aminmax(dim=0)).cpu().numpy()
+    if not (np.all(np.isfinite(lo)) and np.all(np.isfinite(hi))):
+        raise ValueError("the points bounding the view centres must be finite")
+    if int(n) != n or n < 0:
+        raise ValueError("the view count must be a non-negative integer, got %r" % (n,))
+    rng = np.random.default_rng(int(seed))
+    out = np.tile(np.eye(4, dtype=np.float32), (int(n), 1, 1))
+    for i in range(int(n)):
+        c = lo + (hi - lo) * rng.random(3)
+        while True:
+            d = rng.standard_normal(3)
+            norm = np.linalg.norm(d)
+            if norm > 0 and abs(d[1] / norm) < 0.99:
+                break
+        z = d / norm
+        x = np.cross([0.0, 1.0, 0.0], z)
+        x /= np.linalg.norm(x)
+        R = np.stack([x, np.cross(z, x), z])
+        out[i, :3, :3] = R
+        out[i, :3, 3] = -R @ c
+    return out
+
+
+class _FrameStack:
+    """The frames' depth and gt_w2c (dicts as ``visible_mask`` takes) copied once to the device in chunks of
+    CULL_FRAMES_PER_LAUNCH, for culling many point sets against the same frames.  Holds T H W float32 on the device."""
+
+    def __init__(self, frames, dev):
+        self.device = dev
+        self.chunks = []
+        ds, ws, hw = [], [], None
+        for fr in frames:
+            d = torch.as_tensor(fr["depth"]).to(dev, torch.float32)
+            hw = hw or tuple(d.shape[-2:])
+            if d.numel() != hw[0] * hw[1]:
+                raise ValueError("frames differ in size: %s after %s" % (tuple(d.shape), hw))
+            ds.append(d.reshape(hw))
+            ws.append(torch.as_tensor(fr["gt_w2c"]).to(dev, torch.float32).reshape(4, 4))
+            if len(ds) == CULL_FRAMES_PER_LAUNCH:
+                self.chunks.append((torch.stack(ds), torch.stack(ws)))
+                ds, ws = [], []
+        if ds:
+            self.chunks.append((torch.stack(ds), torch.stack(ws)))
+        if not self.chunks:
+            raise ValueError("frames is empty")
+
+    def cull(self, points, K, occlusion_eps, mask=None):
+        """visible_mask's result for points [N,3] on the device: one sb_points_visible launch per chunk."""
+        eps = float(occlusion_eps)
+        if not (np.isfinite(eps) and eps >= 0):
+            raise ValueError("occlusion_eps must be finite and >= 0, got %r" % (occlusion_eps,))
+        pts = points.to(self.device, torch.float32).reshape(-1, 3).contiguous()
+        if mask is None:
+            mask = torch.zeros(pts.shape[0], dtype=torch.uint8, device=self.device)
+        K = np.asarray(K, np.float64)
+        for d, w in self.chunks:
+            _lib.call("sb_points_visible", pts.shape[0], pts, d.shape[0], d.shape[1], d.shape[2], d, w,
+                      float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]), eps, mask, device=self.device)
+        return mask
+
+
+def backproject(depth, w2c, K):
+    """The points [B,H,W,3] (float32, map frame) that depth [B,H,W] puts on the pixel centres of cameras w2c
+    [B,4,4] with intrinsics K: camera (x, y, z) = ((c - cx) d / fx, (r - cy) d / fy, d), then R^T (p - t)."""
+    B, H, W = depth.shape
+    K = np.asarray(K, np.float64)
+    dev = depth.device
+    c = (torch.arange(W, device=dev, dtype=torch.float32) - float(K[0, 2])) / float(K[0, 0])
+    r = (torch.arange(H, device=dev, dtype=torch.float32) - float(K[1, 2])) / float(K[1, 1])
+    cam = torch.stack([c[None, None, :] * depth, r[None, :, None] * depth, depth], dim=-1)
+    R, t = w2c[:, :3, :3], w2c[:, :3, 3]
+    return (cam - t[:, None, None, :]) @ R[:, None]
+
+
+def depth_sums(d_pred, d_gt, scored):
+    """Per-view float64 sums [B,4] of depth maps [B,H,W] over their scored pixels (bool [B,H,W]): the scored pixel
+    count, the sum of |d_pred - d_gt| (a hole, d_pred = 0, costs d_gt), the count of scored pixels where the
+    prediction has a surface (d_pred > 0) and the sum of |d_pred - d_gt| over those."""
+    sc = scored.double()
+    err = (d_pred.double() - d_gt.double()).abs() * sc
+    surf = sc * (d_pred > 0).double()
+    return torch.stack([sc.sum((1, 2)), err.sum((1, 2)), surf.sum((1, 2)), (err * surf).sum((1, 2))], dim=1)
+
+
+def depth_scores(sums, pixels, views):
+    """The metric from per-view sums [n,4] (``depth_sums``, read on the host) of views with `pixels` pixels each: a
+    view is accepted when at least half its pixels are scored, in order, up to `views` of them.  depth_l1 is the mean
+    over accepted views of the view's mean |d_pred - d_gt|; depth_l1_surface the same over the pixels with a predicted
+    surface (over the accepted views that have any; NaN if none has); hole_ratio the share of all accepted scored
+    pixels without a predicted surface.  ValueError when no view is accepted."""
+    s = np.asarray(sums, np.float64).reshape(-1, 4)
+    acc = s[s[:, 0] >= 0.5 * pixels][:int(views)]
+    if len(acc) == 0:
+        raise ValueError("no view had at least half its pixels on an observed ground-truth surface: check that the "
+                         "meshes are in the map's frame (datasets.SequenceFiles.world_to_map)")
+    has = acc[:, 2] > 0
+    return dict(depth_l1=float(np.mean(acc[:, 1] / acc[:, 0])),
+                depth_l1_surface=float(np.mean(acc[has, 3] / acc[has, 2])) if has.any() else float("nan"),
+                hole_ratio=float(1.0 - acc[:, 2].sum() / acc[:, 0].sum()), views_used=len(acc))
+
+
+def depth_l1(pred, gt, frames=None, K=None, views=1000, seed=0, occlusion_eps=0.03, batch=8, *, gt_kept=None,
+             device="cuda"):
+    """Scores the reconstruction `pred` against the ground truth `gt` (both (vertices [V,3], faces [F,3]) in the
+    map's frame) by rendered depth, from ``depth_views`` cameras at DEPTH_VIEW_HW with DEPTH_VIEW_K and near
+    DEPTH_VIEW_NEAR.  Views are drawn `batch` at a time and each batch is rendered once per mesh (``MeshDepth``).
+
+    A view's scored pixels are those where the ground-truth render has a surface; with `frames` (as for
+    ``evaluate_mesh``; K their intrinsics, default the first frame's) only those whose surface point -- the pixel
+    back-projected at the ground-truth depth -- some frame observed, by ``visible_mask``'s rule with
+    `occlusion_eps` (sb_points_visible; the frames' depth is held on the device).  The host reads the per-view sums
+    once per batch; drawing stops after `views` accepted views (``depth_scores``) or 20 views draws.
+
+    gt_kept: the points whose box holds the view centres; default 200,000 area samples of `gt` (torch.Generator
+    seeded with `seed`), culled by `frames`.  Returns depth_l1, depth_l1_surface (metres), hole_ratio, views_used,
+    views_drawn, and the device times render_ms and cull_ms."""
+    dev = _device(device)
+    if dev.type != "cuda":
+        raise _lib.SplatamB200Error("depth_l1 needs a CUDA device (there is no CPU fallback)")
+    if int(views) != views or views < 1:
+        raise ValueError("views must be a positive integer, got %r" % (views,))
+    if int(batch) != batch or batch < 1:
+        raise ValueError("batch must be a positive integer, got %r" % (batch,))
+    if not (np.isfinite(occlusion_eps) and occlusion_eps >= 0):
+        raise ValueError("occlusion_eps must be finite and >= 0, got %r" % (occlusion_eps,))
+    if frames is not None and K is None and not isinstance(frames, _FrameStack):
+        K, frames = _first_intrinsics(frames)
+    H, W = DEPTH_VIEW_HW
+    t_render, t_cull = _Timer(), _Timer()
+    with torch.cuda.device(dev):
+        if frames is not None and not isinstance(frames, _FrameStack):
+            frames = _FrameStack(frames, dev)
+        g_mesh, p_mesh = MeshDepth(*gt, dev), MeshDepth(*pred, dev)
+        if gt_kept is None:
+            gen = torch.Generator(dev).manual_seed(int(seed))
+            gt_kept, _ = sample_surface(*gt, 200_000, gen, dev)
+            if frames is not None:
+                gt_kept = gt_kept[frames.cull(gt_kept, K, occlusion_eps).bool()]
+        cams = torch.from_numpy(depth_views(gt_kept, 20 * int(views), seed)).to(dev)
+        bufs = None
+        sums, drawn, used = [], 0, 0
+        while used < views and drawn < cams.shape[0]:
+            nb = min(int(batch), cams.shape[0] - drawn)
+            w = cams[drawn:drawn + nb]
+            t_render.start()
+            d_gt, _ = g_mesh.render(w, DEPTH_VIEW_K, H, W)
+            d_pred, _ = p_mesh.render(w, DEPTH_VIEW_K, H, W)
+            t_render.stop()
+            scored = d_gt > 0
+            if frames is not None:
+                t_cull.start()
+                pts = backproject(d_gt, w, DEPTH_VIEW_K)
+                if bufs is None or bufs.numel() != nb * H * W:
+                    bufs = torch.empty(nb * H * W, dtype=torch.uint8, device=dev)
+                bufs.zero_()
+                frames.cull(pts, K, occlusion_eps, bufs)
+                scored &= bufs.view(nb, H, W).bool()
+                t_cull.stop()
+            s = depth_sums(d_pred, d_gt, scored).cpu().numpy()
+            drawn += nb
+            sums.append(s)
+            used += int((s[:, 0] >= 0.5 * H * W).sum())
+        out = depth_scores(np.concatenate(sums), H * W, views)
+        torch.cuda.synchronize(dev)
+    out.update(views_drawn=drawn, render_ms=t_render.ms(), cull_ms=t_cull.ms() if t_cull.pairs else 0.0)
     return out

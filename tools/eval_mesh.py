@@ -13,7 +13,12 @@ should select the run's frames.  The ground-truth mesh is moved from the dataset
 (datasets.SequenceFiles.world_to_map: the first selected camera is the map's origin), and only the ground-truth samples
 that some --every-th selected frame observed, by its depth at the native image size and its ground-truth pose, are
 kept.  --no-cull keeps every sample; with --no-cull and no dataset flags the two meshes are scored as they are, for a
-ground truth that is already in the map's frame and culled.  One GPU."""
+ground truth that is already in the map's frame and culled.
+
+--depth-views N also renders both meshes from N random views (mesh_eval.depth_l1: 500x500, fx = fy = 300, centres in
+the box of the kept ground-truth samples) and adds depth_l1_cm, depth_l1_surface_cm, hole_ratio, depth_views_used,
+depth_views_drawn and render_ms to the line; with culling only pixels whose ground-truth surface was observed count.
+One GPU."""
 import argparse
 import json
 import os
@@ -44,6 +49,8 @@ def parse_args(argv=None):
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--batch", type=int, default=8, help="frames per culling launch")
     ap.add_argument("--no-cull", action="store_true", help="keep every ground-truth sample")
+    ap.add_argument("--depth-views", type=int, default=0,
+                    help="also score depth L1 over this many accepted random views (0: off)")
     a = ap.parse_args(argv)
     for flag, path in (("--mesh", a.mesh), ("--gt-mesh", a.gt_mesh)):
         if not os.path.isfile(path):
@@ -58,6 +65,8 @@ def parse_args(argv=None):
             ap.error("culling needs the sequence: pass --dataset, --basedir and --sequence, or --no-cull")
         if selection:
             ap.error("%s select frames: they need --dataset, --basedir and --sequence" % ", ".join(selection))
+    if a.depth_views < 0:
+        ap.error("--depth-views must be >= 0")
     if a.every < 1 or a.batch < 1 or a.samples < 1:
         ap.error("--every, --batch and --samples must be positive")
     if not (np.isfinite(a.threshold) and a.threshold > 0):
@@ -91,7 +100,8 @@ def main(argv=None):
                 K = seq.intrinsics.cpu().numpy()
                 frames = (seq[t] for t in range(0, len(seq), a.every))
         out = mesh_eval.evaluate_mesh((pv, pf), (gv, gf), frames, K, samples=a.samples, threshold=a.threshold,
-                                      occlusion_eps=a.occlusion_eps, seed=a.seed, device=dev, batch=a.batch)
+                                      occlusion_eps=a.occlusion_eps, seed=a.seed, device=dev, batch=a.batch,
+                                      depth_views=a.depth_views)
     finally:
         if seq is not None:
             seq.close()
@@ -102,6 +112,10 @@ def main(argv=None):
                 pred_samples=out["pred_samples"], gt_samples=out["gt_samples"],
                 gt_samples_kept=out["gt_samples_kept"], cull_ms=out["cull_ms"], grid_ms=out["grid_ms"],
                 query_ms=out["query_ms"])
+    if a.depth_views:
+        line.update(depth_l1_cm=100 * out["depth_l1"], depth_l1_surface_cm=100 * out["depth_l1_surface"],
+                    hole_ratio=out["hole_ratio"], depth_views_used=out["depth_views_used"],
+                    depth_views_drawn=out["depth_views_drawn"], render_ms=out["depth_render_ms"])
     print(json.dumps(line))
     return line
 
