@@ -192,16 +192,21 @@ def calc_ssim(img1, img2, window_size=11):
     return (((2 * mu12 + c1) * (2 * s12 + c2)) / ((mu1_sq + mu2_sq + c1) * (s1 + s2 + c2))).mean()
 
 
-def _render_pair(params, frame, render, fused, camera_grad, max_rendered=None):
-    """The RGB and depth/silhouette renders of `frame` -> (image, depth_sil, radii, means2D of the RGB render).  Either
-    the Gaussians get gradient or, with `camera_grad`, only the camera pose.  fused: one kernel builds both rendervars
+def _render_pair(params, frame, render, fused, camera_grad, max_rendered=None, gaussians_grad=None):
+    """The RGB and depth/silhouette renders of `frame` -> (image, depth_sil, radii, means2D of the RGB render).  The
+    camera pose gets gradient iff `camera_grad`.  `gaussians_grad` (default: not `camera_grad`) decides whether the
+    Gaussians get gradient on the torch glue path (transform_to_frame's flag); both together give both gradients
+    from one backward (the reference's do_ba=True).  The fused path's kernel (csrc/prepare.cu) gives gradient to
+    whichever Gaussian tensors require it, so a caller that wants only the pose passes detached Gaussian tensors, as
+    tracking does.  fused: one kernel builds both rendervars
     (csrc/prepare.cu), and the product rasterizer blends both colour sets in one pass (N1), with a fixed instance
     capacity if `max_rendered`; otherwise the PyTorch glue and two `render` calls.  Both render at frame["pose"]
     (w2c, normalised quaternion) if given, else at the frame's pose in params."""
     if fused:
         rv_rgb, rv_depth = fused_rendervars(params, frame["id"], frame["w2c"], camera_grad, pose=frame.get("pose"))
     else:
-        tg = transform_to_frame(params, frame["id"], gaussians_grad=not camera_grad, camera_grad=camera_grad,
+        gaussians_grad = (not camera_grad) if gaussians_grad is None else gaussians_grad
+        tg = transform_to_frame(params, frame["id"], gaussians_grad=gaussians_grad, camera_grad=camera_grad,
                                 pose=frame.get("pose"))
         rv_rgb, rv_depth = rgb_rendervar(params, tg), depth_sil_rendervar(params, frame["w2c"], tg)
     if fused and render is default_render:
@@ -216,13 +221,13 @@ def _render_pair(params, frame, render, fused, camera_grad, max_rendered=None):
 
 
 def mapping_loss(params, frame, render, loss_weights=(0.5, 1.0), ignore_outlier_depth_loss=False, fused_loss=False,
-                 max_rendered=None, keep=None):
-    """SplaTAM get_loss(mapping=True): Gaussians get gradient, camera does not
-    (R/scripts/splatam.py:214-347 with tracking=False, mapping=True, do_ba=False, use_l1=True).
+                 max_rendered=None, keep=None, camera_grad=False):
+    """SplaTAM get_loss(mapping=True): the Gaussians get gradient, and with `camera_grad` the keyframe's pose too
+    (R/scripts/splatam.py:214-347 with tracking=False, mapping=True, do_ba=camera_grad, use_l1=True).
     frame: dict(im [3,H,W], depth [1,H,W], cam settings, w2c [4,4] first-frame w2c, id time index).
     render(settings, **rendervar) -> (image, radii, depth)."""
-    im, depth_sil, radius, means2D = _render_pair(params, frame, render, fused_loss, camera_grad=False,
-                                                  max_rendered=max_rendered)
+    im, depth_sil, radius, means2D = _render_pair(params, frame, render, fused_loss, camera_grad=camera_grad,
+                                                  max_rendered=max_rendered, gaussians_grad=True)
     if keep is not None:       # the caller wants d loss / d means2D of the RGB render (densification statistic)
         means2D.retain_grad()
         keep["means2D"] = means2D
@@ -491,21 +496,24 @@ def _track_frame_graphed(params, frame, num_iters, lr_rot, lr_trans, build=True,
 class FlatGaussians:
     """The five Gaussian parameter tensors as views into ONE flat fp32 buffer, their gradients as
     views into ONE flat gradient bucket of the same layout -- the packed send buffer of the
-    all-reduce (48-56 B per Gaussian)."""
+    all-reduce (48-56 B per Gaussian).  `pose_numel` > 0 appends the pose-gradient table of keyframe-pose refinement
+    ([7, T]: the 4 quaternion rows, then the 3 translation rows) to the bucket."""
 
-    def __init__(self, tensors):
+    def __init__(self, tensors, pose_numel=0):
         self.shapes = {k: tuple(tensors[k].shape) for k in GAUSSIAN_KEYS}
         n = sum(math.prod(s) for s in self.shapes.values())
         dev = tensors["means3D"].device
         self.flat = torch.zeros(n, dtype=torch.float32, device=dev)
         # ONE all-reduce bucket: [per-Gaussian gradients (n) | per-Gaussian "seen" flags as 0/1 floats (P) | loss (1) |
-        # capacity-overflow flag of the sync-free rasterizer (1): non-zero on ANY rank => every rank skips the update]
+        # capacity-overflow flag of the sync-free rasterizer (1): non-zero on ANY rank => every rank skips the update |
+        # pose-gradient table (pose_numel, refinement only)]
         P_ = tensors["means3D"].shape[0]
-        self.bucket = torch.zeros(n + P_ + 2, dtype=torch.float32, device=dev)
+        self.bucket = torch.zeros(n + P_ + 2 + pose_numel, dtype=torch.float32, device=dev)
         self.flat_grad = self.bucket[:n]
         self.seen_f = self.bucket[n:n + P_]
         self.loss_slot = self.bucket[n + P_:n + P_ + 1]
-        self.overflow_slot = self.bucket[n + P_ + 1:]
+        self.overflow_slot = self.bucket[n + P_ + 1:n + P_ + 2]
+        self.pose_grad = self.bucket[n + P_ + 2:]
         self.params, grads = self.views(self.flat), self.views(self.flat_grad)
         for k, p in self.params.items():
             p.copy_(tensors[k].detach().reshape(self.shapes[k]))
@@ -537,8 +545,19 @@ def default_render(settings, **rendervar):
     return GaussianRasterizer(raster_settings=settings)(**rendervar)
 
 
+CAM_KEYS = ("cam_unnorm_rots", "cam_trans")
+
+
 class ShardedMapper:
-    """Data-parallel mapping over keyframes.  `lrs` follow R/configs/replica/splatam.py:92-100."""
+    """Data-parallel mapping over keyframes.  `lrs` follow R/configs/replica/splatam.py:92-100.
+
+    Keyframe-pose refinement (the reference's get_loss(mapping=True, do_ba=True)) is on iff the `lrs` of
+    cam_unnorm_rots or cam_trans is non-zero.  The mapper then owns the cameras: `cam` holds two views of one flat
+    [4T | 3T] buffer, and camera tensors a caller puts into `cam` (tracking, `sync_camera`) are copied into it before
+    the next step.  Each step's render gives gradient to the Gaussians and to its keyframe's pose; the [7, T] pose
+    gradient (zero outside the keyframe's column) travels in the all-reduce bucket, and an Adam over the whole two
+    tensors (torch.optim.Adam on the torch path, FusedAdam on the fused one) steps them on every step.  Its moments
+    reset with `reset_optimizer` and survive map edits.  At zero camera rates nothing of this exists."""
 
     DEFAULT_LRS = dict(means3D=0.0001, rgb_colors=0.0025, unnorm_rotations=0.001, logit_opacities=0.05,
                        log_scales=0.001)
@@ -553,7 +572,11 @@ class ShardedMapper:
         self.group = group
         self.rank = self.dist.get_rank(group) if self.dist else 0
         self.world = self.dist.get_world_size(group) if self.dist else 1
-        self.g = FlatGaussians(gaussians)
+        lrs = dict(self.DEFAULT_LRS, **(lrs or {}))
+        self.lrs = lrs
+        self.refine_poses = any(float(lrs.get(k, 0.0)) != 0.0 for k in CAM_KEYS)
+        T = cam_trans.shape[-1]
+        self.g = FlatGaussians(gaussians, pose_numel=7 * T if self.refine_poses else 0)
         P, dev = self.g.shapes["means3D"][0], self.g.flat.device
         # per-Gaussian creation frame: kept beside the flat buffer, outside the gradient / Adam / all-reduce layout, and
         # edited with the same masks as the parameters, so every replica holds the same one
@@ -564,12 +587,19 @@ class ShardedMapper:
             if self.timestep.shape[0] != P:
                 raise ValueError("timestep has %d entries for a map of %d Gaussians" % (self.timestep.shape[0], P))
         self.cam = dict(cam_unnorm_rots=cam_unnorm_rots.detach(), cam_trans=cam_trans.detach())
-        lrs = dict(self.DEFAULT_LRS, **(lrs or {}))
-        self.lrs = lrs
         # fused = hand-written Adam over the flat buffer + fused L1/SSIM loss (CUDA only); the torch path is
         # the reference formulation (R/scripts/splatam.py:160-166) and the one the CPU/gloo test exercises
         self.fused = self.g.flat.is_cuda if fused is None else bool(fused)
         self._make_optimizer()
+        if self.refine_poses:
+            self._cam_flat = torch.zeros(7 * T, dtype=torch.float32, device=dev)
+            self._cam_views = {"cam_unnorm_rots": self._cam_flat[:4 * T].view(1, 4, T),
+                               "cam_trans": self._cam_flat[4 * T:].view(1, 3, T)}
+            for v in self._cam_views.values():
+                v.requires_grad_(True)
+            self._bind_pose_grad()
+            self._bind_cameras()
+            self._make_cam_optimizer()
         self.render = render
         self.gen = torch.Generator().manual_seed(seed)   # shared seed -> identical schedule on every rank
         self.step_idx = 0
@@ -631,9 +661,64 @@ class ShardedMapper:
             return self.opt.applied_steps()[0]
         return int(self.opt.state[self.g.params["means3D"]]["step"])
 
+    # ---- keyframe-pose refinement ---------------------------------------------------------------------------------
+    def _bind_pose_grad(self):
+        """The camera views' gradients are the bucket's pose table (autograd accumulates into it in place)."""
+        T = self._cam_flat.numel() // 7
+        self._cam_views["cam_unnorm_rots"].grad = self.g.pose_grad[:4 * T].view(1, 4, T)
+        self._cam_views["cam_trans"].grad = self.g.pose_grad[4 * T:].view(1, 3, T)
+
+    def _bind_cameras(self):
+        """Copies camera tensors a caller put into `cam` into the mapper's buffer, whose views `cam` holds again."""
+        if all(self.cam[k] is self._cam_views[k] for k in CAM_KEYS):
+            return
+        T = self._cam_flat.numel() // 7
+        with torch.no_grad():
+            self._cam_flat[:4 * T].copy_(self.cam["cam_unnorm_rots"].reshape(-1))
+            self._cam_flat[4 * T:].copy_(self.cam["cam_trans"].reshape(-1))
+        self.cam = dict(self._cam_views)
+
+    def _make_cam_optimizer(self):
+        """Fresh Adam over the two whole camera tensors (initialize_optimizer(tracking=False), R/scripts/splatam.py:
+        160-166): the fused path steps the flat buffer with FusedAdam, the torch path uses torch.optim.Adam groups."""
+        lr = [self.lrs.get(k, 0.0) for k in CAM_KEYS]
+        if self.fused:
+            from .train_ops import FusedAdam
+            T = self._cam_flat.numel() // 7
+            self.cam_opt = FusedAdam(self._cam_flat, self.g.pose_grad, [4 * T, 3 * T], lr, eps=1e-15)
+        else:
+            self.cam_opt = torch.optim.Adam([{"params": [self._cam_views[k]], "name": k, "lr": r}
+                                             for k, r in zip(CAM_KEYS, lr)], lr=0.0, eps=1e-15)
+
+    def _cam_step(self, guard=None):
+        """Adam step of the cameras; `guard`: the overflow slot of a graph step (a no-op when it is non-zero)."""
+        if self.fused:
+            self.cam_opt.flat_grad = self.g.pose_grad
+            if guard is None:
+                self.cam_opt.step()
+            else:
+                self.cam_opt.step_guarded(guard)
+            # the kernel writes through a raw pointer: bump the version the pose cache (fused_pose_cached) keys on
+            torch.autograd.graph.increment_version(self._cam_flat)
+        else:
+            self.cam_opt.step()
+
     def set_lr(self, key, lr):
-        """Learning rate of Gaussian tensor `key` from the next Adam step on, and for the optimizers a map edit
-        rebuilds (update_learning_rate, R/utils/gs_external.py:260-266)."""
+        """Learning rate of parameter tensor `key` from the next Adam step on, and for the optimizers a map edit
+        rebuilds (update_learning_rate, R/utils/gs_external.py:260-266).  A camera key needs a mapper built with
+        refinement on (a non-zero camera rate), or a zero rate."""
+        if key in CAM_KEYS:
+            if not self.refine_poses:
+                if float(lr) != 0.0:
+                    raise ValueError("keyframe-pose refinement is off: build the mapper with a non-zero %s rate" % key)
+                return
+            self.lrs[key] = float(lr)
+            i = CAM_KEYS.index(key)
+            if self.fused:
+                self.cam_opt.set_lr(i, lr)
+            else:
+                self.cam_opt.param_groups[i]["lr"] = float(lr)
+            return
         self.lrs[key] = float(lr)
         i = GAUSSIAN_KEYS.index(key)
         if self.fused:
@@ -643,8 +728,10 @@ class ShardedMapper:
 
     def reset_optimizer(self):
         """Fresh Adam state, as the reference re-creates its optimizer at the start of every frame's mapping
-        phase (R/scripts/splatam.py:822)."""
+        phase (R/scripts/splatam.py:822), the cameras' included."""
         self._make_optimizer()
+        if self.refine_poses:
+            self._make_cam_optimizer()
 
     def _widths(self):
         return [self.g.shapes[k][1] if len(self.g.shapes[k]) > 1 else 1 for k in GAUSSIAN_KEYS]
@@ -656,7 +743,11 @@ class ShardedMapper:
         for k, w in zip(GAUSSIAN_KEYS, self._widths()):
             tensors[k] = flat[off:off + w * P_new].view(P_new, w)
             off += w * P_new
-        self.g = FlatGaussians(tensors)
+        old_pose_grad = self.g.pose_grad
+        self.g = FlatGaussians(tensors, pose_numel=old_pose_grad.numel())
+        if self.refine_poses:       # map edits leave the cameras alone (R/utils/slam_external.py:141): keep the gradient
+            self.g.pose_grad.copy_(old_pose_grad)
+            self._bind_pose_grad()
         self._make_optimizer(m, v, t)
         self._graph = None                      # shapes changed: a captured graph is stale
 
@@ -765,16 +856,36 @@ class ShardedMapper:
         # a geometry pass per probed frame sizes the capacity (an overflow later is safe: it skips the step and
         # re-captures, see the docstring)
         probe = window if len(window) <= 3 else [window[0], window[len(window) // 2], window[-1]]
+        if self.refine_poses:
+            self._bind_cameras()
         step = _CapturedStep(self.params(), window[0], probe, slack, capacity)
         step.frame["pose"] = tuple(t.clone() for t in fused_pose_cached(self.params(), window[0]["id"]))
         self._slack = slack
         self._polls = []                 # (event, pinned copy of the overflow slot) of steps in flight
         self._pin = [torch.empty(1, dtype=torch.float32, pin_memory=True) for _ in range(8)]
+        refine = self.refine_poses
+        if refine:
+            # the keyframe's pose as two static leaves [1,4], [1,3] loaded from its column before each replay; the
+            # backward leaves their gradient in static .grad buffers, scattered into column `col` of the pose table
+            T = self._cam_flat.numel() // 7
+            t0 = window[0]["id"]
+            with torch.cuda.stream(step.side):
+                q = self.cam["cam_unnorm_rots"][..., t0].detach().clone().requires_grad_(True)
+                tr = self.cam["cam_trans"][..., t0].detach().clone().requires_grad_(True)
+                q.grad, tr.grad = torch.zeros_like(q), torch.zeros_like(tr)
+                col = torch.full((1,), int(t0), dtype=torch.long, device=step.dev)
+            step.pose_leaves = (q, tr, col)
 
         def body():
             self.g.bucket.zero_()
-            loss, radius = mapping_loss(self.params(), step.frame, self.render, fused_loss=True, max_rendered=step.cap)
+            frame = step.frame
+            if refine:
+                q.grad.zero_(); tr.grad.zero_()
+                frame = dict(step.frame, pose=camera_w2c(q, tr))
+            loss, radius = mapping_loss(self.params(), frame, self.render, fused_loss=True, max_rendered=step.cap)
             loss.backward()
+            if refine:
+                self.g.pose_grad.view(7, T).index_copy_(1, col, torch.cat([q.grad, tr.grad], 1).reshape(7, 1))
             self.g.seen_f.copy_(radius > 0)
             self.g.loss_slot.copy_(loss.detach().reshape(1))
             self.g.overflow_slot.copy_(step.overflow())     # int32 0/1 -> float
@@ -838,7 +949,10 @@ class ShardedMapper:
     def accumulate(self, frame):
         """Local backward of one keyframe into the flat gradient bucket (no communication)."""
         keep = {} if self.track_means2D else None
-        loss, radius = mapping_loss(self.params(), frame, self.render, fused_loss=self.fused, keep=keep)
+        if self.refine_poses:
+            self._bind_cameras()
+        loss, radius = mapping_loss(self.params(), frame, self.render, fused_loss=self.fused, keep=keep,
+                                    camera_grad=self.refine_poses)
         loss.backward()
         if keep is not None:      # gradient of the RGB render's 2D means: the densification statistic (splatam.py:250)
             self.last_means2D_grad = keep["means2D"].grad
@@ -958,8 +1072,16 @@ class ShardedMapper:
             self.poll_overflow(window)
             step, frame = self._graph, window[picks[self.rank]]
             step.load(frame)
-            for static, v in zip(step.frame["pose"], fused_pose_cached(self.params(), frame["id"])):
-                static.copy_(v, non_blocking=True)
+            if self.refine_poses:
+                self._bind_cameras()
+                q, tr, col = step.pose_leaves
+                with torch.no_grad():
+                    q.copy_(self.cam["cam_unnorm_rots"][..., frame["id"]])
+                    tr.copy_(self.cam["cam_trans"][..., frame["id"]])
+                col.fill_(int(frame["id"]))
+            else:
+                for static, v in zip(step.frame["pose"], fused_pose_cached(self.params(), frame["id"])):
+                    static.copy_(v, non_blocking=True)
             step.graph.replay()
         else:
             self.g.zero_grad()
@@ -971,6 +1093,8 @@ class ShardedMapper:
             self.dist.all_reduce(self.g.bucket, op=self.dist.ReduceOp.SUM, group=self.group)
         if graphed:
             self.opt.step_guarded(self.g.overflow_slot)    # no-op on every rank if any rank's render overflowed
+            if self.refine_poses:
+                self._cam_step(self.g.overflow_slot)
             host = self._pin[self.step_idx % len(self._pin)]
             host.copy_(self.g.overflow_slot, non_blocking=True)
             ev = torch.cuda.Event()
@@ -978,6 +1102,8 @@ class ShardedMapper:
             self._polls.append((ev, host))
         else:
             self.opt.step()
+            if self.refine_poses:
+                self._cam_step()
         self.step_idx += 1
         seen = self.g.seen_f > 0
         loss = self.g.loss_slot[0] / self.world

@@ -96,6 +96,15 @@ def optimize_map(mapper, frames, iters, means3D_lr_final, densify_dict, scene_ra
     return counts
 
 
+def _map_lrs(lrs):
+    """`lrs` without camera keys: the offline loops render with camera_grad=False whatever their camera rates
+    (R/scripts/post_splatam_opt.py), so a non-zero camera rate is an error rather than a request for pose refinement."""
+    bad = {k: v for k, v in lrs.items() if k in M.CAM_KEYS and float(v) != 0.0}
+    if bad:
+        raise ValueError("offline map optimisation keeps the poses fixed; got camera rates %s" % bad)
+    return {k: v for k, v in lrs.items() if k not in M.CAM_KEYS}
+
+
 def from_record(path, frames, frame_indices, device, lrs=LRS, render=M.default_render, fused=None):
     """post_splatam_opt.py's start (initialize_first_timestep_from_ckpt, :68-124, and the frame loading, :243-262):
     the map of a SplaTAM record -- formats.save_run_record's or the reference's params.npz -- with its five Gaussian
@@ -115,7 +124,7 @@ def from_record(path, frames, frame_indices, device, lrs=LRS, render=M.default_r
     t = formats.record_tensors(rec, formats.CHECKPOINT_KEYS, device)
     rots, trans = t["cam_unnorm_rots"], t["cam_trans"]
     train = [dict(frames[i], pose=M.camera_w2c(rots[..., k], trans[..., k])) for i, k in enumerate(idx)]
-    mapper = M.ShardedMapper({k: t[k] for k in formats.GAUSSIAN_KEYS}, rots, trans, lrs=lrs, render=render,
+    mapper = M.ShardedMapper({k: t[k] for k in formats.GAUSSIAN_KEYS}, rots, trans, lrs=_map_lrs(lrs), render=render,
                              fused=fused, timestep=rec["timestep"])
     return mapper, train, float(frames[0]["depth"].max()) / 2.0, rec
 
@@ -134,7 +143,8 @@ def from_gt_poses(init_frames, frames, lrs=LRS, sil_thres=0.5, render=M.default_
     init, _ = slam.initialize_map(f0, f0["intrinsics"].cpu())
     rots = torch.zeros(1, 4, T, device=dev)
     rots[:, 0] = 1.0
-    mapper = M.ShardedMapper(init, rots, torch.zeros(1, 3, T, device=dev), lrs=lrs, render=render, fused=fused)
+    mapper = M.ShardedMapper(init, rots, torch.zeros(1, 3, T, device=dev), lrs=_map_lrs(lrs), render=render,
+                             fused=fused)
     K = f0["intrinsics"].cpu()
     for t in range(T):
         fr = init_frames[t]

@@ -10,6 +10,7 @@ By default the map starts from a perturbed copy of the generating scene; with `i
 """
 import math
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -67,18 +68,28 @@ def _without_densify(frame):
 
 def keyframes_from_checkpoint(frames, ckpt):
     """The keyframe list of a checkpoint (formats.load_checkpoint): frames[k] for every stored id k, with est_w2c
-    rebuilt from the stored camera column k (F.normalize + build_rotation, as R/scripts/splatam.py:619-638 does)."""
+    rebuilt from the stored camera column k (F.normalize + build_rotation, as R/scripts/splatam.py:619-638 does) -- or,
+    when the checkpoint's sidecar holds `keyframe_est_w2c` (a run with keyframe-pose refinement, whose later mapping
+    phases move a column after its keyframe stored its pose), the stored matrices themselves."""
     rots, trans = ckpt["cam_unnorm_rots"], ckpt["cam_trans"]
-    return [dict(_without_densify(frames[k]), est_w2c=_curr_w2c(rots, trans, k)) for k in ckpt["keyframe_time_indices"]]
+    ids = ckpt["keyframe_time_indices"]
+    state = ckpt.get("state")
+    if state is not None and "keyframe_est_w2c" in state:
+        est = torch.from_numpy(np.array(state["keyframe_est_w2c"], dtype=np.float32)).to(rots.device)
+        if est.shape != (len(ids), 4, 4):
+            raise ValueError("the checkpoint's run state holds %s keyframe poses for %d keyframes"
+                             % (tuple(est.shape), len(ids)))
+        return [dict(_without_densify(frames[k]), est_w2c=est[i]) for i, k in enumerate(ids)]
+    return [dict(_without_densify(frames[k]), est_w2c=_curr_w2c(rots, trans, k)) for k in ids]
 
 
-def _run_state(mapper, counts):
+def _run_state(mapper, counts, keyframes=None):
     """The sidecar of a checkpoint (formats.save_checkpoint's `run_state`): what continues a run exactly and the
     reference's params{t}.npz cannot carry -- the mapper's own state (ShardedMapper.run_state: the Gaussians'
     `timestep`, its schedule and device generators, the densification statistic), torch's CPU RNG and the CUDA RNG of
     the map's device (keyframe selection and densification draw from the global generators), NumPy's global RNG
-    (keyframe_selection_overlap's permutation) and the Gaussian counts so far.  Numeric arrays only."""
-    import numpy as np
+    (keyframe_selection_overlap's permutation) and the Gaussian counts so far; with `keyframes` (runs with keyframe-pose
+    refinement) also their stored est_w2c, which the refined camera columns no longer give.  Numeric arrays only."""
     dev = mapper.g.flat.device
     _, keys, pos, has_gauss, cached = np.random.get_state()
     st = dict(mapper.run_state(), torch_rng=torch.get_rng_state().numpy(),
@@ -87,12 +98,13 @@ def _run_state(mapper, counts):
               numpy_rng_cached_gaussian=np.array(cached, dtype=np.float64), counts=np.array(counts, dtype=np.int64))
     if dev.type == "cuda":
         st["cuda_rng"] = torch.cuda.get_rng_state(dev).numpy()
+    if keyframes is not None:
+        st["keyframe_est_w2c"] = torch.stack([kf["est_w2c"].detach().float() for kf in keyframes]).cpu().numpy()
     return st
 
 
 def _restore_run_state(mapper, st):
     """Inverse of _run_state on a mapper built from the checkpoint's map; returns the Gaussian counts so far."""
-    import numpy as np
     mapper.load_run_state(st)
     dev = mapper.g.flat.device
     torch.set_rng_state(torch.from_numpy(np.array(st["torch_rng"], dtype=np.uint8)))
@@ -128,10 +140,11 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
              window=4, fused=None, seed=0, intrinsics=None, add_new_gaussians=False, sil_thres=0.5, prune_dict=None,
              scene_radius=None, select_keyframes=False, checkpoint_dir=None, first_frame_iters=0, map_every=None,
              graph=False, timing=None, densify_dict=None, tracking_lrs=(0.0004, 0.002), depth_loss_thres=None,
-             checkpoint_every=None, resume=None):
+             checkpoint_every=None, resume=None, mapping_cam_lrs=(0.0, 0.0)):
     """Tracks every frame and maps on keyframes.  gauss_init: dict of the five Gaussian tensors (the map's
     starting point); frames: list of dict(id, cam, w2c, im, depth).  Returns dict(rots, trans, psnr, gauss, counts,
-    timestep, keyframe_time_indices): `timestep` is the frame that created each Gaussian of the final map.
+    timestep, keyframe_time_indices, keyframe_est_w2c): `timestep` is the frame that created each Gaussian of the final
+    map, `keyframe_est_w2c` the pose each keyframe stored when it joined the list.
 
     The optional stages follow the reference's main loop (R/scripts/splatam.py:776-925): `add_new_gaussians` grows
     the map from each mapped frame's silhouette holes before mapping -- from the frame's ``densify`` entry, with that
@@ -147,8 +160,11 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     densification inside the mapping iterations (the reference's `use_gaussian_splatting_densification` branch,
     splatam.py:863-864; eager steps only -- the map size changes).  `tracking_lrs`: the tracking learning rates of
     (cam_unnorm_rots, cam_trans); the default is Replica's.  `depth_loss_thres`: track_frame's rule that doubles a
-    frame's tracking iterations while the depth loss stays high (ScanNet++: 20000).  `timing`: dict that receives the
-    accumulated wall seconds of tracking / mapping (synchronised), the tracking and mapping iteration counts, and
+    frame's tracking iterations while the depth loss stays high (ScanNet++: 20000).  `mapping_cam_lrs`: the mapping
+    learning rates of (cam_unnorm_rots, cam_trans); non-zero turns on keyframe-pose refinement (the reference's
+    do_ba=True, `ShardedMapper`): each mapping iteration also steps its keyframe's pose, and a keyframe joins the
+    keyframe list with its pose after its own mapping phase, as the reference stores it.  `timing`: dict that receives
+    the accumulated wall seconds of tracking / mapping (synchronised), the tracking and mapping iteration counts, and
     `setup_s`, the wall seconds from the call to the start of the frame loop.
 
     Checkpoints and resume (R/scripts/splatam.py:604-643,927-931).  With `checkpoint_dir` and `checkpoint_every` = N,
@@ -160,10 +176,12 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     `resume` = formats.load_checkpoint(dir, t, device), with gauss_init None: the map, the cameras and the keyframe list
     come from the checkpoint (keyframe k is frames[k] with est_w2c rebuilt from the stored camera column, as
     splatam.py:619-638 does); with a sidecar every RNG, the schedule generator, the densification statistic, `timestep`
-    and `counts` are restored, without one (a checkpoint the reference wrote) `timestep` is zeros, `counts` starts at
-    the loaded map and the RNGs are left as they are.  `first_frame_iters` does not run.  The loop continues at frame
-    t + 1, unlike the reference, which restarts at t: it tracks and maps frame t a second time and appends it to its
-    keyframe list twice.  Continuing at t + 1 is what makes a resumed run equal the uninterrupted one."""
+    and `counts` are restored -- with refinement also the keyframes' stored est_w2c, since later mapping phases move
+    a keyframe's column after it stored its pose --, without one (a checkpoint the reference wrote) `timestep` is
+    zeros, `counts` starts at the loaded map and the RNGs are left as they are.  `first_frame_iters` does not run.
+    The loop continues at frame t + 1, unlike the reference, which restarts at t: it tracks and maps frame t a second
+    time and appends it to its keyframe list twice.  Continuing at t + 1 is what makes a resumed run equal the
+    uninterrupted one."""
     import time
     t_setup = time.perf_counter()
     map_every = keyframe_every if map_every is None else map_every
@@ -173,6 +191,8 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     _check_resume(gauss_init, resume, T, checkpoint_every, checkpoint_dir)
     kw = {} if render is None else {"render": render}
     track_m2d = densify_dict is not None
+    kw["lrs"] = dict(cam_unnorm_rots=float(mapping_cam_lrs[0]), cam_trans=float(mapping_cam_lrs[1]))
+    refine = any(v != 0.0 for v in kw["lrs"].values())
     if resume is None:
         dev = gauss_init["means3D"].device
         rots = torch.zeros(1, 4, T, device=dev); rots[:, 0] = 1.0
@@ -199,12 +219,20 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
             return
         from . import formats
         formats.save_checkpoint(checkpoint_dir, t, dict(mapper.g.params, cam_unnorm_rots=rots, cam_trans=trans),
-                                [kf["id"] for kf in keyframes], _run_state(mapper, counts))
+                                [kf["id"] for kf in keyframes],
+                                _run_state(mapper, counts, keyframes if refine else None))
+
+    def refined_cameras():
+        """Refinement: copies of the mapper's cameras after a mapping phase (tracking then works on its own tensors)."""
+        return tuple(mapper.cam[k].detach().clone() for k in M.CAM_KEYS)
 
     for it in range(first_frame_iters):       # the reference maps frame 0 before it tracks frame 1 (splatam.py:777)
         mapper.step([keyframes[0]])
         if prune_dict is not None:
             mapper.prune_gaussians(it, prune_dict, scene_radius)
+    if refine and first_frame_iters > 0:
+        rots, trans = refined_cameras()
+        keyframes[0]["est_w2c"] = _curr_w2c(rots, trans, 0)
     if resume is None:
         checkpoint(0)
     torch.cuda.synchronize(dev) if dev.type == "cuda" else None
@@ -264,6 +292,9 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
             timing["mapping_s"] += time.perf_counter() - t0
             timing["mapping_iters"] += mapping_iters
             counts.append(mapper.g.shapes["means3D"][0])
+            if refine:
+                rots, trans = refined_cameras()
+                cur["est_w2c"] = _curr_w2c(rots, trans, t)
         if t % keyframe_every == 0:
             keyframes.append(cur)
             if checkpoint_dir is not None and checkpoint_every is None:
@@ -280,7 +311,8 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
         from . import formats
         formats.save_params(dict(final, cam_unnorm_rots=rots, cam_trans=trans), checkpoint_dir)
     return dict(rots=rots, trans=trans, psnr=sum(vals) / len(vals), gauss=final, counts=counts,
-                timestep=mapper.timestep.detach().clone(), keyframe_time_indices=[int(kf["id"]) for kf in keyframes])
+                timestep=mapper.timestep.detach().clone(), keyframe_time_indices=[int(kf["id"]) for kf in keyframes],
+                keyframe_est_w2c=[kf["est_w2c"] for kf in keyframes])
 
 
 def w2c_list(rots, trans):

@@ -131,6 +131,9 @@ def main():
                     help="continue from the checkpoint of frame T under --out")
     ap.add_argument("--save-frames", action="store_true",
                     help="save the evaluation's rendered and ground-truth frames under --out")
+    ap.add_argument("--mapping-cam-lrs", type=float, nargs=2, default=(0.0, 0.0), metavar=("ROT", "TRANS"),
+                    help="mapping learning rates of cam_unnorm_rots and cam_trans; non-zero refines each mapping "
+                         "iteration's keyframe pose (the reference's do_ba=True); default 0 0, as every shipped config")
     a = ap.parse_args()
     if (a.lpips_alexnet is None) != (a.lpips_lin is None):
         ap.error("--lpips-alexnet and --lpips-lin go together")
@@ -187,7 +190,8 @@ def main():
                         scene_radius=radius, select_keyframes=True, first_frame_iters=h["mapping_iters"],
                         checkpoint_dir=a.out if a.checkpoint_every else None,
                         checkpoint_every=a.checkpoint_every or None, resume=ckpt,
-                        tracking_lrs=h["tracking_lrs"], depth_loss_thres=h["depth_loss_thres"])
+                        tracking_lrs=h["tracking_lrs"], depth_loss_thres=h["depth_loss_thres"],
+                        mapping_cam_lrs=tuple(a.mapping_cam_lrs))
     torch.cuda.synchronize(dev)
     wall = time.perf_counter() - t0
     # --resume: wall time from reading the checkpoint to the first tracked frame (frame-0 read, load, keyframe rebuild)
@@ -220,6 +224,7 @@ def main():
         dataset=a.dataset, sequence=a.sequence, variant=a.variant, frames=T, width=seq.width, height=seq.height,
         densify_height=seq.densify_height, densify_width=seq.densify_width, hyper=h,
         initial_gaussians=initial_gaussians, resumed_from=a.resume, resume_s=resume_s,
+        mapping_cam_lrs=list(a.mapping_cam_lrs),
         ate_m=res["ate"], psnr_db=res["psnr"], ms_ssim=res["ms_ssim"], depth_l1_m=res["depth_l1"],
         gaussians=int(out["counts"][-1]), wall_s=wall, tracking_s=timing["tracking_s"], mapping_s=timing["mapping_s"],
         load_wait_ms_per_frame=1e3 * load_wait / max(T - 1, 1), evaluated_frames=len(res["frame_ids"]),
