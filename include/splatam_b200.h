@@ -171,6 +171,25 @@ SB_API int sb_forward_async(const sb_settings* s, int P, const float* means3D, c
 SB_API int sb_read_counts(const void* geom_ws, size_t geom_ws_bytes, int P, int* num_rendered, int* overflow,
                           void* stream);
 
+/* ---- blend statistics of a finished render (splatam_b200/contrib.py) -------------------------------------------
+ * Replays the per-pixel walk of the forward that filled the three workspaces (sb_forward / sb_forward_render, or
+ * sb_forward_async with num_rendered := capacity and sync_free = 1), with the forward's own culling, thresholds,
+ * early-outs and float operation order, and ADDS into the caller's per-Gaussian arrays [P] (kept across calls, so
+ * one set gathers many views):
+ *   blended[g]          pixels where g was composited: alpha >= 1/255 and test_T = T (1 - alpha) >= 1e-4
+ *   ended[g]            pixels whose walk g stopped: alpha >= 1/255 and test_T < 1e-4 (g blends nothing there)
+ *   max_weight_bits[g]  atomicMax of the float32 bits of alpha * T over the pixels g blended (weights are >= 0)
+ * Writes no image and leaves the workspaces as they are.  A plain and a two-set render of the same geometry give
+ * the same statistics (the binning workspace of either is accepted).  sync_free = 1: an overflowed render (flag word 2
+ * of the geometry workspace set) adds nothing.  Integer and max atomics only: the result is deterministic.  The
+ * caller keeps the counters from wrapping (at most 2^32 - 1 accumulated pixels).  No host synchronisation.
+ * SB_ERR_BAD_ARG, before any launch, for bad settings, P < 0, num_rendered < 0, a null workspace or array the call
+ * reads; SB_ERR_WORKSPACE for a workspace smaller than its size query gives. */
+SB_API int sb_blend_stats(const sb_settings* s, int P, int num_rendered, int sync_free, const void* geom_ws,
+                          size_t geom_ws_bytes, const void* binning_ws, size_t binning_ws_bytes, const void* image_ws,
+                          size_t image_ws_bytes, uint32_t* blended, uint32_t* ended, uint32_t* max_weight_bits,
+                          void* stream);
+
 /* ---- spherical-harmonics colour branch (shs / sh_degree, X/cuda_rasterizer/forward.cu:20-71,
  *      backward.cu:20-139).  sb_sh_forward turns shs [P,max_coeffs,3] into the rgb [P,3] the render consumes
  *      (plus one clamp-flag byte per Gaussian); sb_sh_backward turns dL/drgb into dL/dshs and ADDS the

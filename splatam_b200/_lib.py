@@ -57,6 +57,7 @@ _SIGNATURES = {
     "sb_read_counts": (_i, [_vp, _sz, _i, ctypes.POINTER(_i), ctypes.POINTER(_i), _vp]),
     "sb_forward_render": (_i, [ctypes.POINTER(SbSettings), _i, _i, _vp, _vp, _vp, _sz, _vp, _sz, _vp, _sz,
                                _vp, _vp, _vp, _vp]),
+    "sb_blend_stats": (_i, [ctypes.POINTER(SbSettings), _i, _i, _i, _vp, _sz, _vp, _sz, _vp, _sz, _vp, _vp, _vp, _vp]),
     "sb_backward": (_i, [ctypes.POINTER(SbSettings), _i, _i, _vp, _vp, _vp, _vp, _vp, _vp,
                          _vp, _sz, _vp, _sz, _vp, _sz, _vp, _sz,
                          _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),

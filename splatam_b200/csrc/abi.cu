@@ -257,6 +257,27 @@ SB_API int sb_forward_render(const sb_settings* s, int P, int num_rendered, cons
     return launch_blend_forward(*s, num_rendered, g, b, img, out_color, out_color2, out_depth, nullptr, st);
 }
 
+SB_API int sb_blend_stats(const sb_settings* s, int P, int num_rendered, int sync_free, const void* geom_ws,
+                          size_t geom_ws_bytes, const void* binning_ws, size_t binning_ws_bytes, const void* image_ws,
+                          size_t image_ws_bytes, uint32_t* blended, uint32_t* ended, uint32_t* max_weight_bits,
+                          void* stream) {
+    if (!settings_ok(s) || P < 0 || num_rendered < 0) return SB_ERR_BAD_ARG;
+    if (P == 0) return SB_OK;
+    if (!geom_ws || !image_ws || !blended || !ended || !max_weight_bits) return SB_ERR_BAD_ARG;
+    if (num_rendered > 0 && !binning_ws) return SB_ERR_BAD_ARG;
+    size_t need = 0;
+    GeometryWs g = carve_geometry(const_cast<void*>(geom_ws), P, &need);
+    if (geom_ws_bytes < need) return SB_ERR_WORKSPACE;
+    // the one-set layout is a prefix of the two-set one, and the walk reads only that prefix
+    BinningWs b = carve_binning(const_cast<void*>(binning_ws), num_rendered, tiles_of(s), 1, &need);
+    if (num_rendered > 0 && binning_ws_bytes < need) return SB_ERR_WORKSPACE;
+    ImageWs img = carve_image(const_cast<void*>(image_ws), s->image_width, s->image_height, &need);
+    if (image_ws_bytes < need) return SB_ERR_WORKSPACE;
+    if (num_rendered == 0) return SB_OK;      // every tile range is empty: nothing blended
+    return launch_blend_stats(*s, b, img, sync_free ? g.header + 2 : nullptr, blended, ended, max_weight_bits,
+                              static_cast<cudaStream_t>(stream));
+}
+
 SB_API int sb_backward(const sb_settings* s, int P, int num_rendered, const float* means3D, const float* colors,
                 const float* scales, const float* rotations, const float* cov3D_precomp, const int32_t* radii,
                 const void* geom_ws, size_t geom_ws_bytes, const void* binning_ws, size_t binning_ws_bytes,

@@ -13,6 +13,11 @@
 //      (dx,dy,power,expf,alpha,test_T,fma accumulate), so colour / final_T / n_contrib are
 //      bit-identical -- culled pairs are precisely pairs the reference skips (alpha < 1/255);
 //   3. a warp whose 32 pixels are all saturated (T < 1e-4) stops evaluating (warp-vote early-out).
+//
+// kStats = true replays the same walk over a finished render's workspaces and writes no image: per Gaussian it counts
+// the (pixel) pairs it blended (alpha >= 1/255, test_T >= 1e-4), the pairs it ended (test_T < 1e-4: it sets `done`),
+// and atomicMax-es the bits of its largest weight alpha * T.  Each survivor step folds its 32 lanes with one ballot
+// per count and one __reduce_max_sync, then one lane issues at most three integer atomics (deterministic).
 #include "common.cuh"
 #include "pipeline.cuh"
 
@@ -37,7 +42,7 @@ struct __align__(128) FwdSmem {
     uint64_t empty[kStages];
 };
 
-template <int NCH, int kMinBlocks>
+template <int NCH, int kMinBlocks, bool kStats = false>
 __global__ void __launch_bounds__(kBlendThreads, kMinBlocks)
 blend_forward_kernel(const uint2* __restrict__ ranges, const float4* __restrict__ recA,
                      const float4* __restrict__ recB, const float4* __restrict__ recC,
@@ -46,8 +51,12 @@ blend_forward_kernel(const uint2* __restrict__ ranges, const float4* __restrict_
                      const float* __restrict__ bg, float* __restrict__ out_color,
                      float* __restrict__ out_color2,
                      float* __restrict__ out_depth, float* __restrict__ final_T,
-                     uint32_t* __restrict__ n_contrib, const int32_t* __restrict__ overflow_flag) {
+                     uint32_t* __restrict__ n_contrib, const int32_t* __restrict__ overflow_flag,
+                     uint32_t* __restrict__ st_blended = nullptr, uint32_t* __restrict__ st_ended = nullptr,
+                     uint32_t* __restrict__ st_max_weight = nullptr) {
     __shared__ FwdSmem<NCH> sm;
+    // an overflowed sync-free render had truncated lists: its statistics add nothing (block-uniform exit)
+    if (kStats && overflow_flag != nullptr && __ldg(overflow_flag) != 0) return;
     const uint32_t tile = blockIdx.x;
     const uint2 range = ranges[tile];
     const int n = (int)(range.y - range.x);
@@ -109,6 +118,8 @@ blend_forward_kernel(const uint2* __restrict__ ranges, const float4* __restrict_
                 while (mask) {
                     const int j = c + (__ffs(mask) - 1);
                     mask &= mask - 1;
+                    bool st_b = false, st_e = false;
+                    uint32_t st_w = 0u;
                     if (!done) {
                         const float4 a = sm.A[s][j];
                         const float4 q = sm.B[s][j];
@@ -121,6 +132,11 @@ blend_forward_kernel(const uint2* __restrict__ ranges, const float4* __restrict_
                                 const float test_T = __fmul_rn(T, __fsub_rn(1.0f, alpha));
                                 if (test_T < 0.0001f) {
                                     done = true;
+                                    if (kStats) st_e = true;
+                                } else if (kStats) {
+                                    st_b = true;
+                                    st_w = __float_as_uint(__fmul_rn(alpha, T));
+                                    T = test_T;
                                 } else {
                                     const float4 col = sm.C[s][j];
                                     C0 = __fmaf_rn(T, __fmul_rn(alpha, col.x), C0);
@@ -140,6 +156,17 @@ blend_forward_kernel(const uint2* __restrict__ ranges, const float4* __restrict_
                             }
                         }
                     }
+                    if (kStats) {
+                        const uint32_t nbl = __popc(__ballot_sync(0xffffffffu, st_b));
+                        const uint32_t nen = __popc(__ballot_sync(0xffffffffu, st_e));
+                        const uint32_t wmax = __reduce_max_sync(0xffffffffu, st_w);
+                        if (lane == 0 && (nbl | nen) != 0u) {
+                            const uint32_t g = __float_as_uint(sm.C[s][j].w);
+                            if (nbl) atomicAdd(st_blended + g, nbl);
+                            if (nen) atomicAdd(st_ended + g, nen);
+                            if (wmax) atomicMax(st_max_weight + g, wmax);
+                        }
+                    }
                 }
                 warp_done = __all_sync(0xffffffffu, done);
             }
@@ -148,7 +175,7 @@ blend_forward_kernel(const uint2* __restrict__ ranges, const float4* __restrict_
         if (lane == 0) mbar_arrive(&sm.empty[s]);
     }
 
-    if (inside) {
+    if (!kStats && inside) {
         const size_t pix = (size_t)py * W + px, hw = (size_t)H * W;
         // sync-free mode: if the scene needed more tile instances than the caller's capacity, the lists are truncated;
         // poison the images so that an incomplete render can never be mistaken for a valid one
@@ -187,6 +214,19 @@ int launch_blend_forward(const sb_settings& s, int R, const GeometryWs& g, const
                                                                       nullptr, out_depth, img.final_T,
                                                                       img.n_contrib, overflow_flag);
     SB_LAUNCH_CHECK("blend_forward_kernel");
+    return SB_OK;
+}
+
+int launch_blend_stats(const sb_settings& s, const BinningWs& b, const ImageWs& img, const int32_t* overflow_flag,
+                       uint32_t* blended, uint32_t* ended, uint32_t* max_weight_bits, cudaStream_t st) {
+    const int W = s.image_width, H = s.image_height;
+    const uint32_t gx = (W + kTile - 1) / kTile, gy = (H + kTile - 1) / kTile;
+    // the walk reads geometry (recA, recB) and the index (recC.w) only, so one instantiation serves both colour sets
+    blend_forward_kernel<3, 5, true><<<gx * gy, kBlendThreads, 0, st>>>(img.ranges, b.recA, b.recB, b.recC, nullptr,
+                                                                        nullptr, W, H, gx, nullptr, nullptr, nullptr,
+                                                                        nullptr, nullptr, nullptr, overflow_flag,
+                                                                        blended, ended, max_weight_bits);
+    SB_LAUNCH_CHECK("blend_forward_kernel<stats>");
     return SB_OK;
 }
 

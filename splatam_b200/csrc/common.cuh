@@ -124,6 +124,10 @@ int launch_finalize_count(int P, const GeometryWs& g, int capacity, cudaStream_t
 int launch_blend_forward(const sb_settings& s, int R, const GeometryWs& g, const BinningWs& b,
                          const ImageWs& img, float* out_color, float* out_color2, float* out_depth,
                          const int32_t* overflow_flag, cudaStream_t st);
+// the blend forward's walk over a finished render, adding per-Gaussian statistics instead of writing images
+// (sb_blend_stats); overflow_flag as for launch_blend_forward
+int launch_blend_stats(const sb_settings& s, const BinningWs& b, const ImageWs& img, const int32_t* overflow_flag,
+                       uint32_t* blended, uint32_t* ended, uint32_t* max_weight_bits, cudaStream_t st);
 int launch_blend_backward(const sb_settings& s, int R, const BinningWs& b, const ImageWs& img,
                           const float* dL_dout_color, const float* dL_dout_color2, float* accum,
                           cudaStream_t st);

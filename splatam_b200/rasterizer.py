@@ -5,6 +5,7 @@ Same names, kwargs, return tuple and error behaviour as
 every stage runs in the hand-written sm_90a kernels behind ``libsplatam_b200.so``; torch is only
 used for device memory, the current stream and autograd bookkeeping.
 """
+import contextlib
 import ctypes
 from typing import NamedTuple
 
@@ -81,6 +82,21 @@ def _settings_pack(rs, device):
 _SIZE_CACHE = {}
 _R_HINT = {}
 _LAST_ASYNC_STATE = {}      # device index -> state of the most recent sync-free forward on that device
+_STATE_SINKS = []           # the lists of the open `forward_states` blocks, innermost last
+
+
+@contextlib.contextmanager
+def forward_states():
+    """Yields a list that collects, in call order, the workspace `_State` of every forward this module runs while the
+    block is open (plain, two-set and sync-free alike), so a caller can read what a render left in its workspaces
+    (e.g. contrib.BlendStats) without changing what the render returns.  A collected state keeps its workspaces
+    alive until the list is dropped."""
+    sink = []
+    _STATE_SINKS.append(sink)
+    try:
+        yield sink
+    finally:
+        _STATE_SINKS.remove(sink)
 
 
 def _sizes(P, W, H, sets):
@@ -107,7 +123,7 @@ def _binning_ws(num_rendered, W, H, sets, device):
 class _State:
     """Scratch kept alive between forward and backward (the reference saves its three byte buffers
     on the autograd ctx, __init__.py:82-84)."""
-    __slots__ = ("geom", "binning", "image", "num_rendered", "settings", "P")
+    __slots__ = ("geom", "binning", "image", "num_rendered", "settings", "P", "sync_free")
 
     def header(self):
         """int32 view [num_rendered, num_visible, overflow flag] of the device-side counters (no synchronisation)."""
@@ -149,6 +165,9 @@ def _forward_impl(means3D, colors_precomp, opacities, scales, rotations, cov3Ds_
     state = _State()
     state.settings = pack
     state.P = P
+    state.sync_free = capacity is not None
+    if _STATE_SINKS:
+        _STATE_SINKS[-1].append(state)
     geom_bytes, img_bytes, _ = _sizes(P, W, H, sets)
     state.geom = _ws(geom_bytes, device)
     state.image = _ws(img_bytes, device)
