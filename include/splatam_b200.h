@@ -220,6 +220,10 @@ SB_API int sb_export_binning(const sb_settings* s, int P, int num_rendered,
                       const void* image_ws, size_t image_ws_bytes,
                       uint64_t* keys, uint32_t* point_list, uint32_t* ranges,
                       float* final_T, uint32_t* n_contrib, void* stream);
+/*   cover [R] u8: per sorted tile instance, bit w set iff the Gaussian can blend a pixel of the 8x4 rectangle
+ *   (16 tx + 8 (w & 1), 16 ty + 4 (w >> 1)) of its tile (tx, ty) -- the only pairs the blend kernels evaluate */
+SB_API int sb_export_cover(const sb_settings* s, int num_rendered, const void* binning_ws, size_t binning_ws_bytes,
+                           uint8_t* cover, void* stream);
 
 /* ---- per-iteration training ops around the rasterizer (SURVEY.md section 8(f) row N3) -----------------
  * sb_adam_step: torch.optim.Adam (no amsgrad / weight decay) over ONE flat parameter buffer whose segments

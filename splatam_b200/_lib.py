@@ -116,6 +116,7 @@ _SIGNATURES = {
     "sb_stage_name": (ctypes.c_char_p, [_i]),
     "sb_export_binning": (_i, [ctypes.POINTER(SbSettings), _i, _i, _vp, _sz, _vp, _sz, _vp, _sz,
                                _vp, _vp, _vp, _vp, _vp, _vp]),
+    "sb_export_cover": (_i, [ctypes.POINTER(SbSettings), _i, _vp, _sz, _vp, _vp]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 

@@ -107,6 +107,10 @@ __global__ void export_keys_kernel(int R, const KeyT* tile_sorted, const uint32_
     if (keys) keys[i] = ((uint64_t)tile_sorted[i] << 32) | (uint64_t)depth_key[g];
     if (list) list[i] = g;
 }
+__global__ void export_cover_kernel(int R, const float4* recA, uint8_t* cover) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < R) cover[i] = (uint8_t)__float_as_uint(recA[i].z);
+}
 
 }  // namespace sb
 
@@ -359,6 +363,19 @@ SB_API int sb_export_binning(const sb_settings* s, int P, int num_rendered, cons
     if (ranges) SB_CUDA_CHECK(cudaMemcpyAsync(ranges, img.ranges, sizeof(uint2) * (size_t)tiles, cudaMemcpyDeviceToDevice, st));
     if (final_T) SB_CUDA_CHECK(cudaMemcpyAsync(final_T, img.final_T, sizeof(float) * hw, cudaMemcpyDeviceToDevice, st));
     if (n_contrib) SB_CUDA_CHECK(cudaMemcpyAsync(n_contrib, img.n_contrib, sizeof(uint32_t) * hw, cudaMemcpyDeviceToDevice, st));
+    return SB_OK;
+}
+
+SB_API int sb_export_cover(const sb_settings* s, int num_rendered, const void* binning_ws, size_t binning_ws_bytes,
+                           uint8_t* cover, void* stream) {
+    if (!settings_ok(s) || num_rendered < 0 || (num_rendered > 0 && !cover)) return SB_ERR_BAD_ARG;
+    if (num_rendered == 0) return SB_OK;
+    size_t need = 0;
+    BinningWs b = carve_binning(const_cast<void*>(binning_ws), num_rendered, tiles_of(s), 1, &need);
+    if (!binning_ws || binning_ws_bytes < need) return SB_ERR_WORKSPACE;
+    export_cover_kernel<<<(num_rendered + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(num_rendered,
+                                                                                                  b.recA, cover);
+    SB_LAUNCH_CHECK("export_cover_kernel");
     return SB_OK;
 }
 

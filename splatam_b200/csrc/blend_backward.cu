@@ -7,10 +7,11 @@
 // ring (as blend_forward.cu); 8 autonomous consumer warps own one 8x4 pixel rectangle each.  The reference
 // issues 9 global float atomics per contributing (pixel, Gaussian) pair (backward.cu:523-554) from a loop
 // in which, on SplaTAM-sized splats, only ~10 of a warp's 32 pixels lie inside any one Gaussian.  Here the
-// work of a warp is split by what it depends on, over a WINDOW of KW box-culled survivors at a time:
+// work of a warp is split by what it depends on, over a WINDOW of KW mask-culled survivors at a time:
 //
-//   gather   (lane = record)  : ballot-cull 32 staged records against the warp's rectangle with the
-//                               projection kernel's conservative boxes, compact survivors into the window;
+//   gather   (lane = record)  : ballot-cull 32 staged records with their coverage bit for the warp's rectangle
+//                               (recA.z, binning.cu's conservative ellipse-vs-rectangle test), compact survivors
+//                               into the window;
 //   evaluate (lane = pixel, lock-step over the window's slots): the part that needs no running state --
 //                               G = exp(power), opacity*G, the skip decisions with the forward's exact float
 //                               sequence, and c.dL/dpixel -- parked in a [slot][pixel] matrix in shared
@@ -301,7 +302,7 @@ blend_backward_kernel(const uint2* __restrict__ ranges, const float4* __restrict
     }
 
     const float pxf = (float)px, pyf = (float)py;
-    const float fx0 = (float)x0, fx1 = (float)(x0 + 7), fy0 = (float)y0, fy1 = (float)(y0 + 3);
+    const float fx0 = (float)x0, fy0 = (float)y0;
     const float bg0 = __ldg(bg), bg1 = __ldg(bg + 1), bg2 = __ldg(bg + 2);
     const float bg_dot1 = bg0 * dLa.x + bg1 * dLa.y + bg2 * dLa.z;
     const float bg_dot = NCH == 6 ? bg_dot1 + (bg0 * dLb.x + bg1 * dLb.y + bg2 * dLb.z) : bg_dot1;
@@ -318,17 +319,14 @@ blend_backward_kernel(const uint2* __restrict__ ranges, const float4* __restrict
         if (lo < (int)warp_nc) {
             for (int c = 0; c < cnt; c += 32) {
                 const int jl = cnt - 1 - (c + lane);       // ascending lane = descending list index
-                bool hit = false;
-                float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (jl >= 0 && lo + jl < (int)warp_nc) {
-                    a = sm.A[s][jl];
-                    hit = (a.x + a.z >= fx0) && (a.x - a.z <= fx1) && (a.y + a.w >= fy0) && (a.y - a.w <= fy1);
-                }
+                bool hit = jl >= 0 && lo + jl < (int)warp_nc &&
+                           ((__float_as_uint(sm.A[s][jl].z) >> warp) & 1u) != 0u;   // coverage bit of this warp
                 uint32_t mask = __ballot_sync(full, hit);
                 while (mask != 0u) {
                     const int pos = wcount + __popc(mask & lt_mask);
                     const bool take = hit && pos < KW;
                     if (take) {
+                        const float4 a = sm.A[s][jl];
                         sm.WA[warp][pos] = make_float4(a.x, a.y, __uint_as_float((uint32_t)(lo + jl)), 0.f);
                         sm.WB[warp][pos] = sm.B[s][jl];
                         sm.WC[warp][pos] = sm.C[s][jl];

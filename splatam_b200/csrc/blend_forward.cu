@@ -7,8 +7,9 @@
 // (recA/recB/recC, 16 B each) into a 4-stage shared-memory ring with cp.async.bulk + mbarrier
 // complete_tx.  Warps 0-7 each own an 8x4 pixel sub-rectangle and consume the ring independently
 // (no __syncthreads in the loop):
-//   1. each lane tests ONE staged Gaussian's conservative contributing box {x+-hx, y+-hy} against the
-//      warp's pixel rectangle; __ballot_sync gives the survivors of 32 Gaussians at once;
+//   1. each lane reads ONE staged record's coverage bit for the warp's pixel rectangle (recA.z, computed once per
+//      tile instance by binning.cu from the conservative ellipse-vs-rectangle test); __ballot_sync gives the
+//      survivors of 32 Gaussians at once;
 //   2. only survivors are evaluated per pixel, with exactly the reference's float operation order
 //      (dx,dy,power,expf,alpha,test_T,fma accumulate), so colour / final_T / n_contrib are
 //      bit-identical -- culled pairs are precisely pairs the reference skips (alpha < 1/255);
@@ -94,7 +95,7 @@ blend_forward_kernel(const uint2* __restrict__ ranges, const float4* __restrict_
     const int px = x0 + (lane & 7), py = y0 + (lane >> 3);
     const bool inside = px < W && py < H;
     const float pxf = (float)px, pyf = (float)py;
-    const float fx0 = (float)x0, fx1 = (float)(x0 + 7), fy0 = (float)y0, fy1 = (float)(y0 + 3);
+    const uint32_t wbit = 1u << warp;   // this warp's bit of the records' coverage masks
 
     float T = 1.0f, C0 = 0.f, C1 = 0.f, C2 = 0.f, E0 = 0.f, E1 = 0.f, E2 = 0.f;
     float D = 15.0f;  // median depth default (forward.cu:308)
@@ -109,11 +110,7 @@ blend_forward_kernel(const uint2* __restrict__ ranges, const float4* __restrict_
             const int cnt = min(kBatch, n - k * kBatch);
             for (int c = 0; c < cnt && !warp_done; c += 32) {
                 const int jl = c + lane;
-                bool hit = false;
-                if (jl < cnt) {
-                    const float4 a = sm.A[s][jl];
-                    hit = (a.x + a.z >= fx0) && (a.x - a.z <= fx1) && (a.y + a.w >= fy0) && (a.y - a.w <= fy1);
-                }
+                const bool hit = jl < cnt && (__float_as_uint(sm.A[s][jl].z) & wbit) != 0u;
                 uint32_t mask = __ballot_sync(0xffffffffu, hit);
                 while (mask) {
                     const int j = c + (__ffs(mask) - 1);

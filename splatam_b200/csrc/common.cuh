@@ -71,7 +71,9 @@ GeometryWs carve_geometry(void* ws, int P, size_t* total);
 
 // ---- per-instance state (R = num_rendered tile instances) -------------------------------
 // Sorted SoA splat records staged by TMA into shared memory, 16 B each per array:
-// recA = geomA of the instance's Gaussian, recB = geomB, recC = {r, g, b, bits(index)}.
+// recA = {pixel x, pixel y, bits(coverage mask), 0}: bit w of the mask is set iff the Gaussian can blend a pixel of
+// blend-kernel warp w's 8x4 rectangle of the instance's tile (binning.cu, cover_mask);
+// recB = geomB, recC = {r, g, b, bits(index)}.
 struct BinningWs {
     uint32_t* tile_unsorted; // [R] tile id per instance, (depth,index) order
     uint32_t* val_unsorted;  // [R] Gaussian index per instance

@@ -13,6 +13,9 @@ the same conservative cull boxes as csrc/project.cu and counts what the instruct
       - "exact" : an exact ellipse-vs-rectangle test instead of the bounding box (upper bound on what better culling buys)
       - "4x8"   : 4-wide x 8-tall rectangles instead of 8x4 (isotropic splats: same)
 
+`cover_masks` restates csrc/binning.cu's per-instance coverage masks, which the shipped kernels cull with; the
+tests/test_cover_mask_*.py suites check the device masks and the per-pixel alpha test against it.
+
 Run:  python tools/lane_packing_model.py [--tiles 150] [--gaussians 1000000]
 """
 import argparse
@@ -44,6 +47,67 @@ def cull_half_extents(conic, opacity, radius):
     hx[ok & ~good] = 1e30
     hy[ok & ~good] = 1e30
     return hx, hy
+
+
+def cull_half_extents_f32(conic, opacity, radius):
+    """hx, hy as csrc/project.cu stores them: rounded to float32, anything not below 1e30 clamped to 1e30."""
+    with np.errstate(over="ignore", invalid="ignore"):
+        out = [h.astype(np.float32) for h in cull_half_extents(conic, opacity, radius)]
+    return [np.where(h < np.float32(1e30), h, np.float32(1e30)) for h in out]
+
+
+def cover_masks(xy, conic, hx, hy, tile, grid_x, near_rel=1e-6):
+    """Per tile instance, the 8-bit coverage mask of csrc/binning.cu (cover_mask), restated in numpy with the same
+    float32 box comparisons and the same float64 operations in the same order: bit w stands for the blend kernels'
+    warp w, pixel centres x0..x0+7 by y0..y0+3 with x0 = 16 tx + 8 (w & 1), y0 = 16 ty + 4 (w >> 1).
+
+    xy [n,2] and conic [n,3] float32 as the projection stores them, hx, hy [n] float32 (cull_half_extents_f32), tile [n]
+    tile ids.  Returns (mask, box, near), uint8 [n] each: the coverage mask; the box test alone, of which the mask is a
+    subset; and the bits whose decision lies within a relative `near_rel` of a threshold (where a last-ulp difference
+    in hx, hy between this model and the device can flip the bit)."""
+    xy = np.asarray(xy, np.float32)
+    gx32, gy32 = xy[:, 0], xy[:, 1]
+    hx32, hy32 = np.asarray(hx, np.float32), np.asarray(hy, np.float32)
+    gx, gy = gx32.astype(np.float64), gy32.astype(np.float64)
+    a, b, c = (np.asarray(conic[:, k], np.float32).astype(np.float64) for k in range(3))
+    hx64, hy64 = hx32.astype(np.float64), hy32.astype(np.float64)
+    tile = np.asarray(tile, np.int64)
+    tx, ty = tile % grid_x, tile // grid_x
+    dc = a * c - b * b
+    thr_x, thr_y = dc * (hx64 * hx64), dc * (hy64 * hy64)
+    culled = ~(hx32 > 0)
+    skip = (hx32 >= np.float32(1e30)) | (hy32 >= np.float32(1e30))
+    mask, box_all, near = (np.zeros(tile.shape, np.uint8) for _ in range(3))
+
+    def close(x, y):
+        return np.abs(x - y) <= near_rel * np.maximum(np.abs(x), np.abs(y))
+
+    with np.errstate(invalid="ignore", over="ignore"):
+        for w in range(8):
+            x0, y0 = tx * 16 + (w & 1) * 8, ty * 16 + (w >> 1) * 4
+            fx0, fx1, fy0, fy1 = (v.astype(np.float32) for v in (x0, x0 + 7, y0, y0 + 3))
+            lx, rx, ly, ry = gx32 + hx32, gx32 - hx32, gy32 + hy32, gy32 - hy32
+            box = (lx >= fx0) & (rx <= fx1) & (ly >= fy0) & (ry <= fy1)
+            box_near = (close(lx, fx0) | close(rx, fx1) | close(ly, fy0) | close(ry, fy1))
+            u0, u1 = gx - (x0 + 7.0), gx - x0
+            v0, v1 = gy - (y0 + 3.0), gy - y0
+            inside = (u0 <= 0) & (u1 >= 0) & (v0 <= 0) & (v1 >= 0)
+            hv, hu = (v0 > 0) | (v1 < 0), (u0 > 0) | (u1 < 0)
+            v = np.where(v0 > 0, v0, v1)
+            bv = b * v
+            d = np.maximum(np.maximum(a * u0 + bv, -(a * u1 + bv)), 0.0)
+            sh = d * d + dc * v * v
+            u = np.where(u0 > 0, u0, u1)
+            bu = b * u
+            d = np.maximum(np.maximum(c * v0 + bu, -(c * v1 + bu)), 0.0)
+            sv = d * d + dc * u * u
+            ell = inside | (hv & (sh <= thr_y)) | (hu & (sv <= thr_x))
+            ell_near = (hv & close(sh, thr_y)) | (hu & close(sv, thr_x))
+            bit = box & ~culled & (skip | ell)
+            mask |= bit.astype(np.uint8) << w
+            box_all |= box.astype(np.uint8) << w
+            near |= ((box_near | (box & ~skip & ell_near)) & ~culled).astype(np.uint8) << w
+    return mask, box_all, near
 
 
 def main():
