@@ -57,6 +57,16 @@ class Scene:
         out["means2D"] = torch.zeros_like(out["means3D"], requires_grad=requires_grad)
         return out
 
+    def splatam_params(self, device=None, opacity_clamp=(0.02, 0.98), isotropic=True):
+        """The scene as SplaTAM's five-tensor map (pre-activation opacities and log scales). Opacities are clamped
+        into `opacity_clamp` (None: not clamped) so that their logits stay finite; `isotropic` keeps the first
+        scale column only, as SplaTAM's isotropic Gaussians do."""
+        op = self.opacities if opacity_clamp is None else self.opacities.clamp(*opacity_clamp)
+        scales = self.scales[:, :1] if isotropic else self.scales
+        d = dict(means3D=self.means3D, rgb_colors=self.colors, unnorm_rotations=self.rotations,
+                 logit_opacities=torch.logit(op), log_scales=torch.log(scales))
+        return d if device is None else {k: v.to(device) for k, v in d.items()}
+
     def oracle_cam(self):
         from oracle import oracle as O
         return O.make_cam(self.w, self.h, self.tanfovx, self.tanfovy, self.bg.numpy(), self.view.numpy().reshape(-1),

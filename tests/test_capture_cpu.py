@@ -4,7 +4,6 @@ make_golden_capture.py); the uint8 / float32 / uint16 rules of oracle/capture_nu
 packet validation; argument checks of sb_ingest_capture and sb_capture_depth_u16; the DDS adapter against a stand-in
 cyclonedds module (no socket is opened)."""
 import hashlib
-import importlib.util
 import os
 import sys
 import types
@@ -13,24 +12,16 @@ import numpy as np
 import pytest
 import torch
 
-from util import GOLDEN
+from util import GOLDEN, bits_equal, load
 from oracle import capture_numpy as N, ingest_numpy
 from splatam_b200 import _lib, capture as C, datasets as D
 
 FIX = os.path.join(GOLDEN, "capture", "ref_capture.npz")
 
 
-def _generator():
-    spec = importlib.util.spec_from_file_location("make_golden_capture",
-                                                  os.path.join(GOLDEN, "capture", "make_golden_capture.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
 @pytest.fixture(scope="module")
 def gen():
-    return _generator()
+    return load("tests/golden/capture/make_golden_capture.py")
 
 
 @pytest.fixture(scope="module")
@@ -57,11 +48,6 @@ def root(fx, tmp_path_factory):
 
 def frames_of(gen):
     return [C.sample_to_frame(s) for s in gen.make_packets()]
-
-
-def bits_equal(a, b):
-    a, b = np.asarray(a), np.asarray(b)
-    return a.shape == b.shape and a.dtype == b.dtype and a.tobytes() == b.tobytes()
 
 
 # ---- the numpy restatement against cv2 and NumPy ---------------------------------------------------------------------

@@ -3,7 +3,6 @@ CaptureWriter (splatam_b200/capture.py) and the NeRFCapture reader (datasets.py)
 code (tests/golden/capture/ref_capture.npz) and cv2's digests on a full-size packet, bit for bit; and a short synthetic
 online run whose capture the reader re-reads and whose params.npz formats and the viewer open."""
 import hashlib
-import importlib.util
 import json
 import os
 import sys
@@ -12,7 +11,7 @@ import numpy as np
 import pytest
 import torch
 
-from util import GOLDEN, ROOT
+from util import GOLDEN, ROOT, bits_equal, load
 from oracle import capture_numpy as N
 from splatam_b200 import capture as C, datasets as D
 
@@ -21,27 +20,14 @@ pytestmark = pytest.mark.gpu
 FIX = os.path.join(GOLDEN, "capture", "ref_capture.npz")
 
 
-def _generator():
-    spec = importlib.util.spec_from_file_location("make_golden_capture",
-                                                  os.path.join(GOLDEN, "capture", "make_golden_capture.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
 @pytest.fixture(scope="module")
 def gen():
-    return _generator()
+    return load("tests/golden/capture/make_golden_capture.py")
 
 
 @pytest.fixture(scope="module")
 def fx():
     return dict(np.load(FIX))
-
-
-def bits_equal(a, b):
-    a, b = np.asarray(a), np.asarray(b)
-    return a.shape == b.shape and a.dtype == b.dtype and a.tobytes() == b.tobytes()
 
 
 def test_full_size_packet_matches_cv2_digests(gen, fx, cuda_device):

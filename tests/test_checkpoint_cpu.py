@@ -2,7 +2,6 @@
 `timestep` of the mapper's torch path, with the float32 brute-force composite from oracle/ standing in for the
 rasterizer.  That renderer and the torch path are deterministic, so a resumed run must equal the uninterrupted one
 bit for bit.  The GPU runs are tests/test_checkpoint_gpu.py."""
-import importlib.util
 import os
 import shutil
 import sys
@@ -14,10 +13,9 @@ import torch.nn.functional as F
 
 import refsrc
 import scenes
-from oracle import bruteforce_torch as BF
+from util import cpu_render, load
 from splatam_b200 import formats, mapping as M, slam
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 T = 8
 # three mapping iterations per mapped frame: densification accumulates in iterations 0 and 1 and edits the map in
 # iteration 0, pruning runs from iteration 2 -- never both in one iteration, where densify would index the step's
@@ -33,28 +31,19 @@ REF_RECORD = dict(means3D=np.float32, rgb_colors=np.float32, unnorm_rotations=np
                   gt_w2c_all_frames=np.float32, keyframe_time_indices=np.int64)
 
 
-def _cpu_render(settings, means3D, means2D, opacities, colors_precomp, scales, rotations):
-    out = BF.render(means3D, colors_precomp, opacities, scales, rotations, width=settings.image_width,
-                    height=settings.image_height, tanfovx=settings.tanfovx, tanfovy=settings.tanfovy, bg=settings.bg,
-                    viewmatrix=settings.viewmatrix[0], projmatrix=settings.projmatrix[0], means2D=means2D,
-                    dtype=torch.float32)
-    return out["color"], out["radii"], out["depth"]
-
-
 @pytest.fixture(scope="module")
 def problem():
     import splatam_b200 as S
     torch.set_num_threads(4)
     sc = scenes.config1(seed=8, P=160, w=48, h=32)
     cam = sc.settings(S.GaussianRasterizationSettings, "cpu")
-    gt = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-              logit_opacities=torch.logit(sc.opacities.clamp(0.05, 0.95)), log_scales=torch.log(sc.scales[:, :1]))
+    gt = sc.splatam_params(opacity_clamp=(0.05, 0.95))
     rots, trans = slam.look_trajectory(T, "cpu", step=(0.004, -0.002, 0.003), rot_step=(0.001, -0.001, 0.0005))
-    frames = [slam.render_frame(gt, rots, trans, t, cam, render=_cpu_render) for t in range(T)]
+    frames = [slam.render_frame(gt, rots, trans, t, cam, render=cpu_render) for t in range(T)]
     K = torch.tensor([[sc.fx, 0, sc.cx], [0, sc.fy, sc.cy], [0, 0, 1]])
     init = dict(gt)
     init["rgb_colors"] = (gt["rgb_colors"] + 0.2).clamp(0, 1)          # a wrong map: densification has gradients
-    kw = dict(render=_cpu_render, fused=False, tracking_iters=3, mapping_iters=3, keyframe_every=2, window=3,
+    kw = dict(render=cpu_render, fused=False, tracking_iters=3, mapping_iters=3, keyframe_every=2, window=3,
               intrinsics=K, prune_dict=PRUNE, densify_dict=DENSIFY, scene_radius=0.5, select_keyframes=True)
     return cam, frames, init, kw
 
@@ -191,9 +180,7 @@ def _final_recon():
     sys.modules["diff_gaussian_rasterization"] = pkg
     path_before = list(sys.path)
     try:
-        spec = importlib.util.spec_from_file_location("_ref_final_recon", path)
-        mod = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(mod)
+        mod = load(path)
     finally:
         sys.path[:] = path_before
         for k in [k for k in sys.modules if owned(k)]:
@@ -239,9 +226,7 @@ def test_argument_checks(problem, full_run, tmp_path):
 
 
 def test_tool_needs_out_for_checkpoints(monkeypatch, capsys):
-    spec = importlib.util.spec_from_file_location("run_slam_dataset", os.path.join(ROOT, "tools", "run_slam_dataset.py"))
-    tool = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(tool)
+    tool = load("tools/run_slam_dataset.py")
     for extra in (["--checkpoint-every", "5"], ["--resume", "10"]):
         monkeypatch.setattr(sys, "argv", ["run_slam_dataset.py", "--dataset", "replica", "--basedir", "x",
                                           "--sequence", "y"] + extra)
@@ -255,7 +240,7 @@ def _mapper(P=24, seed=0):
     gauss = dict(means3D=torch.randn(P, 3, generator=g), rgb_colors=torch.rand(P, 3, generator=g),
                  unnorm_rotations=torch.randn(P, 4, generator=g), logit_opacities=torch.randn(P, 1, generator=g),
                  log_scales=torch.randn(P, 1, generator=g) - 3.0)
-    return M.ShardedMapper(gauss, torch.zeros(1, 4, 2), torch.zeros(1, 3, 2), render=_cpu_render, fused=False), gauss
+    return M.ShardedMapper(gauss, torch.zeros(1, 4, 2), torch.zeros(1, 3, 2), render=cpu_render, fused=False), gauss
 
 
 def test_mapper_timestep_follows_the_map_edits():

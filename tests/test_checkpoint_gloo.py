@@ -10,7 +10,7 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 import scenes
-from oracle import bruteforce_torch as BF
+from util import cpu_render
 from splatam_b200 import formats, slam
 
 T = 6
@@ -21,26 +21,17 @@ DENSIFY = dict(start_after=0, remove_big_after=0, stop_after=1, densify_every=2,
                reset_opacities_every=100)
 
 
-def _cpu_render(settings, means3D, means2D, opacities, colors_precomp, scales, rotations):
-    out = BF.render(means3D, colors_precomp, opacities, scales, rotations, width=settings.image_width,
-                    height=settings.image_height, tanfovx=settings.tanfovx, tanfovy=settings.tanfovy, bg=settings.bg,
-                    viewmatrix=settings.viewmatrix[0], projmatrix=settings.projmatrix[0], means2D=means2D,
-                    dtype=torch.float32)
-    return out["color"], out["radii"], out["depth"]
-
-
 def _problem():
     import splatam_b200 as S
     sc = scenes.config1(seed=8, P=120, w=48, h=32)
     cam = sc.settings(S.GaussianRasterizationSettings, "cpu")
-    gt = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-              logit_opacities=torch.logit(sc.opacities.clamp(0.05, 0.95)), log_scales=torch.log(sc.scales[:, :1]))
+    gt = sc.splatam_params(opacity_clamp=(0.05, 0.95))
     rots, trans = slam.look_trajectory(T, "cpu", step=(0.004, -0.002, 0.003), rot_step=(0.001, -0.001, 0.0005))
-    frames = [slam.render_frame(gt, rots, trans, t, cam, render=_cpu_render) for t in range(T)]
+    frames = [slam.render_frame(gt, rots, trans, t, cam, render=cpu_render) for t in range(T)]
     K = torch.tensor([[sc.fx, 0, sc.cx], [0, sc.fy, sc.cy], [0, 0, 1]])
     init = dict(gt)
     init["rgb_colors"] = (gt["rgb_colors"] + 0.2).clamp(0, 1)
-    kw = dict(render=_cpu_render, fused=False, tracking_iters=2, mapping_iters=3, keyframe_every=2, window=4,
+    kw = dict(render=cpu_render, fused=False, tracking_iters=2, mapping_iters=3, keyframe_every=2, window=4,
               intrinsics=K, prune_dict=PRUNE, densify_dict=DENSIFY, scene_radius=0.5, select_keyframes=True, seed=3)
     return cam, frames, init, kw
 

@@ -1,21 +1,18 @@
 """GPU: the per-Gaussian `timestep` through the fused map edits, end to end through the SLAM loop, checkpoint / resume
 on the fused path (eager and graph), and the dataset tool's --checkpoint-every / --resume.  Two GPU runs are not
 bit-equal (the backward uses float atomics), so resumed runs are held to test_slam_gpu.py's bounds between two arms."""
-import importlib.util
-import json
 import os
-import sys
 
 import numpy as np
 import pytest
 import torch
 
 import scenes
+from util import load, run_tool
 from test_slam_gpu import _opaque_sequence
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 K = torch.tensor([[160.0, 0, 159.5], [0, 160.0, 95.5], [0, 0, 1]])
 PRUNE = dict(start_after=0, remove_big_after=0, stop_after=20, prune_every=4, removal_opacity_threshold=0.005,
              final_removal_opacity_threshold=0.005, reset_opacities=False, reset_opacities_every=500)
@@ -142,25 +139,16 @@ def test_resume_on_the_gpu(cuda_device, tmp_path, monkeypatch):
         assert abs(ate - ate_full) < 0.01 * travelled
 
 
-def _tool():
-    spec = importlib.util.spec_from_file_location("run_slam_dataset", os.path.join(ROOT, "tools", "run_slam_dataset.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
 def test_tool_checkpoints_and_resumes(cuda_device, tmp_path, monkeypatch, capsys):
     T = 12
     scenes.write_replica_sequence(str(tmp_path / "room0"), T, cuda_device)
-    tool = _tool()
+    tool = load("tools/run_slam_dataset.py")
     out_dir = str(tmp_path / "run")
     base = ["run_slam_dataset.py", "--dataset", "replica", "--basedir", str(tmp_path), "--sequence", "room0",
             "--tracking-iters", "10", "--mapping-iters", "10", "--out", out_dir]
     lines = []
     for extra in (["--checkpoint-every", "5"], ["--resume", "10"]):
-        monkeypatch.setattr(sys, "argv", base + extra)
-        tool.main()
-        lines.append(json.loads(capsys.readouterr().out.strip().splitlines()[-1]))
+        lines.append(run_tool(tool, base + extra, monkeypatch, capsys))
         with np.load(os.path.join(out_dir, "params.npz")) as z:
             rec = {k: z[k] for k in z.files}
         if extra[0] == "--checkpoint-every":

@@ -2,8 +2,6 @@
 oracle/blend_stats_numpy.py): the entry point's argument checks, the counter guard, the keep rule, record handling
 around the compaction kernels, the tool's arguments, and the oracle's statistics on hand-checkable stacks."""
 import ctypes
-import importlib.util
-import os
 import types
 
 import numpy as np
@@ -11,16 +9,8 @@ import pytest
 import torch
 
 import scenes
+from util import load
 from splatam_b200 import _lib, contrib, formats
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _tool():
-    spec = importlib.util.spec_from_file_location("compact_record", os.path.join(ROOT, "tools", "compact_record.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def test_blend_stats_is_exported():
@@ -158,7 +148,7 @@ def test_checkpoint_and_in_place_output_are_rejected(tmp_path):
 
 
 def test_tool_arguments(tmp_path):
-    tool = _tool()
+    tool = load("tools/compact_record.py")
     rec = str(tmp_path / "params.npz")
     np.savez(rec, **_synthetic_record())
     a = tool.parse_args(["--record", rec, "--out", str(tmp_path / "c.npz")])

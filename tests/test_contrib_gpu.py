@@ -1,19 +1,17 @@
 """GPU suite for map compaction (splatam_b200/contrib.py, sb_blend_stats): the statistics against the numpy oracle
 (oracle/blend_stats_numpy.py), determinism, bit-identical re-renders of the lossless compaction, and the tool end to
 end on a SplaTAM run record."""
-import importlib.util
 import json
 import os
-import sys
 
 import numpy as np
 import pytest
 import torch
 
 import scenes
+from util import load, run_tool
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _scenes():
@@ -85,8 +83,7 @@ def _map(sc, T, dev):
     """A SplaTAM map of `sc` with T cameras along slam.look_trajectory (frame 0 the identity)."""
     from splatam_b200 import slam
     rots, trans = slam.look_trajectory(T, dev)
-    g = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-             logit_opacities=torch.logit(sc.opacities.clamp(1e-4, 1 - 1e-4)), log_scales=torch.log(sc.scales[:, :1]))
+    g = sc.splatam_params(opacity_clamp=(1e-4, 1 - 1e-4))
     p = {k: v.to(dev).contiguous() for k, v in g.items()}
     p.update(cam_unnorm_rots=rots, cam_trans=trans)
     return p, sc.settings(__import__("splatam_b200").GaussianRasterizationSettings, dev), torch.eye(4, device=dev)
@@ -156,33 +153,20 @@ def test_lossless_compaction_renders_bit_identically(cuda_device, scene):
         assert not _same(ref, _renders(_drop(params, keep & ~end_only), cam, w2c0, ids))
 
 
-def _load(path, name):
-    spec = importlib.util.spec_from_file_location(name, path)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-def _run(tool, argv, monkeypatch, capsys):
-    monkeypatch.setattr(sys, "argv", argv)
-    tool.main()
-    return json.loads(capsys.readouterr().out.strip().splitlines()[-1])
-
-
 def test_compact_record_end_to_end(cuda_device, tmp_path, monkeypatch, capsys):
     from splatam_b200 import contrib, datasets, formats, offline, viewer
     T = 6
     scenes.write_replica_sequence(str(tmp_path / "room0"), T, cuda_device)
     data = ["--dataset", "replica", "--basedir", str(tmp_path), "--sequence", "room0"]
     run_dir = str(tmp_path / "run")
-    _run(_load(os.path.join(ROOT, "tools", "run_slam_dataset.py"), "run_slam_dataset"),
-         ["run_slam_dataset.py"] + data + ["--tracking-iters", "10", "--mapping-iters", "10", "--out", run_dir],
-         monkeypatch, capsys)
+    run_tool(load("tools/run_slam_dataset.py"),
+             ["run_slam_dataset.py"] + data + ["--tracking-iters", "10", "--mapping-iters", "10", "--out", run_dir],
+             monkeypatch, capsys)
     src = os.path.join(run_dir, "params.npz")
     before = open(src, "rb").read()
     dst = str(tmp_path / "compact.npz")
-    tool = _load(os.path.join(ROOT, "tools", "compact_record.py"), "compact_record")
-    line = _run(tool, ["compact_record.py", "--record", src, "--out", dst, "--every", "1"], monkeypatch, capsys)
+    tool = load("tools/compact_record.py")
+    line = run_tool(tool, ["compact_record.py", "--record", src, "--out", dst, "--every", "1"], monkeypatch, capsys)
     assert open(src, "rb").read() == before
     assert line["views"] == T and (line["width"], line["height"]) == (1200, 680)
     assert 0 < line["gaussians_after"] <= line["gaussians_before"]
@@ -193,11 +177,11 @@ def test_compact_record_end_to_end(cuda_device, tmp_path, monkeypatch, capsys):
         assert a[k].dtype == b[k].dtype, k
         if k not in contrib.PER_GAUSSIAN_KEYS:
             assert a[k].tobytes() == b[k].tobytes(), k
-    ev = _load(os.path.join(ROOT, "tools", "eval_record.py"), "eval_record")
+    ev = load("tools/eval_record.py")
     per = []
     for rec, out in ((src, "eval_a"), (dst, "eval_b")):
-        _run(ev, ["eval_record.py"] + data + ["--record", rec, "--out", str(tmp_path / out), "--no-frames",
-                                              "--frames", str(T)], monkeypatch, capsys)
+        run_tool(ev, ["eval_record.py"] + data + ["--record", rec, "--out", str(tmp_path / out), "--no-frames",
+                                                  "--frames", str(T)], monkeypatch, capsys)
         per.append({n: open(str(tmp_path / out / (n + ".txt"))).read() for n in ("psnr", "l1", "rmse", "ssim")})
     assert per[0] == per[1]                                  # per-frame PSNR, depth errors and MS-SSIM, bit for bit
     formats.export_ply(dst, str(tmp_path / "c.ply"))
@@ -211,8 +195,8 @@ def test_compact_record_end_to_end(cuda_device, tmp_path, monkeypatch, capsys):
             assert torch.equal(getattr(cam, f), getattr(seq.cam, f).to(cuda_device)), f
         frames = [seq[t] for t in range(T)]
         offline.from_record(dst, frames, list(range(T)), cuda_device)
-    lossy = _run(tool, ["compact_record.py", "--record", src, "--out", str(tmp_path / "lossy.npz"), "--every", "1",
-                        "--min-weight", "0.05"], monkeypatch, capsys)
+    lossy = run_tool(tool, ["compact_record.py", "--record", src, "--out", str(tmp_path / "lossy.npz"), "--every", "1",
+                            "--min-weight", "0.05"], monkeypatch, capsys)
     print("compact_record --min-weight 0.05:", json.dumps(lossy))
     assert lossy["gaussians_after"] <= line["gaussians_after"] and np.isfinite(lossy["psnr_db"])
     assert np.isfinite(lossy["depth_l1_m"])

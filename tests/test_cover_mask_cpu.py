@@ -2,19 +2,13 @@
 their numpy restatement in tools/lane_packing_model.py: on the C oracle's geometry and binning, no (warp, Gaussian) pair
 with a pixel that passes the kernels' float32 alpha test may have its bit cleared, and every mask is a subset of the
 projection kernel's box test.  The forward's bit-equality on the GPU depends on the first property."""
-import importlib.util
-import os
-
 import numpy as np
 import pytest
 
 import scenes
+from util import load
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_spec = importlib.util.spec_from_file_location("lane_packing_model",
-                                               os.path.join(ROOT, "tools", "lane_packing_model.py"))
-M = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(M)
+M = load("tools/lane_packing_model.py")
 
 
 def blended_pairs(xy, co, tile, grid_x, W, H):

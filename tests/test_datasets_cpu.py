@@ -3,58 +3,21 @@ kernel (oracle/ingest_numpy.py) against the reference's own dataset classes, run
 TUM and ScanNet sequences (tests/golden/datasets/ref_datasets.npz, written by make_golden_datasets.py): file discovery
 and natural order, start / end / stride, TUM's association and 1/32 s subsampling, poses and intrinsics bit for bit,
 colour and depth bit for bit; argument checks of sb_ingest_rgbd; no CPU fallback."""
-import importlib.util
 import os
 
 import numpy as np
 import pytest
 import torch
 
-from util import GOLDEN
+from dataset_fixtures import files_of, sequence_fixtures
+from util import GOLDEN, bits_equal
 from splatam_b200 import _lib
 from splatam_b200 import datasets as D
 
 FIX = os.path.join(GOLDEN, "datasets", "ref_datasets.npz")
 
 
-def _generator():
-    spec = importlib.util.spec_from_file_location("make_golden_datasets",
-                                                  os.path.join(GOLDEN, "datasets", "make_golden_datasets.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-@pytest.fixture(scope="module")
-def gen():
-    return _generator()
-
-
-@pytest.fixture(scope="module")
-def fx():
-    return dict(np.load(FIX))
-
-
-@pytest.fixture(scope="module")
-def root(gen, fx, tmp_path_factory):
-    d = str(tmp_path_factory.mktemp("sequences"))
-    gen.write_sequences(d, fx)
-    return d
-
-
-def files_of(gen, root, read):
-    dataset, kw = gen.READS[read]
-    return D.SequenceFiles(dataset, os.path.join(root, dataset), gen.SEQUENCES[dataset], gen.config(dataset), **kw)
-
-
-def bits_equal(a, b):
-    """Bit-equal float arrays, NaN positions included (the -inf ScanNet pose turns into NaNs)."""
-    a, b = np.asarray(a), np.asarray(b)
-    if a.shape != b.shape or a.dtype != b.dtype:
-        return False
-    na, nb = np.isnan(a), np.isnan(b)
-    return bool(np.array_equal(na, nb) and np.array_equal(np.where(na, 0, a).view(np.uint32),
-                                                          np.where(nb, 0, b).view(np.uint32)))
+gen, fx, root = sequence_fixtures("datasets")
 
 
 def test_fixture_covers_every_case(gen, fx):

@@ -2,52 +2,20 @@
 own dataset classes (tests/golden/datasets/ref_datasets.npz): colour and depth bit for bit in every resize case
 (native, downscale, upscale, exact 2x, ScanNet's mixed colour / depth sizes); the prefetching reader against the
 synchronous one; and SplaTAM's loop plus `evaluate` on a rendered 1200x680 Replica-layout sequence read from disk."""
-import importlib.util
-import os
-
 import numpy as np
 import pytest
 import torch
 
 import scenes
-from util import GOLDEN
+from dataset_fixtures import sequence, sequence_fixtures
 from splatam_b200 import datasets as D
 
 pytestmark = pytest.mark.gpu
 
-FIX = os.path.join(GOLDEN, "datasets", "ref_datasets.npz")
 PIXEL_READS = ["replica_native", "replica_down", "replica_up", "replica_half", "tum_up", "scannet_mixed"]
 
 
-def _generator():
-    spec = importlib.util.spec_from_file_location("make_golden_datasets",
-                                                  os.path.join(GOLDEN, "datasets", "make_golden_datasets.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-@pytest.fixture(scope="module")
-def gen():
-    return _generator()
-
-
-@pytest.fixture(scope="module")
-def fx():
-    return dict(np.load(FIX))
-
-
-@pytest.fixture(scope="module")
-def root(gen, fx, tmp_path_factory):
-    d = str(tmp_path_factory.mktemp("sequences"))
-    gen.write_sequences(d, fx)
-    return d
-
-
-def sequence(gen, root, read, device, prefetch, **extra):
-    dataset, kw = gen.READS[read]
-    return D.RGBDSequence(dataset, os.path.join(root, dataset), gen.SEQUENCES[dataset], gen.config(dataset),
-                          device=device, prefetch=prefetch, **dict(kw, **extra))
+gen, fx, root = sequence_fixtures("datasets")
 
 
 @pytest.mark.parametrize("prefetch", [0, 2])

@@ -3,51 +3,21 @@ ScannetPPDataset and ReplicaV2Dataset run unmodified on tiny synthetic sequences
 (tests/golden/datasets/ref_nvs_datasets.npz, written by make_golden_nvs_datasets.py): file order, split assembly,
 is_bad filtering, start / end / stride on the test split, poses, intrinsics and retained indices bit for bit, colour
 and depth through the float64 restatement of the ingest kernel; and the error cases."""
-import importlib.util
 import json
 import os
 import shutil
 
-import numpy as np
 import pytest
 import torch
 
-from util import GOLDEN
+from dataset_fixtures import files_of, sequence_fixtures
+from util import GOLDEN, bits_equal
 from splatam_b200 import datasets as D
 
 FIX = os.path.join(GOLDEN, "datasets", "ref_nvs_datasets.npz")
 
 
-@pytest.fixture(scope="module")
-def gen():
-    spec = importlib.util.spec_from_file_location("make_golden_nvs_datasets",
-                                                  os.path.join(GOLDEN, "datasets", "make_golden_nvs_datasets.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-@pytest.fixture(scope="module")
-def fx():
-    return dict(np.load(FIX))
-
-
-@pytest.fixture(scope="module")
-def root(gen, fx, tmp_path_factory):
-    d = str(tmp_path_factory.mktemp("nvs_sequences"))
-    gen.write_sequences(d, fx)
-    return d
-
-
-def files_of(gen, root, read):
-    dataset, split, kw = gen.READS[read]
-    config = gen.REPLICAV2_CONFIG if dataset == "replicav2" else None
-    return D.SequenceFiles(dataset, os.path.join(root, dataset), gen.SEQUENCES[dataset], config, split=split, **kw)
-
-
-def bits_equal(a, b):
-    a, b = np.asarray(a), np.asarray(b)
-    return a.shape == b.shape and a.dtype == b.dtype and bool(np.array_equal(a.view(np.uint32), b.view(np.uint32)))
+gen, fx, root = sequence_fixtures("nvs_datasets")
 
 
 READS = ["scannetpp_train", "scannetpp_train_bad", "scannetpp_test", "scannetpp_test_bad", "replicav2_train",

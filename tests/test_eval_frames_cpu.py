@@ -2,7 +2,6 @@
 (tests/golden/eval/ref_eval_frames.npz), the JET table against cv2's, argument checks of sb_eval_frames_u8 before any
 launch, no CPU fallback, save_frames without out_dir, and the argument and record checks of tools/eval_record.py."""
 import ctypes
-import importlib.util
 import os
 
 import numpy as np
@@ -10,24 +9,17 @@ import pytest
 import torch
 
 from splatam_b200 import _lib, evaluate as EV, formats
-from util import GOLDEN, ROOT
-
-
-def _load(path, name):
-    spec = importlib.util.spec_from_file_location(name, path)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
+from util import GOLDEN, load
 
 
 @pytest.fixture(scope="module")
 def gen():
-    return _load(os.path.join(GOLDEN, "eval", "make_golden_eval_frames.py"), "make_golden_eval_frames")
+    return load("tests/golden/eval/make_golden_eval_frames.py")
 
 
 @pytest.fixture(scope="module")
 def tool():
-    return _load(os.path.join(ROOT, "tools", "eval_record.py"), "eval_record")
+    return load("tools/eval_record.py")
 
 
 def test_jet_table_is_cv2s():

@@ -2,36 +2,22 @@
 reference's own `eval` / `eval_nvs` wrote (tests/golden/eval/ref_eval_frames.npz), the kernel against the reference's
 numpy / cv2 statements at 1200x680, save_frames leaving every metric unchanged, and tools/eval_record.py end to end
 against the run that wrote the record."""
-import importlib.util
-import json
 import os
-import sys
 
 import numpy as np
 import pytest
 import torch
 
 import scenes
-from util import GOLDEN, ROOT
+from util import GOLDEN, load, run_tool
 
 pytestmark = pytest.mark.gpu
-
-
-def _load(path, name):
-    spec = importlib.util.spec_from_file_location(name, path)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-def _gen():
-    return _load(os.path.join(GOLDEN, "eval", "make_golden_eval_frames.py"), "make_golden_eval_frames")
 
 
 @pytest.mark.parametrize("name", ["eval", "eval_nvs"])
 def test_saved_frames_equal_the_reference_files(cuda_device, tmp_path, name):
     from splatam_b200.evaluate import evaluate, evaluate_nvs
-    gen = _gen()
+    gen = load("tests/golden/eval/make_golden_eval_frames.py")
     fx = np.load(os.path.join(GOLDEN, "eval", "ref_eval_frames.npz"))
     dev = cuda_device
     case = gen.frames_case(name)
@@ -75,7 +61,7 @@ def test_kernel_equals_the_reference_statements_at_1200x680(cuda_device, tmp_pat
     cv2 = pytest.importorskip("cv2")
     from PIL import Image
     from splatam_b200.evaluate import eval_frames_u8
-    gen = _gen()
+    gen = load("tests/golden/eval/make_golden_eval_frames.py")
     H, W = 680, 1200
     g = torch.Generator().manual_seed(17)
     im, gt = _special(g, (3, H, W), -0.3, 1.3), _special(g, (3, H, W), -0.1, 1.1)
@@ -115,8 +101,7 @@ def test_save_frames_changes_no_result(cuda_device, tmp_path):
     dev = cuda_device
     sc = scenes.room(seed=31, P=30_000, cam=dict(w=320, h=192, fx=160.0, fy=160.0, cx=159.5, cy=95.5))
     cam = sc.settings(S.GaussianRasterizationSettings, dev)
-    gt = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-              logit_opacities=torch.logit(sc.opacities.clamp(0.02, 0.98)), log_scales=torch.log(sc.scales[:, :1]))
+    gt = sc.splatam_params()
     gt = {k: v.to(dev) for k, v in gt.items()}
     T = 9
     rots, trans = slam.look_trajectory(T, dev)
@@ -170,26 +155,20 @@ def _removing_render(path):
     return render
 
 
-def _run(tool, argv, monkeypatch, capsys):
-    monkeypatch.setattr(sys, "argv", argv)
-    tool.main()
-    return json.loads(capsys.readouterr().out.strip().splitlines()[-1])
-
-
 def test_eval_record_reproduces_the_run(cuda_device, tmp_path, monkeypatch, capsys):
     from splatam_b200 import datasets, evaluate, formats
     T = 6
     scenes.write_replica_sequence(str(tmp_path / "room0"), T, cuda_device)
     data = ["--dataset", "replica", "--basedir", str(tmp_path), "--sequence", "room0"]
     run_dir = str(tmp_path / "run")
-    run = _run(_load(os.path.join(ROOT, "tools", "run_slam_dataset.py"), "run_slam_dataset"),
-               ["run_slam_dataset.py"] + data + ["--tracking-iters", "10", "--mapping-iters", "10", "--out", run_dir,
-                                                 "--save-frames"], monkeypatch, capsys)
+    run = run_tool(load("tools/run_slam_dataset.py"),
+                   ["run_slam_dataset.py"] + data + ["--tracking-iters", "10", "--mapping-iters", "10",
+                                                     "--out", run_dir, "--save-frames"], monkeypatch, capsys)
     for d, n in (("rendered_rgb", "gs"), ("rendered_depth", "gs"), ("rgb", "gt"), ("depth", "gt")):
         assert sorted(os.listdir(os.path.join(run_dir, d))) == ["%s_0000.png" % n, "%s_0004.png" % n]
-    tool = _load(os.path.join(ROOT, "tools", "eval_record.py"), "eval_record")
+    tool = load("tools/eval_record.py")
     rec_path = os.path.join(run_dir, "params.npz")
-    line = _run(tool, ["eval_record.py"] + data + ["--record", rec_path], monkeypatch, capsys)
+    line = run_tool(tool, ["eval_record.py"] + data + ["--record", rec_path], monkeypatch, capsys)
     assert line["out"] == os.path.join(run_dir, "eval_train") and line["evaluated_frames"] == 2
     for k in ("psnr_db", "ms_ssim", "depth_l1_m", "ate_m"):
         assert line[k] == run[k], k
@@ -208,8 +187,8 @@ def test_eval_record_reproduces_the_run(cuda_device, tmp_path, monkeypatch, caps
     assert direct["psnr"] == line["psnr_db"] and direct["ms_ssim"] == line["ms_ssim"]
     assert direct["depth_l1"] == line["depth_l1_m"] and direct["ate"] == line["ate_m"]
     no_frames = str(tmp_path / "no_frames")
-    _run(tool, ["eval_record.py"] + data + ["--record", rec_path, "--out", no_frames, "--no-frames"], monkeypatch,
-         capsys)
+    run_tool(tool, ["eval_record.py"] + data + ["--record", rec_path, "--out", no_frames, "--no-frames"],
+             monkeypatch, capsys)
     assert sorted(os.listdir(no_frames)) == ["l1.txt", "psnr.txt", "rmse.txt", "ssim.txt"]
 
 
@@ -219,18 +198,18 @@ def test_eval_record_test_split(cuda_device, tmp_path, monkeypatch, capsys):
     _write_replicav2(str(tmp_path), 11, cuda_device)
     data = ["--dataset", "replicav2", "--basedir", str(tmp_path), "--sequence", "room_0"]
     run_dir = str(tmp_path / "run")
-    run = _run(_load(os.path.join(ROOT, "tools", "run_slam_dataset.py"), "run_slam_dataset"),
-               ["run_slam_dataset.py"] + data + ["--tracking-iters", "10", "--mapping-iters", "10", "--out", run_dir,
-                                                 "--nvs", "--save-frames"], monkeypatch, capsys)
+    run = run_tool(load("tools/run_slam_dataset.py"),
+                   ["run_slam_dataset.py"] + data + ["--tracking-iters", "10", "--mapping-iters", "10",
+                                                     "--out", run_dir, "--nvs", "--save-frames"], monkeypatch, capsys)
     nvs_dir = os.path.join(run_dir, "eval_nvs")
     views = ["0000", "0004"]                             # test views k = t - 1 for t = 1 and 5 (eval_every 5)
     for d, n in (("rendered_rgb", "splatam"), ("rendered_depth", "splatam"), ("rgb", "gt"), ("depth", "gt")):
         assert sorted(os.listdir(os.path.join(nvs_dir, d))) == ["%s_%s.png" % (n, k) for k in views]
-    tool = _load(os.path.join(ROOT, "tools", "eval_record.py"), "eval_record")
+    tool = load("tools/eval_record.py")
     rec_path = os.path.join(run_dir, "params.npz")
     out = str(tmp_path / "nvs")
-    line = _run(tool, ["eval_record.py"] + data + ["--record", rec_path, "--split", "test", "--out", out],
-                monkeypatch, capsys)
+    line = run_tool(tool, ["eval_record.py"] + data + ["--record", rec_path, "--split", "test", "--out", out],
+                    monkeypatch, capsys)
     assert line["psnr_db"] == run["nvs_psnr_db"] and line["ms_ssim"] == run["nvs_ms_ssim"]
     assert line["depth_l1_m"] == run["nvs_depth_l1_m"] and line["valid_frames"] == run["nvs_valid_frames"]
     for d, n in (("rendered_rgb", "splatam"), ("rendered_depth", "splatam"), ("rgb", "gt"), ("depth", "gt")):

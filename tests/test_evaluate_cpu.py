@@ -2,28 +2,20 @@
 reference's own final `eval`, run unmodified with preset renders (tests/golden/eval/ref_eval.npz, written by
 tests/golden/eval/make_golden_eval.py); argument checks of the metric entry points; no CPU fallback."""
 import ctypes
-import importlib.util
 import os
 
 import numpy as np
 import pytest
 import torch
 
-from util import GOLDEN
+from util import GOLDEN, load
 
 FIX = os.path.join(GOLDEN, "eval", "ref_eval.npz")
 
 
-def _generator():
-    spec = importlib.util.spec_from_file_location("make_golden_eval", os.path.join(GOLDEN, "eval", "make_golden_eval.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
 @pytest.fixture(scope="module")
 def gen():
-    return _generator()
+    return load("tests/golden/eval/make_golden_eval.py")
 
 
 @pytest.fixture(scope="module")

@@ -5,7 +5,6 @@ on the SLAM test sequence over the fused and the plain render paths.
 MS-SSIM bound per (image, channel): max(1e-5, 2 x the error of the float32 restatement of the same definition against
 float64 on the same input, both on the CPU) -- the kernel has to be at least as close to the definition as a float32
 PyTorch implementation of it."""
-import importlib.util
 import os
 
 import numpy as np
@@ -13,16 +12,9 @@ import pytest
 import torch
 
 import scenes
-from util import GOLDEN
+from util import GOLDEN, load
 
 pytestmark = pytest.mark.gpu
-
-
-def _gen():
-    spec = importlib.util.spec_from_file_location("make_golden_eval", os.path.join(GOLDEN, "eval", "make_golden_eval.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def ms_ssim_bound(x, y):
@@ -109,7 +101,7 @@ def _frames_from_case(case, dev):
 def test_evaluate_matches_reference_eval(cuda_device, tmp_path, name):
     """evaluate over the fixture's preset renders == the reference's eval over the same renders."""
     from splatam_b200.evaluate import evaluate
-    gen = _gen()
+    gen = load("tests/golden/eval/make_golden_eval.py")
     fx = np.load(os.path.join(GOLDEN, "eval", "ref_eval.npz"))
     dev = cuda_device
     case = gen.eval_case(name)
@@ -154,8 +146,7 @@ def _slam_sequence(dev, T=9):
     from splatam_b200 import slam
     sc = scenes.room(seed=31, P=30_000, cam=dict(w=320, h=192, fx=160.0, fy=160.0, cx=159.5, cy=95.5))
     cam = sc.settings(S.GaussianRasterizationSettings, dev)
-    gt = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-              logit_opacities=torch.logit(sc.opacities.clamp(0.02, 0.98)), log_scales=torch.log(sc.scales[:, :1]))
+    gt = sc.splatam_params()
     gt = {k: v.to(dev) for k, v in gt.items()}
     rots, trans = slam.look_trajectory(T, dev)
     frames = [slam.render_frame(gt, rots, trans, t, cam) for t in range(T)]

@@ -2,7 +2,6 @@
 with the tolerances of test_evaluate_gpu.py, fused against plain rendering at ground-truth poses on an anisotropic map,
 and end to end: SplaTAM on the train split of a rendered ReplicaV2-layout sequence on disk, then evaluate_nvs on its
 test split."""
-import importlib.util
 import os
 
 import numpy as np
@@ -10,18 +9,10 @@ import pytest
 import torch
 
 import scenes
-from util import GOLDEN
+from util import GOLDEN, load
 from test_evaluate_gpu import ms_ssim_bound
 
 pytestmark = pytest.mark.gpu
-
-
-def _gen():
-    spec = importlib.util.spec_from_file_location("make_golden_eval_nvs",
-                                                  os.path.join(GOLDEN, "eval", "make_golden_eval_nvs.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 @pytest.mark.parametrize("name", ["unmasked_every1", "masked_every2", "none_valid"])
@@ -29,7 +20,7 @@ def test_evaluate_nvs_matches_reference_eval_nvs(cuda_device, tmp_path, name):
     """evaluate_nvs over the fixture's preset renders == the reference's eval_nvs over the same renders."""
     from oracle import metrics_torch as O
     from splatam_b200.evaluate import evaluate_nvs
-    gen = _gen()
+    gen = load("tests/golden/eval/make_golden_eval_nvs.py")
     fx = np.load(os.path.join(GOLDEN, "eval", "ref_eval_nvs.npz"))
     dev = cuda_device
     case = gen.nvs_case(name)
@@ -86,9 +77,8 @@ def test_fused_and_plain_render_at_the_ground_truth_pose(cuda_device):
     sc = scenes.room(seed=41, P=30_000, cam=dict(w=320, h=192, fx=160.0, fy=160.0, cx=159.5, cy=95.5))
     cam = sc.settings(S.GaussianRasterizationSettings, dev)
     g = torch.Generator().manual_seed(6)
-    params = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-                  logit_opacities=torch.logit(sc.opacities.clamp(0.02, 0.98)),
-                  log_scales=torch.log(sc.scales) + 0.3 * torch.randn(sc.scales.shape, generator=g))
+    params = sc.splatam_params(isotropic=False)
+    params["log_scales"] = params["log_scales"] + 0.3 * torch.randn(sc.scales.shape, generator=g)
     params = {k: v.to(dev) for k, v in params.items()}
     assert params["log_scales"].shape[1] == 3
     T = 6

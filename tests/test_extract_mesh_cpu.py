@@ -3,23 +3,13 @@ run's frames with run_slam_dataset.py's flags and refuses a selection whose leng
 count, RecordFusion refuses such a source before any device work, and volumes stay within what marching cubes can
 count."""
 import ctypes
-import importlib.util
-import os
 
 import numpy as np
 import pytest
 
+from util import load
 from splatam_b200 import _lib, formats
 from splatam_b200.mesh import MC_MAX_SAMPLES, RecordFusion, TSDFVolume
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _tool():
-    spec = importlib.util.spec_from_file_location("extract_mesh", os.path.join(ROOT, "tools", "extract_mesh.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def _record(tmp_path, T, width=64, height=48):
@@ -63,7 +53,7 @@ def fake_sequence(monkeypatch):
 
 
 def test_parser_takes_the_run_flags_and_keeps_them_to_input(tmp_path):
-    tool = _tool()
+    tool = load("tools/extract_mesh.py")
     rec = _record(tmp_path, 4)
     a = tool.parse_args(["--record", rec, "--out", "m.ply", "--source", "input", "--dataset", "replica", "--basedir",
                          "d", "--sequence", "room0", "--config", "c.yaml", "--start", "100", "--end", "400",
@@ -82,7 +72,7 @@ def _input_args(tool, rec, *extra):
 
 
 def test_open_input_forwards_the_selection_at_the_record_size(tmp_path, fake_sequence):
-    tool = _tool()
+    tool = load("tools/extract_mesh.py")
     rec = _record(tmp_path, 5, width=64, height=48)
     fake_sequence.n = 5
     seq, frames = tool.open_input(_input_args(tool, rec, "--config", "c.yaml", "--start", "100", "--end", "110",
@@ -97,7 +87,7 @@ def test_open_input_forwards_the_selection_at_the_record_size(tmp_path, fake_seq
 
 @pytest.mark.parametrize("n, extra", [(12, []), (4, []), (4, ["--frames", "5"])])
 def test_open_input_rejects_a_selection_of_another_length(tmp_path, fake_sequence, n, extra):
-    tool = _tool()
+    tool = load("tools/extract_mesh.py")
     rec = _record(tmp_path, 5)
     fake_sequence.n = n
     with pytest.raises(ValueError, match="has 5 cameras but .* select %d frames" % min(n, 5 if extra else n)):

@@ -105,8 +105,7 @@ def _slam_problem(dev, P=30_000):
     import splatam_b200 as S
     sc = scenes.room(seed=33, P=P, cam=dict(w=320, h=192, fx=160.0, fy=160.0, cx=159.5, cy=95.5))
     cam = sc.settings(S.GaussianRasterizationSettings, dev)
-    gauss = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-                 logit_opacities=torch.logit(sc.opacities.clamp(0.02, 0.98)), log_scales=torch.log(sc.scales[:, :1]))
+    gauss = sc.splatam_params()
     gauss = {k: v.to(dev).contiguous() for k, v in gauss.items()}
     K = torch.tensor([[160.0, 0, 159.5], [0, 160.0, 95.5], [0, 0, 1]])
     return sc, cam, gauss, K

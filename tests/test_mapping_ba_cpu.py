@@ -2,24 +2,20 @@
 reference's own get_loss(mapping=True, do_ba=True) + initialize_optimizer + prune_gaussians loop
 (tests/golden/ba/ref_ba.npz, written by tests/golden/ba/make_golden_ba.py), and the rules around it: momentum, map
 edits, zero rates, the pose cache and exact resume."""
-import importlib.util
 import os
 
 import numpy as np
 import pytest
 import torch
 
-from util import GOLDEN
+from util import GOLDEN, load
 
 FIX = os.path.join(GOLDEN, "ba", "ref_ba.npz")
 
 
 @pytest.fixture(scope="module")
 def gen():
-    spec = importlib.util.spec_from_file_location("make_golden_ba", os.path.join(GOLDEN, "ba", "make_golden_ba.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
+    return load("tests/golden/ba/make_golden_ba.py")
 
 
 @pytest.fixture(scope="module")
@@ -200,8 +196,7 @@ def _overlap_sequence(gen, T=6):
     import scenes
     from splatam_b200 import slam
     sc = scenes.config1(seed=8, P=240, w=96, h=72)
-    gt = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-              logit_opacities=torch.logit(sc.opacities.clamp(0.05, 0.95)), log_scales=torch.log(sc.scales[:, :1]))
+    gt = sc.splatam_params(opacity_clamp=(0.05, 0.95))
     rots, trans = slam.look_trajectory(T, "cpu", step=(0.12, -0.03, 0.02), rot_step=(0.004, 0.01, 0.002))
     cam = gen.camera(sc)
     frames = [slam.render_frame(gt, rots, trans, t, cam, render=gen.render) for t in range(T)]

@@ -10,7 +10,8 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 from splatam_b200 import mapping as M
-from test_mapping_gloo import _cpu_render, _problem
+from test_mapping_gloo import _problem
+from util import cpu_render
 
 LRS = dict(cam_unnorm_rots=0.0004, cam_trans=0.002)
 PRUNE = dict(start_after=0, remove_big_after=100, stop_after=20, prune_every=1, removal_opacity_threshold=0.1,
@@ -22,7 +23,7 @@ def _worker(rank, world, port, q):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     torch.set_num_threads(2)
     gauss, rots, trans, frames = _problem()
-    mapper = M.ShardedMapper(gauss, rots, trans, render=_cpu_render, seed=123, lrs=LRS)
+    mapper = M.ShardedMapper(gauss, rots, trans, render=cpu_render, seed=123, lrs=LRS)
     _, _, picks = mapper.step(frames)
     first = dict(picks=picks, pose_grad=mapper.g.pose_grad.numpy().copy(),
                  cams=[mapper.cam[k].detach().numpy().copy() for k in M.CAM_KEYS],
@@ -58,7 +59,7 @@ def test_two_ranks_equal_one_process_and_poses_stay_identical():
     assert all(float(g0[:, c].abs().sum()) == 0 for c in range(g0.shape[1]) if c not in drawn)
     # one process accumulating the same two keyframes, one Adam step of map and poses
     gauss, rots, trans, frames = _problem()
-    ref = M.ShardedMapper(gauss, rots, trans, render=_cpu_render, seed=123, lrs=LRS)
+    ref = M.ShardedMapper(gauss, rots, trans, render=cpu_render, seed=123, lrs=LRS)
     ref.g.zero_grad()
     for k in f0["picks"]:
         ref.accumulate(frames[k])

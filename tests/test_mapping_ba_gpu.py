@@ -2,7 +2,6 @@
 csrc/prepare.cu giving Gaussian and pose gradients, the captured step with its static pose leaves and scatter into the
 pose-gradient table -- against the reference's own do_ba=True loop (tests/golden/ba/ref_ba.npz), eager against graph,
 without host synchronisation, and the poses converging back to the ones the frames were rendered at."""
-import importlib.util
 import math
 import os
 
@@ -11,7 +10,7 @@ import pytest
 import torch
 
 import scenes
-from util import GOLDEN
+from util import GOLDEN, load
 
 pytestmark = pytest.mark.gpu
 
@@ -21,10 +20,7 @@ FROZEN = dict(means3D=0.0, rgb_colors=0.0, unnorm_rotations=0.0, logit_opacities
 
 @pytest.fixture(scope="module")
 def gen():
-    spec = importlib.util.spec_from_file_location("make_golden_ba", os.path.join(GOLDEN, "ba", "make_golden_ba.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
+    return load("tests/golden/ba/make_golden_ba.py")
 
 
 def _rel(a, b):
@@ -76,8 +72,7 @@ def _scene(dev, T=3, seed=3):
     sc = scenes.view_filling(seed=31, cam=dict(w=320, h=192, fx=160.0, fy=160.0, cx=159.5, cy=95.5), stride=1,
                              margin=16)
     cam = sc.settings(S.GaussianRasterizationSettings, dev)
-    gauss = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-                 logit_opacities=torch.logit(sc.opacities.clamp(0.02, 0.98)), log_scales=torch.log(sc.scales[:, :1]))
+    gauss = sc.splatam_params()
     gauss = {k: v.clone().to(dev) for k, v in gauss.items()}
     rots, trans = slam.look_trajectory(T, dev, step=(0.01, -0.005, 0.008), rot_step=(0.002, -0.002, 0.001))
     frames = [slam.render_frame(gauss, rots, trans, t, cam) for t in range(T)]

@@ -11,16 +11,8 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 import scenes
-from oracle import bruteforce_torch as BF
+from util import cpu_render
 from splatam_b200 import mapping as M
-
-
-def _cpu_render(settings, means3D, means2D, opacities, colors_precomp, scales, rotations):
-    out = BF.render(means3D, colors_precomp, opacities, scales, rotations, width=settings.image_width,
-                    height=settings.image_height, tanfovx=settings.tanfovx, tanfovy=settings.tanfovy, bg=settings.bg,
-                    viewmatrix=settings.viewmatrix[0], projmatrix=settings.projmatrix[0], means2D=means2D,
-                    dtype=torch.float32)
-    return out["color"], out["radii"], out["depth"]
 
 
 def _problem():
@@ -47,7 +39,7 @@ def _worker(rank, world, port, q):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     torch.set_num_threads(2)
     gauss, rots, trans, frames = _problem()
-    mapper = M.ShardedMapper(gauss, rots, trans, render=_cpu_render, seed=123)
+    mapper = M.ShardedMapper(gauss, rots, trans, render=cpu_render, seed=123)
     before = mapper.g.flat.detach().clone()
     loss, seen, picks = mapper.step(frames)
     q.put((rank, picks, mapper.g.flat_grad.numpy().copy(), mapper.g.flat.detach().numpy().copy(), before.numpy().copy(), loss))
@@ -71,7 +63,7 @@ def test_sharded_mapping_step_matches_single_process_accumulation():
     assert abs(l0 - l1) < 1e-7
     # single-process reference: accumulate the same two keyframes into one bucket, one Adam step
     gauss, rots, trans, frames = _problem()
-    ref = M.ShardedMapper(gauss, rots, trans, render=_cpu_render, seed=123)
+    ref = M.ShardedMapper(gauss, rots, trans, render=cpu_render, seed=123)
     ref.g.zero_grad()
     for k in picks0:
         ref.accumulate(frames[k])
@@ -82,13 +74,13 @@ def test_sharded_mapping_step_matches_single_process_accumulation():
 
 def test_flat_bucket_layout_and_schedule():
     gauss, rots, trans, frames = _problem()
-    m = M.ShardedMapper(gauss, rots, trans, render=_cpu_render, seed=1)
+    m = M.ShardedMapper(gauss, rots, trans, render=cpu_render, seed=1)
     P = gauss["means3D"].shape[0]
     assert m.g.flat.numel() == P * (3 + 3 + 4 + 1 + 1) and m.g.flat_grad.numel() == m.g.flat.numel()
     for k in M.GAUSSIAN_KEYS:
         assert m.g.params[k].grad.data_ptr() >= m.g.flat_grad.data_ptr()
         assert torch.equal(m.g.params[k].detach(), gauss[k])
-    loss, radius = M.mapping_loss(m.params(), frames[0], _cpu_render)
+    loss, radius = M.mapping_loss(m.params(), frames[0], cpu_render)
     loss.backward()
     assert m.g.flat_grad.abs().sum() > 0 and torch.isfinite(m.g.flat_grad).all()
     assert m.schedule(5)[0] in range(5)
@@ -99,7 +91,7 @@ def _worker_edit(rank, world, port, q):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     torch.set_num_threads(2)
     gauss, rots, trans, frames = _problem()
-    mapper = M.ShardedMapper(gauss, rots, trans, render=_cpu_render, seed=123)
+    mapper = M.ShardedMapper(gauss, rots, trans, render=cpu_render, seed=123)
     mapper.step(frames)
     prune = dict(start_after=0, remove_big_after=0, stop_after=20, prune_every=1, removal_opacity_threshold=0.25,
                  final_removal_opacity_threshold=0.25, reset_opacities=False, reset_opacities_every=500)
@@ -133,7 +125,7 @@ def _worker_sync(rank, world, port, q):
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     dist.init_process_group("gloo", rank=rank, world_size=world)
     gauss, rots, trans, frames = _problem()
-    mapper = M.ShardedMapper(gauss, rots, trans, render=_cpu_render, seed=5)
+    mapper = M.ShardedMapper(gauss, rots, trans, render=cpu_render, seed=5)
     mapper.cam = dict(cam_unnorm_rots=rots + 0.1 * rank, cam_trans=trans - 0.2 * rank)    # rank 1 "tracked" differently
     cam = mapper.sync_camera(src=0)
     fr = dict(frames[0], im=frames[0]["im"] + rank, depth=frames[0]["depth"] * (1 + rank), w2c=torch.eye(4) * (1 + rank))
@@ -165,7 +157,7 @@ def _worker_densify(rank, world, port, q):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     torch.set_num_threads(2)
     gauss, rots, trans, frames = _problem()
-    mapper = M.ShardedMapper(gauss, rots, trans, render=_cpu_render, seed=77, track_means2D=True)
+    mapper = M.ShardedMapper(gauss, rots, trans, render=cpu_render, seed=77, track_means2D=True)
     dd = dict(start_after=0, remove_big_after=0, stop_after=10, densify_every=1, grad_thresh=1e-9, num_to_split_into=2,
               removal_opacity_threshold=0.05, final_removal_opacity_threshold=0.05, reset_opacities=False,
               reset_opacities_every=100)

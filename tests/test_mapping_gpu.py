@@ -17,9 +17,7 @@ def _problem(dev, P=20000, nframes=4):
     sc = scenes.room(seed=21, P=P, cam=dict(w=320, h=192, fx=160.0, fy=160.0, cx=159.5, cy=95.5))
     cam = sc.settings(S.GaussianRasterizationSettings, dev)
     g = torch.Generator().manual_seed(0)
-    gauss = dict(means3D=sc.means3D.clone(), rgb_colors=sc.colors.clone(), unnorm_rotations=sc.rotations.clone(),
-                 logit_opacities=torch.logit(sc.opacities.clamp(0.02, 0.98)), log_scales=torch.log(sc.scales[:, :1].clone()))
-    gauss = {k: v.to(dev) for k, v in gauss.items()}
+    gauss = sc.splatam_params(dev)
     rots = torch.zeros(1, 4, nframes); rots[:, 0] = 1.0
     rots[:, 1:] = 0.01 * torch.randn(1, 3, nframes, generator=g)
     trans = 0.02 * torch.randn(1, 3, nframes, generator=g)

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 import torch
 
+from util import look_at
 from oracle import mesh_numpy as O
 from splatam_b200 import _lib, formats, mc_table
 from splatam_b200.mesh import TSDFVolume
@@ -164,20 +165,6 @@ def test_vertices_in_edge_order_and_interpolated():
     assert np.all(np.sum(on, 0) >= 2)
 
 
-def _look_at(cam, target):
-    fwd = target - cam
-    fwd /= np.linalg.norm(fwd)
-    right = np.cross(fwd, [0.0, 1.0, 0.0])
-    if np.linalg.norm(right) < 1e-6:
-        right = np.cross(fwd, [1.0, 0.0, 0.0])
-    right /= np.linalg.norm(right)
-    down = np.cross(fwd, right)
-    R = np.stack([right, down, fwd])
-    w2c = np.eye(4)
-    w2c[:3, :3], w2c[:3, 3] = R, -R @ cam
-    return w2c
-
-
 def _ray_depth(w2c, K, H, W, hit):
     """Camera-z depth image [H,W] of the surface `hit(origin, dirs) -> ray parameter` (dirs have camera z = 1)."""
     u, v = np.meshgrid(np.arange(W, dtype=np.float64), np.arange(H, dtype=np.float64))
@@ -218,7 +205,7 @@ def test_oracle_tsdf_of_analytic_depth_meshes_the_surface(shape):
     weight = np.zeros_like(tsdf)
     color = np.zeros(tuple(dims[::-1]) + (3,), np.float32)
     for cam in cams:
-        w2c = _look_at(cam, target(cam))
+        w2c = look_at(cam, target(cam))
         depth = _ray_depth(w2c, K, H, W, hit)
         rgb = np.full((3, H, W), 0.5, np.float32)
         O.integrate(tsdf, weight, color, origin, voxel, 4 * voxel, depth, rgb, w2c, K)

@@ -3,7 +3,6 @@ kernel against scipy's KD-tree, the metric definitions on hand-built cases, load
 ground-truth meshes, world_to_map on the synthetic sequences of every reader, eval_mesh.py's argument checks and the
 library's refusal to run without a GPU."""
 import ctypes
-import importlib.util
 import json
 import os
 
@@ -12,18 +11,9 @@ import pytest
 import torch
 from scipy.spatial import cKDTree
 
-from util import GOLDEN
+from util import GOLDEN, load
 from oracle import mesh_eval_numpy as O
 from splatam_b200 import _lib, datasets as D, formats, mesh_eval as E
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _module(path, name):
-    spec = importlib.util.spec_from_file_location(name, path)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 # ---- the brute-force restatement and the metric ------------------------------------------------------------------
@@ -195,8 +185,8 @@ def test_bad_files_are_rejected_with_their_path(tmp_path):
 
 @pytest.fixture(scope="module")
 def roots(tmp_path_factory):
-    base = _module(os.path.join(GOLDEN, "datasets", "make_golden_datasets.py"), "make_golden_datasets")
-    nvs = _module(os.path.join(GOLDEN, "datasets", "make_golden_nvs_datasets.py"), "make_golden_nvs_datasets")
+    base = load("tests/golden/datasets/make_golden_datasets.py")
+    nvs = load("tests/golden/datasets/make_golden_nvs_datasets.py")
     d = str(tmp_path_factory.mktemp("w2m"))
     base.write_sequences(d, dict(np.load(os.path.join(GOLDEN, "datasets", "ref_datasets.npz"))))
     nvs.write_sequences(d, dict(np.load(os.path.join(GOLDEN, "datasets", "ref_nvs_datasets.npz"))))
@@ -270,7 +260,7 @@ def test_world_to_map_refuses_a_non_finite_first_pose(roots):
 # ---- the tool and the library without a GPU -----------------------------------------------------------------------
 
 def test_eval_mesh_argument_errors(tmp_path):
-    tool = _module(os.path.join(ROOT, "tools", "eval_mesh.py"), "eval_mesh")
+    tool = load("tools/eval_mesh.py")
     mesh = formats.save_mesh_ply(str(tmp_path / "m.ply"), VERTS, np.zeros((8, 3)), FANNED)
     ok = ["--mesh", mesh, "--gt-mesh", mesh]
     data = ["--dataset", "replica", "--basedir", str(tmp_path), "--sequence", "room0"]
@@ -287,7 +277,7 @@ def test_eval_mesh_argument_errors(tmp_path):
 
 
 def test_to_map_applies_the_transform_in_float64():
-    tool = _module(os.path.join(ROOT, "tools", "eval_mesh.py"), "eval_mesh")
+    tool = load("tools/eval_mesh.py")
     M = np.eye(4)
     M[:3, :3] = [[0, -1, 0], [1, 0, 0], [0, 0, 1]]
     M[:3, 3] = [1, 2, 3]

@@ -2,35 +2,22 @@
 (oracle/mesh_eval_numpy.py), the grid search on the clouds where it is easiest to get wrong, area sampling, and
 evaluate_mesh / eval_mesh.py end to end on a meshed synthetic run record, with the culling loop free of host
 synchronisation."""
-import importlib.util
 import json
-import os
 
 import numpy as np
 import pytest
 import torch
 from scipy.spatial import cKDTree
 
+from util import load, look_at
 from oracle import mesh_eval_numpy as O
 from splatam_b200 import formats
 from splatam_b200 import mesh_eval as E
 from splatam_b200.mesh import RecordFusion, mesh_record
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 H, W = 32, 40
 K = np.array([[40.0, 0, 19.5], [0, 40.0, 15.5], [0, 0, 1]], np.float32)
-
-
-def _look_at(cam, target):
-    fwd = target - cam
-    fwd /= np.linalg.norm(fwd)
-    right = np.cross(fwd, [0.0, 1.0, 0.0])
-    right /= np.linalg.norm(right)
-    R = np.stack([right, np.cross(fwd, right), fwd])
-    w2c = np.eye(4)
-    w2c[:3, :3], w2c[:3, 3] = R, -R @ cam
-    return w2c.astype(np.float32)
 
 
 def _frames(B, seed):
@@ -41,7 +28,7 @@ def _frames(B, seed):
     for b in range(B):
         r = 0.2 if b % 3 == 0 else g.uniform(1.2, 2.0)
         d = g.normal(size=3)
-        w2c.append(_look_at(r * d / np.linalg.norm(d), g.uniform(-0.1, 0.1, 3)))
+        w2c.append(look_at(r * d / np.linalg.norm(d), g.uniform(-0.1, 0.1, 3)).astype(np.float32))
         base = r + g.uniform(-0.4, 0.4) + 0.2 * g.standard_normal((H, W))
         base[g.uniform(size=(H, W)) < 0.1] = 0.0
         base[g.uniform(size=(H, W)) < 0.05] = 1e6
@@ -232,9 +219,7 @@ def test_wall_scores_with_and_without_culling(cuda_device, wall):
 
 
 def test_eval_mesh_tool_prints_the_same_numbers(cuda_device, wall, capsys):
-    spec = importlib.util.spec_from_file_location("eval_mesh", os.path.join(ROOT, "tools", "eval_mesh.py"))
-    tool = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(tool)
+    tool = load("tools/eval_mesh.py")
     tool.main(["--mesh", wall["pred"], "--gt-mesh", wall["gt"], "--no-cull", "--samples", "50000", "--seed", "4"])
     line = json.loads(capsys.readouterr().out.strip().splitlines()[-1])
     pred, gt = formats.load_mesh_ply(wall["pred"]), formats.load_mesh_ply(wall["gt"])

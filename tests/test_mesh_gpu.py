@@ -1,33 +1,20 @@
 """GPU suite of mesh extraction: sb_tsdf_integrate and the marching-cubes passes bit for bit against the numpy
 restatement (oracle/mesh_numpy.py), batching, the empty and fully inside volumes, and mesh_record / extract_mesh.py
 end to end on a synthetic run record, with its fusion loop free of host synchronisation."""
-import importlib.util
 import json
-import os
 
 import numpy as np
 import pytest
 import torch
 
+from util import load, look_at
 from oracle import mesh_numpy as O
 from splatam_b200 import formats
 from splatam_b200.mesh import RecordFusion, TSDFVolume, mesh_record
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 H, W = 32, 40
 K = np.array([[40.0, 0, 19.5], [0, 40.0, 15.5], [0, 0, 1]], np.float32)
-
-
-def _look_at(cam, target):
-    fwd = target - cam
-    fwd /= np.linalg.norm(fwd)
-    right = np.cross(fwd, [0.0, 1.0, 0.0])
-    right /= np.linalg.norm(right)
-    R = np.stack([right, np.cross(fwd, right), fwd])
-    w2c = np.eye(4)
-    w2c[:3, :3], w2c[:3, 3] = R, -R @ cam
-    return w2c.astype(np.float32)
 
 
 def _frames(B, seed):
@@ -39,7 +26,7 @@ def _frames(B, seed):
         r = 0.3 if b % 3 == 0 else g.uniform(1.2, 1.8)
         d = g.normal(size=3)
         cam = r * d / np.linalg.norm(d)
-        w2c.append(_look_at(cam, g.uniform(-0.1, 0.1, 3)))
+        w2c.append(look_at(cam, g.uniform(-0.1, 0.1, 3)).astype(np.float32))
         base = r + g.uniform(-0.3, 0.3) + 0.1 * np.sin(np.arange(W) / 5.0)[None, :] + 0.05 * g.standard_normal((H, W))
         base[g.uniform(size=(H, W)) < 0.15] = 0.0
         base[g.uniform(size=(H, W)) < 0.05] = 3.0
@@ -195,9 +182,7 @@ def test_mesh_record_from_input_frames(cuda_device, wall_record):
 
 
 def test_extract_mesh_tool(cuda_device, wall_record, tmp_path, capsys):
-    spec = importlib.util.spec_from_file_location("extract_mesh", os.path.join(ROOT, "tools", "extract_mesh.py"))
-    tool = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(tool)
+    tool = load("tools/extract_mesh.py")
     out = str(tmp_path / "mesh.ply")
     tool.main(["--record", wall_record, "--out", out, "--voxel", "0.02", "--every", "2", "--batch", "2"])
     line = json.loads(capsys.readouterr().out.strip().splitlines()[-1])

@@ -2,17 +2,15 @@
 the random-view protocol, the depth-L1 arithmetic on hand-built depth maps, and the library's and the tool's argument
 checks without a GPU."""
 import ctypes
-import importlib.util
-import os
 
 import numpy as np
 import pytest
 import torch
 
+from util import load
 from oracle.mesh_render_numpy import mesh_depth
 from splatam_b200 import _lib, mesh_eval as E
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EYE = np.eye(4, dtype=np.float32)[None]
 
 
@@ -160,9 +158,7 @@ def test_depth_l1_arithmetic_on_hand_built_maps():
 
 
 def test_eval_mesh_depth_views_argument(tmp_path):
-    spec = importlib.util.spec_from_file_location("eval_mesh", os.path.join(ROOT, "tools", "eval_mesh.py"))
-    tool = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(tool)
+    tool = load("tools/eval_mesh.py")
     from splatam_b200 import formats
     mesh = formats.save_mesh_ply(str(tmp_path / "m.ply"), QUAD, np.zeros((4, 3)), TWO)
     ok = ["--mesh", mesh, "--gt-mesh", mesh, "--no-cull"]

@@ -1,37 +1,24 @@
 """GPU suite of mesh depth rendering: sb_mesh_depth bit for bit against the numpy restatement
 (oracle/mesh_render_numpy.py) on the meshes where a rasterizer is easiest to get wrong, MeshDepth free of host
 synchronisation, and depth_l1 / eval_mesh.py --depth-views end to end on a meshed wall of Gaussians."""
-import importlib.util
 import json
-import os
 
 import numpy as np
 import pytest
 import torch
 
+from util import load, look_at
 from oracle.mesh_render_numpy import mesh_depth
 from splatam_b200 import _lib, formats
 from splatam_b200 import mesh_eval as E
 from splatam_b200.mesh import RecordFusion, mesh_record
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _K(H, W):
     f = 0.8 * max(H, W)
     return np.array([[f, 0, (W - 1) / 2], [0, f, (H - 1) / 2], [0, 0, 1]])
-
-
-def _look_at(cam, target):
-    fwd = np.asarray(target, np.float64) - cam
-    fwd /= np.linalg.norm(fwd)
-    right = np.cross([0.0, 1.0, 0.0], fwd)
-    right /= np.linalg.norm(right)
-    R = np.stack([right, np.cross(fwd, right), fwd])
-    w2c = np.eye(4)
-    w2c[:3, :3], w2c[:3, 3] = R, -R @ cam
-    return w2c.astype(np.float32)
 
 
 def _random_mesh(seed, n_small=3000, n_big=12, nan=True):
@@ -66,7 +53,8 @@ def _poses(B, seed, inside=False):
     for b in range(B):
         d = g.normal(size=3)
         r = g.uniform(0.0, 0.4) if inside or b % 3 == 0 else g.uniform(1.0, 2.5)
-        out.append(_look_at(r * d / np.linalg.norm(d), g.uniform(-0.2, 0.2, 3)))
+        # up = -y: image x = y x fwd, these views' camera rolled 180 degrees about the view axis
+        out.append(look_at(r * d / np.linalg.norm(d), g.uniform(-0.2, 0.2, 3), up=(0.0, -1.0, 0.0)).astype(np.float32))
     return np.stack(out)
 
 
@@ -234,9 +222,7 @@ def test_evaluate_mesh_and_the_tool_report_depth_l1(cuda_device, wall, tmp_path,
     assert {k: full[k] for k in base if not k.endswith("_ms")} == {k: base[k] for k in base if not k.endswith("_ms")}
     assert set(full) - set(base) == {"depth_l1", "depth_l1_surface", "hole_ratio", "depth_views_used",
                                      "depth_views_drawn", "depth_render_ms", "depth_cull_ms"}
-    spec = importlib.util.spec_from_file_location("eval_mesh", os.path.join(ROOT, "tools", "eval_mesh.py"))
-    tool = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(tool)
+    tool = load("tools/eval_mesh.py")
     tool.main(["--mesh", wall["pred"], "--gt-mesh", room, "--no-cull", "--samples", "50000", "--seed", "4",
                "--depth-views", "5"])
     line = json.loads(capsys.readouterr().out.strip().splitlines()[-1])

@@ -2,30 +2,23 @@
 reference's own get_loss_gs, densify, get_expon_lr_func and update_learning_rate produced over the same map, frames
 and float32 brute-force renderer; plus the record reader, the original-index pose lookup and the torch counterpart of
 FusedAdam.set_lr.  The GPU runs are tests/test_offline_gpu.py."""
-import importlib.util
 import os
 
 import numpy as np
 import pytest
 import torch
 
+from util import load
 from splatam_b200 import formats, mapping as M, offline
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLDEN = os.path.join(HERE, "golden", "offline")
 
 
-def _generator():
-    spec = importlib.util.spec_from_file_location("make_golden_offline", os.path.join(GOLDEN, "make_golden_offline.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
 @pytest.fixture(scope="module")
 def gen():
     torch.set_num_threads(4)
-    mod = _generator()
+    mod = load("tests/golden/offline/make_golden_offline.py")
     return mod, mod.problem()
 
 

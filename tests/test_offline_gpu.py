@@ -1,20 +1,17 @@
 """GPU: the densification statistic kernel (sb_densify_accumulate), FusedAdam.set_lr, the fused offline loop against
 the torch path, and tools/run_offline_opt.py end to end in both modes on a synthetic Replica-layout sequence."""
-import importlib.util
-import json
 import os
-import sys
 
 import numpy as np
 import pytest
 import torch
 
 import scenes
+from util import load, run_tool
 from splatam_b200 import evaluate, formats, map_ops, mapping as M, offline, slam
 from splatam_b200.train_ops import FusedAdam
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def test_densify_accumulate_is_bit_equal_to_the_torch_statement(cuda_device):
@@ -56,8 +53,7 @@ def _problem(dev, T=4):
     import splatam_b200 as S
     sc = scenes.config1(seed=8, P=2000, w=96, h=64)
     cam = sc.settings(S.GaussianRasterizationSettings, dev)
-    gt = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-              logit_opacities=torch.logit(sc.opacities.clamp(0.05, 0.95)), log_scales=torch.log(sc.scales[:, :1]))
+    gt = sc.splatam_params(opacity_clamp=(0.05, 0.95))
     gt = {k: v.to(dev) for k, v in gt.items()}
     rots, trans = slam.look_trajectory(T, dev)
     frames = [slam.render_frame(gt, rots, trans, t, cam) for t in range(T)]
@@ -84,31 +80,19 @@ def test_fused_loop_matches_the_torch_path(cuda_device):
     assert abs(c_f[-1] - c_t[-1]) <= 0.05 * c_t[-1] and lr_f == lr_t
 
 
-def _tool(name):
-    spec = importlib.util.spec_from_file_location(name, os.path.join(ROOT, "tools", name + ".py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-def _run(tool, argv, monkeypatch, capsys):
-    monkeypatch.setattr(sys, "argv", argv)
-    tool.main()
-    return json.loads(capsys.readouterr().out.strip().splitlines()[-1])
-
-
 def test_tool_runs_both_modes_and_its_evaluation_is_evaluate(cuda_device, tmp_path, monkeypatch, capsys):
     T = 11
     scenes.write_replica_sequence(str(tmp_path / "room0"), T, cuda_device)
     data = ["--dataset", "replica", "--basedir", str(tmp_path), "--sequence", "room0"]
     slam_dir = str(tmp_path / "slam")
-    _run(_tool("run_slam_dataset"), ["run_slam_dataset.py"] + data + ["--tracking-iters", "10", "--mapping-iters", "10",
-                                                                       "--out", slam_dir], monkeypatch, capsys)
-    opt = _tool("run_offline_opt")
+    run_tool(load("tools/run_slam_dataset.py"),
+             ["run_slam_dataset.py"] + data + ["--tracking-iters", "10", "--mapping-iters", "10", "--out", slam_dir],
+             monkeypatch, capsys)
+    opt = load("tools/run_offline_opt.py")
     post_dir = str(tmp_path / "post")
-    line = _run(opt, ["run_offline_opt.py", "--mode", "post_splatam", "--record", os.path.join(slam_dir, "params.npz"),
-                      "--stride", "5", "--iters", "120", "--eval-frames", "3", "--out", post_dir] + data,
-                monkeypatch, capsys)
+    line = run_tool(opt, ["run_offline_opt.py", "--mode", "post_splatam", "--record",
+                          os.path.join(slam_dir, "params.npz"), "--stride", "5", "--iters", "120", "--eval-frames", "3",
+                          "--out", post_dir] + data, monkeypatch, capsys)
     assert line["frames"] == 3 and line["iters"] == 120 and line["eval_frames"] == 3
     assert line["train_psnr_after_db"] >= line["train_psnr_before_db"]
     rec = formats.load_params(os.path.join(post_dir, "params.npz"))
@@ -147,8 +131,8 @@ def test_tool_runs_both_modes_and_its_evaluation_is_evaluate(cuda_device, tmp_pa
     assert direct_40["psnr"] != direct["psnr"]
     np.testing.assert_array_equal(np.loadtxt(str(tmp_path / "eval_7k" / "psnr.txt")), direct_40["psnr_per_frame"])
     gt_dir = str(tmp_path / "gt")
-    line = _run(opt, ["run_offline_opt.py", "--mode", "gt_poses", "--iters", "120", "--eval-frames", "2",
-                      "--out", gt_dir] + data, monkeypatch, capsys)
+    line = run_tool(opt, ["run_offline_opt.py", "--mode", "gt_poses", "--iters", "120", "--eval-frames", "2",
+                          "--out", gt_dir] + data, monkeypatch, capsys)
     assert line["frames"] == T and line["initial_gaussians"] > 0 and np.isfinite(line["psnr_db"])
     assert line["train_psnr_after_db"] >= line["train_psnr_before_db"]
     assert line["width"] == 600 and line["height"] == 340

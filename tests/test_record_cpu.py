@@ -1,16 +1,15 @@
 """CPU: formats.read_record, the one checked reader of a run record, driven with the `need` of each of its callers: a
 valid record reads as np.load gives it, and each malformed one raises the same message whichever tool opens it --
 offline.from_record, tools/eval_record.py and tools/render_record.py --camera-from included."""
-import importlib.util
 import os
 
 import numpy as np
 import pytest
 import torch
 
+from util import load
 from splatam_b200 import formats, offline
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 NEEDS = {
     "viewer": formats.CHECKPOINT_KEYS + formats.CAMERA_KEYS,      # viewer.load_record, mesh.RecordFusion, extract_mesh
@@ -20,13 +19,6 @@ NEEDS = {
     "camera_from": formats.CAMERA_KEYS,                            # tools/render_record.py --camera-from
 }
 WITH_CAMERAS = ("viewer", "offline", "eval_train")
-
-
-def _tool(name):
-    spec = importlib.util.spec_from_file_location(name, os.path.join(ROOT, "tools", name + ".py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def _record(out_dir, T=4, P=6, **override):
@@ -156,7 +148,7 @@ def _replica_layout(root, T):
 
 
 def test_eval_record_rejects_a_malformed_record_at_read_time(tmp_path):
-    tool = _tool("eval_record")
+    tool = load("tools/eval_record.py")
     _replica_layout(str(tmp_path), 12)
     base = ["--dataset", "replica", "--basedir", str(tmp_path), "--sequence", "room0", "--record"]
     # 12 cameras with one cam_trans column short: each evaluated frame (0, 4, 9) still has a column in both tensors
@@ -169,7 +161,7 @@ def test_eval_record_rejects_a_malformed_record_at_read_time(tmp_path):
 
 
 def test_render_record_camera_from_names_what_it_lacks(tmp_path):
-    tool = _tool("render_record")
+    tool = load("tools/render_record.py")
     path = _record(tmp_path / "run")
     formats.save_checkpoint(str(tmp_path / "ckpt"), 3, dict(np.load(path)), [0])
     ckpt = str(tmp_path / "ckpt" / "params3.npz")

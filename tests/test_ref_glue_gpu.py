@@ -104,8 +104,7 @@ def test_fused_losses_match_reference_get_loss(fx, mode, cuda_device):
 def _loop_problem(dev, P=40_000):
     sc = scenes.view_filling(seed=31, cam=dict(w=320, h=192, fx=160.0, fy=160.0, cx=159.5, cy=95.5), stride=1)
     g = torch.Generator().manual_seed(5)
-    gauss = dict(means3D=sc.means3D.clone(), rgb_colors=sc.colors.clone(), unnorm_rotations=sc.rotations.clone(),
-                 logit_opacities=torch.logit(sc.opacities.clamp(0.02, 0.98)), log_scales=torch.log(sc.scales[:, :1].clone()))
+    gauss = sc.splatam_params()
     rots = torch.zeros(1, 4, 2); rots[:, 0] = 1.0
     rots[0, 1:, 1] = torch.tensor([0.004, -0.003, 0.002])
     trans = torch.zeros(1, 3, 2); trans[0, :, 1] = torch.tensor([0.010, -0.006, 0.008])

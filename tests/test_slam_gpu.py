@@ -18,8 +18,7 @@ def _sequence(dev, Settings, T=9):
     from splatam_b200 import slam
     sc = scenes.room(seed=31, P=30_000, cam=dict(w=320, h=192, fx=160.0, fy=160.0, cx=159.5, cy=95.5))
     cam = sc.settings(Settings, dev)
-    gt = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-              logit_opacities=torch.logit(sc.opacities.clamp(0.02, 0.98)), log_scales=torch.log(sc.scales[:, :1]))
+    gt = sc.splatam_params()
     gt = {k: v.to(dev) for k, v in gt.items()}
     rots, trans = slam.look_trajectory(T, dev)
     g = torch.Generator().manual_seed(5)

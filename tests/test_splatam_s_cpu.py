@@ -1,7 +1,6 @@
 """CPU: SplaTAM-S's densification resolution on the host side -- the reader's size arguments, its densification
 intrinsics and camera against the reference's own initialize_first_timestep (tests/golden/slam_s/ref_splatam_s.npz,
 written by make_golden_splatam_s.py), the SLAM loop's choice of frame for map growth, and the tool's variant check."""
-import importlib.util
 import os
 import sys
 
@@ -10,32 +9,23 @@ import pytest
 import torch
 
 import scenes
-from util import GOLDEN
-from oracle import bruteforce_torch as BF
+from dataset_fixtures import sequence_fixtures
+from util import GOLDEN, bits_equal, cpu_render, load
 from splatam_b200 import datasets as D
 from splatam_b200 import mapping as M
 from splatam_b200 import slam
 
-ROOT = os.path.dirname(os.path.dirname(GOLDEN))
 FIX = os.path.join(GOLDEN, "slam_s", "ref_splatam_s.npz")
 CAM_FIELDS = ("image_height", "image_width", "tanfovx", "tanfovy", "viewmatrix", "projmatrix", "campos")
 
 
-def _load(name, path):
-    spec = importlib.util.spec_from_file_location(name, path)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-@pytest.fixture(scope="module")
-def gen():
-    return _load("make_golden_datasets", os.path.join(GOLDEN, "datasets", "make_golden_datasets.py"))
+gen, _, root = sequence_fixtures("datasets")
+del _                   # this module's own `fx` is ref_splatam_s.npz
 
 
 @pytest.fixture(scope="module")
 def sgen():
-    return _load("make_golden_splatam_s", os.path.join(GOLDEN, "slam_s", "make_golden_splatam_s.py"))
+    return load("tests/golden/slam_s/make_golden_splatam_s.py")
 
 
 @pytest.fixture(scope="module")
@@ -43,21 +33,9 @@ def fx():
     return dict(np.load(FIX))
 
 
-@pytest.fixture(scope="module")
-def root(gen, tmp_path_factory):
-    d = str(tmp_path_factory.mktemp("sequences"))
-    gen.write_sequences(d, np.load(os.path.join(GOLDEN, "datasets", "ref_datasets.npz")))
-    return d
-
-
 def replica(gen, root, kw, **extra):
     return D.RGBDSequence("replica", os.path.join(root, "replica"), gen.SEQUENCES["replica"], gen.config("replica"),
                           device="cpu", prefetch=0, **dict(kw, **extra))
-
-
-def bits_equal(a, b):
-    a, b = np.asarray(a), np.asarray(b)
-    return a.shape == b.shape and a.dtype == b.dtype and a.tobytes() == b.tobytes()
 
 
 def field(cam, k):
@@ -105,14 +83,6 @@ def test_default_desired_size_is_the_config_size(gen, root):
     assert seq.densify_cam is None
 
 
-def _cpu_render(settings, means3D, means2D, opacities, colors_precomp, scales, rotations):
-    out = BF.render(means3D, colors_precomp, opacities, scales, rotations, width=settings.image_width,
-                    height=settings.image_height, tanfovx=settings.tanfovx, tanfovy=settings.tanfovy, bg=settings.bg,
-                    viewmatrix=settings.viewmatrix[0], projmatrix=settings.projmatrix[0], means2D=means2D,
-                    dtype=torch.float32)
-    return out["color"], out["radii"], out["depth"]
-
-
 def test_run_slam_grows_the_map_from_the_densify_entry(monkeypatch):
     """Mapped frames that carry ``densify`` are grown from it with its own intrinsics; frames without it from
     themselves with the `intrinsics` argument; no mapping window ever holds a ``densify`` entry.  (Map growth itself is
@@ -121,11 +91,10 @@ def test_run_slam_grows_the_map_from_the_densify_entry(monkeypatch):
     torch.set_num_threads(4)
     sc = scenes.config1(seed=8, P=120, w=48, h=32)
     cam = sc.settings(S.GaussianRasterizationSettings, "cpu")
-    gt = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-              logit_opacities=torch.logit(sc.opacities.clamp(0.05, 0.95)), log_scales=torch.log(sc.scales[:, :1]))
+    gt = sc.splatam_params(opacity_clamp=(0.05, 0.95))
     T = 5
     rots, trans = slam.look_trajectory(T, "cpu", step=(0.004, -0.002, 0.003), rot_step=(0.001, -0.001, 0.0005))
-    frames = [slam.render_frame(gt, rots, trans, t, cam, render=_cpu_render) for t in range(T)]
+    frames = [slam.render_frame(gt, rots, trans, t, cam, render=cpu_render) for t in range(T)]
     K = torch.tensor([[sc.fx, 0, sc.cx], [0, sc.fy, sc.cy], [0, 0, 1]])
     K_d = K.clone()
     K_d[:2] *= 0.5
@@ -142,7 +111,7 @@ def test_run_slam_grows_the_map_from_the_densify_entry(monkeypatch):
         return step(self, window, *a, **k)
     monkeypatch.setattr(M.ShardedMapper, "step", recording_step)
     torch.manual_seed(1); np.random.seed(1)
-    slam.run_slam(gt, frames, cam, render=_cpu_render, fused=False, tracking_iters=2, mapping_iters=1,
+    slam.run_slam(gt, frames, cam, render=cpu_render, fused=False, tracking_iters=2, mapping_iters=1,
                   keyframe_every=2, map_every=1, window=3, intrinsics=K, add_new_gaussians=True,
                   select_keyframes=True, first_frame_iters=1)
     assert [t for _, t, _ in grown] == [1, 2, 3, 4]
@@ -156,7 +125,7 @@ def test_run_slam_grows_the_map_from_the_densify_entry(monkeypatch):
 
 
 def test_tool_accepts_splatam_s_for_replica_only(monkeypatch, capsys):
-    tool = _load("run_slam_dataset", os.path.join(ROOT, "tools", "run_slam_dataset.py"))
+    tool = load("tools/run_slam_dataset.py")
     assert set(tool.HYPER_S) == {"replica"}
     row = tool.HYPER_S["replica"]
     assert (row["height"], row["width"], row["densify_height"], row["densify_width"]) == (680, 1200, 340, 600)

@@ -3,7 +3,6 @@ reference's dataset classes (ref_datasets.npz) and the numpy restatement of the 
 prefetch; the initial map and add_new_gaussians on the densification-size frame against the reference's own
 initialize_first_timestep / add_new_gaussians (ref_splatam_s.npz); and a SplaTAM-S run plus `evaluate` on a rendered
 1200x680 Replica-layout sequence read from disk."""
-import importlib.util
 import os
 
 import numpy as np
@@ -11,6 +10,7 @@ import pytest
 import torch
 
 import scenes
+from dataset_fixtures import sequence, sequence_fixtures
 from util import GOLDEN
 from splatam_b200 import datasets as D
 
@@ -25,39 +25,12 @@ PRUNE = dict(start_after=0, remove_big_after=0, stop_after=20, prune_every=20, r
              final_removal_opacity_threshold=0.005, reset_opacities=False, reset_opacities_every=500)
 
 
-def _load(name, path):
-    spec = importlib.util.spec_from_file_location(name, path)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-@pytest.fixture(scope="module")
-def gen():
-    return _load("make_golden_datasets", os.path.join(GOLDEN, "datasets", "make_golden_datasets.py"))
-
-
-@pytest.fixture(scope="module")
-def fx():
-    return dict(np.load(os.path.join(GOLDEN, "datasets", "ref_datasets.npz")))
+gen, fx, root = sequence_fixtures("datasets")
 
 
 @pytest.fixture(scope="module")
 def sfx():
     return dict(np.load(os.path.join(GOLDEN, "slam_s", "ref_splatam_s.npz")))
-
-
-@pytest.fixture(scope="module")
-def root(gen, fx, tmp_path_factory):
-    d = str(tmp_path_factory.mktemp("sequences"))
-    gen.write_sequences(d, fx)
-    return d
-
-
-def sequence(gen, root, read, device, prefetch, **extra):
-    dataset, kw = gen.READS[read]
-    return D.RGBDSequence(dataset, os.path.join(root, dataset), gen.SEQUENCES[dataset], gen.config(dataset),
-                          device=device, prefetch=prefetch, **dict(kw, **extra))
 
 
 def size(gen, read):

@@ -37,9 +37,7 @@ def _problem(dev):
     sc = scenes.view_filling(seed=41, cam=dict(w=256, h=160, fx=128.0, fy=128.0, cx=127.5, cy=79.5))
     cam = sc.settings(S.GaussianRasterizationSettings, dev)
     g = torch.Generator().manual_seed(2)
-    gauss = dict(means3D=sc.means3D.clone(), rgb_colors=sc.colors.clone(), unnorm_rotations=sc.rotations.clone(),
-                 logit_opacities=torch.logit(sc.opacities.clamp(0.02, 0.98)), log_scales=torch.log(sc.scales[:, :1].clone()))
-    gauss = {k: v.to(dev) for k, v in gauss.items()}
+    gauss = sc.splatam_params(dev)
     rots = torch.zeros(1, 4, 1); rots[:, 0] = 1.0
     trans = torch.zeros(1, 3, 1)
     frames = [dict(id=0, cam=cam, w2c=torch.eye(4, device=dev), im=torch.rand(3, sc.h, sc.w, generator=g).to(dev),

@@ -17,8 +17,7 @@ pytestmark = pytest.mark.gpu
 def _setup(dev, Settings, P=50_000):
     sc = scenes.room(seed=1, P=P, cam=dict(w=400, h=224, fx=200.0, fy=200.0, cx=199.5, cy=111.5))
     cam = sc.settings(Settings, dev)
-    gauss = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-                 logit_opacities=torch.logit(sc.opacities.clamp(0.02, 0.98)), log_scales=torch.log(sc.scales[:, :1]))
+    gauss = sc.splatam_params()
     gauss = {k: v.to(dev) for k, v in gauss.items()}
     return sc, cam, gauss
 

@@ -6,8 +6,8 @@ continues as the reference's `losses['depth'] < thres` test does."""
 import torch
 
 import scenes
+from util import cpu_render
 from splatam_b200 import mapping as M, slam
-from test_slam_cpu import _cpu_render
 
 N = 4
 
@@ -17,16 +17,15 @@ def _problem():
     torch.set_num_threads(4)
     sc = scenes.config1(seed=8, P=160, w=48, h=32)
     cam = sc.settings(S.GaussianRasterizationSettings, "cpu")
-    gauss = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-                 logit_opacities=torch.logit(sc.opacities.clamp(0.05, 0.95)), log_scales=torch.log(sc.scales[:, :1]))
+    gauss = sc.splatam_params(opacity_clamp=(0.05, 0.95))
     rots, trans = slam.look_trajectory(2, "cpu", step=(0.02, -0.01, 0.015), rot_step=(0.01, -0.01, 0.005))
-    return gauss, slam.render_frame(gauss, rots, trans, 1, cam, render=_cpu_render)
+    return gauss, slam.render_frame(gauss, rots, trans, 1, cam, render=cpu_render)
 
 
 def _track(gauss, frame, num_iters, **kw):
     rots = torch.zeros(1, 4, 2); rots[:, 0] = 1.0
     p = dict(gauss, cam_unnorm_rots=rots, cam_trans=torch.zeros(1, 3, 2))
-    losses = M.track_frame(p, frame, render=_cpu_render, num_iters=num_iters, fused=False, **kw)
+    losses = M.track_frame(p, frame, render=cpu_render, num_iters=num_iters, fused=False, **kw)
     return losses, p["cam_unnorm_rots"][..., 1].detach().clone(), p["cam_trans"][..., 1].detach().clone()
 
 
@@ -45,7 +44,7 @@ def test_rule_is_bit_equal_to_fixed_iteration_runs():
     p = dict(gauss, cam_unnorm_rots=torch.zeros(1, 4, 2), cam_trans=torch.zeros(1, 3, 2))
     p["cam_unnorm_rots"][:, 0] = 1.0
     with torch.no_grad():
-        M.tracking_loss(p, frame, _cpu_render, keep=keep)
+        M.tracking_loss(p, frame, cpu_render, keep=keep)
     assert keep["depth"] > 0
     run = _track(gauss, frame, N, depth_loss_thres=float("nan"))          # never below: the reference continues
     assert _equal(run, base_2n)

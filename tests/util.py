@@ -1,11 +1,72 @@
-"""Shared helpers for the parity tests."""
+"""Shared helpers for the tests."""
 import hashlib
+import importlib.util
+import json
 import os
+import sys
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
+
+
+def load(relpath):
+    """Execute the file at `relpath` (relative to the repository root, or absolute) as a module. Every call returns
+    a fresh module object, so a test that monkeypatches a tool changes nothing another test sees."""
+    path = os.path.join(ROOT, relpath)
+    spec = importlib.util.spec_from_file_location(os.path.splitext(os.path.basename(path))[0], path)
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    return mod
+
+
+def run_tool(tool, argv, monkeypatch, capsys):
+    """Run a tool module's main() with `argv` as sys.argv; return the last line it printed, parsed as JSON."""
+    monkeypatch.setattr(sys, "argv", argv)
+    tool.main()
+    return json.loads(capsys.readouterr().out.strip().splitlines()[-1])
+
+
+def cpu_render(settings, means3D, means2D, opacities, colors_precomp, scales, rotations):
+    """The float32 brute-force composite of oracle/bruteforce_torch.py as the `render(settings, **rendervar)`
+    callable the mapper and the SLAM loop take."""
+    import torch
+    from oracle import bruteforce_torch as BF
+    out = BF.render(means3D, colors_precomp, opacities, scales, rotations, width=settings.image_width,
+                    height=settings.image_height, tanfovx=settings.tanfovx, tanfovy=settings.tanfovy, bg=settings.bg,
+                    viewmatrix=settings.viewmatrix[0], projmatrix=settings.projmatrix[0], means2D=means2D,
+                    dtype=torch.float32)
+    return out["color"], out["radii"], out["depth"]
+
+
+def bits_equal(a, b):
+    """Same shape, dtype and bytes, except that NaNs compare by position only: a NaN that arithmetic produces (the
+    inverse of ScanNet's -inf pose, for one) has no portable sign or payload."""
+    a, b = np.asarray(a), np.asarray(b)
+    if a.shape != b.shape or a.dtype != b.dtype:
+        return False
+    if a.dtype.kind in "fc":
+        na, nb = np.isnan(a), np.isnan(b)
+        if not np.array_equal(na, nb):
+            return False
+        a, b = np.where(na, 0, a), np.where(nb, 0, b)
+    return a.tobytes() == b.tobytes()
+
+
+def look_at(cam, target, up=(0.0, 1.0, 0.0)):
+    """Float64 world-to-camera matrix of a camera at `cam` looking at `target`, x = fwd x up, y = fwd x x (image
+    down for the default `up`); a view direction parallel to `up` takes x = fwd x (1, 0, 0) instead."""
+    fwd = np.asarray(target, np.float64) - cam
+    fwd /= np.linalg.norm(fwd)
+    right = np.cross(fwd, up)
+    if np.linalg.norm(right) < 1e-6:
+        right = np.cross(fwd, [1.0, 0.0, 0.0])
+    right /= np.linalg.norm(right)
+    R = np.stack([right, np.cross(fwd, right), fwd])
+    w2c = np.eye(4)
+    w2c[:3, :3], w2c[:3, 3] = R, -R @ cam
+    return w2c
 
 
 def rel_err(a, b, floor_frac=1e-6):

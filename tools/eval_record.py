@@ -19,7 +19,6 @@ by default <record dir>/eval_train or <record dir>/eval_nvs.  --frames N evaluat
   python tools/eval_record.py --dataset replicav2 --basedir data/ReplicaV2 --sequence room_0 \\
       --record runs/room_0/params.npz --split test"""
 import argparse
-import importlib.util
 import json
 import os
 import sys
@@ -27,17 +26,9 @@ import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 import torch  # noqa: E402
-
-
-def _run_slam_dataset():
-    spec = importlib.util.spec_from_file_location("run_slam_dataset", os.path.join(ROOT, "tools", "run_slam_dataset.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-RSD = _run_slam_dataset()
+import run_slam_dataset as RSD  # noqa: E402
 
 
 def parse_args(argv=None):

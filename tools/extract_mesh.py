@@ -15,7 +15,6 @@ record's image size.  One GPU.
   python tools/extract_mesh.py --record runs/room0/params.npz --out runs/room0/mesh_input.ply --source input \
       --dataset replica --basedir data/Replica --sequence room0 --stride 2"""
 import argparse
-import importlib.util
 import json
 import os
 import sys
@@ -23,6 +22,7 @@ import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 import torch  # noqa: E402
 
 
@@ -70,7 +70,7 @@ def open_input(a, record, device):
     config, start, end and stride, capped at --frames -- read at the record's image size.  Returns (sequence, frames);
     ValueError, with the sequence closed, when the selected frame count differs from the record's camera count."""
     from splatam_b200 import datasets, formats
-    rsd = _run_slam_dataset()
+    import run_slam_dataset as rsd
     raw = formats.read_record(record, formats.CHECKPOINT_KEYS + formats.CAMERA_KEYS)
     T = raw["cam_unnorm_rots"].shape[-1]
     height, width = int(raw["org_height"]), int(raw["org_width"])
@@ -84,13 +84,6 @@ def open_input(a, record, device):
                          "the flags of the run" % (record, T, a.start, a.end, a.stride, a.frames, len(frames),
                                                    a.sequence))
     return seq, frames
-
-
-def _run_slam_dataset():
-    spec = importlib.util.spec_from_file_location("run_slam_dataset", os.path.join(ROOT, "tools", "run_slam_dataset.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
 
 
 def main(argv=None):

@@ -15,8 +15,7 @@ dev = torch.device("cuda:0")
 sc = scenes.room(seed=4, P=1_000_000)
 cam = sc.settings(S.GaussianRasterizationSettings, dev)
 g = torch.Generator().manual_seed(0)
-gauss = {k: v.to(dev) for k, v in dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-         logit_opacities=torch.logit(sc.opacities.clamp(0.02, 0.98)), log_scales=torch.log(sc.scales[:, :1])).items()}
+gauss = sc.splatam_params(dev)
 rots = torch.zeros(1, 4, 8); rots[:, 0] = 1.0
 trans = 0.02 * torch.randn(1, 3, 8, generator=g)
 frames = [dict(id=t, cam=cam, w2c=torch.eye(4, device=dev), im=torch.rand(3, sc.h, sc.w, generator=g).to(dev),

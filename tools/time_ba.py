@@ -22,7 +22,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import scenes  # noqa: E402
-from time_ingest import gpu_info  # noqa: E402
+from gpu_info import gpu_info  # noqa: E402
 
 CAM_LRS = dict(cam_unnorm_rots=0.0004, cam_trans=0.002)
 

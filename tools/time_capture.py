@@ -11,7 +11,6 @@
 import argparse
 import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
@@ -21,12 +20,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
-
-
-def gpu_info():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown"
+from gpu_info import gpu_info  # noqa: E402
 
 
 def event_ms(fn, n):

@@ -15,7 +15,9 @@ import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 import torch  # noqa: E402
+from gpu_info import gpu_info  # noqa: E402
 
 
 def main():
@@ -27,7 +29,7 @@ def main():
     from splatam_b200 import formats, mapping as M, slam
     dev = torch.device("cuda", 0)
     g = torch.Generator(device=dev).manual_seed(0)
-    name = torch.cuda.get_device_name(dev)
+    name = gpu_info()
     for P in a.gaussians:
         gauss = dict(means3D=torch.randn(P, 3, device=dev, generator=g), rgb_colors=torch.rand(P, 3, device=dev, generator=g),
                      unnorm_rotations=torch.randn(P, 4, device=dev, generator=g),

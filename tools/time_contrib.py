@@ -25,7 +25,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import scenes  # noqa: E402
-from time_ingest import gpu_info  # noqa: E402
+from gpu_info import gpu_info  # noqa: E402
 
 
 def stats_pass(dev, reps):
@@ -74,8 +74,7 @@ def compact_timing(dev, views, base):
     idx = torch.arange(views) % 40
     rots, trans = r40[..., idx].contiguous(), t40[..., idx].contiguous()
     K = np.array([[sc.fx, 0, sc.cx], [0, sc.fy, sc.cy], [0, 0, 1]], np.float32)
-    gauss = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-                 logit_opacities=torch.logit(sc.opacities.clamp(1e-4, 1 - 1e-4)), log_scales=torch.log(sc.scales[:, :1]))
+    gauss = sc.splatam_params(opacity_clamp=(1e-4, 1 - 1e-4))
     path = formats.save_run_record(os.path.join(base, "big"), gauss, rots, trans, torch.zeros(sc.P), K, np.eye(4),
                                    sc.w, sc.h, [np.eye(4, dtype=np.float32)] * views, list(range(views)))
     out = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "compact_record.py"), "--record", path, "--out",

@@ -19,24 +19,16 @@ Run:  python tools/time_eval.py [--frames 200] [--reps 100] [--ref-frames 5] [--
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 import torch  # noqa: E402
 
 import scenes  # noqa: E402
-
-
-def gpu_info():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                           text=True, check=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:          # the name still comes from torch
-        q = "%s, power limit unknown (%s)" % (torch.cuda.get_device_name(0), e)
-    return q
+from gpu_info import gpu_info  # noqa: E402
 
 
 def reference_metrics(im, depth_sil, gt_im, gt_depth, sil_thres, use_presence):
@@ -70,8 +62,7 @@ def time_nvs(frames_n, sil_thres):
         cam_d = dict(w=w, h=h, fx=w / 2.0, fy=w / 2.0, cx=(w - 1) / 2.0, cy=(h - 1) / 2.0)
         sc = scenes.view_filling(margin=100, cam=cam_d)
         cam = sc.settings(S.GaussianRasterizationSettings, dev)
-        gt = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-                  logit_opacities=torch.logit(sc.opacities.reshape(-1, 1)), log_scales=torch.log(sc.scales[:, :1]))
+        gt = sc.splatam_params(opacity_clamp=None)
         gt = {k: v.to(dev).contiguous() for k, v in gt.items()}
         rots, trans = slam.look_trajectory(frames_n, dev, step=(0.002, -0.001, 0.001), rot_step=(0.0005, -0.0004, 0.0003))
         frames = [slam.render_frame(gt, rots, trans, t, cam) for t in range(frames_n)]
@@ -171,8 +162,7 @@ def time_lpips(frames_n, reps, sil_thres):
     # evaluate() with and without LPIPS on a 1200x680 view-filling map, run alternately
     sc = scenes.view_filling(margin=100)
     cam = sc.settings(S.GaussianRasterizationSettings, dev)
-    gt = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-              logit_opacities=torch.logit(sc.opacities.reshape(-1, 1)), log_scales=torch.log(sc.scales[:, :1]))
+    gt = sc.splatam_params(opacity_clamp=None)
     gt = {k: v.to(dev).contiguous() for k, v in gt.items()}
     rots, trans = slam.look_trajectory(frames_n, dev, step=(0.002, -0.001, 0.001), rot_step=(0.0005, -0.0004, 0.0003))
     frames = [slam.render_frame(gt, rots, trans, t, cam) for t in range(frames_n)]
@@ -217,8 +207,7 @@ def main():
     print("GPU:", gpu_info(), flush=True)
     sc = scenes.view_filling(margin=100)          # surface beyond the borders: the moving camera sees a covered view
     cam = sc.settings(S.GaussianRasterizationSettings, dev)
-    gt = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-              logit_opacities=torch.logit(sc.opacities.reshape(-1, 1)), log_scales=torch.log(sc.scales[:, :1]))
+    gt = sc.splatam_params(opacity_clamp=None)
     gt = {k: v.to(dev).contiguous() for k, v in gt.items()}
     T = args.frames
     rots, trans = slam.look_trajectory(T, dev, step=(0.002, -0.001, 0.001), rot_step=(0.0005, -0.0004, 0.0003))

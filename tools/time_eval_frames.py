@@ -13,26 +13,19 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import tempfile
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 import torch  # noqa: E402
 
 import scenes  # noqa: E402
+from gpu_info import gpu_info  # noqa: E402
 
 BYTES_PER_PIXEL = 4 * (3 + 1 + 3 + 1) + 4 * 3
-
-
-def gpu_info():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                              capture_output=True, text=True, check=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:          # the name still comes from torch
-        return "%s, power limit unknown (%s)" % (torch.cuda.get_device_name(0), e)
 
 
 def time_kernel(reps):
@@ -78,8 +71,7 @@ def time_evaluate(frames_n, d):
     dev = torch.device("cuda:0")
     sc = scenes.view_filling(margin=100)
     cam = sc.settings(S.GaussianRasterizationSettings, dev)
-    gt = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-              logit_opacities=torch.logit(sc.opacities.reshape(-1, 1)), log_scales=torch.log(sc.scales[:, :1]))
+    gt = sc.splatam_params(opacity_clamp=None)
     gt = {k: v.to(dev).contiguous() for k, v in gt.items()}
     rots, trans = slam.look_trajectory(frames_n, dev, step=(0.002, -0.001, 0.001), rot_step=(0.0005, -0.0004, 0.0003))
     frames = [slam.render_frame(gt, rots, trans, t, cam) for t in range(frames_n)]

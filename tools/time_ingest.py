@@ -17,26 +17,18 @@ Run:  python tools/time_ingest.py [--frames 40] [--reps 200] [--dir DIR]"""
 import argparse
 import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 import scenes  # noqa: E402
-
-
-def gpu_info():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                           text=True, check=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:          # the name still comes from torch
-        q = "%s, power limit unknown (%s)" % (torch.cuda.get_device_name(0), e)
-    return q
+from gpu_info import gpu_info  # noqa: E402
 
 
 def reference_frame(files, t, dev):

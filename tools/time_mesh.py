@@ -8,7 +8,6 @@
 
   python tools/time_mesh.py [--gaussians 1000000] [--frames 2000] [--voxel 0.02] [--reps 20]"""
 import argparse
-import importlib.util
 import json
 import os
 import sys
@@ -17,18 +16,13 @@ import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
+import time_viewer as TV  # noqa: E402
+from gpu_info import gpu_info  # noqa: E402
 
 
-def _time_viewer():
-    spec = importlib.util.spec_from_file_location("time_viewer", os.path.join(ROOT, "tools", "time_viewer.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-TV = _time_viewer()
 H, W = 680, 1200
 K = np.array([[600.0, 0, 599.5], [0, 600.0, 339.5], [0, 0, 1]], np.float32)
 
@@ -58,7 +52,7 @@ def main():
     from splatam_b200.mesh import TSDFVolume, mesh_record
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
-    out = dict(gpu=TV.gpu_info(), frame=[W, H])
+    out = dict(gpu=gpu_info(), frame=[W, H])
     depth, rgb, w2c = frames(32, dev)
     for n in (256, 512):
         # a 4 m cube from z = 0.5: the frustum holds most of it, the wall's band a tenth

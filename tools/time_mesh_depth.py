@@ -13,7 +13,6 @@ prints one JSON line with the card's name and power limit:
 
   python tools/time_mesh_depth.py [--side 1000] [--frames 2000] [--views 1000] [--reps 5]"""
 import argparse
-import importlib.util
 import json
 import os
 import sys
@@ -21,18 +20,13 @@ import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
+import time_mesh_eval as TME  # noqa: E402
+from gpu_info import gpu_info  # noqa: E402
 
 
-def _time_mesh_eval():
-    spec = importlib.util.spec_from_file_location("time_mesh_eval", os.path.join(ROOT, "tools", "time_mesh_eval.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-TME = _time_mesh_eval()
 floor_mesh = TME.floor_mesh
 
 SIZES = {"500x500": (500, 500, np.array([[300.0, 0, 249.5], [0, 300.0, 249.5], [0, 0, 1]])),
@@ -65,7 +59,7 @@ def main():
     from splatam_b200 import mesh_eval as E
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
-    out = dict(gpu=TME.TV.gpu_info())
+    out = dict(gpu=gpu_info())
     fv, ff = floor_mesh(a.side)
     out["floor_V_F"] = [len(fv), len(ff)]
     screen_v = np.array([[-10, -10, 1], [10, -10, 1], [10, 10, 1], [-10, 10, 1]], np.float32)

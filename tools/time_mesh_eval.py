@@ -11,7 +11,6 @@ the card's name and power limit:
 
   python tools/time_mesh_eval.py [--side 1000] [--frames 2000] [--reps 5]"""
 import argparse
-import importlib.util
 import json
 import os
 import sys
@@ -19,21 +18,14 @@ import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
+import time_viewer as TV  # noqa: E402
+from gpu_info import gpu_info  # noqa: E402
 
 H, W = 680, 1200
 K = np.array([[600.0, 0, 599.5], [0, 600.0, 339.5], [0, 0, 1]], np.float32)
-
-
-def _time_viewer():
-    spec = importlib.util.spec_from_file_location("time_viewer", os.path.join(ROOT, "tools", "time_viewer.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-TV = _time_viewer()
 
 
 def floor_mesh(side):
@@ -72,7 +64,7 @@ def main():
     from splatam_b200 import _lib, mesh_eval as E
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
-    out = dict(gpu=TV.gpu_info(), frame=[W, H], frames=a.frames)
+    out = dict(gpu=gpu_info(), frame=[W, H], frames=a.frames)
     gv, gf = floor_mesh(a.side)
     out["gt_mesh_V_F"] = [len(gv), len(gf)]
     w2c, depth = cameras(a.frames, dev)

@@ -15,26 +15,19 @@ call.  Prints one JSON line per image size and one for the statistic.
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 import torch  # noqa: E402
 
 import scenes  # noqa: E402
+from gpu_info import gpu_info  # noqa: E402
 
 SIZES = {"1200x680": scenes.REPLICA,
          "876x584": dict(w=876, h=584, fx=438.0, fy=438.0, cx=437.5, cy=291.5)}
-
-
-def gpu_info():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                              capture_output=True, text=True, check=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:          # the name still comes from torch
-        return "%s, power limit unknown (%s)" % (torch.cuda.get_device_name(0), e)
 
 
 def time_loop(P, cam, iters, warmup, dev):
@@ -42,8 +35,7 @@ def time_loop(P, cam, iters, warmup, dev):
     from splatam_b200 import mapping as M, offline, slam
     sc = scenes.config3(P=P, cam=cam)
     settings = sc.settings(S.GaussianRasterizationSettings, dev)
-    gt = dict(means3D=sc.means3D, rgb_colors=sc.colors, unnorm_rotations=sc.rotations,
-              logit_opacities=torch.logit(sc.opacities), log_scales=torch.log(sc.scales[:, :1]))
+    gt = sc.splatam_params(opacity_clamp=None)
     gt = {k: v.to(dev).contiguous() for k, v in gt.items()}
     rots, trans = slam.look_trajectory(4, dev)
     frames = [slam.render_frame(gt, rots, trans, t, settings) for t in range(4)]

@@ -12,7 +12,10 @@ import sys
 
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+from gpu_info import gpu_info  # noqa: E402
 
 
 def median_us(fn, reps):
@@ -82,7 +85,7 @@ def main():
         res["prepare_bwd_kernel_us"].append(median_us(prep_bwd_kernel, a.reps))
         res["image_loss_fwd_bwd_us"].append(median_us(img, a.reps))
         res["masked_l1_fwd_bwd_us"].append(median_us(masked, a.reps))
-    res.update(P=P, gpu=torch.cuda.get_device_name(dev))
+    res.update(P=P, gpu=gpu_info())
     print(json.dumps(res))
 
 

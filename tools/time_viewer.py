@@ -14,23 +14,16 @@ Run:  python tools/time_viewer.py [--gaussians 1000000] [--frames 2000] [--reps 
 import argparse
 import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
-
-
-def gpu_info():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                              capture_output=True, text=True, check=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:          # the name still comes from torch
-        return "%s, power limit unknown (%s)" % (torch.cuda.get_device_name(0), e)
+from gpu_info import gpu_info  # noqa: E402
 
 
 def synthetic_record(path, P, T, seed=0):
@@ -81,8 +74,9 @@ def main():
     a = ap.parse_args()
     from splatam_b200 import viewer as V
     dev = torch.device("cuda:0")
-    print(gpu_info(), flush=True)
-    out = dict(gpu=torch.cuda.get_device_name(0), gaussians=a.gaussians, timesteps=a.frames)
+    gpu = gpu_info()
+    print(gpu, flush=True)
+    out = dict(gpu=gpu, gaussians=a.gaussians, timesteps=a.frames)
     with tempfile.TemporaryDirectory() as tmp:
         rec = V.load_record(synthetic_record(tmp, a.gaussians, a.frames), dev)
         assert rec.monotone
