@@ -511,6 +511,51 @@ SB_API int sb_mesh_depth(int v, const float* vertices, int f, const int* faces, 
                          const float* w2c, float fx, float fy, float cx, float cy, float near, void* workspace,
                          size_t workspace_bytes, float* depth, int* face_id, void* stream);
 
+/* ---- pose initialisation: projective point-to-plane ICP (splatam_b200/icp.py, csrc/icp.cu) -----------------------
+ * sb_icp_align: the pose of frame t from its sensor depth and the map's depth rendered at frame t-1's pose.
+ *   model_depth_sil float32 [2,H,W] (depth_acc, silhouette of the depth/silhouette render at w2c_prev), data_depth
+ *   float32 [H,W] (frame t), one pinhole fx, fy, cx, cy (a pixel's centre at its integer coordinates), w2c_prev and
+ *   w2c_init float32 [4,4] row-major on the device (rows 0..2 read; w2c_init is the constant-velocity guess),
+ *   iters: host int[SB_ICP_LEVELS], the iterations of levels 0 (full size), 1, 2.  Float32, each operation rounded as
+ *   written; oracle/icp_numpy.py restates the rule.
+ *   1. Level 0: model depth = depth_acc / sil where sil > 0.99 and the quotient is finite and positive, else 0
+ *      (invalid); data depth = the sensor depth where finite and positive, else 0.
+ *   2. Level l + 1 (H >> 1, W >> 1): pixel (x, y) averages, in the order (2x,2y), (2x+1,2y), (2x,2y+1), (2x+1,2y+1),
+ *      the block's valid samples within 0.05 m of the block's smallest one (sum / count), 0 if none is valid.
+ *      Intrinsics: fx/2, fy/2, (cx - 0.5)/2, (cy - 0.5)/2.
+ *   3. Vertex (u, v) = ((u - cx)/fx z, (v - cy)/fy z, z), 0 where invalid.  Model normal = cross(V(u+1) - V(u-1),
+ *      V(v+1) - V(v-1)) / its norm, 0 (invalid) on the border, where a neighbour is invalid or where
+ *      |z_neighbour - z| fx > 5 z (fx of the level).
+ *   4. T = w2c_prev inv(w2c_init) (double; camera t -> camera t-1).  Levels 2, 1, 0, iters[l] times each: every valid
+ *      data vertex v goes to p = R v + t (T rounded to float32), is projected to (floor(fx px/pz + cx + 0.5),
+ *      floor(fy py/pz + cy + 0.5)) and pairs with the model vertex q and normal n there if pz > 0, the pixel is in
+ *      the image, q and n are valid and |p - q|^2 <= (0.1 2^l m)^2.  r = n.(p - q), J = [p x n, n]; JtJ, Jtr,
+ *      sum r^2 and the counts are summed in double in a fixed order (the result does not depend on the run).  One
+ *      thread solves JtJ xi = -Jtr by Cholesky and sets T <- exp(xi) T; with fewer than 32 pairs or a matrix that
+ *      is not positive definite the update is skipped.
+ *   5. Accepted iff the last iteration had inliers / valid data pixels >= 0.4, RMS r <= 0.03 m, smallest / largest
+ *      Cholesky pivot >= 1e-5 and its update was applied.  w2c_out [4,4] = inv(T) w2c_prev (double, rounded) if
+ *      accepted, else w2c_init.
+ *   stats double[SB_ICP_STATS]: 0 accepted (1/0), 1 inlier fraction, 2 RMS residual [m], 3 inliers, 4 valid data
+ *   pixels, 5 pivot ratio (0: not positive definite or too few pairs), 6 some update skipped, 7 the last update
+ *   skipped -- all of the last iteration --, 8..28 its JtJ (upper triangle, row-major), 29..34 its Jtr, 35 its sum r^2.
+ *   No host synchronisation: the call can be captured into a CUDA graph.
+ * sb_icp_export: copies level `level`'s maps out of a workspace an sb_icp_align call has filled (stream-ordered):
+ *   model_depth, data_depth [H_l, W_l], model_vertex, model_normal, data_vertex [3, H_l, W_l] (x, y, z planes) and
+ *   assoc uint8 [H_l, W_l] (0 no valid data, 1 not paired, 2 paired) of the latest iteration at that level.
+ * SB_ERR_BAD_ARG, before any launch, for null pointers, H or W < 4, H W >= 2^31, a non-finite camera, fx or fy <= 0,
+ * iterations outside [0, 1000] and a level outside [0, SB_ICP_LEVELS); SB_ERR_WORKSPACE for a workspace smaller than
+ * sb_icp_workspace_bytes gives. */
+#define SB_ICP_LEVELS 3
+#define SB_ICP_STATS 36
+SB_API int sb_icp_workspace_bytes(int height, int width, size_t* bytes);
+SB_API int sb_icp_align(int height, int width, const float* model_depth_sil, const float* data_depth, float fx,
+                        float fy, float cx, float cy, const float* w2c_prev, const float* w2c_init, const int* iters,
+                        void* workspace, size_t workspace_bytes, float* w2c_out, double* stats, void* stream);
+SB_API int sb_icp_export(int height, int width, const void* workspace, size_t workspace_bytes, int level,
+                         float* model_depth, float* data_depth, float* model_vertex, float* model_normal,
+                         float* data_vertex, uint8_t* assoc, void* stream);
+
 /* ---- per-stage device timing (measurement only; bench.py's roofline pass) -------------------
  * Between sb_profile_begin() and sb_profile_end() every stage launch of this process is bracketed
  * by CUDA events on its stream.  sb_profile_end synchronises, writes the summed milliseconds and call

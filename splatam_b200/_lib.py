@@ -111,6 +111,9 @@ _SIGNATURES = {
     "sb_nn_query": (_i, [_i, _vp, _i, _f, _f, _f, _f, _i, _i, _i, _vp, _sz, _vp, _vp]),
     "sb_mesh_depth_workspace_bytes": (_i, [_i, _i, _i, _i, ctypes.POINTER(_sz)]),
     "sb_mesh_depth": (_i, [_i, _vp, _i, _vp, _i, _i, _i, _vp, _f, _f, _f, _f, _f, _vp, _sz, _vp, _vp, _vp]),
+    "sb_icp_workspace_bytes": (_i, [_i, _i, ctypes.POINTER(_sz)]),
+    "sb_icp_align": (_i, [_i, _i, _vp, _vp, _f, _f, _f, _f, _vp, _vp, ctypes.POINTER(_i), _vp, _sz, _vp, _vp, _vp]),
+    "sb_icp_export": (_i, [_i, _i, _vp, _sz, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "sb_profile_begin": (_i, []),
     "sb_profile_end": (_i, [ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_int)]),
     "sb_stage_name": (ctypes.c_char_p, [_i]),

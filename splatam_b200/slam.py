@@ -140,7 +140,7 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
              window=4, fused=None, seed=0, intrinsics=None, add_new_gaussians=False, sil_thres=0.5, prune_dict=None,
              scene_radius=None, select_keyframes=False, checkpoint_dir=None, first_frame_iters=0, map_every=None,
              graph=False, timing=None, densify_dict=None, tracking_lrs=(0.0004, 0.002), depth_loss_thres=None,
-             checkpoint_every=None, resume=None, mapping_cam_lrs=(0.0, 0.0)):
+             checkpoint_every=None, resume=None, mapping_cam_lrs=(0.0, 0.0), pose_init="constant_velocity"):
     """Tracks every frame and maps on keyframes.  gauss_init: dict of the five Gaussian tensors (the map's
     starting point); frames: list of dict(id, cam, w2c, im, depth).  Returns dict(rots, trans, psnr, gauss, counts,
     timestep, keyframe_time_indices, keyframe_est_w2c): `timestep` is the frame that created each Gaussian of the final
@@ -166,6 +166,13 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     keyframe list with its pose after its own mapping phase, as the reference stores it.  `timing`: dict that receives
     the accumulated wall seconds of tracking / mapping (synchronised), the tracking and mapping iteration counts, and
     `setup_s`, the wall seconds from the call to the start of the frame loop.
+    `pose_init`: how each frame's tracking starts.  "constant_velocity" (the default) is the reference's guess
+    (splatam.py:423-444).  "icp" follows that guess with icp.init_pose: the map's depth rendered at frame t-1's pose is
+    aligned with frame t's depth by point-to-plane ICP on the GPU (needs CUDA tensors and `intrinsics`), and the ICP
+    pose replaces the guess when it passes its acceptance test.  Every rank computes the same pose.  With "icp",
+    `timing` also receives `pose_init_s` (synchronised wall seconds) and the result holds `icp`: per tracked frame
+    dict(frame, accepted, inlier_frac, rms), read from the device once at the end.  `pose_init` is not stored in
+    checkpoints: a resumed run passes it again.
 
     Checkpoints and resume (R/scripts/splatam.py:604-643,927-931).  With `checkpoint_dir` and `checkpoint_every` = N,
     after frame t's mapping and keyframe step, for every t % N == 0 (frame 0 included, after `first_frame_iters`),
@@ -189,6 +196,17 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     timing.update(tracking_s=0.0, mapping_s=0.0, mapping_iters=0, tracking_iters=0, setup_s=0.0)
     T = len(frames)
     _check_resume(gauss_init, resume, T, checkpoint_every, checkpoint_dir)
+    if pose_init not in ("constant_velocity", "icp"):
+        raise ValueError("pose_init must be 'constant_velocity' or 'icp', got %r" % (pose_init,))
+    use_icp = pose_init == "icp"
+    if use_icp:
+        if intrinsics is None:
+            raise ValueError("pose_init='icp' needs the intrinsics")
+        from . import _lib, icp
+        _lib.need_cuda("run_slam(pose_init='icp')", (gauss_init or resume["gauss"])["means3D"])
+        K_icp = np.asarray(torch.as_tensor(intrinsics).detach().cpu(), dtype=np.float64)
+        timing["pose_init_s"] = 0.0
+        icp_stats = []
     kw = {} if render is None else {"render": render}
     track_m2d = densify_dict is not None
     kw["lrs"] = dict(cam_unnorm_rots=float(mapping_cam_lrs[0]), cam_trans=float(mapping_cam_lrs[1]))
@@ -248,6 +266,11 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
                 trans[0, :, t] = trans[0, :, t - 1]
         params = dict({k: v.detach() for k, v in mapper.g.params.items()}, cam_unnorm_rots=rots, cam_trans=trans)
         torch.cuda.synchronize(dev) if dev.type == "cuda" else None
+        if use_icp:
+            t0 = time.perf_counter()
+            icp_stats.append(icp.init_pose(params, frames[t], t, K_icp, render=render, fused=fused))
+            torch.cuda.synchronize(dev)
+            timing["pose_init_s"] += time.perf_counter() - t0
         t0 = time.perf_counter()
         losses = M.track_frame(params, frames[t], render=render, num_iters=tracking_iters, lr_rot=tracking_lrs[0],
                                lr_trans=tracking_lrs[1], fused=fused, depth_loss_thres=depth_loss_thres)
@@ -310,9 +333,14 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     if checkpoint_dir is not None and (checkpoint_every is None or mapper.rank == 0):
         from . import formats
         formats.save_params(dict(final, cam_unnorm_rots=rots, cam_trans=trans), checkpoint_dir)
-    return dict(rots=rots, trans=trans, psnr=sum(vals) / len(vals), gauss=final, counts=counts,
-                timestep=mapper.timestep.detach().clone(), keyframe_time_indices=[int(kf["id"]) for kf in keyframes],
-                keyframe_est_w2c=[kf["est_w2c"] for kf in keyframes])
+    out = dict(rots=rots, trans=trans, psnr=sum(vals) / len(vals), gauss=final, counts=counts,
+               timestep=mapper.timestep.detach().clone(), keyframe_time_indices=[int(kf["id"]) for kf in keyframes],
+               keyframe_est_w2c=[kf["est_w2c"] for kf in keyframes])
+    if use_icp:
+        st = torch.stack(icp_stats).cpu().numpy() if icp_stats else np.zeros((0, icp.STATS))
+        out["icp"] = [dict(frame=start + i, accepted=bool(s[0]), inlier_frac=float(s[1]), rms=float(s[2]))
+                      for i, s in enumerate(st)]
+    return out
 
 
 def w2c_list(rots, trans):

@@ -13,7 +13,8 @@ frame, keyframe_every = frames // 5 below 25 frames (else 5), tracking rates (0.
 20000, scene radius = max depth / 3.  --out receives rgb/N.png, depth/N.png and transforms.json (which
 `run_slam_dataset.py --dataset nerfcapture` reads back) and the reference's params.npz (formats.save_run_record;
 org_width / org_height the tracking size, gt_w2c_all_frames the ARKit poses), which eval_record.py and
-render_record.py open.  --capture-only writes the capture without SLAM, as nerfcapture2dataset.py does.  Prints one
+render_record.py open.  --pose-init icp starts each frame's tracking from a point-to-plane ICP alignment of its
+depth with the map's (splatam_b200.icp; default constant_velocity, the reference's guess).  --capture-only writes the capture without SLAM, as nerfcapture2dataset.py does.  Prints one
 JSON line: ATE against the ARKit poses (the reference's Horn-aligned mean), Gaussian count, wall times, frames/s."""
 import argparse
 import json
@@ -34,7 +35,8 @@ HYPER = dict(height=720, width=960, densify_height=360, densify_width=480, downs
 SIL_THRES = 0.5
 
 
-def run(packets, frames, out, capture_only=False, device="cuda:0", tracking_iters=None, mapping_iters=None):
+def run(packets, frames, out, capture_only=False, device="cuda:0", tracking_iters=None, mapping_iters=None,
+        pose_init="constant_velocity"):
     """The demo over an iterable of CaptureFrame packets; returns the JSON-able result dict."""
     from splatam_b200 import capture, formats, slam
     sys.path.insert(0, os.path.join(ROOT, "tools"))
@@ -66,12 +68,14 @@ def run(packets, frames, out, capture_only=False, device="cuda:0", tracking_iter
                               map_every=h["map_every"], window=h["window"], sil_thres=SIL_THRES, intrinsics=K,
                               add_new_gaussians=True, prune_dict=_PRUNE, scene_radius=radius, select_keyframes=True,
                               first_frame_iters=h["mapping_iters"], tracking_lrs=h["tracking_lrs"],
-                              depth_loss_thres=h["depth_loss_thres"])
+                              depth_loss_thres=h["depth_loss_thres"], pose_init=pose_init)
             torch.cuda.synchronize(dev)
             est = slam.w2c_list(o["rots"], o["trans"])
             res.update(ate_m=slam.ate_horn(seq.gt_w2c, est), gaussians=int(o["counts"][-1]),
                        tracking_s=timing["tracking_s"], mapping_s=timing["mapping_s"],
-                       tracking_iters=timing["tracking_iters"])
+                       tracking_iters=timing["tracking_iters"], pose_init=pose_init)
+            if pose_init == "icp":
+                res.update(pose_init_s=timing["pose_init_s"], icp_accepted=sum(s["accepted"] for s in o["icp"]))
             formats.save_run_record(out, o["gauss"], o["rots"], o["trans"], o["timestep"], K, seq.w2c, seq.width,
                                     seq.height, seq.gt_w2c, o["keyframe_time_indices"])
     torch.cuda.synchronize(dev)
@@ -91,6 +95,8 @@ def main():
     ap.add_argument("--tracking-iters", type=int, default=0)
     ap.add_argument("--mapping-iters", type=int, default=0)
     ap.add_argument("--seed", type=int, default=14, help="generating scene of --source synthetic")
+    ap.add_argument("--pose-init", default="constant_velocity", choices=("constant_velocity", "icp"),
+                    help="tracking start: the reference's constant-velocity guess, or that guess refined by ICP")
     a = ap.parse_args()
     if not a.capture_only and a.frames < 5:
         ap.error("SLAM needs at least 5 frames (keyframe_every = frames // 5)")
@@ -102,7 +108,7 @@ def main():
         packets = capture.dds_frames(a.domain_id)
     else:
         packets = capture.synthetic_frames(a.frames, dev, seed=a.seed)
-    res = run(packets, a.frames, a.out, a.capture_only, dev, a.tracking_iters, a.mapping_iters)
+    res = run(packets, a.frames, a.out, a.capture_only, dev, a.tracking_iters, a.mapping_iters, a.pose_init)
     res["source"] = a.source
     print(json.dumps(res))
 
