@@ -556,6 +556,51 @@ SB_API int sb_icp_export(int height, int width, const void* workspace, size_t wo
                          float* model_depth, float* data_depth, float* model_vertex, float* model_normal,
                          float* data_vertex, uint8_t* assoc, void* stream);
 
+/* ---- loop closure: map deformation and the keyframe pose graph (splatam_b200/loop.py, csrc/loop.cu) ---------------
+ * A correction is a rigid map from the old world to the new one, float32 [12] row-major 3x4 [R | t]; the table holds
+ * one per frame.  oracle/loop_numpy.py restates every rule below.
+ * sb_deform_gaussians: in place, one thread per Gaussian i, nothing at all if *apply_flag (device int) is 0.  The
+ *   Gaussian takes the correction c of frame timestep[i] (float32 [P], the creation frame); a timestep outside [0, T)
+ *   and an exact identity correction leave it unchanged.  Float32, each operation rounded as written:
+ *     mean:  x'_r = ((c_r0 x + c_r1 y) + c_r2 z) + c_r3 for r = 0, 1, 2;
+ *     q_c:   f0 = ((1 + r00) + r11) + r22, f1 = ((1 + r00) - r11) - r22, f2 = ((1 - r00) + r11) - r22,
+ *            f3 = ((1 - r00) - r11) + r22; k = the first largest; row k of
+ *            [[f0, r21 - r12, r02 - r20, r10 - r01], [r21 - r12, f1, r10 + r01, r02 + r20],
+ *             [r02 - r20, r10 + r01, f2, r12 + r21], [r10 - r01, r02 + r20, r12 + r21, f3]]
+ *            divided by 2 sqrt(max(f_k, 0));
+ *     quaternion (unnormalised, w x y z): q' = q_c q, the Hamilton product with the terms in the order
+ *            w = ((aw bw - ax bx) - ay by) - az bz, x = ((aw bx + ax bw) + ay bz) - az by,
+ *            y = ((aw by - ax bz) + ay bw) + az bx, z = ((aw bz + ax by) - ay bx) + az bw.
+ *   Scales, colours and opacities are not touched.  means3D [P,3] and unnorm_rotations [P,4] need 4-byte alignment.
+ * sb_pose_graph_normal_equations: N nodes (w2c poses, double [N,12]), E edges (device int [E,2]: i, j), measurements
+ *   Z double [E,12] and weights double [E,2] (w_rot, w_trans).  Edge e has the residual r = log(Z T_i T_j^-1) in se(3)
+ *   (tangent order: rotation, translation; the log takes the angle atan2(|vee(R - R^T)| / 2, (tr R - 1) / 2) and
+ *   assumes it is below pi), weighted by
+ *   diag(w_rot I3, w_trans I3), with the left perturbation T <- exp(xi) T:
+ *     d r / d xi_i = Jl^-1(r) Ad(Z), d r / d xi_j = -Jl^-1(r) Ad(Z T_i T_j^-1), Ad(T) = [[R, 0], [t^ R, R]],
+ *     Jl^-1(r) = I - ad(r)/2 + ad(r)^2/12 (the series to the second order), ad(r) = [[phi^, 0], [rho^, phi^]].
+ *   Writes residuals double [E,6], jacobians double [E,72] (the two row-major 6x6 blocks) and the dense normal equations
+ *   of the free nodes 1..N-1 (node 0 is fixed): H double [6(N-1)]^2 = sum_e A^T W A and b double [6(N-1)] = sum_e
+ *   A^T W r, accumulated edge by edge in order, so every call gives the same bits.  An edge with a node outside
+ *   [0, N) or i == j adds nothing and gets NaN residuals.
+ * sb_pose_graph_update: T_n <- exp(xi_n) T_n for n = 1..N-1 (xi double [6(N-1)], node n at 6(n-1)); then every edge's
+ *   E = Z T_i T_j^-1 gives edge_err double [E,2] = (|t_E| in m, its rotation angle in rad, as above) and
+ *   *apply_flag = 1 iff every
+ *   edge has |t_E| <= max_residual_m and angle <= max_residual_rad (NaN fails); then corrections float32 [T,12]:
+ *   frame s takes C = T_n^-1 T_n_old (double, rounded) of node n = frame_node[s] (device int [T]), the exact identity
+ *   where node n did not move or frame_node[s] is outside [0, N).  One block, no host synchronisation.
+ * SB_ERR_BAD_ARG, before any launch, for null pointers, P < 0, T < 1, N outside [2, 20000], E < 1 and negative or NaN
+ * bounds. */
+SB_API int sb_deform_gaussians(int P, float* means3D, float* unnorm_rotations, const float* timestep, int T,
+                               const float* corrections, const int* apply_flag, void* stream);
+SB_API int sb_pose_graph_normal_equations(int N, int E, const double* poses, const int* edges, const double* Z,
+                                          const double* weights, double* residuals, double* jacobians, double* H,
+                                          double* b, void* stream);
+SB_API int sb_pose_graph_update(int N, int E, int T, double* poses, const double* poses_old, const double* xi,
+                                const int* edges, const double* Z, const int* frame_node, double max_residual_m,
+                                double max_residual_rad, float* corrections, int* apply_flag, double* edge_err,
+                                void* stream);
+
 /* ---- per-stage device timing (measurement only; bench.py's roofline pass) -------------------
  * Between sb_profile_begin() and sb_profile_end() every stage launch of this process is bracketed
  * by CUDA events on its stream.  sb_profile_end synchronises, writes the summed milliseconds and call

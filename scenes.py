@@ -556,6 +556,153 @@ def write_replica_sequence(dst, num_frames, device, seed=14, cam=REPLICA, png_de
     return torch.stack(w2cs)
 
 
+LOOP_CAM = dict(w=320, h=192, fx=160.0, fy=160.0, cx=159.5, cy=95.5)
+
+
+def loop_room(seed=21, P=400_000, cam=LOOP_CAM, half=(2.0, 1.2, 2.0), centre=(0.0, 0.0, 0.3)):
+    """A closed box room (half extents `half` [m] around `centre`) whose walls, floor and ceiling are densely covered
+    with opaque, textured, isotropic splats (about 1.2 cm): from anywhere inside, every pixel sees a wall, so the
+    rendered depth behaves like a sensor's.  Faces are drawn in proportion to their area."""
+    g = torch.Generator().manual_seed(seed)
+    h = torch.tensor(half)
+    area = torch.tensor([h[1] * h[2], h[1] * h[2], h[0] * h[2], h[0] * h[2], h[0] * h[1], h[0] * h[1]])
+    face = torch.multinomial(area / area.sum(), P, replacement=True, generator=g)
+    a, b = _rand(g, P) * 2 - 1, _rand(g, P) * 2 - 1
+    pts = torch.zeros(P, 3)
+    for f in range(6):
+        m = face == f
+        ax = f // 2
+        o = [i for i in range(3) if i != ax]
+        pts[m, ax] = (1.0 if f % 2 else -1.0) * h[ax]
+        pts[m, o[0]] = a[m] * h[o[0]]
+        pts[m, o[1]] = b[m] * h[o[1]]
+    pts = pts + torch.tensor(centre)
+    col = 0.5 + 0.25 * torch.sin(pts * 7.0 + torch.tensor([0.0, 2.0, 4.0])) + 0.2 * torch.sin(
+        pts[:, [1, 2, 0]] * 23.0 + torch.tensor([1.0, 3.0, 5.0]))
+    scales = torch.full((P, 3), 0.012)
+    q = torch.zeros(P, 4)
+    q[:, 0] = 1.0
+    return Scene("loop_room_%d" % P, cam["w"], cam["h"], cam["fx"], cam["fy"], cam["cx"], cam["cy"], pts,
+                 col.clamp(0, 1), torch.full((P,), 0.95), scales, q)
+
+
+def loop_trajectory(num_frames, device, radius=0.3, yaw=25.0):
+    """A camera that travels once around a circle of `radius` [m] in the horizontal plane while its heading swings by
+    up to `yaw` degrees either way, and comes back to where it started: frame s is at angle th = 2 pi s /
+    (num_frames - 1) with heading yaw sin(th), so the last frame repeats frame 0's pose (the identity).  Returns
+    (unnormalised quaternions [1,4,T], translations [1,3,T])."""
+    rots = torch.zeros(1, 4, num_frames, device=device)
+    trans = torch.zeros(1, 3, num_frames, device=device)
+    for s in range(num_frames):
+        th = 2 * math.pi * s / max(num_frames - 1, 1)
+        a = math.radians(yaw) * math.sin(th)
+        c = torch.tensor([radius * math.sin(th), 0.0, radius * (1 - math.cos(th))])
+        R = torch.tensor([[math.cos(a), 0.0, -math.sin(a)], [0.0, 1.0, 0.0], [math.sin(a), 0.0, math.cos(a)]])
+        rots[0, :, s] = torch.tensor([math.cos(a / 2), 0.0, -math.sin(a / 2), 0.0])
+        trans[0, :, s] = (-(R @ c)).to(device)
+    return rots, trans
+
+
+def write_loop_sequence(dst, num_frames, device, seed=21, cam=LOOP_CAM, png_depth_scale=6553.5, quality=95):
+    """Writes a sequence in Replica's on-disk layout (results/frame<t>.jpg, results/depth<t>.png, traj.txt of c2w rows)
+    under `dst`, as write_replica_sequence does: the frames are rendered on `device` from `loop_room` along
+    `loop_trajectory`, a camera inside a densely walled room that comes back to where it started.  Depth is
+    alpha-normalised, 0 where the silhouette is below 0.9.  Returns the ground-truth w2c matrices [T,4,4] (CPU)."""
+    import os
+    from PIL import Image
+    import splatam_b200 as S
+    from splatam_b200 import mapping as M, slam
+    sc = loop_room(seed=seed, cam=cam)
+    rs = sc.settings(S.GaussianRasterizationSettings, device)
+    gt = sc.splatam_params(device)
+    rots, trans = loop_trajectory(num_frames, device)
+    os.makedirs(os.path.join(dst, "results"), exist_ok=True)
+    w2cs, traj = [], []
+    for t in range(num_frames):
+        f = slam.render_frame(gt, rots, trans, t, rs)
+        depth = torch.where(f["sil"] > 0.9, f["depth"] / f["sil"].clamp(min=1e-6), torch.zeros_like(f["depth"]))
+        rgb = (f["im"].clamp(0, 1) * 255).round().to(torch.uint8).permute(1, 2, 0).cpu().numpy()
+        raw = (depth[0] * png_depth_scale).round().clamp(0, 65535).cpu().numpy().astype(np.uint16)
+        Image.fromarray(rgb).save(os.path.join(dst, "results", "frame%06d.jpg" % t), quality=quality)
+        Image.fromarray(raw).save(os.path.join(dst, "results", "depth%06d.png" % t))
+        w2c = M.camera_w2c(rots[..., t], trans[..., t])[0].detach().double().cpu()
+        w2cs.append(w2c)
+        traj.append(" ".join("%.17g" % v for v in torch.linalg.inv(w2c).reshape(-1).tolist()))
+    with open(os.path.join(dst, "traj.txt"), "w") as fh:
+        fh.write("\n".join(traj) + "\n")
+    return torch.stack(w2cs)
+
+
+def loop_data_config(cam=LOOP_CAM, png_depth_scale=6553.5):
+    """The data config (datasets.load_config's shape) that reads a `write_loop_sequence` sequence back with
+    datasets.RGBDSequence("replica", ...)."""
+    return dict(camera_params=dict(image_height=cam["h"], image_width=cam["w"], fx=cam["fx"], fy=cam["fy"],
+                                   cx=cam["cx"], cy=cam["cy"], png_depth_scale=png_depth_scale))
+
+
+def drifted_loop(dev, T=81, P=200_000, drift=((0.0, 1.0, 0.0), 0.06, (0.0025, 0.0005, 0.0015)), keyframe_every=5):
+    """A SLAM state that has drifted, built from a ground-truth loop, for loop-closure tests and measurements.  Ground
+    truth: `loop_room` (P Gaussians) seen along `loop_trajectory` (T frames, the last one back at frame 0).  The
+    estimate of frame s is gt_s W^s for the small rigid world drift W = `drift` (axis, degrees, translation [m]) a
+    frame; every `keyframe_every`-th frame is a keyframe; each Gaussian belongs to the first keyframe that sees it
+    (its `timestep`) and sits where that keyframe's drifted pose puts it; keyframes hold colour and depth rendered from
+    the ground truth.  Returns a dict of all of it (see the keys at the end)."""
+    import torch.nn.functional as F
+    import splatam_b200 as SB
+    from oracle import loop_numpy as O
+    from splatam_b200 import mapping as M, slam
+    sc = loop_room(P=P)
+    cam = sc.settings(SB.GaussianRasterizationSettings, dev)
+    gt = {k: v.contiguous() for k, v in sc.splatam_params(dev).items()}
+    rots_gt, trans_gt = loop_trajectory(T, dev)
+    W = O.rigid(*drift)
+    gt_w2c = [M.camera_w2c(rots_gt[..., s], trans_gt[..., s])[0].double().cpu().numpy() for s in range(T)]
+    est = [gt_w2c[s] @ np.linalg.matrix_power(W, s) for s in range(T)]
+    rots = torch.zeros(1, 4, T, device=dev)
+    trans = torch.zeros(1, 3, T, device=dev)
+    for s in range(T):
+        m = torch.from_numpy(est[s]).float().to(dev)
+        q = F.normalize(M.matrix_to_quaternion(m[:3, :3]), dim=0)
+        rots[0, :, s] = q if float(q[0]) >= 0 else -q
+        trans[0, :, s] = m[:3, 3]
+    kf_ids = list(range(0, T, keyframe_every))
+    ts = torch.full((P,), -1.0, device=dev)
+    X = torch.cat([gt["means3D"], torch.ones(P, 1, device=dev)], 1)
+    for k in kf_ids:
+        c = (torch.from_numpy(gt_w2c[k]).float().to(dev) @ X.T).T
+        u, v = sc.fx * c[:, 0] / c[:, 2] + sc.cx, sc.fy * c[:, 1] / c[:, 2] + sc.cy
+        seen = (c[:, 2] > 0.05) & (u >= 0) & (u < sc.w) & (v >= 0) & (v < sc.h) & (ts < 0)
+        ts[seen] = float(k)
+    ts[ts < 0] = 0.0
+    table = torch.zeros(T, 12, device=dev)
+    for s in range(T):
+        table[s] = torch.from_numpy(np.linalg.matrix_power(O.inv(W), s)[:3].reshape(12)).float()
+    drifted = {k: v.clone() for k, v in gt.items()}
+    from splatam_b200 import loop
+    loop.deform_gaussians(drifted["means3D"], drifted["unnorm_rotations"], ts, table,
+                          torch.ones(1, dtype=torch.int32, device=dev))
+    frames = {}
+    for k in kf_ids:
+        f = slam.render_frame(gt, rots_gt, trans_gt, k, cam)
+        f["depth"] = torch.where(f["sil"] > 0.9, f["depth"] / f["sil"].clamp(min=1e-6), torch.zeros_like(f["depth"]))
+        frames[k] = f
+    return dict(cam=cam, gt=gt, drifted=drifted, timestep=ts, rots=rots, trans=trans, rots_gt=rots_gt,
+                trans_gt=trans_gt, frames=frames, kf_ids=kf_ids, T=T)
+
+
+def drifted_loop_at(st, t):
+    """The state of `drifted_loop` just before loop closure at keyframe frame t: (mapper over the drifted map, the
+    keyframes before t with their est_w2c, the pose graph of those keyframes and t, camera columns rots, trans),
+    fresh copies each call."""
+    from splatam_b200 import loop, mapping as M
+    rots, trans = st["rots"].clone(), st["trans"].clone()
+    mapper = M.ShardedMapper(st["drifted"], rots, trans, timestep=st["timestep"])
+    ids = [k for k in st["kf_ids"] if k < t]
+    kfs = [dict(st["frames"][k], est_w2c=M.camera_w2c(rots[..., k], trans[..., k])[0]) for k in ids]
+    graph = loop.PoseGraph.chain(ids + [t], rots, trans)
+    return mapper, kfs, graph, rots, trans
+
+
 def algorithmic_bytes(P, R, w, h):
     """B_algo of SURVEY.md section 8(d) / BASELINE.md section 4, bytes per fwd+bwd render."""
     tiles = ((w + 15) // 16) * ((h + 15) // 16)

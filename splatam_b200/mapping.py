@@ -824,6 +824,16 @@ class ShardedMapper:
         self.timestep = torch.cat([self.timestep, ts])
         return P + n_new
 
+    def deform(self, table, flag):
+        """Loop closure's map deformation (loop.deform_gaussians): every Gaussian's mean and quaternion move, in place
+        in the flat buffer, by the correction table [T,12] row of its `timestep`; nothing moves if the device int32
+        `flag` is 0.  The storage stays, so a captured mapping step and a cached tracking graph read the moved map at
+        their next replay."""
+        from . import loop
+        p = self.g.params
+        with torch.no_grad():
+            loop.deform_gaussians(p["means3D"], p["unnorm_rotations"], self.timestep.contiguous(), table, flag)
+
     def add_new_gaussians(self, frame, time_idx, intrinsics, sil_thres):
         """add_new_gaussians of the reference (R/scripts/splatam.py:378-420): one depth/silhouette render of the
         current map at the frame's estimated pose, non-presence mask, back-projection of the selected pixels,

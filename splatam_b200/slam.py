@@ -83,13 +83,14 @@ def keyframes_from_checkpoint(frames, ckpt):
     return [dict(_without_densify(frames[k]), est_w2c=_curr_w2c(rots, trans, k)) for k in ids]
 
 
-def _run_state(mapper, counts, keyframes=None):
+def _run_state(mapper, counts, keyframes=None, pose_graph=None):
     """The sidecar of a checkpoint (formats.save_checkpoint's `run_state`): what continues a run exactly and the
     reference's params{t}.npz cannot carry -- the mapper's own state (ShardedMapper.run_state: the Gaussians'
     `timestep`, its schedule and device generators, the densification statistic), torch's CPU RNG and the CUDA RNG of
     the map's device (keyframe selection and densification draw from the global generators), NumPy's global RNG
     (keyframe_selection_overlap's permutation) and the Gaussian counts so far; with `keyframes` (runs with keyframe-pose
-    refinement) also their stored est_w2c, which the refined camera columns no longer give.  Numeric arrays only."""
+    refinement) also their stored est_w2c, which the refined camera columns no longer give; with `pose_graph` (runs
+    with loop closure) also its edges and their measurements (loop.PoseGraph.state).  Numeric arrays only."""
     dev = mapper.g.flat.device
     _, keys, pos, has_gauss, cached = np.random.get_state()
     st = dict(mapper.run_state(), torch_rng=torch.get_rng_state().numpy(),
@@ -100,6 +101,8 @@ def _run_state(mapper, counts, keyframes=None):
         st["cuda_rng"] = torch.cuda.get_rng_state(dev).numpy()
     if keyframes is not None:
         st["keyframe_est_w2c"] = torch.stack([kf["est_w2c"].detach().float() for kf in keyframes]).cpu().numpy()
+    if pose_graph is not None:
+        st.update(pose_graph.state())
     return st
 
 
@@ -140,7 +143,8 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
              window=4, fused=None, seed=0, intrinsics=None, add_new_gaussians=False, sil_thres=0.5, prune_dict=None,
              scene_radius=None, select_keyframes=False, checkpoint_dir=None, first_frame_iters=0, map_every=None,
              graph=False, timing=None, densify_dict=None, tracking_lrs=(0.0004, 0.002), depth_loss_thres=None,
-             checkpoint_every=None, resume=None, mapping_cam_lrs=(0.0, 0.0), pose_init="constant_velocity"):
+             checkpoint_every=None, resume=None, mapping_cam_lrs=(0.0, 0.0), pose_init="constant_velocity",
+             loop_closure=None):
     """Tracks every frame and maps on keyframes.  gauss_init: dict of the five Gaussian tensors (the map's
     starting point); frames: list of dict(id, cam, w2c, im, depth).  Returns dict(rots, trans, psnr, gauss, counts,
     timestep, keyframe_time_indices, keyframe_est_w2c): `timestep` is the frame that created each Gaussian of the final
@@ -173,6 +177,15 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     `timing` also receives `pose_init_s` (synchronised wall seconds) and the result holds `icp`: per tracked frame
     dict(frame, accepted, inlier_frac, rms), read from the device once at the end.  `pose_init` is not stored in
     checkpoints: a resumed run passes it again.
+    `loop_closure`: None (the default: off, and nothing of it runs) or a dict of loop.DEFAULTS keys (needs CUDA tensors
+    and `intrinsics`).  Every keyframe frame t > 0 becomes a node of a keyframe pose graph, with an odometry edge from
+    the previous node measured from the camera columns after tracking; then, before new Gaussians are added,
+    loop.close_loop looks for an old keyframe frame t sees again, measures the loop by ICP against that keyframe's
+    depth, solves the graph and, if every edge fits, moves every camera column, every keyframe's est_w2c and every
+    Gaussian (by its `timestep`) with the correction of its node; frame t's mapping window then holds the loop keyframe
+    in place of its first entry.  `timing` also receives `loop_closure_s` and the result holds `loops`: one dict(frame,
+    keyframe, accepted, inlier_frac, rms, correction_m, correction_deg) per measured candidate.  Checkpoints then also
+    hold the graph and every keyframe's est_w2c; `loop_closure` itself is not stored: a resumed run passes it again.
 
     Checkpoints and resume (R/scripts/splatam.py:604-643,927-931).  With `checkpoint_dir` and `checkpoint_every` = N,
     after frame t's mapping and keyframe step, for every t % N == 0 (frame 0 included, after `first_frame_iters`),
@@ -207,6 +220,15 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
         K_icp = np.asarray(torch.as_tensor(intrinsics).detach().cpu(), dtype=np.float64)
         timing["pose_init_s"] = 0.0
         icp_stats = []
+    use_loop = loop_closure is not None
+    if use_loop:
+        from . import _lib, loop
+        loop_cfg = loop.config(loop_closure)
+        if intrinsics is None:
+            raise ValueError("loop_closure needs the intrinsics")
+        _lib.need_cuda("run_slam(loop_closure=...)", (gauss_init or resume["gauss"])["means3D"])
+        timing["loop_closure_s"] = 0.0
+        loops = []
     kw = {} if render is None else {"render": render}
     track_m2d = densify_dict is not None
     kw["lrs"] = dict(cam_unnorm_rots=float(mapping_cam_lrs[0]), cam_trans=float(mapping_cam_lrs[1]))
@@ -231,6 +253,12 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
             counts = [mapper.g.shapes["means3D"][0]]
         start = int(resume["time_idx"]) + 1
         first_frame_iters = 0
+    if use_loop:
+        st = resume["state"] if resume is not None else None
+        if st is not None and "loop_graph_edges" in st:
+            pose_graph = loop.PoseGraph.from_state(st, dev)
+        else:
+            pose_graph = loop.PoseGraph.chain([int(kf["id"]) for kf in keyframes], rots, trans)
 
     def checkpoint(t):
         if checkpoint_every is None or t % checkpoint_every != 0 or mapper.rank != 0:
@@ -238,7 +266,8 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
         from . import formats
         formats.save_checkpoint(checkpoint_dir, t, dict(mapper.g.params, cam_unnorm_rots=rots, cam_trans=trans),
                                 [kf["id"] for kf in keyframes],
-                                _run_state(mapper, counts, keyframes if refine else None))
+                                _run_state(mapper, counts, keyframes if (refine or use_loop) else None,
+                                           pose_graph if use_loop else None))
 
     def refined_cameras():
         """Refinement: copies of the mapper's cameras after a mapping phase (tracking then works on its own tensors)."""
@@ -282,6 +311,16 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
         cam_now = mapper.sync_camera()            # multi-rank runs: rank 0's tracking result is the pose of record
         rots, trans = cam_now["cam_unnorm_rots"], cam_now["cam_trans"]
         frame = frames[t]
+        loop_kf = None
+        if use_loop and t % keyframe_every == 0:
+            t0 = time.perf_counter()
+            pose_graph.add_odometry(pose_graph.nodes()[-1], t, pose_graph.odometry_from(rots, trans, t))
+            recs, loop_kf = loop.close_loop(t, frame, keyframes, rots, trans, pose_graph, intrinsics, loop_cfg, seed,
+                                            mapper)
+            loops += recs
+            rots, trans = mapper.cam["cam_unnorm_rots"], mapper.cam["cam_trans"]    # sync_camera may replace them
+            torch.cuda.synchronize(dev)
+            timing["loop_closure_s"] += time.perf_counter() - t0
         cur = dict(_without_densify(frame), est_w2c=_curr_w2c(rots, trans, t))
         if t % map_every == 0:
             if add_new_gaussians:
@@ -299,6 +338,8 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
                 win = [keyframes[int(i)] for i in sel] + [keyframes[-1], cur]
             else:
                 win = (keyframes + [cur])[-window:]
+            if loop_kf is not None and len(win) >= 2 and all(w is not keyframes[loop_kf] for w in win):
+                win[0] = keyframes[loop_kf]               # the seam between the loop's two ends gets optimised
             mapper.reset_optimizer()                          # splatam.py:822
             if graph and densify_dict is None:
                 mapper.enable_graph(win)
@@ -340,6 +381,8 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
         st = torch.stack(icp_stats).cpu().numpy() if icp_stats else np.zeros((0, icp.STATS))
         out["icp"] = [dict(frame=start + i, accepted=bool(s[0]), inlier_frac=float(s[1]), rms=float(s[2]))
                       for i, s in enumerate(st)]
+    if use_loop:
+        out["loops"] = loops
     return out
 
 
