@@ -601,6 +601,51 @@ SB_API int sb_pose_graph_update(int N, int E, int T, double* poses, const double
                                 double max_residual_rad, float* corrections, int* apply_flag, double* edge_err,
                                 void* stream);
 
+/* ---- relocalisation: thumbnail retrieval and the tracking health check (splatam_b200/reloc.py, csrc/reloc.cu) -----
+ * oracle/reloc_numpy.py restates every rule below.
+ * sb_reloc_thumbnail_size: the descriptor size h x w of an H x W image: s = max(1, H / SB_RELOC_THUMB_ROWS) (integer
+ *   division), h = H / s, w = W / s (the right and bottom remainder is cropped: 1200x680 -> 85x48, 640x480 -> 64x48).
+ * sb_reloc_thumbnails: B images -> out float32 [B,2,h,w] (channel 0 grey, 1 depth); scratch float32 [B,2,h,w].
+ *   rgb float32 [B,3,H,W], depth [B,H,W], sil [B,H,W] or NULL (a map render passes its silhouette and its depth_acc
+ *   as `depth`; a sensor frame passes NULL and its depth).  Float32, each operation rounded as written:
+ *   1. Sample (u, v): grey = (0.299 r + 0.587 g) + 0.114 b; depth = d, or d / sil with a silhouette.  With a silhouette,
+ *      a sample with sil <= 0.99 (or NaN) is invalid in both channels.  A grey sample is valid if finite, a depth
+ *      sample if finite and > 0.
+ *   2. Block (x, y) = samples u in [x s, x s + s), v in [y s, y s + s): sum of the valid samples in row-major order
+ *      (v outer, u inner) starting at 0, divided by their count; NaN (invalid) unless 2 count >= s^2.  Per channel.
+ *   3. Blur: a valid value becomes sum w v / sum w over its valid 3x3 neighbours inside the descriptor (itself
+ *      included), neighbours in row-major order (dy outer), w = (dy == 0 ? 2 : 1) (dx == 0 ? 2 : 1), each sum starting
+ *      at 0; an invalid value stays NaN.
+ * sb_reloc_score: query float32 [2,h,w] against database float32 [N,2,h,w] (pixels = h w) -> scores double [N].  Per
+ *   channel: the pixels valid (not NaN) in both; n their count, m_q, m_d the means of their values (double);
+ *   ncc = sum (q - m_q)(d - m_d) / sqrt(sum (q - m_q)^2 sum (d - m_d)^2), 0 where either sum of squares is 0.  Score =
+ *   (ncc_grey + ncc_depth) / 2, or -2 when, in either channel, the query has no valid pixel, n < 2 or 2 n < the
+ *   query's valid pixel count.  Sums in double in a fixed order (the same bits on every call).
+ * sb_reloc_topk: the k <= SB_RELOC_MAX_K best of scores double [N] (k <= N): indices int [k] and their scores double
+ *   [k], highest first, the lower index on ties (numpy's stable argsort of -score); NaN ranks below every number.
+ * sb_track_health: depth_sil float32 [2,H,W] (depth_acc, silhouette of the map's depth/silhouette render at the tracked
+ *   pose), frame_depth float32 [H,W].  Valid: frame depth finite and > 0; covered: valid and sil > 0.99; r =
+ *   depth_acc / sil - frame depth (float32, rounded as written); inlier: covered and |r| < max(tau_abs, tau_rel *
+ *   frame depth).  stats double [SB_RELOC_HEALTH_STATS]: 0 valid, 1 covered, 2 inliers, 3 RMS of r over the covered
+ *   pixels (inf if none), 4 healthy (1/0): valid > 0, covered > 0, covered / valid >= min_coverage and inliers /
+ *   covered >= min_inliers.  Counts are exact; the sum of r^2 is in double over SB_RELOC_HEALTH_BLOCKS fixed partials
+ *   (scratch double [4 SB_RELOC_HEALTH_BLOCKS]), summed in block order.  No host synchronisation.
+ * SB_ERR_BAD_ARG, before any launch, for null pointers (sil may be NULL), sizes < 1, pixels > SB_RELOC_MAX_PIXELS,
+ * k outside [1, min(N, SB_RELOC_MAX_K)], negative or non-finite tolerances and thresholds outside [0, 1]. */
+#define SB_RELOC_THUMB_ROWS 48
+#define SB_RELOC_MAX_K 8
+#define SB_RELOC_MAX_PIXELS 28000
+#define SB_RELOC_HEALTH_BLOCKS 128
+#define SB_RELOC_HEALTH_STATS 5
+SB_API int sb_reloc_thumbnail_size(int height, int width, int* h, int* w);
+SB_API int sb_reloc_thumbnails(int B, int height, int width, const float* rgb, const float* depth, const float* sil,
+                               float* scratch, float* out, void* stream);
+SB_API int sb_reloc_score(int N, int pixels, const float* query, const float* database, double* scores, void* stream);
+SB_API int sb_reloc_topk(int N, int k, const double* scores, int* indices, double* top_scores, void* stream);
+SB_API int sb_track_health(int height, int width, const float* depth_sil, const float* frame_depth, float tau_abs,
+                           float tau_rel, double min_coverage, double min_inliers, double* scratch, double* stats,
+                           void* stream);
+
 /* ---- per-stage device timing (measurement only; bench.py's roofline pass) -------------------
  * Between sb_profile_begin() and sb_profile_end() every stage launch of this process is bracketed
  * by CUDA events on its stream.  sb_profile_end synchronises, writes the summed milliseconds and call

@@ -608,6 +608,10 @@ def write_loop_sequence(dst, num_frames, device, seed=21, cam=LOOP_CAM, png_dept
     under `dst`, as write_replica_sequence does: the frames are rendered on `device` from `loop_room` along
     `loop_trajectory`, a camera inside a densely walled room that comes back to where it started.  Depth is
     alpha-normalised, 0 where the silhouette is below 0.9.  Returns the ground-truth w2c matrices [T,4,4] (CPU)."""
+    return _write_room_sequence(dst, loop_trajectory(num_frames, device), device, seed, cam, png_depth_scale, quality)
+
+
+def _write_room_sequence(dst, traj, device, seed, cam, png_depth_scale, quality):
     import os
     from PIL import Image
     import splatam_b200 as S
@@ -615,7 +619,8 @@ def write_loop_sequence(dst, num_frames, device, seed=21, cam=LOOP_CAM, png_dept
     sc = loop_room(seed=seed, cam=cam)
     rs = sc.settings(S.GaussianRasterizationSettings, device)
     gt = sc.splatam_params(device)
-    rots, trans = loop_trajectory(num_frames, device)
+    rots, trans = traj
+    num_frames = rots.shape[-1]
     os.makedirs(os.path.join(dst, "results"), exist_ok=True)
     w2cs, traj = [], []
     for t in range(num_frames):
@@ -631,6 +636,37 @@ def write_loop_sequence(dst, num_frames, device, seed=21, cam=LOOP_CAM, png_dept
     with open(os.path.join(dst, "traj.txt"), "w") as fh:
         fh.write("\n".join(traj) + "\n")
     return torch.stack(w2cs)
+
+
+def kidnapped_trajectory(device, num_loop=81, before=41, jump=(12, 31), unmapped=False, shift=1.3):
+    """A camera that jumps: `loop_trajectory(num_loop)` frames 0..before-1, then frames jump[0]..jump[1]-1, so the camera
+    lands back at a place it mapped (frame `before` is the jump).  With `unmapped`, the frames after the jump are those
+    poses turned 180 degrees about the camera's vertical axis and moved `shift` [m] back along world z, so the camera
+    faces the back wall (z = -1.7 m) from 0.5 to 1 m away: a wall the first part never saw, and a depth no pose near
+    the first part's can explain.  Returns (unnormalised quaternions [1,4,T], translations
+    [1,3,T]); frame `before` is the first frame after the jump."""
+    r, t = loop_trajectory(num_loop, device)
+    idx = list(range(before)) + list(range(*jump))
+    rots, trans = r[..., idx].clone(), t[..., idx].clone()
+    if unmapped:
+        from splatam_b200 import mapping as M
+        a = math.pi
+        qy = torch.tensor([math.cos(a / 2), 0.0, math.sin(a / 2), 0.0], device=device)
+        Ry = torch.tensor([[math.cos(a), 0.0, math.sin(a)], [0.0, 1.0, 0.0], [-math.sin(a), 0.0, math.cos(a)]],
+                          device=device)
+        for s in range(before, len(idx)):
+            w2c = M.camera_w2c(rots[..., s], trans[..., s])[0]
+            c = -(w2c[:3, :3].T @ w2c[:3, 3]) + torch.tensor([0.0, 0.0, -shift], device=device)
+            R = Ry @ w2c[:3, :3]
+            rots[0, :, s] = M.quat_mult(qy[None], torch.nn.functional.normalize(rots[..., s]))[0]
+            trans[0, :, s] = -(R @ c)
+    return rots, trans
+
+
+def write_kidnapped_sequence(dst, device, seed=21, cam=LOOP_CAM, png_depth_scale=6553.5, quality=95, **kw):
+    """`kidnapped_trajectory(device, **kw)` in `loop_room`, written as write_loop_sequence writes the loop (read it
+    back with loop_data_config).  Returns the ground-truth w2c matrices [T,4,4] (CPU)."""
+    return _write_room_sequence(dst, kidnapped_trajectory(device, **kw), device, seed, cam, png_depth_scale, quality)
 
 
 def loop_data_config(cam=LOOP_CAM, png_depth_scale=6553.5):

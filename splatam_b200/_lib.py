@@ -118,6 +118,11 @@ _SIGNATURES = {
     "sb_pose_graph_normal_equations": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "sb_pose_graph_update": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double, _vp, _vp,
                                   _vp, _vp]),
+    "sb_reloc_thumbnail_size": (_i, [_i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i)]),
+    "sb_reloc_thumbnails": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "sb_reloc_score": (_i, [_i, _i, _vp, _vp, _vp, _vp]),
+    "sb_reloc_topk": (_i, [_i, _i, _vp, _vp, _vp, _vp]),
+    "sb_track_health": (_i, [_i, _i, _vp, _vp, _f, _f, ctypes.c_double, ctypes.c_double, _vp, _vp, _vp]),
     "sb_profile_begin": (_i, []),
     "sb_profile_end": (_i, [ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_int)]),
     "sb_stage_name": (ctypes.c_char_p, [_i]),

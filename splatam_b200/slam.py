@@ -83,14 +83,15 @@ def keyframes_from_checkpoint(frames, ckpt):
     return [dict(_without_densify(frames[k]), est_w2c=_curr_w2c(rots, trans, k)) for k in ids]
 
 
-def _run_state(mapper, counts, keyframes=None, pose_graph=None):
+def _run_state(mapper, counts, keyframes=None, pose_graph=None, reloc_frames=None):
     """The sidecar of a checkpoint (formats.save_checkpoint's `run_state`): what continues a run exactly and the
     reference's params{t}.npz cannot carry -- the mapper's own state (ShardedMapper.run_state: the Gaussians'
     `timestep`, its schedule and device generators, the densification statistic), torch's CPU RNG and the CUDA RNG of
     the map's device (keyframe selection and densification draw from the global generators), NumPy's global RNG
     (keyframe_selection_overlap's permutation) and the Gaussian counts so far; with `keyframes` (runs with keyframe-pose
     refinement) also their stored est_w2c, which the refined camera columns no longer give; with `pose_graph` (runs
-    with loop closure) also its edges and their measurements (loop.PoseGraph.state).  Numeric arrays only."""
+    with loop closure) also its edges and their measurements (loop.PoseGraph.state); with `reloc_frames` (runs with
+    relocalisation: (lost ids, relocalised ids)) `reloc_lost` and `reloc_relocalised`.  Numeric arrays only."""
     dev = mapper.g.flat.device
     _, keys, pos, has_gauss, cached = np.random.get_state()
     st = dict(mapper.run_state(), torch_rng=torch.get_rng_state().numpy(),
@@ -103,6 +104,9 @@ def _run_state(mapper, counts, keyframes=None, pose_graph=None):
         st["keyframe_est_w2c"] = torch.stack([kf["est_w2c"].detach().float() for kf in keyframes]).cpu().numpy()
     if pose_graph is not None:
         st.update(pose_graph.state())
+    if reloc_frames is not None:
+        st["reloc_lost"] = np.array(sorted(reloc_frames[0]), dtype=np.int64)
+        st["reloc_relocalised"] = np.array(sorted(reloc_frames[1]), dtype=np.int64)
     return st
 
 
@@ -144,7 +148,7 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
              scene_radius=None, select_keyframes=False, checkpoint_dir=None, first_frame_iters=0, map_every=None,
              graph=False, timing=None, densify_dict=None, tracking_lrs=(0.0004, 0.002), depth_loss_thres=None,
              checkpoint_every=None, resume=None, mapping_cam_lrs=(0.0, 0.0), pose_init="constant_velocity",
-             loop_closure=None):
+             loop_closure=None, relocalise=None):
     """Tracks every frame and maps on keyframes.  gauss_init: dict of the five Gaussian tensors (the map's
     starting point); frames: list of dict(id, cam, w2c, im, depth).  Returns dict(rots, trans, psnr, gauss, counts,
     timestep, keyframe_time_indices, keyframe_est_w2c): `timestep` is the frame that created each Gaussian of the final
@@ -186,6 +190,18 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     in place of its first entry.  `timing` also receives `loop_closure_s` and the result holds `loops`: one dict(frame,
     keyframe, accepted, inlier_frac, rms, correction_m, correction_deg) per measured candidate.  Checkpoints then also
     hold the graph and every keyframe's est_w2c; `loop_closure` itself is not stored: a resumed run passes it again.
+    `relocalise`: None (the default: off, and nothing of it runs) or a dict of reloc.DEFAULTS keys (needs CUDA tensors
+    and `intrinsics`; one rank only -- with several ranks it raises ValueError).  Each keyframe's frame adds its
+    descriptor to a reloc.Database when it joins the keyframe list.  After tracking, reloc.health checks every frame
+    against the map's depth/silhouette render at its pose (one render and one small host read per frame); a lost frame
+    calls reloc.relocalise against the keyframe database.  A relocalised frame continues as a normal frame, and the
+    next frame starts with zero velocity.  A frame that stays lost takes column t - 1 (so the next guess has zero
+    velocity) and is not mapped, adds no Gaussians, joins no keyframe list and adds no pose-graph node.  `timing` also
+    receives `health_s` and `reloc_s`, and the result holds `reloc`: per lost frame dict(frame, relocalised, candidate
+    (camera column or None), score, coverage, inlier_frac, rms (the final health), candidates, scores, icp),
+    `reloc_lost` (the ids of frames that stayed lost) and `reloc_database`.  Checkpoints also hold the lost and
+    relocalised ids; on resume the database is rebuilt from the restored keyframes.  `relocalise` itself is not
+    stored: a resumed run passes it again.
 
     Checkpoints and resume (R/scripts/splatam.py:604-643,927-931).  With `checkpoint_dir` and `checkpoint_every` = N,
     after frame t's mapping and keyframe step, for every t % N == 0 (frame 0 included, after `first_frame_iters`),
@@ -229,6 +245,18 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
         _lib.need_cuda("run_slam(loop_closure=...)", (gauss_init or resume["gauss"])["means3D"])
         timing["loop_closure_s"] = 0.0
         loops = []
+    use_reloc = relocalise is not None
+    if use_reloc:
+        from . import _lib, reloc
+        reloc_cfg = reloc.config(relocalise)
+        if intrinsics is None:
+            raise ValueError("relocalise needs the intrinsics")
+        import torch.distributed as dist
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            raise ValueError("relocalise runs on one rank only, got a world of %d" % dist.get_world_size())
+        _lib.need_cuda("run_slam(relocalise=...)", (gauss_init or resume["gauss"])["means3D"])
+        timing.update(health_s=0.0, reloc_s=0.0)
+        reloc_recs, reloc_lost, reloc_done = [], set(), set()
     kw = {} if render is None else {"render": render}
     track_m2d = densify_dict is not None
     kw["lrs"] = dict(cam_unnorm_rots=float(mapping_cam_lrs[0]), cam_trans=float(mapping_cam_lrs[1]))
@@ -259,6 +287,14 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
             pose_graph = loop.PoseGraph.from_state(st, dev)
         else:
             pose_graph = loop.PoseGraph.chain([int(kf["id"]) for kf in keyframes], rots, trans)
+    if use_reloc:
+        st = resume["state"] if resume is not None else None
+        if st is not None and "reloc_lost" in st:
+            reloc_lost = {int(i) for i in np.asarray(st["reloc_lost"]).reshape(-1)}
+            reloc_done = {int(i) for i in np.asarray(st["reloc_relocalised"]).reshape(-1)}
+        reloc_db = reloc.Database()
+        for kf in keyframes:
+            reloc_db.add(kf, int(kf["id"]))
 
     def checkpoint(t):
         if checkpoint_every is None or t % checkpoint_every != 0 or mapper.rank != 0:
@@ -267,7 +303,8 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
         formats.save_checkpoint(checkpoint_dir, t, dict(mapper.g.params, cam_unnorm_rots=rots, cam_trans=trans),
                                 [kf["id"] for kf in keyframes],
                                 _run_state(mapper, counts, keyframes if (refine or use_loop) else None,
-                                           pose_graph if use_loop else None))
+                                           pose_graph if use_loop else None,
+                                           (reloc_lost, reloc_done) if use_reloc else None))
 
     def refined_cameras():
         """Refinement: copies of the mapper's cameras after a mapping phase (tracking then works on its own tensors)."""
@@ -286,7 +323,7 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     timing["setup_s"] = time.perf_counter() - t_setup
     for t in range(start, T):
         with torch.no_grad():           # constant-velocity initialisation (splatam.py:423-444)
-            if t > 1:
+            if t > 1 and not (use_reloc and (t - 1) in reloc_done):
                 r1, r2 = F.normalize(rots[0, :, t - 1], dim=0), F.normalize(rots[0, :, t - 2], dim=0)
                 rots[0, :, t] = F.normalize(r1 + (r1 - r2), dim=0)
                 trans[0, :, t] = trans[0, :, t - 1] + (trans[0, :, t - 1] - trans[0, :, t - 2])
@@ -311,6 +348,37 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
         cam_now = mapper.sync_camera()            # multi-rank runs: rank 0's tracking result is the pose of record
         rots, trans = cam_now["cam_unnorm_rots"], cam_now["cam_trans"]
         frame = frames[t]
+        if use_reloc:
+            t0 = time.perf_counter()
+            now = dict(params, cam_unnorm_rots=rots, cam_trans=trans)
+            healthy = reloc.read_health(reloc.health(now, frame, t, reloc_cfg, render, fused))["ok"]
+            timing["health_s"] += time.perf_counter() - t0
+            if not healthy:
+                t0 = time.perf_counter()
+                rec = reloc.relocalise(now, frame, t, reloc_db, intrinsics, reloc_cfg, render=render, fused=fused,
+                                       tracking=dict(num_iters=tracking_iters, lr_rot=tracking_lrs[0],
+                                                     lr_trans=tracking_lrs[1], depth_loss_thres=depth_loss_thres))
+                rots, trans = now["cam_unnorm_rots"].detach(), now["cam_trans"].detach()
+                h = rec["health"] or {}
+                reloc_recs.append(dict(frame=t, relocalised=rec["accepted"], candidate=(
+                    reloc_db.columns[rec["chosen"]] if rec["chosen"] is not None else None),
+                    score=(rec["scores"][rec["candidates"].index(rec["chosen"])] if rec["chosen"] is not None
+                           else None), coverage=h.get("coverage"), inlier_frac=h.get("inlier_frac"), rms=h.get("rms"),
+                    candidates=rec["columns"], scores=rec["scores"], icp=rec["icp"]))
+                if not rec["accepted"]:
+                    with torch.no_grad():
+                        rots[..., t] = rots[..., t - 1]
+                        trans[..., t] = trans[..., t - 1]
+                mapper.cam = dict(cam_unnorm_rots=rots, cam_trans=trans)
+                cam_now = mapper.sync_camera()
+                rots, trans = cam_now["cam_unnorm_rots"], cam_now["cam_trans"]
+                torch.cuda.synchronize(dev)
+                timing["reloc_s"] += time.perf_counter() - t0
+                if not rec["accepted"]:
+                    reloc_lost.add(t)
+                    checkpoint(t)
+                    continue
+                reloc_done.add(t)
         loop_kf = None
         if use_loop and t % keyframe_every == 0:
             t0 = time.perf_counter()
@@ -361,6 +429,8 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
                 cur["est_w2c"] = _curr_w2c(rots, trans, t)
         if t % keyframe_every == 0:
             keyframes.append(cur)
+            if use_reloc:
+                reloc_db.add(frame, t)
             if checkpoint_dir is not None and checkpoint_every is None:
                 from . import formats
                 formats.save_params_ckpt(dict(mapper.g.params, cam_unnorm_rots=rots, cam_trans=trans), checkpoint_dir, t)
@@ -383,6 +453,8 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
                       for i, s in enumerate(st)]
     if use_loop:
         out["loops"] = loops
+    if use_reloc:
+        out.update(reloc=reloc_recs, reloc_lost=sorted(reloc_lost), reloc_database=reloc_db)
     return out
 
 

@@ -18,7 +18,9 @@ One GPU.
 --stride select frames as the reference does; --frames caps the number of frames; --tracking-iters / --mapping-iters
 override the shipped iteration counts; --pose-init icp starts each frame's tracking from a point-to-plane ICP
 alignment of its depth with the map's (splatam_b200.icp; default constant_velocity, the reference's guess);
---loop-closure closes loops against old keyframes with splatam_b200.loop's defaults and prints every closure attempt.  Prints one JSON line: ATE, PSNR, MS-SSIM, depth L1, initial and final
+--loop-closure closes loops against old keyframes with splatam_b200.loop's defaults and prints every closure attempt.
+--relocalise checks every tracked frame against the map and relocalises lost ones against the keyframes
+(splatam_b200.reloc's defaults) and prints every lost frame.  Prints one JSON line: ATE, PSNR, MS-SSIM, depth L1, initial and final
 Gaussian counts, tracking
 and mapping wall times, and the load time per frame that the SLAM loop waited for (decode + upload not hidden by the
 prefetch).  --out DIR writes the reference's psnr.txt / rmse.txt / l1.txt / ssim.txt and its full params.npz record
@@ -140,6 +142,9 @@ def main():
                     help="tracking start: the reference's constant-velocity guess, or that guess refined by ICP")
     ap.add_argument("--loop-closure", action="store_true",
                     help="close loops against old keyframes (splatam_b200.loop, its DEFAULTS); off by default")
+    ap.add_argument("--relocalise", action="store_true",
+                    help="health-check every frame and relocalise lost ones (splatam_b200.reloc, its DEFAULTS); off by "
+                         "default")
     a = ap.parse_args()
     if (a.lpips_alexnet is None) != (a.lpips_lin is None):
         ap.error("--lpips-alexnet and --lpips-lin go together")
@@ -198,7 +203,7 @@ def main():
                         checkpoint_every=a.checkpoint_every or None, resume=ckpt,
                         tracking_lrs=h["tracking_lrs"], depth_loss_thres=h["depth_loss_thres"],
                         mapping_cam_lrs=tuple(a.mapping_cam_lrs), pose_init=a.pose_init,
-                        loop_closure={} if a.loop_closure else None)
+                        loop_closure={} if a.loop_closure else None, relocalise={} if a.relocalise else None)
     torch.cuda.synchronize(dev)
     wall = time.perf_counter() - t0
     # --resume: wall time from reading the checkpoint to the first tracked frame (frame-0 read, load, keyframe rebuild)
@@ -235,6 +240,8 @@ def main():
         **({} if a.pose_init != "icp" else dict(pose_init_s=timing["pose_init_s"],
                                                 icp_accepted=sum(s["accepted"] for s in out["icp"]))),
         **({} if not a.loop_closure else dict(loop_closure_s=timing["loop_closure_s"], loops=out["loops"])),
+        **({} if not a.relocalise else dict(health_s=timing["health_s"], reloc_s=timing["reloc_s"], reloc=out["reloc"],
+                                            reloc_lost=out["reloc_lost"])),
         ate_m=res["ate"], psnr_db=res["psnr"], ms_ssim=res["ms_ssim"], depth_l1_m=res["depth_l1"],
         gaussians=int(out["counts"][-1]), wall_s=wall, tracking_s=timing["tracking_s"], mapping_s=timing["mapping_s"],
         load_wait_ms_per_frame=1e3 * load_wait / max(T - 1, 1), evaluated_frames=len(res["frame_ids"]),
