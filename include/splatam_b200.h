@@ -556,6 +556,49 @@ SB_API int sb_icp_export(int height, int width, const void* workspace, size_t wo
                          float* model_depth, float* data_depth, float* model_vertex, float* model_normal,
                          float* data_vertex, uint8_t* assoc, void* stream);
 
+/* ---- RGB-D ICP: joint geometric and photometric alignment (splatam_b200/icp.py, csrc/icp.cu) ----------------------
+ * sb_rgbd_icp_align: sb_icp_align's arguments plus model_rgb float32 [3,H,W] (the map's RGB render at w2c_prev),
+ *   data_rgb float32 [3,H,W] (frame t) and weight (lambda, metres per unit of intensity, finite and >= 0).  Float32,
+ *   each operation rounded as written, double sums in a fixed order; oracle/rgbd_icp_numpy.py restates the rule.
+ *   Steps 1-3 and the pairs of step 4 are sb_icp_align's, computed by the same device code.  In addition:
+ *   a. Level 0 grey = (0.299 r + 0.587 g) + 0.114 b; model grey where the model depth is valid, data grey where the
+ *      data depth is valid, NaN elsewhere.  A grey value is valid iff finite.
+ *   b. Level l + 1 grey = (sum of the grey of exactly the samples the depth pyramid averaged, in its order) / their
+ *      count; NaN where the depth is 0.
+ *   c. Model gradient (gu, gv) = ((I(u+1) - I(u-1)) / 2, (I(v+1) - I(v-1)) / 2) where the model normal is valid, NaN
+ *      elsewhere (so no gradient crosses a depth edge).
+ *   d. Every data pixel with a geometric pair at p = R v + t (step 4, whose distance gate is the occlusion test) is
+ *      projected to (uc, vc) = (fx px/pz + cx, fy py/pz + cy); with u0 = floor(uc), v0 = floor(vc), a = uc - u0, b =
+ *      vc - v0 the taps (u0, v0), (u0+1, v0), (u0, v0+1), (u0+1, v0+1) must lie in the image with finite grey and
+ *      gradient.  Weights (1-a)(1-b), a(1-b), (1-a)b, ab; a sample is ((w00 x00 + w10 x10) + w01 x01) + w11 x11.
+ *      r_I = I_model - I_data, paired iff |r_I| <= SB_RGBD_ICP_MAX_RESIDUAL; g = (dpi/dp)^T grad I =
+ *      (gu fx / pz, gv fy / pz, -((gu fx / pz) px + (gv fy / pz) py) / pz); J_I = [p x g, g], paired only if all six
+ *      entries are finite (so the photometric sums stay finite).
+ *   e. JtJ_I, Jtr_I, sum r_I^2 and the pair count are summed in double in the geometric sums' fixed order; the system
+ *      solved is JtJ + weight^2 JtJ_I, Jtr + weight^2 Jtr_I, with sb_icp_align's skip rule and Cholesky.
+ *   f. Accepted iff sb_icp_align's test passes on the joint system and, when weight > 0, the last iteration had at
+ *      least SB_RGBD_ICP_MIN_PAIRS photometric pairs and photometric RMS <= SB_RGBD_ICP_MAX_RMS.
+ *   stats double[SB_RGBD_ICP_STATS]: 0..35 as sb_icp_align's (8..34: the joint system solved; 3, 4, 35 geometric),
+ *   36 photometric pairs, 37 photometric RMS (inf if none), 38..58 JtJ_I, 59..64 Jtr_I, 65 sum r_I^2 -- all of the
+ *   last iteration.  With weight 0 the pose and stats 0..35 equal sb_icp_align's bit for bit.  No host
+ *   synchronisation: the call can be captured into a CUDA graph.
+ * sb_rgbd_icp_workspace_bytes: its workspace, which begins with sb_icp_align's (sb_icp_export reads it).
+ * sb_rgbd_icp_export: level `level`'s model_grey, data_grey [H_l, W_l], model_grad [2, H_l, W_l] and photometric codes
+ *   uint8 [H_l, W_l] (0 no geometric pair, 1 no photometric pair, 2 paired) of the latest iteration at that level.
+ * SB_ERR_BAD_ARG as sb_icp_align, and for a null rgb pointer and a negative or non-finite weight; SB_ERR_WORKSPACE for
+ * a workspace smaller than sb_rgbd_icp_workspace_bytes gives. */
+#define SB_RGBD_ICP_STATS 66
+#define SB_RGBD_ICP_MAX_RESIDUAL 0.3f
+#define SB_RGBD_ICP_MAX_RMS 0.1
+#define SB_RGBD_ICP_MIN_PAIRS 32.0
+SB_API int sb_rgbd_icp_workspace_bytes(int height, int width, size_t* bytes);
+SB_API int sb_rgbd_icp_align(int height, int width, const float* model_depth_sil, const float* model_rgb,
+                             const float* data_depth, const float* data_rgb, float fx, float fy, float cx, float cy,
+                             const float* w2c_prev, const float* w2c_init, const int* iters, float weight,
+                             void* workspace, size_t workspace_bytes, float* w2c_out, double* stats, void* stream);
+SB_API int sb_rgbd_icp_export(int height, int width, const void* workspace, size_t workspace_bytes, int level,
+                              float* model_grey, float* data_grey, float* model_grad, uint8_t* photo, void* stream);
+
 /* ---- loop closure: map deformation and the keyframe pose graph (splatam_b200/loop.py, csrc/loop.cu) ---------------
  * A correction is a rigid map from the old world to the new one, float32 [12] row-major 3x4 [R | t]; the table holds
  * one per frame.  oracle/loop_numpy.py restates every rule below.
@@ -630,13 +673,24 @@ SB_API int sb_pose_graph_update(int N, int E, int T, double* poses, const double
  *   pixels (inf if none), 4 healthy (1/0): valid > 0, covered > 0, covered / valid >= min_coverage and inliers /
  *   covered >= min_inliers.  Counts are exact; the sum of r^2 is in double over SB_RELOC_HEALTH_BLOCKS fixed partials
  *   (scratch double [4 SB_RELOC_HEALTH_BLOCKS]), summed in block order.  No host synchronisation.
+ * sb_track_health_rgb: sb_track_health's inputs plus map_rgb float32 [3,H,W] (the map's RGB render at the tracked pose)
+ *   and frame_rgb float32 [3,H,W].  Entries 0..3 equal sb_track_health's bit for bit.  Over the inliers whose six
+ *   colour values (map and frame r, g, b) are all finite: 5 their count, 6 the colour NCC of the map against the
+ *   frame: each channel centred on its own mean, ncc = sum_c sum (m_c - mm_c)(f_c - mf_c) / sqrt(sum_c sum (m_c -
+ *   mm_c)^2 sum_c sum (f_c - mf_c)^2), 0 where either sum of squares is 0.  In double, in two passes (the means, then
+ *   the centred sums) over SB_RELOC_HEALTH_BLOCKS fixed partials summed in block order (scratch double
+ *   [22 SB_RELOC_HEALTH_BLOCKS]).  4 healthy: sb_track_health's test, ncc >= min_ncc and count >=
+ *   SB_RELOC_MIN_NCC_PAIRS.  No host synchronisation.
  * SB_ERR_BAD_ARG, before any launch, for null pointers (sil may be NULL), sizes < 1, pixels > SB_RELOC_MAX_PIXELS,
- * k outside [1, min(N, SB_RELOC_MAX_K)], negative or non-finite tolerances and thresholds outside [0, 1]. */
+ * k outside [1, min(N, SB_RELOC_MAX_K)], negative or non-finite tolerances, thresholds outside [0, 1] and min_ncc
+ * outside [-1, 1]. */
 #define SB_RELOC_THUMB_ROWS 48
 #define SB_RELOC_MAX_K 8
 #define SB_RELOC_MAX_PIXELS 28000
 #define SB_RELOC_HEALTH_BLOCKS 128
 #define SB_RELOC_HEALTH_STATS 5
+#define SB_RELOC_HEALTH_RGB_STATS 7
+#define SB_RELOC_MIN_NCC_PAIRS 64.0
 SB_API int sb_reloc_thumbnail_size(int height, int width, int* h, int* w);
 SB_API int sb_reloc_thumbnails(int B, int height, int width, const float* rgb, const float* depth, const float* sil,
                                float* scratch, float* out, void* stream);
@@ -645,6 +699,10 @@ SB_API int sb_reloc_topk(int N, int k, const double* scores, int* indices, doubl
 SB_API int sb_track_health(int height, int width, const float* depth_sil, const float* frame_depth, float tau_abs,
                            float tau_rel, double min_coverage, double min_inliers, double* scratch, double* stats,
                            void* stream);
+SB_API int sb_track_health_rgb(int height, int width, const float* depth_sil, const float* frame_depth,
+                               const float* map_rgb, const float* frame_rgb, float tau_abs, float tau_rel,
+                               double min_coverage, double min_inliers, double min_ncc, double* scratch, double* stats,
+                               void* stream);
 
 /* ---- per-stage device timing (measurement only; bench.py's roofline pass) -------------------
  * Between sb_profile_begin() and sb_profile_end() every stage launch of this process is bracketed

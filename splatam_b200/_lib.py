@@ -114,6 +114,10 @@ _SIGNATURES = {
     "sb_icp_workspace_bytes": (_i, [_i, _i, ctypes.POINTER(_sz)]),
     "sb_icp_align": (_i, [_i, _i, _vp, _vp, _f, _f, _f, _f, _vp, _vp, ctypes.POINTER(_i), _vp, _sz, _vp, _vp, _vp]),
     "sb_icp_export": (_i, [_i, _i, _vp, _sz, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "sb_rgbd_icp_workspace_bytes": (_i, [_i, _i, ctypes.POINTER(_sz)]),
+    "sb_rgbd_icp_align": (_i, [_i, _i, _vp, _vp, _vp, _vp, _f, _f, _f, _f, _vp, _vp, ctypes.POINTER(_i), _f, _vp, _sz,
+                               _vp, _vp, _vp]),
+    "sb_rgbd_icp_export": (_i, [_i, _i, _vp, _sz, _i, _vp, _vp, _vp, _vp, _vp]),
     "sb_deform_gaussians": (_i, [_i, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     "sb_pose_graph_normal_equations": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "sb_pose_graph_update": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double, _vp, _vp,
@@ -123,6 +127,8 @@ _SIGNATURES = {
     "sb_reloc_score": (_i, [_i, _i, _vp, _vp, _vp, _vp]),
     "sb_reloc_topk": (_i, [_i, _i, _vp, _vp, _vp, _vp]),
     "sb_track_health": (_i, [_i, _i, _vp, _vp, _f, _f, ctypes.c_double, ctypes.c_double, _vp, _vp, _vp]),
+    "sb_track_health_rgb": (_i, [_i, _i, _vp, _vp, _vp, _vp, _f, _f, ctypes.c_double, ctypes.c_double, ctypes.c_double,
+                                 _vp, _vp, _vp]),
     "sb_profile_begin": (_i, []),
     "sb_profile_end": (_i, [ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_int)]),
     "sb_stage_name": (ctypes.c_char_p, [_i]),

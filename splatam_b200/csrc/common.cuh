@@ -166,4 +166,11 @@ __device__ __forceinline__ float xform_row(const float* __restrict__ m, int k, f
     return __fadd_rn(__fmaf_rn(pz, m[k + 8], __fmaf_rn(px, m[k], __fmul_rn(py, m[k + 4]))), m[k + 12]);
 }
 
+// Grey of sample i of a planar RGB image (planes `plane` samples apart): (0.299 r + 0.587 g) + 0.114 b, each operation
+// rounded as written (relocalisation thumbnails, RGB-D ICP)
+__device__ __forceinline__ float grey_of(const float* __restrict__ rgb, size_t plane, size_t i) {
+    return __fadd_rn(__fadd_rn(__fmul_rn(0.299f, rgb[i]), __fmul_rn(0.587f, rgb[plane + i])),
+                     __fmul_rn(0.114f, rgb[2 * plane + i]));
+}
+
 }  // namespace sb

@@ -33,6 +33,11 @@ constexpr double kMinCount = 32.0;     // fewer associated pixels: the update is
 constexpr double kMinInlierFrac = 0.4; // acceptance: inliers / valid data pixels of the last iteration
 constexpr double kMaxRms = 0.03;       // acceptance: RMS point-to-plane residual [m] of the last iteration
 constexpr double kMinPivotRatio = 1e-5;// acceptance: smallest / largest Cholesky pivot of the last system
+constexpr int kRgbdStats = SB_RGBD_ICP_STATS;
+constexpr int kPhotoTerms = 29;        // 21 JtJ_I, 6 Jtr_I, sum r_I^2, photometric pairs
+constexpr float kMaxPhotoRes = SB_RGBD_ICP_MAX_RESIDUAL;      // |I_model - I_data| gate of a photometric pair
+constexpr double kMaxPhotoRms = SB_RGBD_ICP_MAX_RMS;          // acceptance with weight > 0: photometric RMS
+constexpr double kMinPhotoPairs = SB_RGBD_ICP_MIN_PAIRS;      // ... and at least this many photometric pairs
 
 inline unsigned int blocks_for(long long n) { return (unsigned int)((n + kThreads - 1) / kThreads); }
 
@@ -53,8 +58,7 @@ struct IcpWs {
     double* T;            // [12] row-major 3x4, camera t -> camera t-1
 };
 
-IcpWs carve_icp(void* ws, int H, int W, size_t* total) {
-    Carver c(ws);
+IcpWs carve_icp(Carver& c, int H, int W) {
     IcpWs w;
     for (int l = 0; l < kLevels; ++l) {
         Level& L = w.lv[l];
@@ -70,6 +74,42 @@ IcpWs carve_icp(void* ws, int H, int W, size_t* total) {
     }
     w.partials = c.take<double>((size_t)kBlocks * kTerms);
     w.T = c.take<double>(12);
+    return w;
+}
+
+IcpWs carve_icp(void* ws, int H, int W, size_t* total) {
+    Carver c(ws);
+    IcpWs w = carve_icp(c, H, W);
+    if (total) *total = c.used();
+    return w;
+}
+
+struct GreyLevel {
+    float* model_grey;    // [H W], NaN where invalid (the model depth is invalid)
+    float* data_grey;     // [H W], NaN where the data depth is invalid
+    float* model_grad;    // [2, H, W] dI/du, dI/dv; NaN where invalid (the model normal is invalid)
+    uint8_t* photo;       // [H W] 0 no geometric pair, 1 no photometric pair, 2 paired (latest iteration)
+};
+
+// sb_icp_align's workspace first (sb_icp_export reads it), then the grey pyramid and the photometric partials
+struct RgbdWs {
+    IcpWs g;
+    GreyLevel lv[kLevels];
+    double* photo_partials;   // [kBlocks, kPhotoTerms]
+};
+
+RgbdWs carve_rgbd(void* ws, int H, int W, size_t* total) {
+    Carver c(ws);
+    RgbdWs w;
+    w.g = carve_icp(c, H, W);
+    for (int l = 0; l < kLevels; ++l) {
+        const size_t n = (size_t)(H >> l) * (W >> l);
+        w.lv[l].model_grey = c.take<float>(n);
+        w.lv[l].data_grey = c.take<float>(n);
+        w.lv[l].model_grad = c.take<float>(2 * n);
+        w.lv[l].photo = c.take<uint8_t>(n);
+    }
+    w.photo_partials = c.take<double>((size_t)kBlocks * kPhotoTerms);
     if (total) *total = c.used();
     return w;
 }
@@ -91,8 +131,10 @@ icp_level0_kernel(int n, const float* __restrict__ depth_sil, const float* __res
 }
 
 // 2x2 reduction of a level into the next: the mean, in sample order, of the block's valid samples within kPyrBand of
-// the block's smallest valid depth
-__device__ __forceinline__ float reduce_block(const float* __restrict__ src, int Ws, int x, int y) {
+// the block's smallest valid depth.  kGrey: the mean of `grey` over exactly those samples instead (NaN if none)
+template <bool kGrey>
+__device__ __forceinline__ float reduce_block(const float* __restrict__ src, int Ws, int x, int y,
+                                              const float* __restrict__ grey) {
     const float s[4] = {src[(size_t)(2 * y) * Ws + 2 * x], src[(size_t)(2 * y) * Ws + 2 * x + 1],
                         src[(size_t)(2 * y + 1) * Ws + 2 * x], src[(size_t)(2 * y + 1) * Ws + 2 * x + 1]};
     float m = INFINITY;
@@ -104,9 +146,13 @@ __device__ __forceinline__ float reduce_block(const float* __restrict__ src, int
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
         const bool use = s[k] > 0.f && __fsub_rn(s[k], m) <= kPyrBand;
-        sum = __fadd_rn(sum, use ? s[k] : 0.f);
+        if constexpr (kGrey)
+            sum = __fadd_rn(sum, use ? grey[(size_t)(2 * y + (k >> 1)) * Ws + 2 * x + (k & 1)] : 0.f);
+        else
+            sum = __fadd_rn(sum, use ? s[k] : 0.f);
         cnt += use;
     }
+    if constexpr (kGrey) return cnt ? __fdiv_rn(sum, (float)cnt) : NAN;
     return cnt ? __fdiv_rn(sum, (float)cnt) : 0.f;
 }
 
@@ -116,8 +162,8 @@ icp_downsample_kernel(int Hd, int Wd, int Ws, const float* __restrict__ model_sr
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= Hd * Wd) return;
     const int x = i % Wd, y = i / Wd;
-    model_dst[i] = reduce_block(model_src, Ws, x, y);
-    data_dst[i] = reduce_block(data_src, Ws, x, y);
+    model_dst[i] = reduce_block<false>(model_src, Ws, x, y, nullptr);
+    data_dst[i] = reduce_block<false>(data_src, Ws, x, y, nullptr);
 }
 
 __device__ __forceinline__ float3 backproject(float z, int u, int v, float fx, float fy, float cx, float cy) {
@@ -204,6 +250,43 @@ __global__ void icp_init_kernel(const float* __restrict__ w2c_prev, const float*
     for (int k = 0; k < kStats; ++k) stats[k] = 0.0;
 }
 
+// the geometric pair of a valid data vertex v (rule 4 of the header): true if paired, with p = R v + t, the model
+// normal nm at the pair and d = p - q
+__device__ __forceinline__ bool geo_pair(const Level L, const float (&R)[12], float dist2, float3 v, int n, float3& p,
+                                         float3& nm, float3& d) {
+    p = make_float3(__fadd_rn(dot3(make_float3(R[0], R[1], R[2]), v), R[3]),
+                    __fadd_rn(dot3(make_float3(R[4], R[5], R[6]), v), R[7]),
+                    __fadd_rn(dot3(make_float3(R[8], R[9], R[10]), v), R[11]));
+    if (p.z > 0.f) {
+        const float uf = floorf(__fadd_rn(__fadd_rn(__fdiv_rn(__fmul_rn(L.fx, p.x), p.z), L.cx), 0.5f));
+        const float vf = floorf(__fadd_rn(__fadd_rn(__fdiv_rn(__fmul_rn(L.fy, p.y), p.z), L.cy), 0.5f));
+        if (uf >= 0.f && uf < (float)L.W && vf >= 0.f && vf < (float)L.H) {
+            const int j = (int)vf * L.W + (int)uf;
+            const float3 q = make_float3(L.model_vertex[j], L.model_vertex[n + j], L.model_vertex[2 * n + j]);
+            nm = make_float3(L.model_normal[j], L.model_normal[n + j], L.model_normal[2 * n + j]);
+            d = sub3(p, q);
+            if (q.z > 0.f && (nm.x != 0.f || nm.y != 0.f || nm.z != 0.f) && dot3(d, d) <= dist2) return true;
+        }
+    }
+    return false;
+}
+
+// a paired pixel's point-to-plane terms: r = n.(p - q), J = [p x n, n] into acc[0..29) (kTerms' layout)
+__device__ __forceinline__ void geo_accumulate(double* acc, float3 p, float3 nm, float3 d) {
+    const float r = dot3(nm, d);
+    const float3 pn = cross3(p, nm);
+    const double J[6] = {pn.x, pn.y, pn.z, nm.x, nm.y, nm.z};
+    int k = 0;
+#pragma unroll
+    for (int a = 0; a < 6; ++a)
+#pragma unroll
+        for (int b = a; b < 6; ++b) acc[k++] += J[a] * J[b];
+#pragma unroll
+    for (int a = 0; a < 6; ++a) acc[21 + a] += J[a] * (double)r;
+    acc[27] += (double)r * (double)r;
+    acc[28] += 1.0;
+}
+
 __global__ void __launch_bounds__(kThreads)
 icp_associate_kernel(Level L, float dist2, const double* __restrict__ T, double* __restrict__ partials) {
     __shared__ double red[kThreads / 32][kTerms];
@@ -220,33 +303,10 @@ icp_associate_kernel(Level L, float dist2, const double* __restrict__ T, double*
         if (v.z > 0.f) {
             code = 1;
             acc[29] += 1.0;
-            const float3 p = make_float3(__fadd_rn(dot3(make_float3(R[0], R[1], R[2]), v), R[3]),
-                                         __fadd_rn(dot3(make_float3(R[4], R[5], R[6]), v), R[7]),
-                                         __fadd_rn(dot3(make_float3(R[8], R[9], R[10]), v), R[11]));
-            if (p.z > 0.f) {
-                const float uf = floorf(__fadd_rn(__fadd_rn(__fdiv_rn(__fmul_rn(L.fx, p.x), p.z), L.cx), 0.5f));
-                const float vf = floorf(__fadd_rn(__fadd_rn(__fdiv_rn(__fmul_rn(L.fy, p.y), p.z), L.cy), 0.5f));
-                if (uf >= 0.f && uf < (float)L.W && vf >= 0.f && vf < (float)L.H) {
-                    const int j = (int)vf * L.W + (int)uf;
-                    const float3 q = make_float3(L.model_vertex[j], L.model_vertex[n + j], L.model_vertex[2 * n + j]);
-                    const float3 nm = make_float3(L.model_normal[j], L.model_normal[n + j], L.model_normal[2 * n + j]);
-                    const float3 d = sub3(p, q);
-                    if (q.z > 0.f && (nm.x != 0.f || nm.y != 0.f || nm.z != 0.f) && dot3(d, d) <= dist2) {
-                        code = 2;
-                        const float r = dot3(nm, d);
-                        const float3 pn = cross3(p, nm);
-                        const double J[6] = {pn.x, pn.y, pn.z, nm.x, nm.y, nm.z};
-                        int k = 0;
-#pragma unroll
-                        for (int a = 0; a < 6; ++a)
-#pragma unroll
-                            for (int b = a; b < 6; ++b) acc[k++] += J[a] * J[b];
-#pragma unroll
-                        for (int a = 0; a < 6; ++a) acc[21 + a] += J[a] * (double)r;
-                        acc[27] += (double)r * (double)r;
-                        acc[28] += 1.0;
-                    }
-                }
+            float3 p, nm, d;
+            if (geo_pair(L, R, dist2, v, n, p, nm, d)) {
+                code = 2;
+                geo_accumulate(acc, p, nm, d);
             }
         }
         L.assoc[i] = code;
@@ -268,17 +328,33 @@ icp_associate_kernel(Level L, float dist2, const double* __restrict__ T, double*
 }
 
 // sum the partials (thread k: term k, blocks in order), then thread 0 solves JtJ xi = -Jtr by Cholesky and applies
-// T <- exp(xi) T; the latest system goes to the stats record
+// T <- exp(xi) T; the latest system goes to the stats record.  kJoint (sb_rgbd_icp_align): threads 32.. also sum the
+// photometric partials, which go to stats[36..66), and the system solved is JtJ + lam2 JtJ_I, Jtr + lam2 Jtr_I
+template <bool kJoint>
 __global__ void icp_solve_kernel(const double* __restrict__ partials, double* __restrict__ T,
-                                 double* __restrict__ stats) {
-    __shared__ double s[kTerms];
+                                 double* __restrict__ stats, const double* __restrict__ photo_partials, double lam2) {
+    __shared__ double s[kJoint ? 32 + kPhotoTerms : kTerms];
     if (threadIdx.x < kTerms) {
         double a = 0.0;
         for (int b = 0; b < kBlocks; ++b) a += partials[(size_t)b * kTerms + threadIdx.x];
         s[threadIdx.x] = a;
     }
+    if constexpr (kJoint) {
+        if (threadIdx.x >= 32 && threadIdx.x < 32 + kPhotoTerms) {
+            double a = 0.0;
+            for (int b = 0; b < kBlocks; ++b) a += photo_partials[(size_t)b * kPhotoTerms + threadIdx.x - 32];
+            s[threadIdx.x] = a;
+        }
+    }
     __syncthreads();
     if (threadIdx.x != 0) return;
+    if constexpr (kJoint) {
+        const double* ph = s + 32;               // 21 JtJ_I, 6 Jtr_I, sum r_I^2, photometric pairs
+        stats[36] = ph[28];
+        stats[37] = ph[28] > 0.0 ? sqrt(ph[27] / ph[28]) : INFINITY;
+        for (int k = 0; k < 28; ++k) stats[38 + k] = ph[k];
+        for (int k = 0; k < 27; ++k) s[k] += lam2 * ph[k];
+    }
     double A[6][6], L[6][6], y[6], xi[6];
     int k = 0;
     for (int a = 0; a < 6; ++a)
@@ -350,16 +426,15 @@ __global__ void icp_solve_kernel(const double* __restrict__ partials, double* __
     for (int q = 0; q < 12; ++q) T[q] = Tn[q];
 }
 
-// acceptance and the chosen pose: w2c_out = inv(T) w2c_prev if accepted, else w2c_init
-__global__ void icp_select_kernel(const double* __restrict__ T, const float* __restrict__ w2c_prev,
-                                  const float* __restrict__ w2c_init, float* __restrict__ w2c_out,
-                                  double* __restrict__ stats) {
-    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+// acceptance (rule 5, and `extra`) and the chosen pose: w2c_out = inv(T) w2c_prev if accepted, else w2c_init
+__device__ __forceinline__ void select_pose(const double* __restrict__ T, const float* __restrict__ w2c_prev,
+                                            const float* __restrict__ w2c_init, float* __restrict__ w2c_out,
+                                            double* __restrict__ stats, bool extra) {
     const double inl = stats[3], valid = stats[4];
     const double frac = valid > 0.0 ? inl / valid : 0.0;
     const double rms = inl > 0.0 ? sqrt(stats[35] / inl) : INFINITY;
     const bool acc = valid > 0.0 && frac >= kMinInlierFrac && rms <= kMaxRms && stats[5] >= kMinPivotRatio &&
-                     stats[7] == 0.0;
+                     stats[7] == 0.0 && extra;
     stats[0] = acc ? 1.0 : 0.0;
     stats[1] = frac;
     stats[2] = rms;
@@ -375,6 +450,159 @@ __global__ void icp_select_kernel(const double* __restrict__ T, const float* __r
     w2c_out[12] = 0.f; w2c_out[13] = 0.f; w2c_out[14] = 0.f; w2c_out[15] = 1.f;
 }
 
+__global__ void icp_select_kernel(const double* __restrict__ T, const float* __restrict__ w2c_prev,
+                                  const float* __restrict__ w2c_init, float* __restrict__ w2c_out,
+                                  double* __restrict__ stats) {
+    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    select_pose(T, w2c_prev, w2c_init, w2c_out, stats, true);
+}
+
+// ---- RGB-D ICP (sb_rgbd_icp_align): the grey pyramid, the model gradient and the fused association ----------------
+
+// level 0 grey where the level-0 depth is valid (rule a), NaN elsewhere
+__global__ void __launch_bounds__(kThreads)
+rgbd_grey0_kernel(int n, const float* __restrict__ model_rgb, const float* __restrict__ data_rgb,
+                  const float* __restrict__ model_depth, const float* __restrict__ data_depth,
+                  float* __restrict__ model_grey, float* __restrict__ data_grey) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    model_grey[i] = model_depth[i] > 0.f ? grey_of(model_rgb, n, i) : NAN;
+    data_grey[i] = data_depth[i] > 0.f ? grey_of(data_rgb, n, i) : NAN;
+}
+
+__global__ void __launch_bounds__(kThreads)
+rgbd_grey_downsample_kernel(int Hd, int Wd, int Ws, const float* __restrict__ model_depth,
+                            const float* __restrict__ data_depth, const float* __restrict__ model_src,
+                            const float* __restrict__ data_src, float* __restrict__ model_dst,
+                            float* __restrict__ data_dst) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= Hd * Wd) return;
+    const int x = i % Wd, y = i / Wd;
+    model_dst[i] = reduce_block<true>(model_depth, Ws, x, y, model_src);
+    data_dst[i] = reduce_block<true>(data_depth, Ws, x, y, data_src);
+}
+
+// central differences of the model grey where the model normal is valid (rule c)
+__global__ void __launch_bounds__(kThreads)
+rgbd_gradient_kernel(Level L, GreyLevel G) {
+    const int n = L.H * L.W;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    float gu = NAN, gv = NAN;
+    if (L.model_normal[i] != 0.f || L.model_normal[n + i] != 0.f || L.model_normal[2 * n + i] != 0.f) {
+        gu = __fmul_rn(__fsub_rn(G.model_grey[i + 1], G.model_grey[i - 1]), 0.5f);
+        gv = __fmul_rn(__fsub_rn(G.model_grey[i + L.W], G.model_grey[i - L.W]), 0.5f);
+    }
+    G.model_grad[i] = gu;
+    G.model_grad[n + i] = gv;
+}
+
+// the photometric pair of a data pixel whose geometric pair is p (rule d): true with r_I and J_I
+__device__ __forceinline__ bool photo_pair(const Level& L, const GreyLevel& G, int n, float3 p, float data_grey,
+                                           float& r, float (&J)[6]) {
+    const float uc = __fadd_rn(__fdiv_rn(__fmul_rn(L.fx, p.x), p.z), L.cx);
+    const float vc = __fadd_rn(__fdiv_rn(__fmul_rn(L.fy, p.y), p.z), L.cy);
+    const float u0 = floorf(uc), v0 = floorf(vc);
+    if (!(u0 >= 0.f && __fadd_rn(u0, 1.f) < (float)L.W && v0 >= 0.f && __fadd_rn(v0, 1.f) < (float)L.H)) return false;
+    const float a = __fsub_rn(uc, u0), b = __fsub_rn(vc, v0);
+    const float a1 = __fsub_rn(1.f, a), b1 = __fsub_rn(1.f, b);
+    const float w[4] = {__fmul_rn(a1, b1), __fmul_rn(a, b1), __fmul_rn(a1, b), __fmul_rn(a, b)};
+    const int j0 = (int)v0 * L.W + (int)u0;
+    const int tap[4] = {j0, j0 + 1, j0 + L.W, j0 + L.W + 1};
+    float I = 0.f, gu = 0.f, gv = 0.f;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const float ik = G.model_grey[tap[k]], uk = G.model_grad[tap[k]], vk = G.model_grad[n + tap[k]];
+        if (!(isfinite(ik) && isfinite(uk) && isfinite(vk))) return false;
+        I = __fadd_rn(I, __fmul_rn(w[k], ik));
+        gu = __fadd_rn(gu, __fmul_rn(w[k], uk));
+        gv = __fadd_rn(gv, __fmul_rn(w[k], vk));
+    }
+    r = __fsub_rn(I, data_grey);
+    if (!(fabsf(r) <= kMaxPhotoRes)) return false;
+    const float g0 = __fdiv_rn(__fmul_rn(gu, L.fx), p.z), g1 = __fdiv_rn(__fmul_rn(gv, L.fy), p.z);
+    const float g2 = -__fdiv_rn(__fadd_rn(__fmul_rn(g0, p.x), __fmul_rn(g1, p.y)), p.z);
+    const float3 g = make_float3(g0, g1, g2);
+    const float3 pg = cross3(p, g);
+    J[0] = pg.x; J[1] = pg.y; J[2] = pg.z; J[3] = g0; J[4] = g1; J[5] = g2;
+    bool ok = true;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) ok = ok && isfinite(J[k]);
+    return ok;
+}
+
+// icp_associate_kernel's geometric pass with the photometric term fused in: the geometric partials in kTerms' layout
+// (summed exactly as icp_associate_kernel sums them), the photometric ones in kPhotoTerms' layout
+__global__ void __launch_bounds__(kThreads)
+rgbd_associate_kernel(Level L, GreyLevel G, float dist2, const double* __restrict__ T, double* __restrict__ partials,
+                      double* __restrict__ photo_partials) {
+    constexpr int kAll = kTerms + kPhotoTerms;
+    __shared__ double red[kThreads / 32][kAll];
+    float R[12];
+#pragma unroll
+    for (int k = 0; k < 12; ++k) R[k] = __double2float_rn(T[k]);
+    const int n = L.H * L.W;
+    double acc[kAll];
+#pragma unroll
+    for (int k = 0; k < kAll; ++k) acc[k] = 0.0;
+    for (int i = blockIdx.x * kThreads + threadIdx.x; i < n; i += kBlocks * kThreads) {
+        const float3 v = make_float3(L.data_vertex[i], L.data_vertex[n + i], L.data_vertex[2 * n + i]);
+        uint8_t code = 0, photo = 0;
+        if (v.z > 0.f) {
+            code = 1;
+            acc[29] += 1.0;
+            float3 p, nm, d;
+            if (geo_pair(L, R, dist2, v, n, p, nm, d)) {
+                code = 2;
+                photo = 1;
+                geo_accumulate(acc, p, nm, d);
+                float r, J[6];
+                if (photo_pair(L, G, n, p, G.data_grey[i], r, J)) {
+                    photo = 2;
+                    double* ph = acc + kTerms;
+                    int k = 0;
+#pragma unroll
+                    for (int a = 0; a < 6; ++a)
+#pragma unroll
+                        for (int b = a; b < 6; ++b) ph[k++] += (double)J[a] * (double)J[b];
+#pragma unroll
+                    for (int a = 0; a < 6; ++a) ph[21 + a] += (double)J[a] * (double)r;
+                    ph[27] += (double)r * (double)r;
+                    ph[28] += 1.0;
+                }
+            }
+        }
+        L.assoc[i] = code;
+        G.photo[i] = photo;
+    }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < kAll; ++k) {
+        double s = acc[k];
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+        if (lane == 0) red[warp][k] = s;
+    }
+    __syncthreads();
+    if (threadIdx.x < kAll) {
+        double s = 0.0;
+        for (int w = 0; w < kThreads / 32; ++w) s += red[w][threadIdx.x];
+        if (threadIdx.x < kTerms)
+            partials[(size_t)blockIdx.x * kTerms + threadIdx.x] = s;
+        else
+            photo_partials[(size_t)blockIdx.x * kPhotoTerms + threadIdx.x - kTerms] = s;
+    }
+}
+
+// rule f on top of rule 5
+__global__ void rgbd_select_kernel(const double* __restrict__ T, const float* __restrict__ w2c_prev,
+                                   const float* __restrict__ w2c_init, float* __restrict__ w2c_out,
+                                   double* __restrict__ stats, float weight) {
+    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    const bool photo_ok = weight == 0.f || (stats[36] >= kMinPhotoPairs && stats[37] <= kMaxPhotoRms);
+    select_pose(T, w2c_prev, w2c_init, w2c_out, stats, photo_ok);
+}
+
 void level_intrinsics(IcpWs& w, float fx, float fy, float cx, float cy) {
     for (int l = 0; l < kLevels; ++l) {
         Level& L = w.lv[l];
@@ -382,6 +610,36 @@ void level_intrinsics(IcpWs& w, float fx, float fy, float cx, float cy) {
         // a coarse pixel's centre is the mean of its block's centres: u_{l+1} = (u_l - 0.5) / 2
         fx = fx * 0.5f; fy = fy * 0.5f; cx = (cx - 0.5f) * 0.5f; cy = (cy - 0.5f) * 0.5f;
     }
+}
+
+bool valid_camera(float fx, float fy, float cx, float cy) {
+    return std::isfinite(fx) && fx > 0.f && std::isfinite(fy) && fy > 0.f && std::isfinite(cx) && std::isfinite(cy);
+}
+
+bool valid_iters(const int* iters) {
+    for (int l = 0; l < kLevels; ++l)
+        if (iters[l] < 0 || iters[l] > 1000) return false;
+    return true;
+}
+
+// steps 1-3 of sb_icp_align: the depth pyramid and the vertex and normal maps of every level
+int launch_maps(IcpWs& w, int height, int width, const float* model_depth_sil, const float* data_depth,
+                cudaStream_t st) {
+    const int n0 = height * width;
+    icp_level0_kernel<<<blocks_for(n0), kThreads, 0, st>>>(n0, model_depth_sil, data_depth, w.lv[0].model_depth,
+                                                           w.lv[0].data_depth);
+    SB_LAUNCH_CHECK("icp_level0_kernel");
+    for (int l = 1; l < kLevels; ++l) {
+        const Level &S = w.lv[l - 1], &D = w.lv[l];
+        icp_downsample_kernel<<<blocks_for((long long)D.H * D.W), kThreads, 0, st>>>(
+            D.H, D.W, S.W, S.model_depth, S.data_depth, D.model_depth, D.data_depth);
+        SB_LAUNCH_CHECK("icp_downsample_kernel");
+    }
+    for (int l = 0; l < kLevels; ++l) {
+        icp_maps_kernel<<<blocks_for((long long)w.lv[l].H * w.lv[l].W), kThreads, 0, st>>>(w.lv[l]);
+        SB_LAUNCH_CHECK("icp_maps_kernel");
+    }
+    return SB_OK;
 }
 
 }  // namespace
@@ -402,31 +660,16 @@ SB_API int sb_icp_align(int height, int width, const float* model_depth_sil, con
                         float fy, float cx, float cy, const float* w2c_prev, const float* w2c_init, const int* iters,
                         void* workspace, size_t workspace_bytes, float* w2c_out, double* stats, void* stream) {
     if (!valid_sizes(height, width) || !model_depth_sil || !data_depth || !w2c_prev || !w2c_init || !iters ||
-        !workspace || !w2c_out || !stats || !(std::isfinite(fx) && fx > 0.f) || !(std::isfinite(fy) && fy > 0.f) ||
-        !std::isfinite(cx) || !std::isfinite(cy))
+        !workspace || !w2c_out || !stats || !valid_camera(fx, fy, cx, cy) || !valid_iters(iters))
         return SB_ERR_BAD_ARG;
-    for (int l = 0; l < kLevels; ++l)
-        if (iters[l] < 0 || iters[l] > 1000) return SB_ERR_BAD_ARG;
     size_t need = 0;
     carve_icp(nullptr, height, width, &need);
     if (workspace_bytes < need) return SB_ERR_WORKSPACE;
     IcpWs w = carve_icp(workspace, height, width, &need);
     level_intrinsics(w, fx, fy, cx, cy);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int n0 = height * width;
-    icp_level0_kernel<<<blocks_for(n0), kThreads, 0, st>>>(n0, model_depth_sil, data_depth, w.lv[0].model_depth,
-                                                           w.lv[0].data_depth);
-    SB_LAUNCH_CHECK("icp_level0_kernel");
-    for (int l = 1; l < kLevels; ++l) {
-        const Level &S = w.lv[l - 1], &D = w.lv[l];
-        icp_downsample_kernel<<<blocks_for((long long)D.H * D.W), kThreads, 0, st>>>(
-            D.H, D.W, S.W, S.model_depth, S.data_depth, D.model_depth, D.data_depth);
-        SB_LAUNCH_CHECK("icp_downsample_kernel");
-    }
-    for (int l = 0; l < kLevels; ++l) {
-        icp_maps_kernel<<<blocks_for((long long)w.lv[l].H * w.lv[l].W), kThreads, 0, st>>>(w.lv[l]);
-        SB_LAUNCH_CHECK("icp_maps_kernel");
-    }
+    const int rc = launch_maps(w, height, width, model_depth_sil, data_depth, st);
+    if (rc != SB_OK) return rc;
     icp_init_kernel<<<1, 1, 0, st>>>(w2c_prev, w2c_init, w.T, stats);
     SB_LAUNCH_CHECK("icp_init_kernel");
     for (int l = kLevels - 1; l >= 0; --l) {
@@ -434,12 +677,90 @@ SB_API int sb_icp_align(int height, int width, const float* model_depth_sil, con
         for (int it = 0; it < iters[l]; ++it) {
             icp_associate_kernel<<<kBlocks, kThreads, 0, st>>>(w.lv[l], d * d, w.T, w.partials);
             SB_LAUNCH_CHECK("icp_associate_kernel");
-            icp_solve_kernel<<<1, 32, 0, st>>>(w.partials, w.T, stats);
+            icp_solve_kernel<false><<<1, 32, 0, st>>>(w.partials, w.T, stats, nullptr, 0.0);
             SB_LAUNCH_CHECK("icp_solve_kernel");
         }
     }
     icp_select_kernel<<<1, 1, 0, st>>>(w.T, w2c_prev, w2c_init, w2c_out, stats);
     SB_LAUNCH_CHECK("icp_select_kernel");
+    return SB_OK;
+}
+
+SB_API int sb_rgbd_icp_workspace_bytes(int height, int width, size_t* bytes) {
+    if (!valid_sizes(height, width) || !bytes) return SB_ERR_BAD_ARG;
+    carve_rgbd(nullptr, height, width, bytes);
+    return SB_OK;
+}
+
+SB_API int sb_rgbd_icp_align(int height, int width, const float* model_depth_sil, const float* model_rgb,
+                             const float* data_depth, const float* data_rgb, float fx, float fy, float cx, float cy,
+                             const float* w2c_prev, const float* w2c_init, const int* iters, float weight,
+                             void* workspace, size_t workspace_bytes, float* w2c_out, double* stats, void* stream) {
+    if (!valid_sizes(height, width) || !model_depth_sil || !model_rgb || !data_depth || !data_rgb || !w2c_prev ||
+        !w2c_init || !iters || !workspace || !w2c_out || !stats || !valid_camera(fx, fy, cx, cy) ||
+        !valid_iters(iters) || !(std::isfinite(weight) && weight >= 0.f))
+        return SB_ERR_BAD_ARG;
+    size_t need = 0;
+    carve_rgbd(nullptr, height, width, &need);
+    if (workspace_bytes < need) return SB_ERR_WORKSPACE;
+    RgbdWs w = carve_rgbd(workspace, height, width, &need);
+    level_intrinsics(w.g, fx, fy, cx, cy);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int rc = launch_maps(w.g, height, width, model_depth_sil, data_depth, st);
+    if (rc != SB_OK) return rc;
+    const int n0 = height * width;
+    rgbd_grey0_kernel<<<blocks_for(n0), kThreads, 0, st>>>(n0, model_rgb, data_rgb, w.g.lv[0].model_depth,
+                                                           w.g.lv[0].data_depth, w.lv[0].model_grey,
+                                                           w.lv[0].data_grey);
+    SB_LAUNCH_CHECK("rgbd_grey0_kernel");
+    for (int l = 1; l < kLevels; ++l) {
+        const Level &S = w.g.lv[l - 1], &D = w.g.lv[l];
+        rgbd_grey_downsample_kernel<<<blocks_for((long long)D.H * D.W), kThreads, 0, st>>>(
+            D.H, D.W, S.W, S.model_depth, S.data_depth, w.lv[l - 1].model_grey, w.lv[l - 1].data_grey,
+            w.lv[l].model_grey, w.lv[l].data_grey);
+        SB_LAUNCH_CHECK("rgbd_grey_downsample_kernel");
+    }
+    for (int l = 0; l < kLevels; ++l) {
+        rgbd_gradient_kernel<<<blocks_for((long long)w.g.lv[l].H * w.g.lv[l].W), kThreads, 0, st>>>(w.g.lv[l],
+                                                                                                     w.lv[l]);
+        SB_LAUNCH_CHECK("rgbd_gradient_kernel");
+    }
+    icp_init_kernel<<<1, 1, 0, st>>>(w2c_prev, w2c_init, w.g.T, stats);
+    SB_LAUNCH_CHECK("icp_init_kernel");
+    SB_CUDA_CHECK(cudaMemsetAsync(stats + kStats, 0, (kRgbdStats - kStats) * sizeof(double), st));
+    const double lam2 = (double)weight * (double)weight;
+    for (int l = kLevels - 1; l >= 0; --l) {
+        const float d = kDist0 * (float)(1 << l);
+        for (int it = 0; it < iters[l]; ++it) {
+            rgbd_associate_kernel<<<kBlocks, kThreads, 0, st>>>(w.g.lv[l], w.lv[l], d * d, w.g.T, w.g.partials,
+                                                                w.photo_partials);
+            SB_LAUNCH_CHECK("rgbd_associate_kernel");
+            icp_solve_kernel<true><<<1, 64, 0, st>>>(w.g.partials, w.g.T, stats, w.photo_partials, lam2);
+            SB_LAUNCH_CHECK("icp_solve_kernel");
+        }
+    }
+    rgbd_select_kernel<<<1, 1, 0, st>>>(w.g.T, w2c_prev, w2c_init, w2c_out, stats, weight);
+    SB_LAUNCH_CHECK("rgbd_select_kernel");
+    return SB_OK;
+}
+
+SB_API int sb_rgbd_icp_export(int height, int width, const void* workspace, size_t workspace_bytes, int level,
+                              float* model_grey, float* data_grey, float* model_grad, uint8_t* photo, void* stream) {
+    if (!valid_sizes(height, width) || !workspace || level < 0 || level >= kLevels || !model_grey || !data_grey ||
+        !model_grad || !photo)
+        return SB_ERR_BAD_ARG;
+    size_t need = 0;
+    carve_rgbd(nullptr, height, width, &need);
+    if (workspace_bytes < need) return SB_ERR_WORKSPACE;
+    RgbdWs w = carve_rgbd(const_cast<void*>(workspace), height, width, &need);
+    const GreyLevel& G = w.lv[level];
+    const size_t n = (size_t)(height >> level) * (width >> level);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const cudaMemcpyKind k = cudaMemcpyDeviceToDevice;
+    SB_CUDA_CHECK(cudaMemcpyAsync(model_grey, G.model_grey, n * sizeof(float), k, st));
+    SB_CUDA_CHECK(cudaMemcpyAsync(data_grey, G.data_grey, n * sizeof(float), k, st));
+    SB_CUDA_CHECK(cudaMemcpyAsync(model_grad, G.model_grad, 2 * n * sizeof(float), k, st));
+    SB_CUDA_CHECK(cudaMemcpyAsync(photo, G.photo, n, k, st));
     return SB_OK;
 }
 

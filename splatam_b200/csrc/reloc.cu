@@ -22,6 +22,7 @@ constexpr int kThreads = 256;
 constexpr int kTopkThreads = 1024;
 constexpr int kHealthBlocks = SB_RELOC_HEALTH_BLOCKS;   // fixed, so the summation order does not depend on the device
 constexpr float kSilThres = 0.99f;                      // a pixel is observed where the silhouette exceeds this
+constexpr int kHealthRgbTerms = 11;                    // sb_track_health_rgb's partials: four counts, seven NCC sums
 constexpr int kScoreTerms = 5;                          // per channel: n, n_query, then pass 1 sums q, d / pass 2 cross
 
 inline unsigned int blocks_for(long long n) { return (unsigned int)((n + kThreads - 1) / kThreads); }
@@ -52,8 +53,7 @@ thumb_means_kernel(int B, int H, int W, int s, int h, int w, const float* __rest
                 seen = sv > kSilThres;
                 d = __fdiv_rn(d, sv);
             }
-            const float g = __fadd_rn(__fadd_rn(__fmul_rn(0.299f, R[p]), __fmul_rn(0.587f, R[plane + p])),
-                                      __fmul_rn(0.114f, R[2 * plane + p]));
+            const float g = grey_of(R, plane, p);
             if (seen && isfinite(g)) { gs = __fadd_rn(gs, g); ++gn; }
             if (seen && depth_ok(d)) { ds = __fadd_rn(ds, d); ++dn; }
         }
@@ -222,12 +222,28 @@ reloc_topk_kernel(int N, int k, const double* __restrict__ scores, int* __restri
 }
 
 // per-block partial counts: valid frame depth, covered (valid and observed by the map), inliers, sum of squared
-// residuals over the covered pixels
+// residuals over the covered pixels.  kMode 0: sb_track_health.  kMode 1 and 2, the two passes of
+// sb_track_health_rgb's colour NCC over the inliers whose six colour values are all finite: [4] pairs, [5..8) sums of
+// the map's r, g, b, [8..11) of the frame's; then, with the per-channel means from pass 1's partials (summed in block
+// order), [4] sum over channels of (m - mm)(f - mf), [5] of (m - mm)^2, [6] of (f - mf)^2
+template <int kMode>
 __global__ void __launch_bounds__(kThreads)
 health_partials_kernel(int n, const float* __restrict__ depth_sil, const float* __restrict__ frame_depth, float tau_abs,
-                       float tau_rel, double* __restrict__ partials) {
-    __shared__ double red[kThreads / 32][4];
-    double a[4] = {0.0, 0.0, 0.0, 0.0};
+                       float tau_rel, double* __restrict__ partials, const float* __restrict__ map_rgb,
+                       const float* __restrict__ frame_rgb, const double* __restrict__ pass1) {
+    constexpr int N = kMode == 0 ? 4 : kHealthRgbTerms;
+    __shared__ double red[kThreads / 32][N];
+    double a[N] = {0.0, 0.0, 0.0, 0.0};
+    double mm[3] = {0.0, 0.0, 0.0}, mf[3] = {0.0, 0.0, 0.0};
+    if constexpr (kMode == 2) {
+        double s[7] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+        for (int b = 0; b < kHealthBlocks; ++b)
+            for (int k = 0; k < 7; ++k) s[k] += pass1[(size_t)b * N + 4 + k];
+        for (int c = 0; c < 3; ++c) {
+            mm[c] = s[1 + c] / s[0];
+            mf[c] = s[4 + c] / s[0];
+        }
+    }
     for (int i = blockIdx.x * kThreads + threadIdx.x; i < n; i += kHealthBlocks * kThreads) {
         const float df = frame_depth[i];
         if (!depth_ok(df)) continue;
@@ -238,10 +254,38 @@ health_partials_kernel(int n, const float* __restrict__ depth_sil, const float* 
         const float r = __fsub_rn(__fdiv_rn(depth_sil[i], sil), df);
         a[2] += fabsf(r) < fmaxf(tau_abs, __fmul_rn(tau_rel, df)) ? 1.0 : 0.0;
         a[3] += (double)r * (double)r;
+        if constexpr (kMode != 0) {
+            if (!(fabsf(r) < fmaxf(tau_abs, __fmul_rn(tau_rel, df)))) continue;
+            float cm[3], cf[3];
+            bool ok = true;
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                cm[c] = map_rgb[(size_t)c * n + i];
+                cf[c] = frame_rgb[(size_t)c * n + i];
+                ok = ok && isfinite(cm[c]) && isfinite(cf[c]);
+            }
+            if (!ok) continue;
+            if constexpr (kMode == 1) {
+                a[4] += 1.0;
+#pragma unroll
+                for (int c = 0; c < 3; ++c) {
+                    a[5 + c] += (double)cm[c];
+                    a[8 + c] += (double)cf[c];
+                }
+            } else {
+#pragma unroll
+                for (int c = 0; c < 3; ++c) {
+                    const double em = (double)cm[c] - mm[c], ef = (double)cf[c] - mf[c];
+                    a[4] += em * ef;
+                    a[5] += em * em;
+                    a[6] += ef * ef;
+                }
+            }
+        }
     }
-    block_sum<4>(a, red);
+    block_sum<N>(a, red);
     if (threadIdx.x == 0)
-        for (int k = 0; k < 4; ++k) partials[(size_t)blockIdx.x * 4 + k] = a[k];
+        for (int k = 0; k < N; ++k) partials[(size_t)blockIdx.x * N + k] = a[k];
 }
 
 __global__ void health_finish_kernel(const double* __restrict__ partials, double min_coverage, double min_inliers,
@@ -255,6 +299,27 @@ __global__ void health_finish_kernel(const double* __restrict__ partials, double
     stats[2] = s[2];
     stats[3] = s[1] > 0.0 ? sqrt(s[3] / s[1]) : INFINITY;
     stats[4] = (s[0] > 0.0 && s[1] > 0.0 && s[1] / s[0] >= min_coverage && s[2] / s[1] >= min_inliers) ? 1.0 : 0.0;
+}
+
+// sb_track_health_rgb's record: sb_track_health's five entries (the same sums), the NCC pairs and the colour NCC
+__global__ void health_rgb_finish_kernel(const double* __restrict__ pass1, const double* __restrict__ pass2,
+                                         double min_coverage, double min_inliers, double min_ncc,
+                                         double* __restrict__ stats) {
+    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    double s[5] = {0.0, 0.0, 0.0, 0.0, 0.0}, c[3] = {0.0, 0.0, 0.0};
+    for (int b = 0; b < kHealthBlocks; ++b) {
+        for (int k = 0; k < 5; ++k) s[k] += pass1[(size_t)b * kHealthRgbTerms + k];
+        for (int k = 0; k < 3; ++k) c[k] += pass2[(size_t)b * kHealthRgbTerms + 4 + k];
+    }
+    stats[0] = s[0];
+    stats[1] = s[1];
+    stats[2] = s[2];
+    stats[3] = s[1] > 0.0 ? sqrt(s[3] / s[1]) : INFINITY;
+    const bool geo = s[0] > 0.0 && s[1] > 0.0 && s[1] / s[0] >= min_coverage && s[2] / s[1] >= min_inliers;
+    const double ncc = (c[1] > 0.0 && c[2] > 0.0) ? c[0] / sqrt(c[1] * c[2]) : 0.0;
+    stats[5] = s[4];
+    stats[6] = ncc;
+    stats[4] = (geo && s[4] >= SB_RELOC_MIN_NCC_PAIRS && ncc >= min_ncc) ? 1.0 : 0.0;
 }
 
 }  // namespace
@@ -315,11 +380,35 @@ SB_API int sb_track_health(int height, int width, const float* depth_sil, const 
         || !(min_coverage >= 0.0 && min_coverage <= 1.0) || !(min_inliers >= 0.0 && min_inliers <= 1.0))
         return SB_ERR_BAD_ARG;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    health_partials_kernel<<<kHealthBlocks, kThreads, 0, st>>>(height * width, depth_sil, frame_depth, tau_abs, tau_rel,
-                                                               scratch);
+    health_partials_kernel<0><<<kHealthBlocks, kThreads, 0, st>>>(height * width, depth_sil, frame_depth, tau_abs,
+                                                                  tau_rel, scratch, nullptr, nullptr, nullptr);
     SB_LAUNCH_CHECK("health_partials_kernel");
     health_finish_kernel<<<1, 1, 0, st>>>(scratch, min_coverage, min_inliers, stats);
     SB_LAUNCH_CHECK("health_finish_kernel");
+    return SB_OK;
+}
+
+SB_API int sb_track_health_rgb(int height, int width, const float* depth_sil, const float* frame_depth,
+                               const float* map_rgb, const float* frame_rgb, float tau_abs, float tau_rel,
+                               double min_coverage, double min_inliers, double min_ncc, double* scratch, double* stats,
+                               void* stream) {
+    if (height < 1 || width < 1 || (long long)height * width >= (1LL << 31) || !depth_sil || !frame_depth ||
+        !map_rgb || !frame_rgb || !scratch || !stats || !(std::isfinite(tau_abs) && tau_abs >= 0.f) ||
+        !(std::isfinite(tau_rel) && tau_rel >= 0.f) || !(min_coverage >= 0.0 && min_coverage <= 1.0) ||
+        !(min_inliers >= 0.0 && min_inliers <= 1.0) || !(min_ncc >= -1.0 && min_ncc <= 1.0))
+        return SB_ERR_BAD_ARG;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    double* pass1 = scratch;
+    double* pass2 = scratch + (size_t)kHealthRgbTerms * kHealthBlocks;
+    const int n = height * width;
+    health_partials_kernel<1><<<kHealthBlocks, kThreads, 0, st>>>(n, depth_sil, frame_depth, tau_abs, tau_rel, pass1,
+                                                                  map_rgb, frame_rgb, nullptr);
+    SB_LAUNCH_CHECK("health_partials_kernel");
+    health_partials_kernel<2><<<kHealthBlocks, kThreads, 0, st>>>(n, depth_sil, frame_depth, tau_abs, tau_rel, pass2,
+                                                                  map_rgb, frame_rgb, pass1);
+    SB_LAUNCH_CHECK("health_partials_kernel");
+    health_rgb_finish_kernel<<<1, 1, 0, st>>>(pass1, pass2, min_coverage, min_inliers, min_ncc, stats);
+    SB_LAUNCH_CHECK("health_rgb_finish_kernel");
     return SB_OK;
 }
 

@@ -12,7 +12,9 @@ pose; the best verified pose is refined by tracking and kept only if it passes t
 * ``thumbnails``         sb_reloc_thumbnails: [B,2,h,w] descriptors of B RGB-D images
 * ``score`` / ``topk``   sb_reloc_score and sb_reloc_topk
 * ``Database``           descriptors with their camera columns; poses are read from camera columns at query time
-* ``health``             sb_track_health on the render at column t; ``read_health`` is its host view
+* ``health``             sb_track_health (with cfg["photometric"], sb_track_health_rgb, which adds the colour NCC of the
+                         map's RGB render against the frame's) on the render at column t; ``read_health`` is its host
+                         view
 * ``relocalise``         retrieval, ICP verification, tracking and the health check; writes column t only on success
 * ``localise_sequence``  tracks a new sequence in a saved map that stays frozen, relocalising lost frames
 
@@ -37,10 +39,14 @@ DEFAULTS = dict(
     min_inliers=0.5,                # health: inliers / covered pixels
     min_inlier_frac=0.6,            # ICP acceptance of a candidate, on top of sb_icp_align's own
     max_rms=0.02,                   # [m]
+    photometric=False,              # health: sb_track_health_rgb; candidates verified by icp.align_rgbd
+    min_ncc=0.7,                    # photometric health: colour NCC of the map render against the frame (inliers)
 )
 MAX_K = 8
 HEALTH_STATS = 5
+HEALTH_RGB_STATS = 7
 HEALTH_BLOCKS = 128
+HEALTH_RGB_SCRATCH = 22 * HEALTH_BLOCKS     # two passes of 11 partial sums per block
 
 
 def config(relocalise):
@@ -68,6 +74,9 @@ def config(relocalise):
     for key in ("min_coverage", "min_inliers", "min_inlier_frac"):
         cfg[key] = num(key, 0.0, 1.0)
     cfg["max_rms"] = num("max_rms", 0.0, lo_open=True)
+    if not isinstance(cfg["photometric"], bool):
+        raise ValueError("relocalise['photometric'] = %r must be True or False" % (cfg["photometric"],))
+    cfg["min_ncc"] = num("min_ncc", -1.0, 1.0)
     return cfg
 
 
@@ -186,28 +195,49 @@ def _health_of(ds, depth, cfg):
     return stats
 
 
+def _health_rgb_of(ds, im, depth, rgb, cfg):
+    _lib.need_cuda("reloc.health", ds, im, depth, rgb)
+    H, W = ds.shape[-2:]
+    scratch = torch.empty(HEALTH_RGB_SCRATCH, dtype=torch.float64, device=ds.device)
+    stats = torch.empty(HEALTH_RGB_STATS, dtype=torch.float64, device=ds.device)
+    _lib.call("sb_track_health_rgb", H, W, ds[:2].float().contiguous(), depth.reshape(H, W).float().contiguous(),
+              im.reshape(3, H, W).float().contiguous(), rgb.reshape(3, H, W).float().contiguous(), cfg["tau_abs"],
+              cfg["tau_rel"], cfg["min_coverage"], cfg["min_inliers"], cfg["min_ncc"], scratch, stats,
+              device=ds.device)
+    return stats
+
+
 def health(params, frame, t, cfg=None, render=None, fused=None):
     """The health record (device float64 [5]: valid, covered, inliers, rms, healthy) of frame t: its depth against
-    the map's depth/silhouette render at column t of params (sb_track_health)."""
+    the map's depth/silhouette render at column t of params (sb_track_health).  With cfg["photometric"], [7]: also
+    the NCC pairs and the colour NCC of the map's RGB render against the frame's, which `healthy` then includes
+    (sb_track_health_rgb)."""
     cfg = config({}) if cfg is None else cfg
+    if cfg["photometric"]:
+        im, ds = icp.model_render(params, t, frame, render, fused)
+        return _health_rgb_of(ds, im, frame["depth"], frame["im"], cfg)
     return _health_of(icp.model_depth_sil(params, t, frame, render, fused), frame["depth"], cfg)
 
 
 def read_health(stats):
-    """Host dict of a health record (one device read): ok, valid, covered, inliers, coverage, inlier_frac, rms."""
+    """Host dict of a health record (one device read): ok, valid, covered, inliers, coverage, inlier_frac, rms; for
+    a photometric record also ncc_pairs and ncc."""
     s = stats.detach().cpu().numpy()
-    return dict(ok=bool(s[4]), valid=int(s[0]), covered=int(s[1]), inliers=int(s[2]),
-                coverage=float(s[1] / s[0]) if s[0] > 0 else 0.0, inlier_frac=float(s[2] / s[1]) if s[1] > 0 else 0.0,
-                rms=float(s[3]))
+    d = dict(ok=bool(s[4]), valid=int(s[0]), covered=int(s[1]), inliers=int(s[2]),
+             coverage=float(s[1] / s[0]) if s[0] > 0 else 0.0, inlier_frac=float(s[2] / s[1]) if s[1] > 0 else 0.0,
+             rms=float(s[3]))
+    if len(s) >= HEALTH_RGB_STATS:
+        d.update(ncc_pairs=int(s[5]), ncc=float(s[6]))
+    return d
 
 
-def _render_at(params, frame, pose, render, fused):
+def _render_at(params, frame, pose, render, fused, rgb=False):
     render = M.default_render if render is None else render
     fused = (params["means3D"].is_cuda and render is M.default_render) if fused is None else fused
     with torch.no_grad():
-        _, ds, _, _ = M._render_pair(params, dict(id=frame["id"], cam=frame["cam"], w2c=frame["w2c"], pose=pose),
-                                     render, fused, camera_grad=False)
-    return ds
+        im, ds, _, _ = M._render_pair(params, dict(id=frame["id"], cam=frame["cam"], w2c=frame["w2c"], pose=pose),
+                                      render, fused, camera_grad=False)
+    return (im, ds) if rgb else ds
 
 
 def _column_of(w2c, w2c0):
@@ -223,8 +253,9 @@ def relocalise(params, frame, t, db, intrinsics, cfg=None, tracking=None, render
 
     1. The frame's descriptor is scored against `db` and the k best entries (scores above -2) are the candidates.
     2. Each candidate's pose (db.w2c) renders the map's depth/silhouette; icp.align aligns the frame's depth with it,
-       the candidate pose being both w2c_prev and w2c_init.  A candidate is accepted if sb_icp_align accepts it and its
-       inlier fraction >= min_inlier_frac and RMS <= max_rms.
+       the candidate pose being both w2c_prev and w2c_init (with cfg["photometric"], icp.align_rgbd against the
+       candidate render's RGB too).  A candidate is accepted if the alignment accepts it and its inlier fraction >=
+       min_inlier_frac and RMS <= max_rms.
     3. The first accepted candidate in score order wins (the higher score, then the lower index); its ICP pose goes
        into column t and mapping.track_frame refines it (`tracking`: its keyword arguments; the map is detached).
     4. The health check at column t decides: healthy keeps the column, otherwise column t is restored bit for bit.
@@ -253,8 +284,12 @@ def relocalise(params, frame, t, db, intrinsics, cfg=None, tracking=None, render
     for i, _ in cands:
         w2c_c, q_c = db.w2c(rots, trans, i)
         pose = w2c0 @ w2c_c
-        ds = _render_at(params, frame, (w2c_c, q_c), render, fused)
-        out, st = icp.align(ds, frame["depth"], intrinsics, pose, pose)
+        if cfg["photometric"]:
+            im, ds = _render_at(params, frame, (w2c_c, q_c), render, fused, rgb=True)
+            out, st = icp.align_rgbd(ds, im, frame["depth"], frame["im"], intrinsics, pose, pose)
+        else:
+            ds = _render_at(params, frame, (w2c_c, q_c), render, fused)
+            out, st = icp.align(ds, frame["depth"], intrinsics, pose, pose)
         outs.append(out)
         stats.append(st)
     host = torch.stack(stats).cpu().numpy()                               # host read 2
@@ -291,9 +326,10 @@ def localise_sequence(params, frames, intrinsics, db, cfg=None, pose_init="const
     refined by icp.init_pose), is tracked, health-checked and relocalised when lost.  A frame that stays lost takes
     the previous frame's column; the frame after a relocalised or lost one starts with zero velocity.  The map's
     Gaussians in `params` are used detached; `db` holds the record's cameras.  Returns dict(rots [1,4,T], trans
-    [1,3,T] in the map's frame, lost, relocalised (bool lists), health [T, 5] (host), reloc (relocalise records))."""
-    if pose_init not in ("constant_velocity", "icp"):
-        raise ValueError("pose_init must be 'constant_velocity' or 'icp', got %r" % (pose_init,))
+    [1,3,T] in the map's frame, lost, relocalised (bool lists), health [T, 5] (host; [T, 7] with cfg["photometric"]:
+    also the NCC pairs and the NCC), reloc (relocalise records))."""
+    if pose_init not in ("constant_velocity", "icp", "rgbd_icp"):
+        raise ValueError("pose_init must be 'constant_velocity', 'icp' or 'rgbd_icp', got %r" % (pose_init,))
     cfg = config({}) if cfg is None else cfg
     tracking = {} if tracking is None else tracking
     dev = params["means3D"].device
@@ -316,8 +352,9 @@ def localise_sequence(params, frames, intrinsics, db, cfg=None, pose_init="const
         p = dict(gauss, cam_unnorm_rots=rots, cam_trans=trans)
         h = None
         if t > 0:
-            if pose_init == "icp":
-                icp.init_pose(p, frames[t], t, intrinsics, render=render, fused=fused)
+            if pose_init != "constant_velocity":
+                icp.init_pose(p, frames[t], t, intrinsics, render=render, fused=fused,
+                              photometric=pose_init == "rgbd_icp")
             M.track_frame(p, frames[t], render=render, fused=fused, **tracking)
             rots, trans = p["cam_unnorm_rots"].detach(), p["cam_trans"].detach()
             p = dict(gauss, cam_unnorm_rots=rots, cam_trans=trans)
@@ -336,6 +373,7 @@ def localise_sequence(params, frames, intrinsics, db, cfg=None, pose_init="const
                         trans[..., t] = trans[..., t - 1]
                 if h is None:
                     h = read_health(health(p, frames[t], t, cfg, render, fused))
-        healths.append([h["valid"], h["covered"], h["inliers"], h["rms"], float(h["ok"])])
+        healths.append([h["valid"], h["covered"], h["inliers"], h["rms"], float(h["ok"])] +
+                       ([h["ncc_pairs"], h["ncc"]] if cfg["photometric"] else []))
     return dict(rots=rots, trans=trans, lost=lost, relocalised=relocd, health=np.array(healths, dtype=np.float64),
                 reloc=recs)

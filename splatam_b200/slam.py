@@ -177,7 +177,9 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     `pose_init`: how each frame's tracking starts.  "constant_velocity" (the default) is the reference's guess
     (splatam.py:423-444).  "icp" follows that guess with icp.init_pose: the map's depth rendered at frame t-1's pose is
     aligned with frame t's depth by point-to-plane ICP on the GPU (needs CUDA tensors and `intrinsics`), and the ICP
-    pose replaces the guess when it passes its acceptance test.  Every rank computes the same pose.  With "icp",
+    pose replaces the guess when it passes its acceptance test.  "rgbd_icp" aligns with icp.align_rgbd instead: the
+    map's RGB render and frame t's colour add a photometric term at icp.DEFAULT_WEIGHT, and the records also hold
+    `photo_rms`.  Every rank computes the same pose.  With "icp",
     `timing` also receives `pose_init_s` (synchronised wall seconds) and the result holds `icp`: per tracked frame
     dict(frame, accepted, inlier_frac, rms), read from the device once at the end.  `pose_init` is not stored in
     checkpoints: a resumed run passes it again.
@@ -190,7 +192,9 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     in place of its first entry.  `timing` also receives `loop_closure_s` and the result holds `loops`: one dict(frame,
     keyframe, accepted, inlier_frac, rms, correction_m, correction_deg) per measured candidate.  Checkpoints then also
     hold the graph and every keyframe's est_w2c; `loop_closure` itself is not stored: a resumed run passes it again.
-    `relocalise`: None (the default: off, and nothing of it runs) or a dict of reloc.DEFAULTS keys (needs CUDA tensors
+    `relocalise`: None (the default: off, and nothing of it runs) or a dict of reloc.DEFAULTS keys (`photometric`: the
+    health check also compares the map's RGB render with the frame's by colour NCC, and candidates are verified with
+    icp.align_rgbd; needs CUDA tensors
     and `intrinsics`; one rank only -- with several ranks it raises ValueError).  Each keyframe's frame adds its
     descriptor to a reloc.Database when it joins the keyframe list.  After tracking, reloc.health checks every frame
     against the map's depth/silhouette render at its pose (one render and one small host read per frame); a lost frame
@@ -225,14 +229,14 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     timing.update(tracking_s=0.0, mapping_s=0.0, mapping_iters=0, tracking_iters=0, setup_s=0.0)
     T = len(frames)
     _check_resume(gauss_init, resume, T, checkpoint_every, checkpoint_dir)
-    if pose_init not in ("constant_velocity", "icp"):
-        raise ValueError("pose_init must be 'constant_velocity' or 'icp', got %r" % (pose_init,))
-    use_icp = pose_init == "icp"
+    if pose_init not in ("constant_velocity", "icp", "rgbd_icp"):
+        raise ValueError("pose_init must be 'constant_velocity', 'icp' or 'rgbd_icp', got %r" % (pose_init,))
+    use_icp = pose_init != "constant_velocity"
     if use_icp:
         if intrinsics is None:
-            raise ValueError("pose_init='icp' needs the intrinsics")
+            raise ValueError("pose_init=%r needs the intrinsics" % (pose_init,))
         from . import _lib, icp
-        _lib.need_cuda("run_slam(pose_init='icp')", (gauss_init or resume["gauss"])["means3D"])
+        _lib.need_cuda("run_slam(pose_init=%r)" % (pose_init,), (gauss_init or resume["gauss"])["means3D"])
         K_icp = np.asarray(torch.as_tensor(intrinsics).detach().cpu(), dtype=np.float64)
         timing["pose_init_s"] = 0.0
         icp_stats = []
@@ -334,7 +338,8 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
         torch.cuda.synchronize(dev) if dev.type == "cuda" else None
         if use_icp:
             t0 = time.perf_counter()
-            icp_stats.append(icp.init_pose(params, frames[t], t, K_icp, render=render, fused=fused))
+            icp_stats.append(icp.init_pose(params, frames[t], t, K_icp, render=render, fused=fused,
+                                           photometric=pose_init == "rgbd_icp"))
             torch.cuda.synchronize(dev)
             timing["pose_init_s"] += time.perf_counter() - t0
         t0 = time.perf_counter()
@@ -364,7 +369,8 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
                     reloc_db.columns[rec["chosen"]] if rec["chosen"] is not None else None),
                     score=(rec["scores"][rec["candidates"].index(rec["chosen"])] if rec["chosen"] is not None
                            else None), coverage=h.get("coverage"), inlier_frac=h.get("inlier_frac"), rms=h.get("rms"),
-                    candidates=rec["columns"], scores=rec["scores"], icp=rec["icp"]))
+                    candidates=rec["columns"], scores=rec["scores"], icp=rec["icp"],
+                    **({"ncc": h.get("ncc")} if reloc_cfg["photometric"] else {})))
                 if not rec["accepted"]:
                     with torch.no_grad():
                         rots[..., t] = rots[..., t - 1]
@@ -449,7 +455,8 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
                keyframe_est_w2c=[kf["est_w2c"] for kf in keyframes])
     if use_icp:
         st = torch.stack(icp_stats).cpu().numpy() if icp_stats else np.zeros((0, icp.STATS))
-        out["icp"] = [dict(frame=start + i, accepted=bool(s[0]), inlier_frac=float(s[1]), rms=float(s[2]))
+        out["icp"] = [dict(frame=start + i, accepted=bool(s[0]), inlier_frac=float(s[1]), rms=float(s[2]),
+                           **({"photo_rms": float(s[37])} if pose_init == "rgbd_icp" else {}))
                       for i, s in enumerate(st)]
     if use_loop:
         out["loops"] = loops

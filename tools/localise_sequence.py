@@ -33,7 +33,10 @@ def parse_args(argv=None):
     ap.add_argument("--config", default=None, help="data YAML (camera_params) of the query; default: the shipped camera")
     ap.add_argument("--frames", type=int, default=0, help="use only the first N frames (0: all)")
     ap.add_argument("--every", type=int, default=5, help="database columns when the record has no keyframe list")
-    ap.add_argument("--pose-init", default="constant_velocity", choices=("constant_velocity", "icp"))
+    ap.add_argument("--pose-init", default="constant_velocity", choices=("constant_velocity", "icp", "rgbd_icp"))
+    ap.add_argument("--photometric", action="store_true",
+                    help="photometric health check (colour NCC of the map's render against the frame) and RGB-D ICP "
+                         "verification of the candidates")
     ap.add_argument("--tracking-iters", type=int, default=40)
     ap.add_argument("--k", type=int, default=5, help="candidates verified by ICP")
     ap.add_argument("--map-dataset", default=None)
@@ -92,7 +95,8 @@ def main(argv=None):
         frames = [seq[t] for t in range(n)]
         K = seq.intrinsics.cpu().double().numpy()
         db = reloc.Database.from_record(params, cols, seq.cam, w2c0=frames[0]["w2c"])
-        res = reloc.localise_sequence(params, frames, K, db, reloc.config(dict(k=a.k)), pose_init=a.pose_init,
+        cfg = reloc.config(dict(k=a.k, photometric=a.photometric))
+        res = reloc.localise_sequence(params, frames, K, db, cfg, pose_init=a.pose_init,
                                       tracking=dict(num_iters=a.tracking_iters))
         query_to_world = np.linalg.inv(seq.files.world_to_map)
         rel = [seq.files.poses[t].double().numpy() for t in range(n)]

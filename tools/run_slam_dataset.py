@@ -17,10 +17,12 @@ One GPU.
 --config takes a data YAML of the reference's shape (default: the shipped camera of the dataset); --start / --end /
 --stride select frames as the reference does; --frames caps the number of frames; --tracking-iters / --mapping-iters
 override the shipped iteration counts; --pose-init icp starts each frame's tracking from a point-to-plane ICP
-alignment of its depth with the map's (splatam_b200.icp; default constant_velocity, the reference's guess);
+alignment of its depth with the map's (splatam_b200.icp; default constant_velocity, the reference's guess), and
+--pose-init rgbd_icp from a joint alignment of its depth and colour with the map's renders;
 --loop-closure closes loops against old keyframes with splatam_b200.loop's defaults and prints every closure attempt.
 --relocalise checks every tracked frame against the map and relocalises lost ones against the keyframes
-(splatam_b200.reloc's defaults) and prints every lost frame.  Prints one JSON line: ATE, PSNR, MS-SSIM, depth L1, initial and final
+(splatam_b200.reloc's defaults) and prints every lost frame; --relocalise-photometric does so with the photometric
+health check and RGB-D ICP verification.  Prints one JSON line: ATE, PSNR, MS-SSIM, depth L1, initial and final
 Gaussian counts, tracking
 and mapping wall times, and the load time per frame that the SLAM loop waited for (decode + upload not hidden by the
 prefetch).  --out DIR writes the reference's psnr.txt / rmse.txt / l1.txt / ssim.txt and its full params.npz record
@@ -138,14 +140,19 @@ def main():
     ap.add_argument("--mapping-cam-lrs", type=float, nargs=2, default=(0.0, 0.0), metavar=("ROT", "TRANS"),
                     help="mapping learning rates of cam_unnorm_rots and cam_trans; non-zero refines each mapping "
                          "iteration's keyframe pose (the reference's do_ba=True); default 0 0, as every shipped config")
-    ap.add_argument("--pose-init", default="constant_velocity", choices=("constant_velocity", "icp"),
-                    help="tracking start: the reference's constant-velocity guess, or that guess refined by ICP")
+    ap.add_argument("--pose-init", default="constant_velocity", choices=("constant_velocity", "icp", "rgbd_icp"),
+                    help="tracking start: the reference's constant-velocity guess, or that guess refined by ICP "
+                         "(rgbd_icp: depth and colour)")
     ap.add_argument("--loop-closure", action="store_true",
                     help="close loops against old keyframes (splatam_b200.loop, its DEFAULTS); off by default")
     ap.add_argument("--relocalise", action="store_true",
                     help="health-check every frame and relocalise lost ones (splatam_b200.reloc, its DEFAULTS); off by "
                          "default")
+    ap.add_argument("--relocalise-photometric", action="store_true",
+                    help="--relocalise with the photometric health check and RGB-D ICP verification (implies "
+                         "--relocalise)")
     a = ap.parse_args()
+    a.relocalise = a.relocalise or a.relocalise_photometric
     if (a.lpips_alexnet is None) != (a.lpips_lin is None):
         ap.error("--lpips-alexnet and --lpips-lin go together")
     if a.checkpoint_every < 0:
@@ -203,7 +210,9 @@ def main():
                         checkpoint_every=a.checkpoint_every or None, resume=ckpt,
                         tracking_lrs=h["tracking_lrs"], depth_loss_thres=h["depth_loss_thres"],
                         mapping_cam_lrs=tuple(a.mapping_cam_lrs), pose_init=a.pose_init,
-                        loop_closure={} if a.loop_closure else None, relocalise={} if a.relocalise else None)
+                        loop_closure={} if a.loop_closure else None,
+                        relocalise=((dict(photometric=True) if a.relocalise_photometric else {}) if a.relocalise
+                                    else None))
     torch.cuda.synchronize(dev)
     wall = time.perf_counter() - t0
     # --resume: wall time from reading the checkpoint to the first tracked frame (frame-0 read, load, keyframe rebuild)
@@ -237,7 +246,7 @@ def main():
         densify_height=seq.densify_height, densify_width=seq.densify_width, hyper=h,
         initial_gaussians=initial_gaussians, resumed_from=a.resume, resume_s=resume_s,
         mapping_cam_lrs=list(a.mapping_cam_lrs), pose_init=a.pose_init,
-        **({} if a.pose_init != "icp" else dict(pose_init_s=timing["pose_init_s"],
+        **({} if a.pose_init == "constant_velocity" else dict(pose_init_s=timing["pose_init_s"],
                                                 icp_accepted=sum(s["accepted"] for s in out["icp"]))),
         **({} if not a.loop_closure else dict(loop_closure_s=timing["loop_closure_s"], loops=out["loops"])),
         **({} if not a.relocalise else dict(health_s=timing["health_s"], reloc_s=timing["reloc_s"], reloc=out["reloc"],

@@ -4,6 +4,7 @@ power limit first:
 
 (a) icp.align's device time per frame at 1200x680 and 960x720 (CUDA events over `--launches` back-to-back calls,
     default iterations 10 / 5 / 4), and the depth/silhouette render of the map it needs (scenes.room, `--gaussians`);
+    then icp.align and icp.align_rgbd alternated three times;
 (b) tools/run_slam_dataset.py on a synthetic Replica-layout sequence (scenes.write_replica_sequence, `--frames`
     frames) at each `--strides` value, for constant velocity with 40 tracking iterations, ICP with 40 and ICP with 10:
     ATE, tracking and pose-initialisation wall time per frame and the accepted ICP poses.  One JSON line per run.
@@ -27,7 +28,7 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 import scenes  # noqa: E402
 from gpu_info import gpu_info  # noqa: E402
 
-RUNS = (("constant_velocity", 40), ("icp", 40), ("icp", 10))
+RUNS = (("constant_velocity", 40), ("icp", 40), ("icp", 10), ("rgbd_icp", 40))
 
 
 def _size(s):
@@ -69,9 +70,28 @@ def align_time(dev, w, h, gaussians, launches):
     truth = M.camera_w2c(rots[..., 1], trans[..., 1])[0]
     w2c, st = icp.align(ds0, data, K, eye, eye)
     err = (w2c @ torch.linalg.inv(truth)).double().cpu()
+    # sb_rgbd_icp_align against sb_icp_align, alternated three times on the same inputs
+    im0, _ = icp.model_render(params, 0, frame)
+    im1, _ = icp.model_render(params, 1, frame)
+    icp.align_rgbd(ds0, im0, data, im1, K, eye, eye)
+    geo, rgbd = [], []
+    for _ in range(3):
+        for fn, acc in ((lambda: icp.align(ds0, data, K, eye, eye), geo),
+                        (lambda: icp.align_rgbd(ds0, im0, data, im1, K, eye, eye), rgbd)):
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            for _ in range(launches):
+                fn()
+            b.record()
+            torch.cuda.synchronize(dev)
+            acc.append(round(a.elapsed_time(b) / launches, 4))
+    w2c_r, st_r = icp.align_rgbd(ds0, im0, data, im1, K, eye, eye)
+    err_r = (w2c_r @ torch.linalg.inv(truth)).double().cpu()
     return dict(render_ms=e0.elapsed_time(e1) / launches, align_ms=e1.elapsed_time(e2) / launches,
                 stats=icp.read_stats(st), trans_err_mm=1e3 * float(err[:3, 3].abs().max()),
-                rot_err_deg=math.degrees(math.acos(max(-1.0, min(1.0, (float(err[:3, :3].trace()) - 1) / 2)))))
+                rot_err_deg=math.degrees(math.acos(max(-1.0, min(1.0, (float(err[:3, :3].trace()) - 1) / 2)))),
+                alternated_align_ms=geo, alternated_rgbd_align_ms=rgbd, rgbd_stats=icp.read_stats(st_r),
+                rgbd_trans_err_mm=1e3 * float(err_r[:3, 3].abs().max()))
 
 
 def main():

@@ -4,7 +4,8 @@
   score_us[N]            sb_reloc_score of one 85x48 query against N = 400, 2000, 10000 entries, with the byte bound
                          (N * 2 * 85 * 48 * 4 bytes read once, at 3.35 TB/s) and its share
   topk_us                sb_reloc_topk, k = 5 of 10000
-  health_ms              sb_track_health at 1200x680 (kernel only), and health_frame_ms: the depth/silhouette render of
+  health_ms              sb_track_health at 1200x680 (kernel only); health_alternated_ms: it and sb_track_health_rgb
+                         alternated three times; health_frame_ms: the depth/silhouette render of
                          the loop room at 320x192 plus the check and its host read, as run_slam pays per frame
   relocalise_ms          one reloc.relocalise call in the loop room at k = 5 (40 tracking iterations)
   slam_ms_per_frame      run_slam on scenes.write_replica_sequence (12 frames), relocalise=None and {} alternated twice
@@ -62,6 +63,12 @@ def main():
     ds = torch.stack([d[0], torch.ones_like(d[0])])
     cfg = reloc.config({})
     out["health_ms"] = _events(lambda: reloc._health_of(ds, d[0], cfg), 50)
+    cfg_rgb = reloc.config(dict(photometric=True))
+    hm, hr = [], []
+    for _ in range(3):                              # alternated: depth-only and photometric health
+        hm.append(_events(lambda: reloc._health_of(ds, d[0], cfg), 50))
+        hr.append(_events(lambda: reloc._health_rgb_of(ds, im[0], d[0], im[1], cfg_rgb), 50))
+    out["health_alternated_ms"] = dict(depth=[round(x, 4) for x in hm], rgb=[round(x, 4) for x in hr])
 
     sc = scenes.loop_room()
     cam = sc.settings(SB.GaussianRasterizationSettings, dev)
