@@ -704,6 +704,25 @@ SB_API int sb_track_health_rgb(int height, int width, const float* depth_sil, co
                                double min_coverage, double min_inliers, double min_ncc, double* scratch, double* stats,
                                void* stream);
 
+/* ---- per-frame exposure and white balance (splatam_b200/train_ops.py `exposure`, csrc/exposure.cu) --------------
+ * A frame's colour correction is ab float32 [6] (device) = (a_r, a_g, a_b, b_r, b_g, b_b): log-gains and biases.
+ * Images are float32 [3,H,W] (device), channel c the values c*H*W .. (c+1)*H*W - 1; no alignment is assumed.
+ * Every call reads ab from device memory (a graph replay picks up new values) and never synchronises the host.
+ * sb_exposure_apply: g_c = float(exp(double(a_c))), or float(exp(-double(a_c))) when `inverse`;
+ *   y = __fadd_rn(__fmul_rn(g_c, x), b_c), or when `inverse` y = __fmul_rn(__fsub_rn(x, b_c), g_c).  y may be x.
+ * sb_exposure_backward: the gradient of the forward transform for an upstream gy [3,H,W]: gx = __fmul_rn(g_c, gy)
+ *   (float32 [3,H,W], may be gy) and g_ab double [6] = (exp(double(a_c)) S_c, G_c) with S_c = sum over channel c of
+ *   double(gy) double(x) and G_c = sum of double(gy): each sum over SB_EXPOSURE_BLOCKS fixed partials added in block
+ *   order, no atomics, so a call gives the same bits every time.  workspace: sb_exposure_workspace_bytes.
+ * SB_ERR_BAD_ARG, before any launch, for sizes < 1, null pointers and `inverse` outside {0, 1}; SB_ERR_WORKSPACE for
+ * a short workspace. */
+#define SB_EXPOSURE_BLOCKS 264
+SB_API int sb_exposure_workspace_bytes(int height, int width, size_t* bytes);
+SB_API int sb_exposure_apply(int height, int width, const float* x, const float* ab, int inverse, float* y,
+                             void* stream);
+SB_API int sb_exposure_backward(int height, int width, const float* x, const float* ab, const float* gy, float* gx,
+                                double* g_ab, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- per-stage device timing (measurement only; bench.py's roofline pass) -------------------
  * Between sb_profile_begin() and sb_profile_end() every stage launch of this process is bracketed
  * by CUDA events on its stream.  sb_profile_end synchronises, writes the summed milliseconds and call

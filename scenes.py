@@ -524,11 +524,39 @@ def adversarial(small=False):
     return d
 
 
-def write_replica_sequence(dst, num_frames, device, seed=14, cam=REPLICA, png_depth_scale=6553.5, quality=95):
+def _exposed_u8(im, exposure, t):
+    """Frame t's colour as uint8 HWC: clip(exp(a) im + b, 0, 1) with row t of the [T,6] `exposure` table (log-gains,
+    biases) when given, then the quantisation every writer uses."""
+    if exposure is not None:
+        row = torch.as_tensor(np.asarray(exposure, dtype=np.float32)[t]).to(im.device)
+        im = torch.exp(row[:3, None, None]) * im + row[3:, None, None]
+    return (im.clamp(0, 1) * 255).round().to(torch.uint8).permute(1, 2, 0).cpu().numpy()
+
+
+def exposure_profile(num_frames, gain=0.3, bias=0.04, period=12.0):
+    """A [T,6] float32 table of per-frame colour changes (log-gains a_r, a_g, a_b, biases b_r, b_g, b_b) as
+    auto-exposure and white balance make them: a common log-gain that swings between 0 and -`gain` with a period of
+    `period` frames, red and blue log-gains that drift a further 0 to -gain/2 at other rates (white balance), and
+    biases up to `bias`.  Every log-gain is <= 0 and every bias lies in [0, 1 - exp(a_c)], so exp(a) x + b maps [0, 1]
+    into itself: the profile clips no colour value of [0, 1].  Frame 0 is the identity, so the estimates relative to
+    frame 0 are the table itself."""
+    w = 2 * np.pi * np.arange(num_frames, dtype=np.float64) / period
+    common = -gain * (1 - np.cos(w)) / 2
+    a = np.stack([common - 0.25 * gain * (1 - np.cos(0.7 * w)), common,
+                  common - 0.25 * gain * (1 - np.cos(1.3 * w))], 1)
+    b = np.minimum(bias * np.stack([(1 - np.cos(0.5 * w)) / 2, (1 - np.cos(0.9 * w)) / 4,
+                                    (1 - np.cos(1.1 * w)) / 2], 1), 1 - np.exp(a))
+    return (np.concatenate([a, b], 1) + 0.0).astype(np.float32)         # + 0.0: frame 0 holds +0, not -0
+
+
+def write_replica_sequence(dst, num_frames, device, seed=14, cam=REPLICA, png_depth_scale=6553.5, quality=95,
+                           exposure=None):
     """Writes a sequence in Replica's on-disk layout (results/frame<t>.jpg, results/depth<t>.png, traj.txt of c2w
     rows) under `dst`: the frames are rendered on `device` from a view-filling surface (`view_filling`) along
     `slam.look_trajectory`, colour as JPEG and depth as a 16-bit PNG at `png_depth_scale`, depth as a sensor reports it
-    (alpha-normalised, 0 where the silhouette is below 0.9).  Returns the ground-truth w2c matrices [T,4,4] (CPU)."""
+    (alpha-normalised, 0 where the silhouette is below 0.9).  `exposure`: None, or a [T,6] table (`exposure_profile`)
+    applied to frame t's colour as clip(exp(a) im + b, 0, 1) before quantisation.  Returns the ground-truth w2c
+    matrices [T,4,4] (CPU)."""
     import os
     from PIL import Image
     import splatam_b200 as S
@@ -544,7 +572,7 @@ def write_replica_sequence(dst, num_frames, device, seed=14, cam=REPLICA, png_de
     for t in range(num_frames):
         f = slam.render_frame(gt, rots, trans, t, rs)
         depth = torch.where(f["sil"] > 0.9, f["depth"] / f["sil"].clamp(min=1e-6), torch.zeros_like(f["depth"]))
-        rgb = (f["im"].clamp(0, 1) * 255).round().to(torch.uint8).permute(1, 2, 0).cpu().numpy()
+        rgb = _exposed_u8(f["im"], exposure, t)
         raw = (depth[0] * png_depth_scale).round().clamp(0, 65535).cpu().numpy().astype(np.uint16)
         Image.fromarray(rgb).save(os.path.join(dst, "results", "frame%06d.jpg" % t), quality=quality)
         Image.fromarray(raw).save(os.path.join(dst, "results", "depth%06d.png" % t))
@@ -603,15 +631,18 @@ def loop_trajectory(num_frames, device, radius=0.3, yaw=25.0):
     return rots, trans
 
 
-def write_loop_sequence(dst, num_frames, device, seed=21, cam=LOOP_CAM, png_depth_scale=6553.5, quality=95):
+def write_loop_sequence(dst, num_frames, device, seed=21, cam=LOOP_CAM, png_depth_scale=6553.5, quality=95,
+                        exposure=None):
     """Writes a sequence in Replica's on-disk layout (results/frame<t>.jpg, results/depth<t>.png, traj.txt of c2w rows)
     under `dst`, as write_replica_sequence does: the frames are rendered on `device` from `loop_room` along
     `loop_trajectory`, a camera inside a densely walled room that comes back to where it started.  Depth is
-    alpha-normalised, 0 where the silhouette is below 0.9.  Returns the ground-truth w2c matrices [T,4,4] (CPU)."""
-    return _write_room_sequence(dst, loop_trajectory(num_frames, device), device, seed, cam, png_depth_scale, quality)
+    alpha-normalised, 0 where the silhouette is below 0.9.  `exposure`: as for write_replica_sequence.  Returns the
+    ground-truth w2c matrices [T,4,4] (CPU)."""
+    return _write_room_sequence(dst, loop_trajectory(num_frames, device), device, seed, cam, png_depth_scale, quality,
+                                exposure)
 
 
-def _write_room_sequence(dst, traj, device, seed, cam, png_depth_scale, quality):
+def _write_room_sequence(dst, traj, device, seed, cam, png_depth_scale, quality, exposure=None):
     import os
     from PIL import Image
     import splatam_b200 as S
@@ -626,7 +657,7 @@ def _write_room_sequence(dst, traj, device, seed, cam, png_depth_scale, quality)
     for t in range(num_frames):
         f = slam.render_frame(gt, rots, trans, t, rs)
         depth = torch.where(f["sil"] > 0.9, f["depth"] / f["sil"].clamp(min=1e-6), torch.zeros_like(f["depth"]))
-        rgb = (f["im"].clamp(0, 1) * 255).round().to(torch.uint8).permute(1, 2, 0).cpu().numpy()
+        rgb = _exposed_u8(f["im"], exposure, t)
         raw = (depth[0] * png_depth_scale).round().clamp(0, 65535).cpu().numpy().astype(np.uint16)
         Image.fromarray(rgb).save(os.path.join(dst, "results", "frame%06d.jpg" % t), quality=quality)
         Image.fromarray(raw).save(os.path.join(dst, "results", "depth%06d.png" % t))

@@ -129,6 +129,9 @@ _SIGNATURES = {
     "sb_track_health": (_i, [_i, _i, _vp, _vp, _f, _f, ctypes.c_double, ctypes.c_double, _vp, _vp, _vp]),
     "sb_track_health_rgb": (_i, [_i, _i, _vp, _vp, _vp, _vp, _f, _f, ctypes.c_double, ctypes.c_double, ctypes.c_double,
                                  _vp, _vp, _vp]),
+    "sb_exposure_workspace_bytes": (_i, [_i, _i, ctypes.POINTER(_sz)]),
+    "sb_exposure_apply": (_i, [_i, _i, _vp, _vp, _i, _vp, _vp]),
+    "sb_exposure_backward": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "sb_profile_begin": (_i, []),
     "sb_profile_end": (_i, [ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_int)]),
     "sb_stage_name": (ctypes.c_char_p, [_i]),

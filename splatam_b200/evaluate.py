@@ -400,6 +400,8 @@ def evaluate(params, frames, cam, sil_thres, mapping_iters, add_new_gaussians, e
     fused / render: as for mapping (`mapping._render_pair`); fused defaults to the fast path on CUDA.
     at_gt_pose: render every frame at its `gt_w2c` instead of its estimated pose, as the offline drivers' `eval` does
     (R/utils/gs_helpers.py:463-510); `params` then needs no camera tensors.
+    When `params` holds `cam_exposure` [1,6,T] (a run with exposure, formats.load_exposure), every frame's RGB render
+    is corrected by its column (`mapping.frame_exposure`) before it is scored, saved or given to LPIPS.
     save_frames: also writes, for each evaluated frame t (its position in `frames`), the reference's four PNGs
     (`eval_frames_u8` of the unmasked renders): out_dir/rendered_rgb/gs_{t:04d}.png, rendered_depth/gs_{t:04d}.png,
     rgb/gt_{t:04d}.png and depth/gt_{t:04d}.png.  Needs `out_dir` (ValueError otherwise); returns once every file is
@@ -455,6 +457,8 @@ def evaluate_nvs(params, frames, cam, sil_thres, mapping_iters, add_new_gaussian
     use_presence = int(mapping_iters == 0 and not add_new_gaussians)
     writer = _FrameWriter(out_dir, "splatam", -1, H, W, params["means3D"].device) if save_frames else None
     try:
+        # held-out views have no exposure estimate: they are scored in the map's (frame 0's) appearance
+        params = {k: v for k, v in params.items() if k != "cam_exposure"}
         metrics, presence = _score_frames(params, frames, ids, cam, sil_thres, use_presence, render, fused,
                                           at_gt_pose=True, count_holes=True, lpips=lpips, writer=writer)
     finally:

@@ -181,6 +181,35 @@ def save_run_record(out_dir, gauss, rots, trans, timestep, intrinsics, first_w2c
     return path
 
 
+def save_exposure(out_dir, cam_exposure):
+    """`<out_dir>/exposure.npz` with one key, `cam_exposure` float32 [1,6,T]: a run's per-frame colour corrections
+    (slam.run_slam's `exposure`).  Kept out of params.npz, whose readers take every key they do not know for a
+    per-Gaussian tensor or an optimised parameter.  Returns the path."""
+    a = np.ascontiguousarray(np.asarray(_host(cam_exposure), dtype=np.float32))
+    if a.ndim != 3 or a.shape[:2] != (1, 6):
+        raise ValueError("cam_exposure must be [1,6,T], got %s" % (a.shape,))
+    os.makedirs(out_dir, exist_ok=True)
+    path = os.path.join(out_dir, "exposure.npz")
+    np.savez(path, cam_exposure=a)
+    return path
+
+
+def load_exposure(path, num_frames=None, device=None):
+    """The `cam_exposure` [1,6,T] of an exposure.npz (`save_exposure`): numpy, or a float32 tensor on `device`.
+    ValueError when the key is missing, the shape is not [1,6,T] or T differs from `num_frames`."""
+    with np.load(path) as z:
+        if "cam_exposure" not in z.files:
+            raise ValueError("%s lacks cam_exposure" % path)
+        a = np.asarray(z["cam_exposure"], dtype=np.float32)
+    if a.ndim != 3 or a.shape[:2] != (1, 6) or (num_frames is not None and a.shape[2] != num_frames):
+        raise ValueError("%s: cam_exposure has shape %s, expected (1, 6, %s)"
+                         % (path, a.shape, "T" if num_frames is None else num_frames))
+    if device is None:
+        return a
+    import torch
+    return torch.from_numpy(np.ascontiguousarray(a)).to(device)
+
+
 def rgb_to_spherical_harmonic(rgb):
     return (rgb - 0.5) / C0
 

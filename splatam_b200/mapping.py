@@ -201,7 +201,8 @@ def _render_pair(params, frame, render, fused, camera_grad, max_rendered=None, g
     tracking does.  fused: one kernel builds both rendervars
     (csrc/prepare.cu), and the product rasterizer blends both colour sets in one pass (N1), with a fixed instance
     capacity if `max_rendered`; otherwise the PyTorch glue and two `render` calls.  Both render at frame["pose"]
-    (w2c, normalised quaternion) if given, else at the frame's pose in params."""
+    (w2c, normalised quaternion) if given, else at the frame's pose in params.  The RGB render is corrected by the
+    frame's exposure (`frame_exposure`) when it has one: train_ops.exposure when fused, its torch statement otherwise."""
     if fused:
         rv_rgb, rv_depth = fused_rendervars(params, frame["id"], frame["w2c"], camera_grad, pose=frame.get("pose"))
     else:
@@ -217,7 +218,21 @@ def _render_pair(params, frame, render, fused, camera_grad, max_rendered=None, g
     else:
         im, radius, _ = render(frame["cam"], **rv_rgb)
         depth_sil, _, _ = render(frame["cam"], **rv_depth)
+    ab = frame_exposure(params, frame)
+    if ab is not None:
+        from .train_ops import exposure, exposure_torch
+        im = exposure(im, ab) if fused else exposure_torch(im, ab)
     return im, depth_sil, radius, rv_rgb["means2D"]
+
+
+def frame_exposure(params, frame):
+    """The colour correction ab [6] (log-gains, biases; train_ops.exposure) of `frame`'s RGB render: frame["exposure"]
+    when given, else column frame["id"] of params["cam_exposure"] [1,6,T] when the params hold one, else None (no
+    correction)."""
+    ab = frame.get("exposure")
+    if ab is None and "cam_exposure" in params:
+        ab = params["cam_exposure"][0, :, frame["id"]]
+    return ab
 
 
 def mapping_loss(params, frame, render, loss_weights=(0.5, 1.0), ignore_outlier_depth_loss=False, fused_loss=False,
@@ -276,7 +291,7 @@ def tracking_loss(params, frame, render, sil_thres=0.99, loss_weights=(0.5, 1.0)
 
 
 def track_frame(params, frame, render=None, num_iters=40, lr_rot=0.0004, lr_trans=0.002, fused=None, graph=None,
-                depth_loss_thres=None):
+                depth_loss_thres=None, lr_exposure=None):
     """SplaTAM's tracking inner loop for one frame (R/scripts/splatam.py:676-744): Adam on the frame's camera
     quaternion and translation only, keeping the best-loss pose.  `params` holds detached Gaussian tensors and
     cam_unnorm_rots [1,4,T] / cam_trans [1,3,T] leaf tensors.  Returns the list of per-iteration losses.
@@ -285,7 +300,10 @@ def track_frame(params, frame, render=None, num_iters=40, lr_rot=0.0004, lr_tran
     with the same Adam state and best-pose record; the list then has 2 * num_iters entries.
     graph: the iteration -- loss forward + backward over the sync-free rasterizer, the Adam step and the best-pose
     bookkeeping, all on the device -- is captured once and replayed, so a frame costs one host synchronisation instead of
-    one per iteration (`_TrackingGraph`); None = re-use a cached graph, build one only for loops of >= 100 iterations."""
+    one per iteration (`_TrackingGraph`); None = re-use a cached graph, build one only for loops of >= 100 iterations.
+    lr_exposure: None, or (lr_log_gain, lr_bias): column t of params["cam_exposure"] [1,6,T] (the frame's colour
+    correction, `frame_exposure`) is optimised with the pose, its log-gains and biases as two more Adam groups of these
+    rates, and the best-loss record keeps it together with the pose."""
     render = default_render if render is None else render
     if fused is None:
         fused = params["means3D"].is_cuda and render is default_render
@@ -295,19 +313,25 @@ def track_frame(params, frame, render=None, num_iters=40, lr_rot=0.0004, lr_tran
         # per frame) or on request (graph=True: tracking-only runs over a map that stays put).  Building costs about as
         # much as ~40 eager iterations (capacity probe, warm-up, capture into a fresh memory pool).
         out = _track_frame_graphed(params, frame, num_iters, lr_rot, lr_trans, build=(graph is True or num_iters >= 100),
-                                   depth_loss_thres=depth_loss_thres)
+                                   depth_loss_thres=depth_loss_thres, lr_exposure=lr_exposure)
         if out is not None:
             return out              # None: no graph, or the instance capacity overflowed mid-frame -> run eagerly
     rots, trans = params["cam_unnorm_rots"], params["cam_trans"]
     rots.requires_grad_(True); trans.requires_grad_(True)
-    opt = torch.optim.Adam([{"params": [rots], "lr": lr_rot}, {"params": [trans], "lr": lr_trans}], lr=0.0, eps=1e-15)
+    groups = [{"params": [rots], "lr": lr_rot}, {"params": [trans], "lr": lr_trans}]
     t = frame["id"]
-    best, best_rot, best_tran, losses = None, None, None, []
+    if lr_exposure is not None:         # the column as two [1,3] leaves: log-gains and biases step at their own rates
+        col = params["cam_exposure"][..., t].detach()
+        gain, bias = col[:, :3].clone().requires_grad_(True), col[:, 3:].clone().requires_grad_(True)
+        groups += [{"params": [gain], "lr": lr_exposure[0]}, {"params": [bias], "lr": lr_exposure[1]}]
+    opt = torch.optim.Adam(groups, lr=0.0, eps=1e-15)
+    best, best_rot, best_tran, best_ab, losses = None, None, None, None, []
     keep = None if depth_loss_thres is None else {}
     total = num_iters
     while len(losses) < total:
         opt.zero_grad(set_to_none=True)
-        loss, _ = tracking_loss(params, frame, render, fused=fused, keep=keep)
+        fr = frame if lr_exposure is None else dict(frame, exposure=torch.cat([gain, bias], 1).reshape(6))
+        loss, _ = tracking_loss(params, fr, render, fused=fused, keep=keep)
         loss.backward()
         opt.step()
         with torch.no_grad():
@@ -316,12 +340,16 @@ def track_frame(params, frame, render=None, num_iters=40, lr_rot=0.0004, lr_tran
             lv = float(loss)
             if best is None or lv < best:
                 best, best_rot, best_tran = lv, rots[..., t].detach().clone(), trans[..., t].detach().clone()
+                if lr_exposure is not None:
+                    best_ab = torch.cat([gain, bias], 1).detach().clone()
         losses.append(lv)
         if keep is not None and len(losses) == num_iters and not float(keep["depth"].detach()) < depth_loss_thres:
             total = 2 * num_iters
     with torch.no_grad():
         rots[..., t] = best_rot
         trans[..., t] = best_tran
+        if lr_exposure is not None:
+            params["cam_exposure"][..., t] = best_ab
     return losses
 
 
@@ -383,9 +411,12 @@ class _TrackingGraph:
     With `depth_loss_thres` the graph records the depth L1 sum too and a frame replays 2 * num_iters iterations; the
     decision of track_frame's rule is taken on the device after iteration num_iters, and when the frame stops there
     the remaining replays run gated: they record no loss, update no best pose and raise no overflow.  The frame
-    still costs one host synchronisation; the gated replays cost GPU time."""
+    still costs one host synchronisation; the gated replays cost GPU time.
 
-    def __init__(self, params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres=None):
+    With `lr_exposure` the frame's colour correction travels the same way, as two [1,3] leaves (log-gains, biases)
+    with two more capturable Adam groups and a best-loss record of their own."""
+
+    def __init__(self, params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres=None, lr_exposure=None):
         t = frame["id"]
         rots, trans = params["cam_unnorm_rots"], params["cam_trans"]
         self.gp = gp = {k: params[k].detach() for k in GAUSSIAN_KEYS}        # keeps the storage the graph reads alive
@@ -398,8 +429,17 @@ class _TrackingGraph:
             self.tr = trans[..., t].detach().clone().requires_grad_(True)
             q, tr = self.q, self.tr
             q.grad, tr.grad = torch.zeros_like(q), torch.zeros_like(tr)
-            self.opt = torch.optim.Adam([{"params": [q], "lr": lr_rot}, {"params": [tr], "lr": lr_trans}], lr=0.0,
-                                        eps=1e-15, capturable=True)
+            leaves, groups = [q, tr], [{"params": [q], "lr": lr_rot}, {"params": [tr], "lr": lr_trans}]
+            self.expo = expo = lr_exposure is not None
+            if expo:
+                col = params["cam_exposure"][..., t].detach()
+                self.gain = col[:, :3].clone().requires_grad_(True)
+                self.bias = col[:, 3:].clone().requires_grad_(True)
+                self.gain.grad, self.bias.grad = torch.zeros_like(self.gain), torch.zeros_like(self.bias)
+                leaves += [self.gain, self.bias]
+                groups += [{"params": [self.gain], "lr": lr_exposure[0]}, {"params": [self.bias], "lr": lr_exposure[1]}]
+                self.best_ab = col.clone()
+            self.opt = torch.optim.Adam(groups, lr=0.0, eps=1e-15, capturable=True)
             self.best_loss = torch.full((), float("inf"), device=dev)
             self.best_q, self.best_tr = q.detach().clone(), tr.detach().clone()
             self.hist = torch.zeros(self.replays, device=dev)
@@ -408,15 +448,18 @@ class _TrackingGraph:
             self.live = torch.ones(1, dtype=torch.bool, device=dev)   # rule only: this replay is a real iteration
 
         def body():
-            q.grad.zero_(); tr.grad.zero_()
+            for leaf in leaves:
+                leaf.grad.zero_()
             keep = {} if rule else None
-            loss, _ = tracking_loss(gp, dict(step.frame, pose=camera_w2c(q, tr)), default_render, fused=True,
-                                    max_rendered=step.cap, keep=keep)
+            fr = dict(step.frame, pose=camera_w2c(q, tr))
+            if expo:
+                fr["exposure"] = torch.cat([self.gain, self.bias], 1).reshape(6)
+            loss, _ = tracking_loss(gp, fr, default_render, fused=True, max_rendered=step.cap, keep=keep)
             loss.backward()
             lossd = loss.detach().reshape(1)
             bad = (step.overflow() != 0) | ~torch.isfinite(lossd)
-            q.grad.copy_(torch.where(bad, torch.zeros_like(q.grad), q.grad))
-            tr.grad.copy_(torch.where(bad, torch.zeros_like(tr.grad), tr.grad))
+            for leaf in leaves:
+                leaf.grad.copy_(torch.where(bad, torch.zeros_like(leaf.grad), leaf.grad))
             self.bad_any.add_((bad & self.live).float() if rule else bad.float())
             self.opt.step()
             # the reference's rule (splatam.py:703-712): candidate = pose AFTER the step, ranked by the loss evaluated
@@ -427,6 +470,8 @@ class _TrackingGraph:
             self.best_loss.copy_(torch.where(better, lossd, self.best_loss.reshape(1)).reshape(()))
             self.best_q.copy_(torch.where(better, q.detach(), self.best_q))
             self.best_tr.copy_(torch.where(better, tr.detach(), self.best_tr))
+            if expo:
+                self.best_ab.copy_(torch.where(better, torch.cat([self.gain, self.bias], 1).detach(), self.best_ab))
             self.hist.scatter_(0, self.it, lossd)
             if rule:
                 # a gated replay overwrites slot `it` (the first unused one, num_iters) and does not advance `it`
@@ -445,6 +490,9 @@ class _TrackingGraph:
         with torch.no_grad():
             self.step.load(frame)
             self.q.copy_(params["cam_unnorm_rots"][..., t]); self.tr.copy_(params["cam_trans"][..., t])
+            if self.expo:
+                col = params["cam_exposure"][..., t]
+                self.gain.copy_(col[:, :3]); self.bias.copy_(col[:, 3:]); self.best_ab.copy_(col)
             for st in self.opt.state.values():
                 st["exp_avg"].zero_(); st["exp_avg_sq"].zero_(); st["step"].zero_()
             self.best_loss.fill_(float("inf")); self.best_q.copy_(self.q); self.best_tr.copy_(self.tr)
@@ -463,6 +511,8 @@ class _TrackingGraph:
         with torch.no_grad():
             params["cam_unnorm_rots"][..., frame["id"]] = self.best_q
             params["cam_trans"][..., frame["id"]] = self.best_tr
+            if self.expo:
+                params["cam_exposure"][..., frame["id"]] = self.best_ab
         hist = self.hist.tolist()
         return hist[:int(self.it)] if self.rule else hist
 
@@ -470,18 +520,21 @@ class _TrackingGraph:
 _TRACK_GRAPHS = {}
 
 
-def _tracking_key(params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres):
+def _tracking_key(params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres, lr_exposure=None):
     """What a captured tracking iteration is bound to: the storage (pointer and shape) of each Gaussian tensor it
-    reads, the camera, the image shape, the iteration count, the learning rates and the depth-loss rule."""
+    reads, the camera, the image shape, the iteration count, the learning rates (the exposure rates included) and the
+    depth-loss rule."""
     return (tuple((params[k].data_ptr(), tuple(params[k].shape)) for k in GAUSSIAN_KEYS), id(frame["cam"]),
-            tuple(frame["im"].shape), num_iters, lr_rot, lr_trans, depth_loss_thres)
+            tuple(frame["im"].shape), num_iters, lr_rot, lr_trans, depth_loss_thres,
+            None if lr_exposure is None else tuple(float(r) for r in lr_exposure))
 
 
-def _track_frame_graphed(params, frame, num_iters, lr_rot, lr_trans, build=True, depth_loss_thres=None):
+def _track_frame_graphed(params, frame, num_iters, lr_rot, lr_trans, build=True, depth_loss_thres=None,
+                         lr_exposure=None):
     """Graph-replayed tracking of one frame, or None when no graph is available / an iteration overflowed the instance
     capacity (the caller then runs the frame eagerly).  Graphs are cached per `_tracking_key`; `build` creates one on
     a miss (worth it for long loops or when the map stays put)."""
-    key = _tracking_key(params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres)
+    key = _tracking_key(params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres, lr_exposure)
     tg = _TRACK_GRAPHS.get(key)
     if tg is None:
         if not build:
@@ -489,7 +542,7 @@ def _track_frame_graphed(params, frame, num_iters, lr_rot, lr_trans, build=True,
         if len(_TRACK_GRAPHS) >= 2:
             _TRACK_GRAPHS.clear()
         tg = _TRACK_GRAPHS[key] = _TrackingGraph(params, frame, num_iters, lr_rot, lr_trans,
-                                                 depth_loss_thres=depth_loss_thres)
+                                                 depth_loss_thres=depth_loss_thres, lr_exposure=lr_exposure)
     return tg.run(params, frame)
 
 
@@ -557,13 +610,17 @@ class ShardedMapper:
     the next step.  Each step's render gives gradient to the Gaussians and to its keyframe's pose; the [7, T] pose
     gradient (zero outside the keyframe's column) travels in the all-reduce bucket, and an Adam over the whole two
     tensors (torch.optim.Adam on the torch path, FusedAdam on the fused one) steps them on every step.  Its moments
-    reset with `reset_optimizer` and survive map edits.  At zero camera rates nothing of this exists."""
+    reset with `reset_optimizer` and survive map edits.  At zero camera rates nothing of this exists.
+
+    `cam` may also hold `cam_exposure` [1,6,T], each frame's colour correction (train_ops.exposure): every step's RGB
+    render is corrected by its keyframe's column (which mapping does not step), and `add_new_gaussians` takes the
+    frame's colours mapped back to frame 0's appearance.  Without it nothing of this runs."""
 
     DEFAULT_LRS = dict(means3D=0.0001, rgb_colors=0.0025, unnorm_rotations=0.001, logit_opacities=0.05,
                        log_scales=0.001)
 
     def __init__(self, gaussians, cam_unnorm_rots, cam_trans, lrs=None, render=default_render, group=None, seed=0,
-                 fused=None, track_means2D=False, timestep=None):
+                 fused=None, track_means2D=False, timestep=None, cam_exposure=None):
         """track_means2D: keep d loss / d means2D of every eager step's RGB render and which Gaussians it saw (the
         statistic of `densify`).  timestep: the frame that created each Gaussian ([P], e.g. from a checkpoint); default
         zeros, as the reference starts its initial map (R/scripts/splatam.py:155)."""
@@ -587,6 +644,8 @@ class ShardedMapper:
             if self.timestep.shape[0] != P:
                 raise ValueError("timestep has %d entries for a map of %d Gaussians" % (self.timestep.shape[0], P))
         self.cam = dict(cam_unnorm_rots=cam_unnorm_rots.detach(), cam_trans=cam_trans.detach())
+        if cam_exposure is not None:
+            self.cam["cam_exposure"] = cam_exposure.detach()
         # fused = hand-written Adam over the flat buffer + fused L1/SSIM loss (CUDA only); the torch path is
         # the reference formulation (R/scripts/splatam.py:160-166) and the one the CPU/gloo test exercises
         self.fused = self.g.flat.is_cuda if fused is None else bool(fused)
@@ -618,7 +677,7 @@ class ShardedMapper:
         """Tracking runs on one rank (its backward uses float atomics, so two ranks would not end bit-identical);
         the estimated poses are broadcast so every replica maps with the same cameras."""
         if self.dist and self.world > 1:
-            for k in ("cam_unnorm_rots", "cam_trans"):
+            for k in [k for k in CAM_KEYS + ("cam_exposure",) if k in self.cam]:
                 t = self.cam[k].detach().clone().contiguous()
                 self.dist.broadcast(t, src=src, group=self.group)
                 self.cam[k] = t
@@ -676,7 +735,7 @@ class ShardedMapper:
         with torch.no_grad():
             self._cam_flat[:4 * T].copy_(self.cam["cam_unnorm_rots"].reshape(-1))
             self._cam_flat[4 * T:].copy_(self.cam["cam_trans"].reshape(-1))
-        self.cam = dict(self._cam_views)
+        self.cam = dict(self.cam, **self._cam_views)
 
     def _make_cam_optimizer(self):
         """Fresh Adam over the two whole camera tensors (initialize_optimizer(tracking=False), R/scripts/splatam.py:
@@ -844,6 +903,9 @@ class ShardedMapper:
             tg = transform_to_frame(p, time_idx, gaussians_grad=False, camera_grad=False)
             depth_sil, _, _ = self.render(frame["cam"], **depth_sil_rendervar(p, frame["w2c"], tg))
             curr_w2c, _ = pose_matrices(p, time_idx)
+            if "cam_exposure" in p:         # the new Gaussians take the frame's colour in frame 0's appearance
+                from .train_ops import exposure
+                frame = dict(frame, im=exposure(frame["im"], p["cam_exposure"][0, :, time_idx], inverse=True))
         new, n = map_ops.new_gaussians_from_frame(depth_sil, frame, intrinsics, curr_w2c, sil_thres,
                                                   scale_dim=self._widths()[4])
         if n:
@@ -870,6 +932,8 @@ class ShardedMapper:
             self._bind_cameras()
         step = _CapturedStep(self.params(), window[0], probe, slack, capacity)
         step.frame["pose"] = tuple(t.clone() for t in fused_pose_cached(self.params(), window[0]["id"]))
+        if "cam_exposure" in self.cam:        # static [6]: `step` loads the keyframe's column as it loads its pose
+            step.frame["exposure"] = self.cam["cam_exposure"][0, :, window[0]["id"]].detach().clone()
         self._slack = slack
         self._polls = []                 # (event, pinned copy of the overflow slot) of steps in flight
         self._pin = [torch.empty(1, dtype=torch.float32, pin_memory=True) for _ in range(8)]
@@ -1092,6 +1156,8 @@ class ShardedMapper:
             else:
                 for static, v in zip(step.frame["pose"], fused_pose_cached(self.params(), frame["id"])):
                     static.copy_(v, non_blocking=True)
+            if "exposure" in step.frame:
+                step.frame["exposure"].copy_(self.cam["cam_exposure"][0, :, frame["id"]], non_blocking=True)
             step.graph.replay()
         else:
             self.g.zero_grad()

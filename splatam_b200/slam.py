@@ -83,6 +83,23 @@ def keyframes_from_checkpoint(frames, ckpt):
     return [dict(_without_densify(frames[k]), est_w2c=_curr_w2c(rots, trans, k)) for k in ids]
 
 
+EXPOSURE_DEFAULTS = dict(lr_log_gain=0.01, lr_bias=0.002)
+
+
+def exposure_config(exposure):
+    """run_slam's `exposure` dict with EXPOSURE_DEFAULTS filled in; ValueError for unknown keys or bad rates."""
+    if not isinstance(exposure, dict):
+        raise ValueError("exposure must be None or a dict of %s, got %r" % (sorted(EXPOSURE_DEFAULTS), exposure))
+    unknown = sorted(set(exposure) - set(EXPOSURE_DEFAULTS))
+    if unknown:
+        raise ValueError("unknown exposure keys %s (known: %s)" % (unknown, sorted(EXPOSURE_DEFAULTS)))
+    cfg = dict(EXPOSURE_DEFAULTS, **exposure)
+    for k, v in cfg.items():
+        if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v) or v < 0:
+            raise ValueError("exposure %s must be a finite rate >= 0, got %r" % (k, v))
+    return {k: float(v) for k, v in cfg.items()}
+
+
 def _run_state(mapper, counts, keyframes=None, pose_graph=None, reloc_frames=None):
     """The sidecar of a checkpoint (formats.save_checkpoint's `run_state`): what continues a run exactly and the
     reference's params{t}.npz cannot carry -- the mapper's own state (ShardedMapper.run_state: the Gaussians'
@@ -91,7 +108,8 @@ def _run_state(mapper, counts, keyframes=None, pose_graph=None, reloc_frames=Non
     (keyframe_selection_overlap's permutation) and the Gaussian counts so far; with `keyframes` (runs with keyframe-pose
     refinement) also their stored est_w2c, which the refined camera columns no longer give; with `pose_graph` (runs
     with loop closure) also its edges and their measurements (loop.PoseGraph.state); with `reloc_frames` (runs with
-    relocalisation: (lost ids, relocalised ids)) `reloc_lost` and `reloc_relocalised`.  Numeric arrays only."""
+    relocalisation: (lost ids, relocalised ids)) `reloc_lost` and `reloc_relocalised`; with a `cam_exposure` in the
+    mapper's cameras (runs with exposure) also that table [1,6,T].  Numeric arrays only."""
     dev = mapper.g.flat.device
     _, keys, pos, has_gauss, cached = np.random.get_state()
     st = dict(mapper.run_state(), torch_rng=torch.get_rng_state().numpy(),
@@ -107,6 +125,8 @@ def _run_state(mapper, counts, keyframes=None, pose_graph=None, reloc_frames=Non
     if reloc_frames is not None:
         st["reloc_lost"] = np.array(sorted(reloc_frames[0]), dtype=np.int64)
         st["reloc_relocalised"] = np.array(sorted(reloc_frames[1]), dtype=np.int64)
+    if "cam_exposure" in mapper.cam:
+        st["cam_exposure"] = mapper.cam["cam_exposure"].detach().float().cpu().numpy()
     return st
 
 
@@ -148,7 +168,7 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
              scene_radius=None, select_keyframes=False, checkpoint_dir=None, first_frame_iters=0, map_every=None,
              graph=False, timing=None, densify_dict=None, tracking_lrs=(0.0004, 0.002), depth_loss_thres=None,
              checkpoint_every=None, resume=None, mapping_cam_lrs=(0.0, 0.0), pose_init="constant_velocity",
-             loop_closure=None, relocalise=None):
+             loop_closure=None, relocalise=None, exposure=None):
     """Tracks every frame and maps on keyframes.  gauss_init: dict of the five Gaussian tensors (the map's
     starting point); frames: list of dict(id, cam, w2c, im, depth).  Returns dict(rots, trans, psnr, gauss, counts,
     timestep, keyframe_time_indices, keyframe_est_w2c): `timestep` is the frame that created each Gaussian of the final
@@ -206,6 +226,15 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     `reloc_lost` (the ids of frames that stayed lost) and `reloc_database`.  Checkpoints also hold the lost and
     relocalised ids; on resume the database is rebuilt from the restored keyframes.  `relocalise` itself is not
     stored: a resumed run passes it again.
+    `exposure`: None (the default: off, and nothing of it runs) or a dict of EXPOSURE_DEFAULTS keys (the tracking rates
+    lr_log_gain, lr_bias).  Each frame t gets a colour correction, column t of a [1,6,T] table (log-gains a_r, a_g,
+    a_b, biases b_r, b_g, b_b): its renders are compared with it through exp(a) * render + b (train_ops.exposure).
+    Frame 0 keeps the identity, so the map holds frame 0's appearance; frame t starts from column t - 1 and tracking
+    optimises it with the pose (track_frame's lr_exposure); mapping applies each keyframe's column without stepping
+    it; new Gaussians take the frame's colour mapped back, (c - b) exp(-a); `pose_init="rgbd_icp"` corrects the map's
+    RGB render by column t - 1; the final PSNR is of the corrected renders.  The result holds `exposure` [1,6,T] and
+    checkpoints hold the table in their sidecar (not in params{t}.npz); resuming with `exposure` from a checkpoint
+    without it raises ValueError, and so does `exposure` together with `relocalise`.
 
     Checkpoints and resume (R/scripts/splatam.py:604-643,927-931).  With `checkpoint_dir` and `checkpoint_every` = N,
     after frame t's mapping and keyframe step, for every t % N == 0 (frame 0 included, after `first_frame_iters`),
@@ -231,6 +260,15 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     _check_resume(gauss_init, resume, T, checkpoint_every, checkpoint_dir)
     if pose_init not in ("constant_velocity", "icp", "rgbd_icp"):
         raise ValueError("pose_init must be 'constant_velocity', 'icp' or 'rgbd_icp', got %r" % (pose_init,))
+    use_expo = exposure is not None
+    if use_expo:
+        expo_cfg = exposure_config(exposure)
+        if relocalise is not None:
+            raise ValueError("exposure and relocalise cannot be combined: relocalisation's candidate tracking does not "
+                             "estimate exposure")
+        if resume is not None and (resume["state"] is None or "cam_exposure" not in resume["state"]):
+            raise ValueError("exposure: the checkpoint holds no exposure table (it was written by a run without it)")
+        lr_expo = (expo_cfg["lr_log_gain"], expo_cfg["lr_bias"])
     use_icp = pose_init != "constant_velocity"
     if use_icp:
         if intrinsics is None:
@@ -269,6 +307,8 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
         dev = gauss_init["means3D"].device
         rots = torch.zeros(1, 4, T, device=dev); rots[:, 0] = 1.0
         trans = torch.zeros(1, 3, T, device=dev)
+        if use_expo:
+            kw["cam_exposure"] = torch.zeros(1, 6, T, device=dev)
         mapper = M.ShardedMapper(gauss_init, rots, trans, seed=seed, fused=fused, track_means2D=track_m2d, **kw)
         keyframes = [dict(_without_densify(frames[0]), est_w2c=torch.eye(4, device=dev))]
         counts = [mapper.g.shapes["means3D"][0]]
@@ -277,6 +317,11 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
         dev = resume["gauss"]["means3D"].device
         rots = resume["cam_unnorm_rots"].detach().clone().to(dev)
         trans = resume["cam_trans"].detach().clone().to(dev)
+        if use_expo:
+            kw["cam_exposure"] = torch.from_numpy(np.array(resume["state"]["cam_exposure"], dtype=np.float32)).to(dev)
+            if tuple(kw["cam_exposure"].shape) != (1, 6, T):
+                raise ValueError("the checkpoint's exposure table has shape %s, expected (1, 6, %d)"
+                                 % (tuple(kw["cam_exposure"].shape), T))
         mapper = M.ShardedMapper(resume["gauss"], rots, trans, seed=seed, fused=fused, track_means2D=track_m2d, **kw)
         keyframes = keyframes_from_checkpoint(frames, dict(resume, cam_unnorm_rots=rots, cam_trans=trans))
         if resume["state"] is not None:
@@ -335,6 +380,11 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
                 rots[0, :, t] = rots[0, :, t - 1]
                 trans[0, :, t] = trans[0, :, t - 1]
         params = dict({k: v.detach() for k, v in mapper.g.params.items()}, cam_unnorm_rots=rots, cam_trans=trans)
+        if use_expo:
+            expo = mapper.cam["cam_exposure"]
+            with torch.no_grad():
+                expo[..., t] = expo[..., t - 1]               # zero velocity
+            params["cam_exposure"] = expo
         torch.cuda.synchronize(dev) if dev.type == "cuda" else None
         if use_icp:
             t0 = time.perf_counter()
@@ -344,12 +394,13 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
             timing["pose_init_s"] += time.perf_counter() - t0
         t0 = time.perf_counter()
         losses = M.track_frame(params, frames[t], render=render, num_iters=tracking_iters, lr_rot=tracking_lrs[0],
-                               lr_trans=tracking_lrs[1], fused=fused, depth_loss_thres=depth_loss_thres)
+                               lr_trans=tracking_lrs[1], fused=fused, depth_loss_thres=depth_loss_thres,
+                               lr_exposure=lr_expo if use_expo else None)
         torch.cuda.synchronize(dev) if dev.type == "cuda" else None
         timing["tracking_s"] += time.perf_counter() - t0
         timing["tracking_iters"] += len(losses)
         rots, trans = params["cam_unnorm_rots"].detach(), params["cam_trans"].detach()
-        mapper.cam = dict(cam_unnorm_rots=rots, cam_trans=trans)
+        mapper.cam = dict(mapper.cam, cam_unnorm_rots=rots, cam_trans=trans)
         cam_now = mapper.sync_camera()            # multi-rank runs: rank 0's tracking result is the pose of record
         rots, trans = cam_now["cam_unnorm_rots"], cam_now["cam_trans"]
         frame = frames[t]
@@ -446,6 +497,10 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     vals = []
     for fr in keyframes:
         est = render_frame(final, rots, trans, fr["id"], cam, render)
+        if use_expo:
+            from .train_ops import exposure as _exposure, exposure_torch
+            ab = mapper.cam["cam_exposure"][0, :, fr["id"]]
+            est["im"] = _exposure(est["im"], ab) if mapper.fused else exposure_torch(est["im"], ab)
         vals.append(psnr(est["im"].clamp(0, 1), fr["im"].clamp(0, 1)))
     if checkpoint_dir is not None and (checkpoint_every is None or mapper.rank == 0):
         from . import formats
@@ -453,6 +508,8 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     out = dict(rots=rots, trans=trans, psnr=sum(vals) / len(vals), gauss=final, counts=counts,
                timestep=mapper.timestep.detach().clone(), keyframe_time_indices=[int(kf["id"]) for kf in keyframes],
                keyframe_est_w2c=[kf["est_w2c"] for kf in keyframes])
+    if use_expo:
+        out["exposure"] = mapper.cam["cam_exposure"].detach().clone()
     if use_icp:
         st = torch.stack(icp_stats).cpu().numpy() if icp_stats else np.zeros((0, icp.STATS))
         out["icp"] = [dict(frame=start + i, accepted=bool(s[0]), inlier_frac=float(s[1]), rms=float(s[2]),

@@ -136,3 +136,46 @@ def masked_l1(depth_sil, gt_depth, im=None, gt_im=None, sil_thres=0.99, use_sil=
     channel of the [3,H,W] depth/silhouette/depth^2 render and, if `im` is given, over the RGB image (sum)."""
     _lib.need_cuda("masked_l1", depth_sil)
     return _MaskedL1.apply(depth_sil, gt_depth, im, gt_im, sil_thres, use_sil, depth_mean)
+
+
+class _Exposure(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, im, ab):
+        im, ab = im.contiguous().float(), ab.contiguous().float().reshape(6)
+        _, H, W = im.shape
+        y = torch.empty_like(im)
+        _lib.call("sb_exposure_apply", H, W, im, ab, 0, y, device=im.device)
+        ctx.save_for_backward(im, ab)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        im, ab = ctx.saved_tensors
+        _, H, W = im.shape
+        gx = torch.empty_like(im)
+        g_ab = torch.empty(6, dtype=torch.float64, device=im.device)
+        ws = torch.empty(_lib.nbytes("sb_exposure_workspace_bytes", H, W), dtype=torch.uint8, device=im.device)
+        _lib.call("sb_exposure_backward", H, W, im, ab, gy.contiguous().float(), gx, g_ab, ws, ws.numel(),
+                  device=im.device)
+        return gx, g_ab.float()
+
+
+def exposure_torch(im, ab, inverse=False):
+    """The torch statement of `exposure`: exp(a) * im + b per channel, or (im - b) * exp(-a) when `inverse`."""
+    a, b = ab.reshape(6)[:3, None, None], ab.reshape(6)[3:, None, None]
+    return (im - b) * torch.exp(-a) if inverse else torch.exp(a) * im + b
+
+
+def exposure(im, ab, inverse=False):
+    """A frame's affine colour correction of an image [3,H,W] by ab [6] = (log-gains a_r, a_g, a_b, biases b_r, b_g,
+    b_b): exp(a_c) * im_c + b_c, differentiable in both (csrc/exposure.cu: one pass forward, one pass plus a
+    deterministic reduction backward), or with `inverse` (no gradient) (im_c - b_c) * exp(-a_c), which maps a frame's
+    colours back to the map's appearance.  `exposure_torch` is the same rule in torch operations."""
+    _lib.need_cuda("exposure", im, ab)
+    if not inverse:
+        return _Exposure.apply(im, ab)
+    im = im.contiguous().float()
+    y = torch.empty_like(im)
+    _lib.call("sb_exposure_apply", im.shape[1], im.shape[2], im, ab.detach().contiguous().float().reshape(6), 1, y,
+              device=im.device)
+    return y

@@ -5,7 +5,8 @@ reads the sequence with splatam_b200.datasets and scores the map with the GPU ev
 
   --split train  (default) the record's Gaussians and cameras through evaluate.evaluate, with the ATE of the record's
                  trajectory against the reader's ground truth; the record needs one camera column for every evaluated
-                 frame
+                 frame; --exposure PATH (the run's exposure.npz) scores the renders through each frame's colour
+                 correction
   --split test   the Gaussians through evaluate.evaluate_nvs on the held-out views, at their ground-truth poses
                  (scannetpp, replicav2)
 
@@ -43,7 +44,14 @@ def parse_args(argv=None):
     ap.add_argument("--no-frames", action="store_true", help="do not save the rendered and ground-truth frames")
     ap.add_argument("--lpips-alexnet", default=None, help="torchvision AlexNet weights (alexnet-owt-7be5be79.pth)")
     ap.add_argument("--lpips-lin", default=None, help="LPIPS v0.1 linear heads (alex.pth)")
+    ap.add_argument("--exposure", default=None, metavar="PATH",
+                    help="exposure.npz of the run (--split train): score each frame's render through its colour "
+                         "correction")
     a = ap.parse_args(argv)
+    if a.exposure is not None and a.split != "train":
+        ap.error("--exposure applies to --split train only (held-out views have no exposure estimate)")
+    if a.exposure is not None and not os.path.isfile(a.exposure):
+        ap.error("--exposure %s: no such file" % a.exposure)
     if (a.lpips_alexnet is None) != (a.lpips_lin is None):
         ap.error("--lpips-alexnet and --lpips-lin go together")
     if a.frames < 0:
@@ -81,6 +89,9 @@ def main(argv=None):
         if a.split == "train":
             cams = formats.record_tensors(rec, ("cam_unnorm_rots", "cam_trans"), dev)
             params = dict(gauss, **{k: v[..., :T] for k, v in cams.items()})
+            if a.exposure is not None:
+                expo = formats.load_exposure(a.exposure, num_frames=rec["cam_trans"].shape[-1], device=dev)
+                params["cam_exposure"] = expo[..., :T].contiguous()
             gt_w2c = [torch.linalg.inv(seq.files.poses[t].to(dev)) for t in range(T)]
             res = evaluate.evaluate(params, frames, seq.cam, RSD.SIL_THRES, h["mapping_iters"], True,
                                     eval_every=h["eval_every"], gt_w2c=gt_w2c, out_dir=a.out, lpips=net,
@@ -89,7 +100,8 @@ def main(argv=None):
             res = evaluate.evaluate_nvs(gauss, frames, seq.cam, RSD.SIL_THRES, h["mapping_iters"], True,
                                         eval_every=h["eval_every"], out_dir=a.out, lpips=net, save_frames=save)
         eval_s = time.perf_counter() - t0
-    line = dict(dataset=a.dataset, sequence=a.sequence, split=a.split, record=a.record, out=a.out, frames=T,
+    line = dict(dataset=a.dataset, sequence=a.sequence, split=a.split, record=a.record, exposure=a.exposure, out=a.out,
+                frames=T,
                 width=int(h["width"]), height=int(h["height"]), gaussians=int(gauss["means3D"].shape[0]),
                 evaluated_frames=len(res["frame_ids"]), frames_saved=save, psnr_db=res["psnr"], ms_ssim=res["ms_ssim"],
                 depth_rmse_m=res["depth_rmse"], depth_l1_m=res["depth_l1"], eval_s=eval_s)

@@ -151,8 +151,14 @@ def main():
     ap.add_argument("--relocalise-photometric", action="store_true",
                     help="--relocalise with the photometric health check and RGB-D ICP verification (implies "
                          "--relocalise)")
+    ap.add_argument("--exposure", action="store_true",
+                    help="estimate each frame's exposure and white balance while tracking, and map and evaluate "
+                         "through it (slam.run_slam's `exposure`, its EXPOSURE_DEFAULTS); with --out also writes "
+                         "exposure.npz; off by default")
     a = ap.parse_args()
     a.relocalise = a.relocalise or a.relocalise_photometric
+    if a.exposure and a.relocalise:
+        ap.error("--exposure cannot be combined with --relocalise")
     if (a.lpips_alexnet is None) != (a.lpips_lin is None):
         ap.error("--lpips-alexnet and --lpips-lin go together")
     if a.checkpoint_every < 0:
@@ -212,7 +218,8 @@ def main():
                         mapping_cam_lrs=tuple(a.mapping_cam_lrs), pose_init=a.pose_init,
                         loop_closure={} if a.loop_closure else None,
                         relocalise=((dict(photometric=True) if a.relocalise_photometric else {}) if a.relocalise
-                                    else None))
+                                    else None),
+                        exposure={} if a.exposure else None)
     torch.cuda.synchronize(dev)
     wall = time.perf_counter() - t0
     # --resume: wall time from reading the checkpoint to the first tracked frame (frame-0 read, load, keyframe rebuild)
@@ -222,6 +229,8 @@ def main():
     gt_w2c = [torch.linalg.inv(p.to(dev)) for p in gt]
     gt_w2c_all = seq.gt_w2c[:T]                  # the record's gt_w2c_all_frames: NaN where a pose is invalid
     params = dict(out["gauss"], cam_unnorm_rots=out["rots"], cam_trans=out["trans"])
+    if a.exposure:                               # scored through each frame's estimated colour correction
+        params["cam_exposure"] = out["exposure"]
     res = evaluate.evaluate(params, frames, seq.cam, SIL_THRES, h["mapping_iters"], True, eval_every=h["eval_every"],
                             gt_w2c=gt_w2c, out_dir=a.out, lpips=net, save_frames=a.save_frames)
     seq.close()
@@ -241,11 +250,13 @@ def main():
     if a.out is not None:
         formats.save_run_record(a.out, out["gauss"], out["rots"], out["trans"], out["timestep"], K, seq.w2c, seq.width,
                                 seq.height, gt_w2c_all, out["keyframe_time_indices"])
+        if a.exposure:
+            formats.save_exposure(a.out, out["exposure"])
     print(json.dumps(dict(
         dataset=a.dataset, sequence=a.sequence, variant=a.variant, frames=T, width=seq.width, height=seq.height,
         densify_height=seq.densify_height, densify_width=seq.densify_width, hyper=h,
         initial_gaussians=initial_gaussians, resumed_from=a.resume, resume_s=resume_s,
-        mapping_cam_lrs=list(a.mapping_cam_lrs), pose_init=a.pose_init,
+        mapping_cam_lrs=list(a.mapping_cam_lrs), pose_init=a.pose_init, exposure=a.exposure,
         **({} if a.pose_init == "constant_velocity" else dict(pose_init_s=timing["pose_init_s"],
                                                 icp_accepted=sum(s["accepted"] for s in out["icp"]))),
         **({} if not a.loop_closure else dict(loop_closure_s=timing["loop_closure_s"], loops=out["loops"])),
