@@ -282,6 +282,23 @@ SB_API int sb_masked_l1_backward(const float* depth_sil, const float* gt_depth, 
                                  int H, int W, float sil_thres, int use_sil, int depth_mean, const double* sums,
                                  const float* g_depth, const float* g_im, float* grad_depth_sil, float* grad_im,
                                  void* stream);
+/* The same losses over the pixels whose `keep` byte (uint8 [H,W], device, non-NULL) is non-zero, through the same
+ * device code: with every keep byte set they give the bits of the calls above.  sb_masked_l1_keep_*: mask &= keep.
+ * sb_image_loss_keep_forward: sums[0] = sum over kept pixels and channels of the SSIM map, sums[1] = that of |x-y|,
+ * sums[2] = the kept pixel count (3 device doubles, zeroed here); the loss is w_l1 sums[1] / (C sums[2]) +
+ * w_ssim (1 - sums[0] / (C sums[2])).  sb_image_loss_keep_backward takes the forward's `sums`. */
+SB_API int sb_masked_l1_keep_forward(const uint8_t* keep, const float* depth_sil, const float* gt_depth,
+                                     const float* im, const float* gt_im, int H, int W, float sil_thres, int use_sil,
+                                     double* sums, void* stream);
+SB_API int sb_masked_l1_keep_backward(const uint8_t* keep, const float* depth_sil, const float* gt_depth,
+                                      const float* im, const float* gt_im, int H, int W, float sil_thres, int use_sil,
+                                      int depth_mean, const double* sums, const float* g_depth, const float* g_im,
+                                      float* grad_depth_sil, float* grad_im, void* stream);
+SB_API int sb_image_loss_keep_forward(const uint8_t* keep, const float* x, const float* y, int C, int H, int W,
+                                      float* work, double* sums, void* stream);
+SB_API int sb_image_loss_keep_backward(const uint8_t* keep, const float* x, const float* y, int C, int H, int W,
+                                       const float* work, const double* sums, const float* grad_out, float w_ssim,
+                                       float w_l1, float* grad_x, void* stream);
 
 /* ---- map maintenance: stream compaction (SURVEY.md section 8(f) row N3) ---------------------------------
  * sb_prune_mask: keep[i] = !(sigmoid(logit_opacities[i]) < opacity_threshold || max_k exp(log_scales[i,k]) >
@@ -722,6 +739,40 @@ SB_API int sb_exposure_apply(int height, int width, const float* x, const float*
                              void* stream);
 SB_API int sb_exposure_backward(int height, int width, const float* x, const float* ab, const float* gy, float* gx,
                                 double* g_ab, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- motion masks from the map's depth residual (splatam_b200/dynamic.py, csrc/dynamic.cu) ------------------------
+ * Inputs: depth_sil float32 [3,H,W] (device; d = channel 0, s = channel 1), the frame's depth g float32 [H,W].
+ * valid = g > 0 & isfinite(d) & s > sil_thres;  r = __fdiv_rn(__fsub_rn(d, g), g).
+ * sb_dynamic_residual: writes r [H*W] (every pixel), zeroes then fills hist uint32 [SB_DYNAMIC_BINS] with the counts
+ *   of bits(|r|) >> 16 over valid pixels, zeroes stats float32 [SB_DYNAMIC_STATS] and sets stats[0] = valid count.
+ * sb_dynamic_scale: one CTA; stats[1] = scale = the float with bits b << 16, b the bin holding element (n - 1) / 2 of
+ *   the valid |r| sorted ascending (n = stats[0]; 0 when n = 0).
+ * sb_dynamic_seeds: thr(k, f) = k*scale if k*scale > f else f (float32).  occ = valid & r > thr(k_high, r_min),
+ *   dis = valid & -r > thr(k_high, r_min); a seed is kept when >= 4 of its 8 neighbours are seeds of its kind.
+ *   cand = g > 0 & ((valid & r > thr(k_low, r_min * 0.5f)) | s <= sil_thres).  flags uint8 [H*W] = kept occ (1) |
+ *   kept dis (2) | cand (4); dyn uint8 [H*W] = kept occ (0/1); stats[2], stats[3] += kept occ, dis counts.
+ * sb_dynamic_grow: `radius` Jacobi steps of  dyn'(q) = dyn(q) | (cand(q) & some 4-neighbour p has dyn(p) and
+ *   |g_p - g_q| <= tau * min(g_p, g_q))  (float32, rounded as written), SB_DYNAMIC_GROW_STEPS steps per launch; the
+ *   result is in `dyn`; tmp uint8 [H*W] is scratch.
+ * sb_dynamic_dilate: dynamic = Chebyshev dilation by `dilate` of grown, inconsistent = that of the kept dis seeds
+ *   (uint8 0/1 [H*W]); stats[4], stats[5] += their counts.
+ * stats = (valid, scale, occ seeds, dis seeds, dynamic, inconsistent): counts are float32 sums of integers, exact
+ * because H*W < 2^24.  No call synchronises the host; all can be captured in a CUDA graph.
+ * SB_ERR_BAD_ARG, before any launch, for H or W < 1, H*W >= 2^24, null pointers, NaN k_high / k_low, r_min or tau
+ * not finite and >= 0, radius < 0, dilate outside [0, 64] and dyn == tmp. */
+#define SB_DYNAMIC_BINS 32768
+#define SB_DYNAMIC_STATS 6
+#define SB_DYNAMIC_GROW_STEPS 8
+SB_API int sb_dynamic_residual(int height, int width, const float* depth_sil, const float* gt_depth, float sil_thres,
+                               float* residual, uint32_t* hist, float* stats, void* stream);
+SB_API int sb_dynamic_scale(const uint32_t* hist, float* stats, void* stream);
+SB_API int sb_dynamic_seeds(int height, int width, const float* depth_sil, const float* gt_depth,
+                            const float* residual, float sil_thres, float k_high, float k_low, float r_min,
+                            uint8_t* flags, uint8_t* dyn, float* stats, void* stream);
+SB_API int sb_dynamic_grow(int height, int width, const float* gt_depth, const uint8_t* flags, float tau, int radius,
+                           uint8_t* dyn, uint8_t* tmp, void* stream);
+SB_API int sb_dynamic_dilate(int height, int width, const uint8_t* grown, const uint8_t* flags, int dilate,
+                             uint8_t* dynamic, uint8_t* inconsistent, float* stats, void* stream);
 
 /* ---- per-stage device timing (measurement only; bench.py's roofline pass) -------------------
  * Between sb_profile_begin() and sb_profile_end() every stage launch of this process is bracketed

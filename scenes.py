@@ -700,6 +700,108 @@ def write_kidnapped_sequence(dst, device, seed=21, cam=LOOP_CAM, png_depth_scale
     return _write_room_sequence(dst, kidnapped_trajectory(device, **kw), device, seed, cam, png_depth_scale, quality)
 
 
+DYNAMIC_BOX = (0.5, 1.0, 0.3)          # the moving box's extents [m] (x, y, z)
+DYNAMIC_BOX_Z = 1.3                    # its centre's depth in front of the loop's start [m]
+
+
+def dynamic_box(seed=5, P=30_000, size=DYNAMIC_BOX):
+    """An opaque, textured box of isotropic Gaussians centred on the origin (extents `size` [m]), its faces covered in
+    proportion to their area: the moving object of `write_dynamic_sequence`.  Returns SplaTAM's five-tensor map (CPU)."""
+    g = torch.Generator().manual_seed(seed)
+    h = torch.tensor(size) / 2
+    area = torch.tensor([h[1] * h[2], h[1] * h[2], h[0] * h[2], h[0] * h[2], h[0] * h[1], h[0] * h[1]])
+    face = torch.multinomial(area / area.sum(), P, replacement=True, generator=g)
+    a, b = _rand(g, P) * 2 - 1, _rand(g, P) * 2 - 1
+    pts = torch.zeros(P, 3)
+    for f in range(6):
+        m = face == f
+        ax = f // 2
+        o = [i for i in range(3) if i != ax]
+        pts[m, ax] = (1.0 if f % 2 else -1.0) * h[ax]
+        pts[m, o[0]] = a[m] * h[o[0]]
+        pts[m, o[1]] = b[m] * h[o[1]]
+    col = 0.45 + 0.35 * torch.sign(torch.sin(pts[:, [0]] * 40.0) * torch.sin(pts[:, [1]] * 40.0)) * torch.tensor(
+        [1.0, -0.6, 0.3])
+    q = torch.zeros(P, 4)
+    q[:, 0] = 1.0
+    return dict(means3D=pts, rgb_colors=col.clamp(0, 1), unnorm_rotations=q,
+                logit_opacities=torch.full((P, 1), float(torch.logit(torch.tensor(0.98)))),
+                log_scales=torch.full((P, 1), math.log(0.01)))
+
+
+def dynamic_box_track(num_frames, present_at_start=False, travel=1.6):
+    """The box centre's world position per frame [T,3] (numpy): it crosses the view from x = -travel to +travel at
+    depth DYNAMIC_BOX_Z (out of view at frame 0), or with `present_at_start` it sits in view at x = 0 at frame 0 and
+    leaves to x = +travel by the middle of the sequence."""
+    s = np.arange(num_frames, dtype=np.float64) / max(num_frames - 1, 1)
+    x = travel * np.minimum(1.0, 2.0 * s) if present_at_start else travel * (2.0 * s - 1.0)
+    return np.stack([x, np.zeros_like(x), np.full_like(x, DYNAMIC_BOX_Z)], 1)
+
+
+def write_dynamic_sequence(dst, num_frames, device, seed=21, cam=LOOP_CAM, present_at_start=False,
+                           png_depth_scale=6553.5, quality=95):
+    """`loop_room` along `loop_trajectory` with a box (`dynamic_box`, 0.5 x 1.0 x 0.3 m) moving through the view
+    (`dynamic_box_track`), written in Replica's layout as write_loop_sequence writes the loop (read it back with
+    loop_data_config).  Also writes the ground-truth motion masks masks/mask<t>.png (255 where the box rendered alone
+    has silhouette > 0.5), which the reader ignores.  Returns (ground-truth w2c [T,4,4] (CPU), box-to-world [T,4,4]
+    (numpy float64))."""
+    import os
+    from PIL import Image
+    import splatam_b200 as S
+    from splatam_b200 import mapping as M, slam
+    sc = loop_room(seed=seed, cam=cam)
+    rs = sc.settings(S.GaussianRasterizationSettings, device)
+    room = sc.splatam_params(device)
+    box = {k: v.to(device) for k, v in dynamic_box().items()}
+    track = dynamic_box_track(num_frames, present_at_start)
+    rots, trans = loop_trajectory(num_frames, device)
+    for d in ("results", "masks"):
+        os.makedirs(os.path.join(dst, d), exist_ok=True)
+    w2cs, traj, poses = [], [], []
+    for t in range(num_frames):
+        moved = dict(box, means3D=box["means3D"] + torch.tensor(track[t], dtype=torch.float32, device=device))
+        both = {k: torch.cat([room[k], moved[k]]) for k in room}
+        f = slam.render_frame(both, rots, trans, t, rs)
+        depth = torch.where(f["sil"] > 0.9, f["depth"] / f["sil"].clamp(min=1e-6), torch.zeros_like(f["depth"]))
+        raw = (depth[0] * png_depth_scale).round().clamp(0, 65535).cpu().numpy().astype(np.uint16)
+        Image.fromarray(_exposed_u8(f["im"], None, t)).save(os.path.join(dst, "results", "frame%06d.jpg" % t),
+                                                            quality=quality)
+        Image.fromarray(raw).save(os.path.join(dst, "results", "depth%06d.png" % t))
+        alone = slam.render_frame(moved, rots, trans, t, rs)
+        mask = ((alone["sil"][0] > 0.5).cpu().numpy() * 255).astype(np.uint8)
+        Image.fromarray(mask).save(os.path.join(dst, "masks", "mask%06d.png" % t))
+        w2c = M.camera_w2c(rots[..., t], trans[..., t])[0].detach().double().cpu()
+        w2cs.append(w2c)
+        traj.append(" ".join("%.17g" % v for v in torch.linalg.inv(w2c).reshape(-1).tolist()))
+        pose = np.eye(4)
+        pose[:3, 3] = track[t]
+        poses.append(pose)
+    with open(os.path.join(dst, "traj.txt"), "w") as fh:
+        fh.write("\n".join(traj) + "\n")
+    return torch.stack(w2cs), np.stack(poses)
+
+
+def motion_mask_frame(H, W, seed, objects=2):
+    """A small synthetic input of the motion-mask rule (splatam_b200/dynamic.py): a [3,H,W] depth/silhouette render and
+    a frame depth [H,W] (float32 numpy) with occluding blocks, a disoccluded block, NaN render depth, zero frame depth,
+    silhouettes exactly at 0.99 and uncovered pixels."""
+    rng = np.random.default_rng(seed)
+    g = (2.0 + 0.01 * rng.standard_normal((H, W))).astype(np.float32)
+    d = (g * (1 + 0.01 * rng.standard_normal((H, W)))).astype(np.float32)
+    s = np.ones((H, W), np.float32)
+    for _ in range(objects):
+        y, x = rng.integers(0, H), rng.integers(0, W)
+        h, w = rng.integers(1, max(2, H // 2)), rng.integers(1, max(2, W // 2))
+        g[y:y + h, x:x + w] = rng.uniform(0.8, 1.5)
+    y, x = rng.integers(0, H), rng.integers(0, W)
+    g[y:y + 3, x:x + 3] = 3.0                           # the frame sees past the map
+    s[rng.random((H, W)) < 0.1] = np.float32(0.99)      # exactly at sil_thres: not valid, a candidate
+    s[rng.random((H, W)) < 0.1] = 0.2                   # not covered by the map
+    d[rng.random((H, W)) < 0.03] = np.nan
+    g[rng.random((H, W)) < 0.03] = 0.0
+    return np.stack([d, s, d * d]).astype(np.float32), g
+
+
 def loop_data_config(cam=LOOP_CAM, png_depth_scale=6553.5):
     """The data config (datasets.load_config's shape) that reads a `write_loop_sequence` sequence back with
     datasets.RGBDSequence("replica", ...)."""

@@ -132,6 +132,17 @@ _SIGNATURES = {
     "sb_exposure_workspace_bytes": (_i, [_i, _i, ctypes.POINTER(_sz)]),
     "sb_exposure_apply": (_i, [_i, _i, _vp, _vp, _i, _vp, _vp]),
     "sb_exposure_backward": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "sb_dynamic_residual": (_i, [_i, _i, _vp, _vp, _f, _vp, _vp, _vp, _vp]),
+    "sb_dynamic_scale": (_i, [_vp, _vp, _vp]),
+    "sb_dynamic_seeds": (_i, [_i, _i, _vp, _vp, _vp, _f, _f, _f, _f, _vp, _vp, _vp, _vp]),
+    "sb_dynamic_grow": (_i, [_i, _i, _vp, _vp, _f, _i, _vp, _vp, _vp]),
+    "sb_dynamic_dilate": (_i, [_i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    "sb_masked_l1_keep_forward": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, ctypes.c_float, _i, _vp, _vp]),
+    "sb_masked_l1_keep_backward": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, ctypes.c_float, _i, _i, _vp, _vp, _vp, _vp,
+                                        _vp, _vp]),
+    "sb_image_loss_keep_forward": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
+    "sb_image_loss_keep_backward": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, ctypes.c_float, ctypes.c_float,
+                                         _vp, _vp]),
     "sb_profile_begin": (_i, []),
     "sb_profile_end": (_i, [ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_int)]),
     "sb_stage_name": (ctypes.c_char_p, [_i]),

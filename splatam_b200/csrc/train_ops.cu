@@ -66,14 +66,16 @@ constexpr int kPW = kTW + 2 * kR, kPH = kTH + 2 * kR;   // padded tile 42 x 18
 struct GaussWin { float w[kWin]; };
 
 // Forward: per pixel/channel SSIM map terms; writes the three partial-derivative maps needed by the
-// backward (dS/dmu1, dS/dE[x^2], dS/dE[xy]) and accumulates sum(ssim) and sum|x-y| into sums[0..1].
+// backward (dS/dmu1, dS/dE[x^2], dS/dE[xy]) and accumulates sum(ssim) and sum|x-y| into sums[0..1].  With `keep`
+// (uint8 [H,W]) a pixel whose byte is 0 adds nothing and gets zero derivative maps, and sums[2] counts the kept pixels;
+// NULL keeps every pixel and leaves sums[2] alone.
 __global__ void __launch_bounds__(kTW * kTH)
 ssim_l1_forward_kernel(const float* __restrict__ x, const float* __restrict__ y, int C, int H, int W,
                        float* __restrict__ dmu, float* __restrict__ de11, float* __restrict__ de12,
-                       double* __restrict__ sums, const GaussWin win) {
+                       double* __restrict__ sums, const GaussWin win, const uint8_t* __restrict__ keep) {
     __shared__ float sx[kPH][kPW], sy[kPH][kPW];
     __shared__ float h[5][kPH][kTW];     // horizontally filtered x, y, xx, yy, xy
-    __shared__ float red[2][kTW * kTH / 32];
+    __shared__ float red[3][kTW * kTH / 32];
     const int c = blockIdx.z, x0 = blockIdx.x * kTW, y0 = blockIdx.y * kTH;
     const float* xc = x + (size_t)c * H * W;
     const float* yc = y + (size_t)c * H * W;
@@ -98,8 +100,10 @@ ssim_l1_forward_kernel(const float* __restrict__ x, const float* __restrict__ y,
     }
     __syncthreads();
     const int px = x0 + threadIdx.x, py = y0 + threadIdx.y;
-    float ssim = 0.f, l1 = 0.f;
+    float ssim = 0.f, l1 = 0.f, kept = 0.f;
     if (px < W && py < H) {
+        const bool k = keep == nullptr || keep[(size_t)py * W + px] != 0;
+        kept = k ? 1.f : 0.f;
         float mu1 = 0.f, mu2 = 0.f, e11 = 0.f, e22 = 0.f, e12 = 0.f;
 #pragma unroll
         for (int k = 0; k < kWin; ++k) {
@@ -117,33 +121,37 @@ ssim_l1_forward_kernel(const float* __restrict__ x, const float* __restrict__ y,
         ssim = a1 * a2 * inv;
         const size_t o = (size_t)c * H * W + (size_t)py * W + px;
         // total derivatives w.r.t. mu1 (incl. through sigma terms), E[x^2], E[xy]
-        dmu[o] = 2.f * mu2 * (a2 - a1) * inv - ssim * 2.f * mu1 * (1.f / b1 - 1.f / b2);
-        de11[o] = -ssim / b2;
-        de12[o] = 2.f * a1 * inv;
-        l1 = fabsf(sx[threadIdx.y + kR][threadIdx.x + kR] - sy[threadIdx.y + kR][threadIdx.x + kR]);
+        dmu[o] = k ? 2.f * mu2 * (a2 - a1) * inv - ssim * 2.f * mu1 * (1.f / b1 - 1.f / b2) : 0.f;
+        de11[o] = k ? -ssim / b2 : 0.f;
+        de12[o] = k ? 2.f * a1 * inv : 0.f;
+        l1 = k ? fabsf(sx[threadIdx.y + kR][threadIdx.x + kR] - sy[threadIdx.y + kR][threadIdx.x + kR]) : 0.f;
+        ssim = k ? ssim : 0.f;
     }
     // block reduction of the two sums
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) {
         ssim += __shfl_xor_sync(0xffffffffu, ssim, off);
         l1 += __shfl_xor_sync(0xffffffffu, l1, off);
+        kept += __shfl_xor_sync(0xffffffffu, kept, off);
     }
-    if ((tid & 31) == 0) { red[0][tid >> 5] = ssim; red[1][tid >> 5] = l1; }
+    if ((tid & 31) == 0) { red[0][tid >> 5] = ssim; red[1][tid >> 5] = l1; red[2][tid >> 5] = kept; }
     __syncthreads();
     if (tid == 0) {
-        float a = 0.f, b = 0.f;
-        for (int i = 0; i < kTW * kTH / 32; ++i) { a += red[0][i]; b += red[1][i]; }
+        float a = 0.f, b = 0.f, n = 0.f;
+        for (int i = 0; i < kTW * kTH / 32; ++i) { a += red[0][i]; b += red[1][i]; n += red[2][i]; }
         atomicAdd(&sums[0], (double)a);
         atomicAdd(&sums[1], (double)b);
+        if (keep != nullptr && c == 0) atomicAdd(&sums[2], (double)n);
     }
 }
 
-// Backward: grad_x = gscale_ssim * (conv(dmu) + 2 x conv(de11) + y conv(de12)) + gscale_l1 * sign(x - y)
+// Backward: grad_x = gscale_ssim * (conv(dmu) + 2 x conv(de11) + y conv(de12)) + gscale_l1 * sign(x - y).  With
+// `keep` the sign term is zero where keep is 0 and n = C * the kept count of the forward (sums[2]).
 __global__ void __launch_bounds__(kTW * kTH)
 ssim_l1_backward_kernel(const float* __restrict__ x, const float* __restrict__ y, const float* __restrict__ dmu,
                         const float* __restrict__ de11, const float* __restrict__ de12, int C, int H, int W,
                         const float* __restrict__ grad_out, float w_ssim, float w_l1, float* __restrict__ gx,
-                        const GaussWin win) {
+                        const GaussWin win, const uint8_t* __restrict__ keep, const double* __restrict__ sums) {
     __shared__ float s[3][kPH][kPW];
     __shared__ float h[3][kPH][kTW];
     const int c = blockIdx.z, x0 = blockIdx.x * kTW, y0 = blockIdx.y * kTH;
@@ -181,10 +189,12 @@ ssim_l1_backward_kernel(const float* __restrict__ x, const float* __restrict__ y
     }
     const size_t o = plane + (size_t)py * W + px;
     const float xv = x[o], yv = y[o], go = __ldg(grad_out);
-    const float n = (float)C * (float)H * (float)W;
+    // with `keep`, an empty kept set gives zero gradient (n >= C), not 0/0
+    const float n = keep == nullptr ? (float)C * (float)H * (float)W : (float)C * (float)fmax(sums[2], 1.0);
     // loss = w_l1 * mean|x-y| + w_ssim * (1 - mean(ssim))
     const float diff = xv - yv;
-    const float sgn = diff > 0.f ? 1.f : (diff < 0.f ? -1.f : 0.f);
+    const bool k = keep == nullptr || keep[(size_t)py * W + px] != 0;
+    const float sgn = !k ? 0.f : (diff > 0.f ? 1.f : (diff < 0.f ? -1.f : 0.f));
     gx[o] = go * (w_l1 * sgn / n - w_ssim * (a + 2.f * xv * b + yv * d) / n);
 }
 
@@ -201,12 +211,12 @@ __device__ __forceinline__ bool loss_mask(float gd, float d, float sil, float ds
 __global__ void __launch_bounds__(256)
 masked_l1_forward_kernel(const float* __restrict__ depth_sil, const float* __restrict__ gt_depth,
                          const float* __restrict__ im, const float* __restrict__ gt_im, int HW, float sil_thres,
-                         int use_sil, double* __restrict__ sums) {
+                         int use_sil, double* __restrict__ sums, const uint8_t* __restrict__ keep) {
     __shared__ float red[3][8];
     float sd = 0.f, sm = 0.f, si = 0.f;
     for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < HW; p += gridDim.x * blockDim.x) {
         const float d = depth_sil[p], gd = gt_depth[p];
-        if (loss_mask(gd, d, depth_sil[HW + p], depth_sil[2 * HW + p], sil_thres, use_sil)) {
+        if (loss_mask(gd, d, depth_sil[HW + p], depth_sil[2 * HW + p], sil_thres, use_sil) && (!keep || keep[p])) {
             sd += fabsf(gd - d); sm += 1.f;
             if (im) si += fabsf(gt_im[p] - im[p]) + fabsf(gt_im[HW + p] - im[HW + p]) + fabsf(gt_im[2 * HW + p] - im[2 * HW + p]);
         }
@@ -233,13 +243,14 @@ masked_l1_backward_kernel(const float* __restrict__ depth_sil, const float* __re
                           const float* __restrict__ im, const float* __restrict__ gt_im, int HW, float sil_thres,
                           int use_sil, int depth_mean, const double* __restrict__ sums,
                           const float* __restrict__ g_depth, const float* __restrict__ g_im,
-                          float* __restrict__ grad_depth_sil, float* __restrict__ grad_im) {
+                          float* __restrict__ grad_depth_sil, float* __restrict__ grad_im,
+                          const uint8_t* __restrict__ keep) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= HW) return;
     const float d = depth_sil[p], gd = gt_depth[p];
-    const bool m = loss_mask(gd, d, depth_sil[HW + p], depth_sil[2 * HW + p], sil_thres, use_sil);
+    const bool m = loss_mask(gd, d, depth_sil[HW + p], depth_sil[2 * HW + p], sil_thres, use_sil) && (!keep || keep[p]);
     float scale = g_depth ? __ldg(g_depth) : 0.f;
-    if (depth_mean) scale = scale / (float)sums[1];
+    if (depth_mean) scale = scale / (float)(keep ? fmax(sums[1], 1.0) : sums[1]);
     const float diff = d - gd;
     grad_depth_sil[p] = m ? scale * (diff > 0.f ? 1.f : (diff < 0.f ? -1.f : 0.f)) : 0.f;
     grad_depth_sil[HW + p] = 0.f;
@@ -311,29 +322,61 @@ SB_API int sb_adam_step_guarded(float* params, const float* grads, float* exp_av
 }
 
 /* sums: 3 device doubles (zeroed here).  im / gt_im may be NULL (mapping: the RGB term uses the SSIM loss). */
-SB_API int sb_masked_l1_forward(const float* depth_sil, const float* gt_depth, const float* im, const float* gt_im,
-                                int H, int W, float sil_thres, int use_sil, double* sums, void* stream) {
+static int masked_l1_forward(const uint8_t* keep, const float* depth_sil, const float* gt_depth, const float* im,
+                             const float* gt_im, int H, int W, float sil_thres, int use_sil, double* sums,
+                             void* stream) {
     if (!depth_sil || !gt_depth || !sums || H < 1 || W < 1 || ((im != nullptr) != (gt_im != nullptr))) return SB_ERR_BAD_ARG;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     SB_CUDA_CHECK(cudaMemsetAsync(sums, 0, 3 * sizeof(double), st));
     const int HW = H * W;
     const int blocks = (HW + 255) / 256 < 528 ? (HW + 255) / 256 : 528;   // 132 SMs x 4
-    masked_l1_forward_kernel<<<blocks, 256, 0, st>>>(depth_sil, gt_depth, im, gt_im, HW, sil_thres, use_sil, sums);
+    masked_l1_forward_kernel<<<blocks, 256, 0, st>>>(depth_sil, gt_depth, im, gt_im, HW, sil_thres, use_sil, sums,
+                                                     keep);
     SB_LAUNCH_CHECK("masked_l1_forward_kernel");
     return SB_OK;
+}
+
+static int masked_l1_backward(const uint8_t* keep, const float* depth_sil, const float* gt_depth, const float* im,
+                              const float* gt_im, int H, int W, float sil_thres, int use_sil, int depth_mean,
+                              const double* sums, const float* g_depth, const float* g_im, float* grad_depth_sil,
+                              float* grad_im, void* stream) {
+    if (!depth_sil || !gt_depth || !sums || !grad_depth_sil || H < 1 || W < 1) return SB_ERR_BAD_ARG;
+    if (grad_im && (!im || !gt_im)) return SB_ERR_BAD_ARG;
+    const int HW = H * W;
+    masked_l1_backward_kernel<<<(HW + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        depth_sil, gt_depth, im, gt_im, HW, sil_thres, use_sil, depth_mean, sums, g_depth, g_im, grad_depth_sil, grad_im,
+        keep);
+    SB_LAUNCH_CHECK("masked_l1_backward_kernel");
+    return SB_OK;
+}
+
+SB_API int sb_masked_l1_forward(const float* depth_sil, const float* gt_depth, const float* im, const float* gt_im,
+                                int H, int W, float sil_thres, int use_sil, double* sums, void* stream) {
+    return masked_l1_forward(nullptr, depth_sil, gt_depth, im, gt_im, H, W, sil_thres, use_sil, sums, stream);
 }
 
 SB_API int sb_masked_l1_backward(const float* depth_sil, const float* gt_depth, const float* im, const float* gt_im,
                                  int H, int W, float sil_thres, int use_sil, int depth_mean, const double* sums,
                                  const float* g_depth, const float* g_im, float* grad_depth_sil, float* grad_im,
                                  void* stream) {
-    if (!depth_sil || !gt_depth || !sums || !grad_depth_sil || H < 1 || W < 1) return SB_ERR_BAD_ARG;
-    if (grad_im && (!im || !gt_im)) return SB_ERR_BAD_ARG;
-    const int HW = H * W;
-    masked_l1_backward_kernel<<<(HW + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        depth_sil, gt_depth, im, gt_im, HW, sil_thres, use_sil, depth_mean, sums, g_depth, g_im, grad_depth_sil, grad_im);
-    SB_LAUNCH_CHECK("masked_l1_backward_kernel");
-    return SB_OK;
+    return masked_l1_backward(nullptr, depth_sil, gt_depth, im, gt_im, H, W, sil_thres, use_sil, depth_mean, sums,
+                              g_depth, g_im, grad_depth_sil, grad_im, stream);
+}
+
+SB_API int sb_masked_l1_keep_forward(const uint8_t* keep, const float* depth_sil, const float* gt_depth,
+                                     const float* im, const float* gt_im, int H, int W, float sil_thres, int use_sil,
+                                     double* sums, void* stream) {
+    if (!keep) return SB_ERR_BAD_ARG;
+    return masked_l1_forward(keep, depth_sil, gt_depth, im, gt_im, H, W, sil_thres, use_sil, sums, stream);
+}
+
+SB_API int sb_masked_l1_keep_backward(const uint8_t* keep, const float* depth_sil, const float* gt_depth,
+                                      const float* im, const float* gt_im, int H, int W, float sil_thres, int use_sil,
+                                      int depth_mean, const double* sums, const float* g_depth, const float* g_im,
+                                      float* grad_depth_sil, float* grad_im, void* stream) {
+    if (!keep) return SB_ERR_BAD_ARG;
+    return masked_l1_backward(keep, depth_sil, gt_depth, im, gt_im, H, W, sil_thres, use_sil, depth_mean, sums,
+                              g_depth, g_im, grad_depth_sil, grad_im, stream);
 }
 
 // slam_external.gaussian(): float32 exp values divided by their float32 sum (R/utils/slam_external.py:54-57).  The
@@ -353,27 +396,52 @@ SB_API size_t sb_image_loss_workspace_floats(int C, int H, int W) { return (size
 
 /* loss terms of  w_l1*mean|x-y| + w_ssim*(1-mean(SSIM(x,y))) : writes sums[0]=sum(ssim map), sums[1]=sum|x-y|
  * (device doubles, zeroed here) and the partial-derivative maps into `work` (3*C*H*W floats). */
-SB_API int sb_image_loss_forward(const float* x, const float* y, int C, int H, int W, float* work, double* sums,
-                                 void* stream) {
+static int image_loss_forward(const uint8_t* keep, const float* x, const float* y, int C, int H, int W, float* work,
+                              double* sums, void* stream) {
     if (!x || !y || !work || !sums || C < 1 || H < 1 || W < 1) return SB_ERR_BAD_ARG;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    SB_CUDA_CHECK(cudaMemsetAsync(sums, 0, 2 * sizeof(double), st));
+    SB_CUDA_CHECK(cudaMemsetAsync(sums, 0, (keep ? 3 : 2) * sizeof(double), st));
     const size_t n = (size_t)C * H * W;
     dim3 grid((W + kTW - 1) / kTW, (H + kTH - 1) / kTH, C), block(kTW, kTH);
-    ssim_l1_forward_kernel<<<grid, block, 0, st>>>(x, y, C, H, W, work, work + n, work + 2 * n, sums, gauss_window());
+    ssim_l1_forward_kernel<<<grid, block, 0, st>>>(x, y, C, H, W, work, work + n, work + 2 * n, sums, gauss_window(),
+                                                   keep);
     SB_LAUNCH_CHECK("ssim_l1_forward_kernel");
     return SB_OK;
 }
 
-SB_API int sb_image_loss_backward(const float* x, const float* y, int C, int H, int W, const float* work,
-                                  const float* grad_out, float w_ssim, float w_l1, float* grad_x, void* stream) {
+static int image_loss_backward(const uint8_t* keep, const double* sums, const float* x, const float* y, int C, int H,
+                               int W, const float* work, const float* grad_out, float w_ssim, float w_l1,
+                               float* grad_x, void* stream) {
     if (!x || !y || !work || !grad_out || !grad_x || C < 1 || H < 1 || W < 1) return SB_ERR_BAD_ARG;
     const size_t n = (size_t)C * H * W;
     dim3 grid((W + kTW - 1) / kTW, (H + kTH - 1) / kTH, C), block(kTW, kTH);
     ssim_l1_backward_kernel<<<grid, block, 0, static_cast<cudaStream_t>(stream)>>>(
-        x, y, work, work + n, work + 2 * n, C, H, W, grad_out, w_ssim, w_l1, grad_x, gauss_window());
+        x, y, work, work + n, work + 2 * n, C, H, W, grad_out, w_ssim, w_l1, grad_x, gauss_window(), keep, sums);
     SB_LAUNCH_CHECK("ssim_l1_backward_kernel");
     return SB_OK;
+}
+
+SB_API int sb_image_loss_forward(const float* x, const float* y, int C, int H, int W, float* work, double* sums,
+                                 void* stream) {
+    return image_loss_forward(nullptr, x, y, C, H, W, work, sums, stream);
+}
+
+SB_API int sb_image_loss_backward(const float* x, const float* y, int C, int H, int W, const float* work,
+                                  const float* grad_out, float w_ssim, float w_l1, float* grad_x, void* stream) {
+    return image_loss_backward(nullptr, nullptr, x, y, C, H, W, work, grad_out, w_ssim, w_l1, grad_x, stream);
+}
+
+SB_API int sb_image_loss_keep_forward(const uint8_t* keep, const float* x, const float* y, int C, int H, int W,
+                                      float* work, double* sums, void* stream) {
+    if (!keep) return SB_ERR_BAD_ARG;
+    return image_loss_forward(keep, x, y, C, H, W, work, sums, stream);
+}
+
+SB_API int sb_image_loss_keep_backward(const uint8_t* keep, const float* x, const float* y, int C, int H, int W,
+                                       const float* work, const double* sums, const float* grad_out, float w_ssim,
+                                       float w_l1, float* grad_x, void* stream) {
+    if (!keep || !sums) return SB_ERR_BAD_ARG;
+    return image_loss_backward(keep, sums, x, y, C, H, W, work, grad_out, w_ssim, w_l1, grad_x, stream);
 }
 
 }  // extern "C"

@@ -194,6 +194,45 @@ def save_exposure(out_dir, cam_exposure):
     return path
 
 
+def save_dynamic(out_dir, stats, keyframe_ids, keyframe_masks):
+    """`<out_dir>/dynamic.npz` of a run with motion masks (slam.run_slam's `dynamic`): per tracked frame `frame`
+    (int64), `scale`, `dynamic_frac` and `inconsistent_frac` (float32), from the result's `dynamic` list; the
+    keyframes' ids `keyframe_ids` (int64 [K]) and their masks as `keyframe_masks` (np.packbits of the bool [K,H,W]
+    stack) with `keyframe_masks_shape`.  Kept out of params.npz, as exposure.npz is.  Returns the path."""
+    m = np.stack([np.asarray(_host(x), dtype=bool) for x in keyframe_masks])
+    if m.ndim != 3 or m.shape[0] != len(keyframe_ids):
+        raise ValueError("%d keyframe ids for keyframe masks of shape %s" % (len(keyframe_ids), m.shape))
+    os.makedirs(out_dir, exist_ok=True)
+    path = os.path.join(out_dir, "dynamic.npz")
+    np.savez(path, frame=np.array([r["frame"] for r in stats], dtype=np.int64),
+             scale=np.array([r["scale"] for r in stats], dtype=np.float32),
+             dynamic_frac=np.array([r["dynamic_frac"] for r in stats], dtype=np.float32),
+             inconsistent_frac=np.array([r["inconsistent_frac"] for r in stats], dtype=np.float32),
+             keyframe_ids=np.asarray(keyframe_ids, dtype=np.int64), keyframe_masks=np.packbits(m.reshape(-1)),
+             keyframe_masks_shape=np.array(m.shape, dtype=np.int64))
+    return path
+
+
+def load_dynamic(path):
+    """The record of `save_dynamic`: dict(frame, scale, dynamic_frac, inconsistent_frac, keyframe_ids, keyframe_masks
+    bool [K,H,W]) of numpy arrays.  ValueError when a key is missing or the shapes disagree."""
+    keys = ("frame", "scale", "dynamic_frac", "inconsistent_frac", "keyframe_ids", "keyframe_masks",
+            "keyframe_masks_shape")
+    with np.load(path) as z:
+        missing = [k for k in keys if k not in z.files]
+        if missing:
+            raise ValueError("%s lacks %s" % (path, missing))
+        d = {k: np.asarray(z[k]) for k in keys}
+    shape = tuple(int(x) for x in d.pop("keyframe_masks_shape").reshape(-1))
+    n = int(np.prod(shape)) if len(shape) == 3 else -1
+    if n < 0 or shape[0] != d["keyframe_ids"].shape[0] or d["keyframe_masks"].size * 8 < n:
+        raise ValueError("%s: keyframe masks of shape %s for %d keyframes" % (path, shape, d["keyframe_ids"].shape[0]))
+    if not d["frame"].shape == d["scale"].shape == d["dynamic_frac"].shape == d["inconsistent_frac"].shape:
+        raise ValueError("%s: per-frame arrays of different lengths" % path)
+    d["keyframe_masks"] = np.unpackbits(d["keyframe_masks"].astype(np.uint8))[:n].reshape(shape).astype(bool)
+    return d
+
+
 def load_exposure(path, num_frames=None, device=None):
     """The `cam_exposure` [1,6,T] of an exposure.npz (`save_exposure`): numpy, or a float32 tensor on `device`.
     ValueError when the key is missing, the shape is not [1,6,T] or T differs from `num_frames`."""

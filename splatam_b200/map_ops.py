@@ -114,13 +114,15 @@ def backproject(color, depth, intrinsics, w2c, mask=None, scale_dim=1, plan=None
     return new, msd
 
 
-def new_gaussians_from_frame(depth_sil, frame, intrinsics, curr_w2c, sil_thres, scale_dim=1):
+def new_gaussians_from_frame(depth_sil, frame, intrinsics, curr_w2c, sil_thres, scale_dim=1, exclude=None):
     """add_new_gaussians' selection + initialisation for one frame: `depth_sil` is the [3,H,W] depth/silhouette
-    render of the current map at the frame's pose, `frame` holds `im` [3,H,W] and `depth` [1,H,W].  Returns
-    (new parameter rows, count)."""
+    render of the current map at the frame's pose, `frame` holds `im` [3,H,W] and `depth` [1,H,W].  Pixels set in
+    `exclude` (bool [H,W]) are not selected.  Returns (new parameter rows, count)."""
     err = depth_error(depth_sil, frame["depth"])
     thres = 50.0 * float(err.median())               # splatam.py:392 (torch.median = lower middle element)
     mask = new_gaussian_mask(depth_sil, frame["depth"], sil_thres, thres)
+    if exclude is not None:
+        mask = mask & ~exclude.reshape(-1)
     plan = compact_plan(mask)
     if plan[2] == 0:
         return None, 0

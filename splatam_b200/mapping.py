@@ -181,6 +181,11 @@ def _ssim_window(channel, device, size=11, sigma=1.5):
 
 def calc_ssim(img1, img2, window_size=11):
     """R/utils/slam_external.py:66-97 (mean SSIM, 11x11 Gaussian window, sigma 1.5)."""
+    return ssim_map(img1, img2, window_size).mean()
+
+
+def ssim_map(img1, img2, window_size=11):
+    """The per-pixel, per-channel SSIM of `calc_ssim`."""
     ch = img1.size(-3)
     w = _ssim_window(ch, img1.device, window_size).type_as(img1)
     pad = window_size // 2
@@ -189,7 +194,7 @@ def calc_ssim(img1, img2, window_size=11):
     mu1_sq, mu2_sq, mu12 = mu1.pow(2), mu2.pow(2), mu1 * mu2
     s1, s2, s12 = conv(img1 * img1) - mu1_sq, conv(img2 * img2) - mu2_sq, conv(img1 * img2) - mu12
     c1, c2 = 0.01 ** 2, 0.03 ** 2
-    return (((2 * mu12 + c1) * (2 * s12 + c2)) / ((mu1_sq + mu2_sq + c1) * (s1 + s2 + c2))).mean()
+    return ((2 * mu12 + c1) * (2 * s12 + c2)) / ((mu1_sq + mu2_sq + c1) * (s1 + s2 + c2))
 
 
 def _render_pair(params, frame, render, fused, camera_grad, max_rendered=None, gaussians_grad=None):
@@ -240,7 +245,10 @@ def mapping_loss(params, frame, render, loss_weights=(0.5, 1.0), ignore_outlier_
     """SplaTAM get_loss(mapping=True): the Gaussians get gradient, and with `camera_grad` the keyframe's pose too
     (R/scripts/splatam.py:214-347 with tracking=False, mapping=True, do_ba=camera_grad, use_l1=True).
     frame: dict(im [3,H,W], depth [1,H,W], cam settings, w2c [4,4] first-frame w2c, id time index).
-    render(settings, **rendervar) -> (image, radii, depth)."""
+    render(settings, **rendervar) -> (image, radii, depth).  frame["dynamic"] (bool [H,W], run_slam's motion mask),
+    when given, takes its pixels out of both terms."""
+    dyn = frame.get("dynamic")
+    kept = None if dyn is None else ~dyn
     im, depth_sil, radius, means2D = _render_pair(params, frame, render, fused_loss, camera_grad=camera_grad,
                                                   max_rendered=max_rendered, gaussians_grad=True)
     if keep is not None:       # the caller wants d loss / d means2D of the RGB render (densification statistic)
@@ -248,7 +256,7 @@ def mapping_loss(params, frame, render, loss_weights=(0.5, 1.0), ignore_outlier_
         keep["means2D"] = means2D
     if fused_loss and not ignore_outlier_depth_loss:
         from .train_ops import masked_l1        # validity-masked mean |gt - depth| in one kernel (+ one backward)
-        l_depth, _ = masked_l1(depth_sil, frame["depth"], depth_mean=True)
+        l_depth, _ = masked_l1(depth_sil, frame["depth"], depth_mean=True, keep=kept)
     else:
         depth = depth_sil[0:1]
         uncertainty = (depth_sil[2:3] - depth ** 2).detach()
@@ -256,31 +264,54 @@ def mapping_loss(params, frame, render, loss_weights=(0.5, 1.0), ignore_outlier_
         if ignore_outlier_depth_loss:
             err = torch.abs(frame["depth"] - depth) * (frame["depth"] > 0)
             mask = mask & (err < 10 * err.median())
+        if kept is not None:
+            mask = mask & kept
         mask = mask.detach()
         l_depth = torch.abs(frame["depth"] - depth)[mask].mean()
+        if kept is not None:
+            l_depth = torch.nan_to_num(l_depth, nan=0.0)
     if fused_loss:      # one forward + one backward kernel instead of 5 depthwise convs + autograd (train_ops.cu)
         from .train_ops import image_loss
-        l_im = image_loss(im, frame["im"], 0.8, 0.2)
-    else:
+        l_im = image_loss(im, frame["im"], 0.8, 0.2, keep=kept)
+    elif kept is None:
         l_im = 0.8 * torch.abs(im - frame["im"]).mean() + 0.2 * (1.0 - calc_ssim(im, frame["im"]))
+    else:             # boolean indexing: with every pixel kept, the same elements in the same order as the means above
+        k3 = kept.expand_as(im)
+        l_im = 0.8 * torch.abs(im - frame["im"])[k3].mean() + 0.2 * (1.0 - ssim_map(im, frame["im"])[k3].mean())
+        l_im = torch.nan_to_num(l_im, nan=0.0)        # every pixel masked: the mean of nothing counts as zero
     return loss_weights[0] * l_im + loss_weights[1] * l_depth, radius
 
 
 def tracking_loss(params, frame, render, sil_thres=0.99, loss_weights=(0.5, 1.0), fused=False, max_rendered=None,
-                  keep=None):
+                  keep=None, motion=None):
     """SplaTAM get_loss(tracking=True, use_sil_for_loss=True, use_l1=True): only the camera pose of frame
     `frame["id"]` gets gradient; L1 sums over pixels with silhouette > sil_thres and valid depth
     (R/scripts/splatam.py:220-224,254-288; weights R/configs/replica/splatam.py:65-68).  `keep`: a dict that receives
-    the unweighted depth L1 sum as "depth" (the reference's losses['depth'])."""
+    the unweighted depth L1 sum as "depth" (the reference's losses['depth']).
+    motion: None, or dict(cfg (dynamic.config), exclude (bool [H,W] buffer), refresh (bool, or a device bool [1])):
+    where `refresh` holds, `exclude` is first replaced by dynamic | inconsistent of this render's motion masks
+    (dynamic.masks); the loss then leaves out the `exclude` pixels."""
     im, depth_sil, radius, _ = _render_pair(params, frame, render, fused, camera_grad=True, max_rendered=max_rendered)
+    kept = None
+    if motion is not None:
+        from . import dynamic
+        refresh = motion["refresh"]
+        if isinstance(refresh, torch.Tensor) or refresh:
+            dyn, inc, _ = dynamic.masks(depth_sil.detach(), frame["depth"], motion["cfg"], sil_thres, fused)
+            new = dyn | inc
+            motion["exclude"].copy_(torch.where(refresh, new, motion["exclude"]) if isinstance(refresh, torch.Tensor)
+                                    else new)
+        kept = ~motion["exclude"]
     if fused:
         from .train_ops import masked_l1
         l_depth, l_im = masked_l1(depth_sil, frame["depth"], im, frame["im"], sil_thres=sil_thres, use_sil=True,
-                                  depth_mean=False)
+                                  depth_mean=False, keep=kept)
     else:
         depth, sil = depth_sil[0:1], depth_sil[1]
         uncertainty = (depth_sil[2:3] - depth ** 2).detach()
         mask = (frame["depth"] > 0) & (~torch.isnan(depth)) & (~torch.isnan(uncertainty)) & (sil > sil_thres)
+        if kept is not None:
+            mask = mask & kept
         mask = mask.detach()
         # boolean indexing, as the reference: a NaN depth under a cleared mask bit must not reach the sum
         l_depth = torch.abs(frame["depth"] - depth)[mask].sum()
@@ -291,7 +322,7 @@ def tracking_loss(params, frame, render, sil_thres=0.99, loss_weights=(0.5, 1.0)
 
 
 def track_frame(params, frame, render=None, num_iters=40, lr_rot=0.0004, lr_trans=0.002, fused=None, graph=None,
-                depth_loss_thres=None, lr_exposure=None):
+                depth_loss_thres=None, lr_exposure=None, dynamic=None):
     """SplaTAM's tracking inner loop for one frame (R/scripts/splatam.py:676-744): Adam on the frame's camera
     quaternion and translation only, keeping the best-loss pose.  `params` holds detached Gaussian tensors and
     cam_unnorm_rots [1,4,T] / cam_trans [1,3,T] leaf tensors.  Returns the list of per-iteration losses.
@@ -303,7 +334,9 @@ def track_frame(params, frame, render=None, num_iters=40, lr_rot=0.0004, lr_tran
     one per iteration (`_TrackingGraph`); None = re-use a cached graph, build one only for loops of >= 100 iterations.
     lr_exposure: None, or (lr_log_gain, lr_bias): column t of params["cam_exposure"] [1,6,T] (the frame's colour
     correction, `frame_exposure`) is optimised with the pose, its log-gains and biases as two more Adam groups of these
-    rates, and the best-loss record keeps it together with the pose."""
+    rates, and the best-loss record keeps it together with the pose.
+    dynamic: None, or a dynamic.config dict: at iterations i % refresh_every == 0 the frame's motion mask is recomputed
+    from that iteration's render, and the loss leaves out its pixels (tracking_loss's `motion`)."""
     render = default_render if render is None else render
     if fused is None:
         fused = params["means3D"].is_cuda and render is default_render
@@ -313,7 +346,7 @@ def track_frame(params, frame, render=None, num_iters=40, lr_rot=0.0004, lr_tran
         # per frame) or on request (graph=True: tracking-only runs over a map that stays put).  Building costs about as
         # much as ~40 eager iterations (capacity probe, warm-up, capture into a fresh memory pool).
         out = _track_frame_graphed(params, frame, num_iters, lr_rot, lr_trans, build=(graph is True or num_iters >= 100),
-                                   depth_loss_thres=depth_loss_thres, lr_exposure=lr_exposure)
+                                   depth_loss_thres=depth_loss_thres, lr_exposure=lr_exposure, dynamic=dynamic)
         if out is not None:
             return out              # None: no graph, or the instance capacity overflowed mid-frame -> run eagerly
     rots, trans = params["cam_unnorm_rots"], params["cam_trans"]
@@ -327,11 +360,17 @@ def track_frame(params, frame, render=None, num_iters=40, lr_rot=0.0004, lr_tran
     opt = torch.optim.Adam(groups, lr=0.0, eps=1e-15)
     best, best_rot, best_tran, best_ab, losses = None, None, None, None, []
     keep = None if depth_loss_thres is None else {}
+    motion = None
+    if dynamic is not None:
+        motion = dict(cfg=dynamic, exclude=torch.zeros(frame["depth"].shape[-2:], dtype=torch.bool,
+                                                        device=frame["depth"].device))
     total = num_iters
     while len(losses) < total:
         opt.zero_grad(set_to_none=True)
         fr = frame if lr_exposure is None else dict(frame, exposure=torch.cat([gain, bias], 1).reshape(6))
-        loss, _ = tracking_loss(params, fr, render, fused=fused, keep=keep)
+        if motion is not None:
+            motion["refresh"] = len(losses) % dynamic["refresh_every"] == 0
+        loss, _ = tracking_loss(params, fr, render, fused=fused, keep=keep, motion=motion)
         loss.backward()
         opt.step()
         with torch.no_grad():
@@ -372,12 +411,15 @@ class _CapturedStep:
         self.cap = int(capacity)
         self.frame = dict(id=frame["id"], cam=frame["cam"], w2c=frame["w2c"].clone(), im=frame["im"].clone(),
                           depth=frame["depth"].clone())
+        if frame.get("dynamic") is not None:      # the keyframes' motion masks (run_slam's `dynamic`)
+            self.frame["dynamic"] = frame["dynamic"].clone()
         self.side = torch.cuda.Stream(self.dev)
         self.side.wait_stream(torch.cuda.current_stream(self.dev))      # for state a caller creates on it before capture
 
     def load(self, frame):
-        for k in ("im", "depth", "w2c"):
-            self.frame[k].copy_(frame[k], non_blocking=True)
+        for k in ("im", "depth", "w2c", "dynamic"):
+            if k in self.frame:
+                self.frame[k].copy_(frame[k], non_blocking=True)
 
     def overflow(self):
         """int32 [1] device view of the overflow flag of the latest sync-free render: inside the step, its own."""
@@ -416,7 +458,8 @@ class _TrackingGraph:
     With `lr_exposure` the frame's colour correction travels the same way, as two [1,3] leaves (log-gains, biases)
     with two more capturable Adam groups and a best-loss record of their own."""
 
-    def __init__(self, params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres=None, lr_exposure=None):
+    def __init__(self, params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres=None, lr_exposure=None,
+                 dynamic=None):
         t = frame["id"]
         rots, trans = params["cam_unnorm_rots"], params["cam_trans"]
         self.gp = gp = {k: params[k].detach() for k in GAUSSIAN_KEYS}        # keeps the storage the graph reads alive
@@ -446,6 +489,10 @@ class _TrackingGraph:
             self.it = torch.zeros(1, dtype=torch.long, device=dev)
             self.bad_any = torch.zeros(1, device=dev)
             self.live = torch.ones(1, dtype=torch.bool, device=dev)   # rule only: this replay is a real iteration
+            self.motion = None
+            if dynamic is not None:       # the mask is computed every replay and kept where it % refresh_every == 0
+                self.motion = dict(cfg=dynamic, exclude=torch.zeros(frame["depth"].shape[-2:], dtype=torch.bool,
+                                                                    device=dev))
 
         def body():
             for leaf in leaves:
@@ -454,7 +501,10 @@ class _TrackingGraph:
             fr = dict(step.frame, pose=camera_w2c(q, tr))
             if expo:
                 fr["exposure"] = torch.cat([self.gain, self.bias], 1).reshape(6)
-            loss, _ = tracking_loss(gp, fr, default_render, fused=True, max_rendered=step.cap, keep=keep)
+            if self.motion is not None:
+                self.motion["refresh"] = self.it % self.motion["cfg"]["refresh_every"] == 0
+            loss, _ = tracking_loss(gp, fr, default_render, fused=True, max_rendered=step.cap, keep=keep,
+                                    motion=self.motion)
             loss.backward()
             lossd = loss.detach().reshape(1)
             bad = (step.overflow() != 0) | ~torch.isfinite(lossd)
@@ -520,21 +570,22 @@ class _TrackingGraph:
 _TRACK_GRAPHS = {}
 
 
-def _tracking_key(params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres, lr_exposure=None):
+def _tracking_key(params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres, lr_exposure=None, dynamic=None):
     """What a captured tracking iteration is bound to: the storage (pointer and shape) of each Gaussian tensor it
-    reads, the camera, the image shape, the iteration count, the learning rates (the exposure rates included) and the
-    depth-loss rule."""
+    reads, the camera, the image shape, the iteration count, the learning rates (the exposure rates included), the
+    depth-loss rule and the motion-mask options."""
     return (tuple((params[k].data_ptr(), tuple(params[k].shape)) for k in GAUSSIAN_KEYS), id(frame["cam"]),
             tuple(frame["im"].shape), num_iters, lr_rot, lr_trans, depth_loss_thres,
-            None if lr_exposure is None else tuple(float(r) for r in lr_exposure))
+            None if lr_exposure is None else tuple(float(r) for r in lr_exposure),
+            None if dynamic is None else tuple(sorted(dynamic.items())))
 
 
 def _track_frame_graphed(params, frame, num_iters, lr_rot, lr_trans, build=True, depth_loss_thres=None,
-                         lr_exposure=None):
+                         lr_exposure=None, dynamic=None):
     """Graph-replayed tracking of one frame, or None when no graph is available / an iteration overflowed the instance
     capacity (the caller then runs the frame eagerly).  Graphs are cached per `_tracking_key`; `build` creates one on
     a miss (worth it for long loops or when the map stays put)."""
-    key = _tracking_key(params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres, lr_exposure)
+    key = _tracking_key(params, frame, num_iters, lr_rot, lr_trans, depth_loss_thres, lr_exposure, dynamic)
     tg = _TRACK_GRAPHS.get(key)
     if tg is None:
         if not build:
@@ -542,7 +593,8 @@ def _track_frame_graphed(params, frame, num_iters, lr_rot, lr_trans, build=True,
         if len(_TRACK_GRAPHS) >= 2:
             _TRACK_GRAPHS.clear()
         tg = _TRACK_GRAPHS[key] = _TrackingGraph(params, frame, num_iters, lr_rot, lr_trans,
-                                                 depth_loss_thres=depth_loss_thres, lr_exposure=lr_exposure)
+                                                 depth_loss_thres=depth_loss_thres, lr_exposure=lr_exposure,
+                                                 dynamic=dynamic)
     return tg.run(params, frame)
 
 
@@ -893,10 +945,12 @@ class ShardedMapper:
         with torch.no_grad():
             loop.deform_gaussians(p["means3D"], p["unnorm_rotations"], self.timestep.contiguous(), table, flag)
 
-    def add_new_gaussians(self, frame, time_idx, intrinsics, sil_thres):
+    def add_new_gaussians(self, frame, time_idx, intrinsics, sil_thres, exclude=None):
         """add_new_gaussians of the reference (R/scripts/splatam.py:378-420): one depth/silhouette render of the
         current map at the frame's estimated pose, non-presence mask, back-projection of the selected pixels,
-        append with `timestep` = time_idx (splatam.py:417-418).  CUDA only.  Returns the number of Gaussians added."""
+        append with `timestep` = time_idx (splatam.py:417-418).  CUDA only.  Returns the number of Gaussians added.
+        exclude: a bool mask (the frame's motion mask, max-pooled to the frame's size when that differs) whose pixels
+        grow nothing."""
         from . import map_ops
         p = self.params()
         with torch.no_grad():
@@ -906,8 +960,11 @@ class ShardedMapper:
             if "cam_exposure" in p:         # the new Gaussians take the frame's colour in frame 0's appearance
                 from .train_ops import exposure
                 frame = dict(frame, im=exposure(frame["im"], p["cam_exposure"][0, :, time_idx], inverse=True))
+        if exclude is not None:
+            from .dynamic import footprint
+            exclude = footprint(exclude, frame["depth"].shape[-2:])
         new, n = map_ops.new_gaussians_from_frame(depth_sil, frame, intrinsics, curr_w2c, sil_thres,
-                                                  scale_dim=self._widths()[4])
+                                                  scale_dim=self._widths()[4], exclude=exclude)
         if n:
             self.add_gaussians(new, timestep=time_idx)
         return n

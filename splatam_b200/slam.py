@@ -100,7 +100,7 @@ def exposure_config(exposure):
     return {k: float(v) for k, v in cfg.items()}
 
 
-def _run_state(mapper, counts, keyframes=None, pose_graph=None, reloc_frames=None):
+def _run_state(mapper, counts, keyframes=None, pose_graph=None, reloc_frames=None, masks=None):
     """The sidecar of a checkpoint (formats.save_checkpoint's `run_state`): what continues a run exactly and the
     reference's params{t}.npz cannot carry -- the mapper's own state (ShardedMapper.run_state: the Gaussians'
     `timestep`, its schedule and device generators, the densification statistic), torch's CPU RNG and the CUDA RNG of
@@ -109,7 +109,9 @@ def _run_state(mapper, counts, keyframes=None, pose_graph=None, reloc_frames=Non
     refinement) also their stored est_w2c, which the refined camera columns no longer give; with `pose_graph` (runs
     with loop closure) also its edges and their measurements (loop.PoseGraph.state); with `reloc_frames` (runs with
     relocalisation: (lost ids, relocalised ids)) `reloc_lost` and `reloc_relocalised`; with a `cam_exposure` in the
-    mapper's cameras (runs with exposure) also that table [1,6,T].  Numeric arrays only."""
+    mapper's cameras (runs with exposure) also that table [1,6,T]; with `masks` (runs with motion masks: the
+    keyframes' bool [H,W] masks) `keyframe_dynamic`, np.packbits of their [K,H,W] stack, and `keyframe_dynamic_shape`.
+    Numeric arrays only."""
     dev = mapper.g.flat.device
     _, keys, pos, has_gauss, cached = np.random.get_state()
     st = dict(mapper.run_state(), torch_rng=torch.get_rng_state().numpy(),
@@ -127,7 +129,22 @@ def _run_state(mapper, counts, keyframes=None, pose_graph=None, reloc_frames=Non
         st["reloc_relocalised"] = np.array(sorted(reloc_frames[1]), dtype=np.int64)
     if "cam_exposure" in mapper.cam:
         st["cam_exposure"] = mapper.cam["cam_exposure"].detach().float().cpu().numpy()
+    if masks is not None:
+        m = torch.stack(masks).cpu().numpy()
+        st["keyframe_dynamic"] = np.packbits(m.reshape(-1))
+        st["keyframe_dynamic_shape"] = np.array(m.shape, dtype=np.int64)
     return st
+
+
+def _keyframe_masks(state, n):
+    """The keyframes' motion masks of a checkpoint's sidecar (_run_state's `masks`): a list of n bool [H,W] arrays."""
+    if state is None or "keyframe_dynamic" not in state:
+        raise ValueError("dynamic: the checkpoint holds no keyframe motion masks (it was written by a run without them)")
+    shape = tuple(int(x) for x in np.asarray(state["keyframe_dynamic_shape"]).reshape(-1))
+    if len(shape) != 3 or shape[0] != n:
+        raise ValueError("the checkpoint's motion masks have shape %s for %d keyframes" % (shape, n))
+    bits = np.unpackbits(np.asarray(state["keyframe_dynamic"], dtype=np.uint8))[:int(np.prod(shape))]
+    return list(bits.reshape(shape).astype(bool))
 
 
 def _restore_run_state(mapper, st):
@@ -168,7 +185,7 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
              scene_radius=None, select_keyframes=False, checkpoint_dir=None, first_frame_iters=0, map_every=None,
              graph=False, timing=None, densify_dict=None, tracking_lrs=(0.0004, 0.002), depth_loss_thres=None,
              checkpoint_every=None, resume=None, mapping_cam_lrs=(0.0, 0.0), pose_init="constant_velocity",
-             loop_closure=None, relocalise=None, exposure=None):
+             loop_closure=None, relocalise=None, exposure=None, dynamic=None):
     """Tracks every frame and maps on keyframes.  gauss_init: dict of the five Gaussian tensors (the map's
     starting point); frames: list of dict(id, cam, w2c, im, depth).  Returns dict(rots, trans, psnr, gauss, counts,
     timestep, keyframe_time_indices, keyframe_est_w2c): `timestep` is the frame that created each Gaussian of the final
@@ -235,6 +252,15 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
     RGB render by column t - 1; the final PSNR is of the corrected renders.  The result holds `exposure` [1,6,T] and
     checkpoints hold the table in their sidecar (not in params{t}.npz); resuming with `exposure` from a checkpoint
     without it raises ValueError, and so does `exposure` together with `relocalise`.
+    `dynamic`: None (the default: off, and nothing of it runs) or a dict of dynamic.DEFAULTS keys.  Each tracked frame
+    gets a motion mask from the residual between its depth and the map's depth render (dynamic.py states the rule):
+    tracking leaves out the `dynamic | inconsistent` pixels, recomputing them every `refresh_every` iterations from that
+    iteration's render (track_frame's `dynamic`); after tracking, one render at the pose of record gives the frame's
+    masks; its keyframe stores `dynamic`, which mapping leaves out of its loss and `add_new_gaussians` out of map
+    growth (max-pooled to the densification frame's size for SplaTAM-S).  Frame 0 has an empty mask.  The result holds
+    `dynamic`: per tracked frame dict(frame, scale, dynamic_frac, inconsistent_frac), read from the device once at the
+    end; checkpoints hold the keyframes' masks in their sidecar, and `dynamic` together with `relocalise` raises
+    ValueError.
 
     Checkpoints and resume (R/scripts/splatam.py:604-643,927-931).  With `checkpoint_dir` and `checkpoint_every` = N,
     after frame t's mapping and keyframe step, for every t % N == 0 (frame 0 included, after `first_frame_iters`),
@@ -269,6 +295,14 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
         if resume is not None and (resume["state"] is None or "cam_exposure" not in resume["state"]):
             raise ValueError("exposure: the checkpoint holds no exposure table (it was written by a run without it)")
         lr_expo = (expo_cfg["lr_log_gain"], expo_cfg["lr_bias"])
+    use_dyn = dynamic is not None
+    if use_dyn:
+        from . import dynamic as _dynamic
+        dyn_cfg = _dynamic.config(dynamic)
+        if relocalise is not None:
+            raise ValueError("dynamic and relocalise cannot be combined: relocalisation's health check does not use the "
+                             "motion mask")
+        dyn_stats = []
     use_icp = pose_init != "constant_velocity"
     if use_icp:
         if intrinsics is None:
@@ -313,6 +347,8 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
         keyframes = [dict(_without_densify(frames[0]), est_w2c=torch.eye(4, device=dev))]
         counts = [mapper.g.shapes["means3D"][0]]
         start = 1
+        if use_dyn:
+            keyframes[0]["dynamic"] = torch.zeros(frames[0]["depth"].shape[-2:], dtype=torch.bool, device=dev)
     else:
         dev = resume["gauss"]["means3D"].device
         rots = resume["cam_unnorm_rots"].detach().clone().to(dev)
@@ -330,6 +366,9 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
             counts = [mapper.g.shapes["means3D"][0]]
         start = int(resume["time_idx"]) + 1
         first_frame_iters = 0
+        if use_dyn:
+            for kf, m in zip(keyframes, _keyframe_masks(resume["state"], len(keyframes))):
+                kf["dynamic"] = torch.from_numpy(m).to(dev)
     if use_loop:
         st = resume["state"] if resume is not None else None
         if st is not None and "loop_graph_edges" in st:
@@ -353,7 +392,8 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
                                 [kf["id"] for kf in keyframes],
                                 _run_state(mapper, counts, keyframes if (refine or use_loop) else None,
                                            pose_graph if use_loop else None,
-                                           (reloc_lost, reloc_done) if use_reloc else None))
+                                           (reloc_lost, reloc_done) if use_reloc else None,
+                                           [kf["dynamic"] for kf in keyframes] if use_dyn else None))
 
     def refined_cameras():
         """Refinement: copies of the mapper's cameras after a mapping phase (tracking then works on its own tensors)."""
@@ -395,7 +435,7 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
         t0 = time.perf_counter()
         losses = M.track_frame(params, frames[t], render=render, num_iters=tracking_iters, lr_rot=tracking_lrs[0],
                                lr_trans=tracking_lrs[1], fused=fused, depth_loss_thres=depth_loss_thres,
-                               lr_exposure=lr_expo if use_expo else None)
+                               lr_exposure=lr_expo if use_expo else None, dynamic=dyn_cfg if use_dyn else None)
         torch.cuda.synchronize(dev) if dev.type == "cuda" else None
         timing["tracking_s"] += time.perf_counter() - t0
         timing["tracking_iters"] += len(losses)
@@ -447,12 +487,24 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
             torch.cuda.synchronize(dev)
             timing["loop_closure_s"] += time.perf_counter() - t0
         cur = dict(_without_densify(frame), est_w2c=_curr_w2c(rots, trans, t))
+        grow_kw = {}
+        if use_dyn:       # the frame's masks at its pose of record: identical on every rank (same replica, same kernels)
+            now = dict({k: v.detach() for k, v in mapper.g.params.items()}, cam_unnorm_rots=rots, cam_trans=trans,
+                       **({"cam_exposure": mapper.cam["cam_exposure"]} if use_expo else {}))
+            trk_fused = (dev.type == "cuda" and render is None) if fused is None else bool(fused)
+            with torch.no_grad():
+                _, depth_sil, _, _ = M._render_pair(now, frame, render or M.default_render, trk_fused,
+                                                    camera_grad=False)
+                dyn_now, _, st_now = _dynamic.masks(depth_sil, frame["depth"], dyn_cfg, 0.99, trk_fused)
+            cur["dynamic"] = dyn_now.clone()
+            grow_kw = dict(exclude=cur["dynamic"])
+            dyn_stats.append(st_now)
         if t % map_every == 0:
             if add_new_gaussians:
                 if "densify" in frame:            # SplaTAM-S: grow the map from the densification-size frame
-                    mapper.add_new_gaussians(frame["densify"], t, frame["densify"]["intrinsics"], sil_thres)
+                    mapper.add_new_gaussians(frame["densify"], t, frame["densify"]["intrinsics"], sil_thres, **grow_kw)
                 else:
-                    mapper.add_new_gaussians(frame, t, intrinsics, sil_thres)
+                    mapper.add_new_gaussians(frame, t, intrinsics, sil_thres, **grow_kw)
             if select_keyframes:
                 from .keyframes import keyframe_selection_overlap
                 if mapper.world > 1:      # the selection draws from the global RNGs: every rank must draw the same
@@ -510,6 +562,12 @@ def run_slam(gauss_init, frames, cam, render=None, tracking_iters=20, mapping_it
                keyframe_est_w2c=[kf["est_w2c"] for kf in keyframes])
     if use_expo:
         out["exposure"] = mapper.cam["cam_exposure"].detach().clone()
+    if use_dyn:
+        st = torch.stack(dyn_stats).cpu().numpy() if dyn_stats else np.zeros((0, _dynamic.STATS), np.float32)
+        npx = float(frames[0]["depth"].shape[-2] * frames[0]["depth"].shape[-1])
+        out["dynamic"] = [dict(frame=start + i, scale=float(s[1]), dynamic_frac=float(s[4]) / npx,
+                               inconsistent_frac=float(s[5]) / npx) for i, s in enumerate(st)]
+        out["keyframe_dynamic"] = [kf["dynamic"] for kf in keyframes]
     if use_icp:
         st = torch.stack(icp_stats).cpu().numpy() if icp_stats else np.zeros((0, icp.STATS))
         out["icp"] = [dict(frame=start + i, accepted=bool(s[0]), inlier_frac=float(s[1]), rms=float(s[2]),

@@ -71,37 +71,52 @@ class FusedAdam:
 
 class _ImageLoss(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, y, w_l1, w_ssim):
+    def forward(ctx, x, y, w_l1, w_ssim, keep):
         x, y = x.contiguous().float(), y.contiguous().float()
         C, H, W = x.shape
         dev = x.device
         work = torch.empty(_lib.load().sb_image_loss_workspace_floats(C, H, W), dtype=torch.float32, device=dev)
-        sums = torch.empty(2, dtype=torch.float64, device=dev)
-        _lib.call("sb_image_loss_forward", x, y, C, H, W, work, sums, device=dev)
-        n = float(C * H * W)
-        ctx.save_for_backward(x, y, work)
+        if keep is None:
+            sums = torch.empty(2, dtype=torch.float64, device=dev)
+            _lib.call("sb_image_loss_forward", x, y, C, H, W, work, sums, device=dev)
+            n = float(C * H * W)
+        else:
+            keep = keep.contiguous().view(torch.uint8)
+            sums = torch.empty(3, dtype=torch.float64, device=dev)
+            _lib.call("sb_image_loss_keep_forward", keep, x, y, C, H, W, work, sums, device=dev)
+            n = C * sums[2].clamp(min=1.0)      # a keyframe whose every pixel is masked contributes zero, not 0/0
+        ctx.save_for_backward(x, y, work, sums, *([] if keep is None else [keep]))
         ctx.w = (float(w_l1), float(w_ssim))
-        return (w_l1 * sums[1] / n + w_ssim * (1.0 - sums[0] / n)).float()
+        ssim_term = w_ssim * (1.0 - sums[0] / n)
+        if keep is not None:          # nothing kept: no SSIM term either (x 1.0 leaves the bits of a non-empty set)
+            ssim_term = ssim_term * (sums[2] > 0)
+        return (w_l1 * sums[1] / n + ssim_term).float()
 
     @staticmethod
     def backward(ctx, grad_out):
-        x, y, work = ctx.saved_tensors
+        x, y, work, sums, *keep = ctx.saved_tensors
         C, H, W = x.shape
         gx = torch.empty_like(x)
         go = grad_out.contiguous().float().reshape(1)
-        _lib.call("sb_image_loss_backward", x, y, C, H, W, work, go, ctx.w[1], ctx.w[0], gx, device=x.device)
-        return gx, None, None, None
+        if keep:
+            _lib.call("sb_image_loss_keep_backward", keep[0], x, y, C, H, W, work, sums, go, ctx.w[1], ctx.w[0], gx,
+                      device=x.device)
+        else:
+            _lib.call("sb_image_loss_backward", x, y, C, H, W, work, go, ctx.w[1], ctx.w[0], gx, device=x.device)
+        return gx, None, None, None, None
 
 
-def image_loss(im, gt, w_l1=0.8, w_ssim=0.2):
-    """0.8 * mean|im-gt| + 0.2 * (1 - SSIM(im, gt)) -- SplaTAM's mapping RGB loss (R/scripts/splatam.py:290)."""
+def image_loss(im, gt, w_l1=0.8, w_ssim=0.2, keep=None):
+    """0.8 * mean|im-gt| + 0.2 * (1 - SSIM(im, gt)) -- SplaTAM's mapping RGB loss (R/scripts/splatam.py:290).  With
+    `keep` (bool [H,W]) both means run over the kept pixels only: 0.8 sum keep |im-gt| / (C sum keep) + 0.2 (1 - sum
+    keep SSIM / (C sum keep)); every bit set gives the bits of the call without it."""
     _lib.need_cuda("image_loss", im)
-    return _ImageLoss.apply(im, gt, w_l1, w_ssim)
+    return _ImageLoss.apply(im, gt, w_l1, w_ssim, keep)
 
 
 class _MaskedL1(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, depth_sil, gt_depth, im, gt_im, sil_thres, use_sil, depth_mean):
+    def forward(ctx, depth_sil, gt_depth, im, gt_im, sil_thres, use_sil, depth_mean, keep):
         dev = depth_sil.device
         depth_sil, gt_depth = depth_sil.contiguous().float(), gt_depth.contiguous().float()
         _, H, W = depth_sil.shape
@@ -109,11 +124,18 @@ class _MaskedL1(torch.autograd.Function):
         if have_im:
             im, gt_im = im.contiguous().float(), gt_im.contiguous().float()
         sums = torch.empty(3, dtype=torch.float64, device=dev)
-        _lib.call("sb_masked_l1_forward", depth_sil, gt_depth, im, gt_im, H, W, float(sil_thres), int(use_sil), sums,
-                  device=dev)
+        if keep is None:
+            _lib.call("sb_masked_l1_forward", depth_sil, gt_depth, im, gt_im, H, W, float(sil_thres), int(use_sil),
+                      sums, device=dev)
+        else:
+            keep = keep.contiguous().view(torch.uint8)
+            _lib.call("sb_masked_l1_keep_forward", keep, depth_sil, gt_depth, im, gt_im, H, W, float(sil_thres),
+                      int(use_sil), sums, device=dev)
+        ctx.keep = keep
         ctx.save_for_backward(depth_sil, gt_depth, sums, *([im, gt_im] if have_im else []))
         ctx.cfg = (float(sil_thres), int(use_sil), int(depth_mean), have_im)
-        l_depth = (sums[0] / sums[1] if depth_mean else sums[0]).float()
+        count = sums[1] if keep is None else sums[1].clamp(min=1.0)        # every pixel masked: zero, not 0/0
+        l_depth = (sums[0] / count if depth_mean else sums[0]).float()
         return l_depth, sums[2].float()
 
     @staticmethod
@@ -126,16 +148,21 @@ class _MaskedL1(torch.autograd.Function):
         grad_im = torch.empty_like(im) if have_im else None
         gd = g_depth.contiguous().float().reshape(1)
         gi = g_im.contiguous().float().reshape(1) if have_im else None
-        _lib.call("sb_masked_l1_backward", depth_sil, gt_depth, im, gt_im, H, W, sil_thres, use_sil, depth_mean, sums,
-                  gd, gi, grad_ds, grad_im, device=depth_sil.device)
-        return grad_ds, None, grad_im, None, None, None, None
+        if ctx.keep is None:
+            _lib.call("sb_masked_l1_backward", depth_sil, gt_depth, im, gt_im, H, W, sil_thres, use_sil, depth_mean,
+                      sums, gd, gi, grad_ds, grad_im, device=depth_sil.device)
+        else:
+            _lib.call("sb_masked_l1_keep_backward", ctx.keep, depth_sil, gt_depth, im, gt_im, H, W, sil_thres, use_sil,
+                      depth_mean, sums, gd, gi, grad_ds, grad_im, device=depth_sil.device)
+        return grad_ds, None, grad_im, None, None, None, None, None
 
 
-def masked_l1(depth_sil, gt_depth, im=None, gt_im=None, sil_thres=0.99, use_sil=False, depth_mean=True):
+def masked_l1(depth_sil, gt_depth, im=None, gt_im=None, sil_thres=0.99, use_sil=False, depth_mean=True, keep=None):
     """(loss_depth, loss_im) of SplaTAM's get_loss: validity (and optionally silhouette) masked L1 over the depth
-    channel of the [3,H,W] depth/silhouette/depth^2 render and, if `im` is given, over the RGB image (sum)."""
+    channel of the [3,H,W] depth/silhouette/depth^2 render and, if `im` is given, over the RGB image (sum).  With
+    `keep` (bool [H,W]) only its set pixels count."""
     _lib.need_cuda("masked_l1", depth_sil)
-    return _MaskedL1.apply(depth_sil, gt_depth, im, gt_im, sil_thres, use_sil, depth_mean)
+    return _MaskedL1.apply(depth_sil, gt_depth, im, gt_im, sil_thres, use_sil, depth_mean, keep)
 
 
 class _Exposure(torch.autograd.Function):

@@ -16,7 +16,8 @@ org_width / org_height the tracking size, gt_w2c_all_frames the ARKit poses), wh
 render_record.py open.  --pose-init icp starts each frame's tracking from a point-to-plane ICP alignment of its
 depth with the map's (splatam_b200.icp; default constant_velocity, the reference's guess).  --exposure estimates each
 frame's exposure and white balance while tracking (slam.run_slam's `exposure`) and writes exposure.npz beside
-params.npz.  --capture-only writes the capture without SLAM, as nerfcapture2dataset.py does.  Prints one
+params.npz.  --dynamic keeps each frame's motion mask (moving people, slam.run_slam's `dynamic`) out of tracking,
+mapping and map growth and writes dynamic.npz beside params.npz.  --capture-only writes the capture without SLAM, as nerfcapture2dataset.py does.  Prints one
 JSON line: ATE against the ARKit poses (the reference's Horn-aligned mean), Gaussian count, wall times, frames/s."""
 import argparse
 import json
@@ -38,7 +39,7 @@ SIL_THRES = 0.5
 
 
 def run(packets, frames, out, capture_only=False, device="cuda:0", tracking_iters=None, mapping_iters=None,
-        pose_init="constant_velocity", exposure=False):
+        pose_init="constant_velocity", exposure=False, dynamic=False):
     """The demo over an iterable of CaptureFrame packets; returns the JSON-able result dict."""
     from splatam_b200 import capture, formats, slam
     sys.path.insert(0, os.path.join(ROOT, "tools"))
@@ -71,18 +72,21 @@ def run(packets, frames, out, capture_only=False, device="cuda:0", tracking_iter
                               add_new_gaussians=True, prune_dict=_PRUNE, scene_radius=radius, select_keyframes=True,
                               first_frame_iters=h["mapping_iters"], tracking_lrs=h["tracking_lrs"],
                               depth_loss_thres=h["depth_loss_thres"], pose_init=pose_init,
-                              exposure={} if exposure else None)
+                              exposure={} if exposure else None, dynamic={} if dynamic else None)
             torch.cuda.synchronize(dev)
             est = slam.w2c_list(o["rots"], o["trans"])
             res.update(ate_m=slam.ate_horn(seq.gt_w2c, est), gaussians=int(o["counts"][-1]),
                        tracking_s=timing["tracking_s"], mapping_s=timing["mapping_s"],
-                       tracking_iters=timing["tracking_iters"], pose_init=pose_init, exposure=bool(exposure))
+                       tracking_iters=timing["tracking_iters"], pose_init=pose_init, exposure=bool(exposure),
+                       dynamic=bool(dynamic))
             if pose_init == "icp":
                 res.update(pose_init_s=timing["pose_init_s"], icp_accepted=sum(s["accepted"] for s in o["icp"]))
             formats.save_run_record(out, o["gauss"], o["rots"], o["trans"], o["timestep"], K, seq.w2c, seq.width,
                                     seq.height, seq.gt_w2c, o["keyframe_time_indices"])
             if exposure:
                 formats.save_exposure(out, o["exposure"])
+            if dynamic:
+                formats.save_dynamic(out, o["dynamic"], o["keyframe_time_indices"], o["keyframe_dynamic"])
     torch.cuda.synchronize(dev)
     wall = time.perf_counter() - t0
     res.update(wall_s=wall, frames_per_s=frames / wall, dropped_packets=seq.dropped,
@@ -104,7 +108,11 @@ def main():
                     help="tracking start: the reference's constant-velocity guess, or that guess refined by ICP")
     ap.add_argument("--exposure", action="store_true",
                     help="estimate each frame's exposure and white balance while tracking; writes exposure.npz")
+    ap.add_argument("--dynamic", action="store_true",
+                    help="keep each frame's motion mask out of tracking, mapping and map growth; writes dynamic.npz")
     a = ap.parse_args()
+    if a.dynamic and a.capture_only:
+        ap.error("--dynamic needs SLAM (not --capture-only)")
     if not a.capture_only and a.frames < 5:
         ap.error("SLAM needs at least 5 frames (keyframe_every = frames // 5)")
     from splatam_b200 import capture
@@ -116,7 +124,7 @@ def main():
     else:
         packets = capture.synthetic_frames(a.frames, dev, seed=a.seed)
     res = run(packets, a.frames, a.out, a.capture_only, dev, a.tracking_iters, a.mapping_iters, a.pose_init,
-              a.exposure)
+              a.exposure, a.dynamic)
     res["source"] = a.source
     print(json.dumps(res))
 

@@ -33,6 +33,9 @@ alex.pth, read from disk, never downloaded) add LPIPS to the evaluation: `lpips`
 JSON line and lpips.txt under --out.
 --save-frames (needs --out) also saves the final evaluation's rendered and ground-truth colour and depth PNGs under
 --out (rendered_rgb/, rendered_depth/, rgb/, depth/), and with --nvs those of the novel views under --out/eval_nvs.
+--dynamic (not with --relocalise) gives each frame a motion mask from the map's depth residual and keeps its pixels
+out of tracking, mapping and map growth (slam.run_slam's `dynamic`); the JSON line gains the median and largest
+flagged share of a frame, and --out receives dynamic.npz (formats.save_dynamic: per-frame stats, keyframe masks).
 --checkpoint-every N writes the reference's params{t}.npz / keyframe_time_indices{t}.npy, and a run_state{t}.npz
 sidecar, under --out every N frames; --resume T continues the run from the checkpoint of frame T under --out (one
 written here, or the reference's own, which then continues without the sidecar's RNG states):
@@ -155,10 +158,16 @@ def main():
                     help="estimate each frame's exposure and white balance while tracking, and map and evaluate "
                          "through it (slam.run_slam's `exposure`, its EXPOSURE_DEFAULTS); with --out also writes "
                          "exposure.npz; off by default")
+    ap.add_argument("--dynamic", action="store_true",
+                    help="estimate a motion mask per frame and keep its pixels out of tracking, mapping and map "
+                         "growth (slam.run_slam's `dynamic`, dynamic.DEFAULTS); with --out also writes dynamic.npz; "
+                         "off by default")
     a = ap.parse_args()
     a.relocalise = a.relocalise or a.relocalise_photometric
     if a.exposure and a.relocalise:
         ap.error("--exposure cannot be combined with --relocalise")
+    if a.dynamic and a.relocalise:
+        ap.error("--dynamic cannot be combined with --relocalise")
     if (a.lpips_alexnet is None) != (a.lpips_lin is None):
         ap.error("--lpips-alexnet and --lpips-lin go together")
     if a.checkpoint_every < 0:
@@ -219,7 +228,7 @@ def main():
                         loop_closure={} if a.loop_closure else None,
                         relocalise=((dict(photometric=True) if a.relocalise_photometric else {}) if a.relocalise
                                     else None),
-                        exposure={} if a.exposure else None)
+                        exposure={} if a.exposure else None, dynamic={} if a.dynamic else None)
     torch.cuda.synchronize(dev)
     wall = time.perf_counter() - t0
     # --resume: wall time from reading the checkpoint to the first tracked frame (frame-0 read, load, keyframe rebuild)
@@ -252,11 +261,17 @@ def main():
                                 seq.height, gt_w2c_all, out["keyframe_time_indices"])
         if a.exposure:
             formats.save_exposure(a.out, out["exposure"])
+        if a.dynamic:
+            formats.save_dynamic(a.out, out["dynamic"], out["keyframe_time_indices"], out["keyframe_dynamic"])
+    dyn = {}
+    if a.dynamic:
+        fr = [r["dynamic_frac"] for r in out["dynamic"]]
+        dyn = dict(dynamic_frac_median=float(np.median(fr)) if fr else 0.0, dynamic_frac_max=max(fr, default=0.0))
     print(json.dumps(dict(
         dataset=a.dataset, sequence=a.sequence, variant=a.variant, frames=T, width=seq.width, height=seq.height,
         densify_height=seq.densify_height, densify_width=seq.densify_width, hyper=h,
         initial_gaussians=initial_gaussians, resumed_from=a.resume, resume_s=resume_s,
-        mapping_cam_lrs=list(a.mapping_cam_lrs), pose_init=a.pose_init, exposure=a.exposure,
+        mapping_cam_lrs=list(a.mapping_cam_lrs), pose_init=a.pose_init, exposure=a.exposure, dynamic=a.dynamic, **dyn,
         **({} if a.pose_init == "constant_velocity" else dict(pose_init_s=timing["pose_init_s"],
                                                 icp_accepted=sum(s["accepted"] for s in out["icp"]))),
         **({} if not a.loop_closure else dict(loop_closure_s=timing["loop_closure_s"], loops=out["loops"])),
