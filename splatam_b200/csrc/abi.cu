@@ -35,8 +35,7 @@ GeometryWs carve_geometry(void* ws, int P, size_t* total) {
     g.header = c.take<int32_t>(64);
     g.depth_key = c.take<uint32_t>(n);
     g.tiles_touched = c.take<uint32_t>(n);
-    g.geomA = c.take<float4>(n);
-    g.geomB = c.take<float4>(n);
+    g.geom = c.take<float4>(2 * n);
     g.rect = c.take<uint2>(n);
     g.sorted_key = c.take<uint32_t>(n);
     g.sorted_idx = c.take<uint32_t>(n);
@@ -87,16 +86,18 @@ static int tiles_of(const sb_settings* s) {
 }
 
 // Small helper kernels for the inspection entry points.
-__global__ void export_geometry_kernel(int P, const uint32_t* depth_key, const float4* geomA, const float4* geomB,
+__global__ void export_geometry_kernel(int P, const uint32_t* depth_key, const float4* geom,
                                        const uint32_t* tiles_touched, float* depths, float* means2D,
                                        float* conic_opacity, uint32_t* tt) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P) return;
-    const bool vis = tiles_touched[i] != 0u;
+    const uint32_t n = tiles_touched[i];
+    const bool vis = n != 0u;
     if (depths) depths[i] = vis ? __uint_as_float(depth_key[i]) : 0.f;
-    if (means2D) { means2D[2 * i] = vis ? geomA[i].x : 0.f; means2D[2 * i + 1] = vis ? geomA[i].y : 0.f; }
-    if (conic_opacity) reinterpret_cast<float4*>(conic_opacity)[i] = vis ? geomB[i] : make_float4(0.f, 0.f, 0.f, 0.f);
-    if (tt) tt[i] = tiles_touched[i];
+    if (means2D) { means2D[2 * i] = vis ? geom[2 * i].x : 0.f; means2D[2 * i + 1] = vis ? geom[2 * i].y : 0.f; }
+    if (conic_opacity)
+        reinterpret_cast<float4*>(conic_opacity)[i] = vis ? geom[2 * i + 1] : make_float4(0.f, 0.f, 0.f, 0.f);
+    if (tt) tt[i] = n;
 }
 template <typename KeyT>
 __global__ void export_keys_kernel(int R, const KeyT* tile_sorted, const uint32_t* point_list,
@@ -334,7 +335,7 @@ SB_API int sb_export_geometry(int P, const void* geom_ws, size_t geom_ws_bytes, 
     GeometryWs g = carve_geometry(const_cast<void*>(geom_ws), P, &need);
     if (geom_ws_bytes < need) return SB_ERR_WORKSPACE;
     export_geometry_kernel<<<(P + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        P, g.depth_key, g.geomA, g.geomB, g.tiles_touched, depths, means2D, conic_opacity, tiles_touched);
+        P, g.depth_key, g.geom, g.tiles_touched, depths, means2D, conic_opacity, tiles_touched);
     SB_LAUNCH_CHECK("export_geometry_kernel");
     return SB_OK;
 }

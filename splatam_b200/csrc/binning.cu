@@ -15,26 +15,44 @@ namespace sb {
 
 namespace {
 
+// One warp per 32 consecutive depth-ordered Gaussians.  Their runs of instances are contiguous in the output (the
+// scan's offsets), so the warp walks the span they cover together, lane l writing slots base + l: every store
+// instruction writes 32 consecutive words.  A Gaussian's tile count is the difference of neighbouring offsets, so only
+// the rectangles of Gaussians that touch a tile are gathered (one 8-B entry each).  A slot's Gaussian is the first lane
+// whose run ends after it, found by a 5-step bisection over the lanes' run ends (shuffles); its tile is the slot's
+// index in that run, row-major over the Gaussian's rectangle, as the reference emits them.  Slots at or past `cap`
+// (capacity of the instance arrays in the sync-free mode, else 2^32-1) are not written.
 __global__ void __launch_bounds__(256)
 emit_instances_kernel(int P, const uint32_t* __restrict__ sorted_idx, const uint32_t* __restrict__ offsets,
-                      const uint32_t* __restrict__ tiles_touched, const uint2* __restrict__ rect,
-                      uint32_t grid_x, uint32_t cap, uint32_t* __restrict__ tile_out, uint32_t* __restrict__ val_out) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= P) return;
+                      const uint2* __restrict__ rect, uint32_t grid_x, uint32_t cap, uint32_t* __restrict__ tile_out,
+                      uint32_t* __restrict__ val_out) {
+    const int lane = threadIdx.x & 31;
+    const int i0 = (blockIdx.x * blockDim.x + threadIdx.x) & ~31;
+    if (i0 >= P) return;
+    const int i = min(i0 + lane, P - 1);             // lanes past P repeat the last Gaussian with an empty run
+    const uint32_t end = __ldg(offsets + i);         // inclusive scan: end of this Gaussian's run
+    const uint32_t prev = __shfl_up_sync(0xffffffffu, end, 1);
+    const uint32_t start = lane == 0 ? (i0 == 0 ? 0u : __ldg(offsets + i0 - 1)) : prev;
     const uint32_t g = __ldg(sorted_idx + i);
-    const uint32_t n = __ldg(tiles_touched + g);
-    if (n == 0u) return;
-    uint32_t off = __ldg(offsets + i) - n;  // inclusive scan -> start of this Gaussian's run
-    const uint2 r = __ldg(rect + g);
-    const uint32_t x0 = r.x & 0xFFFFu, y0 = r.x >> 16, x1 = r.y & 0xFFFFu, y1 = r.y >> 16;
-    for (uint32_t y = y0; y < y1; ++y)
-        for (uint32_t x = x0; x < x1; ++x) {
-            if (off < cap) {              // cap = capacity of the instance arrays (sync-free mode), else 2^32-1
-                tile_out[off] = y * grid_x + x;
-                val_out[off] = g;
-            }
-            ++off;
+    const uint2 t = end != start ? __ldg(rect + g) : make_uint2(0u, 0u);
+    const uint32_t span0 = __shfl_sync(0xffffffffu, start, 0);
+    const uint32_t span1 = min(__shfl_sync(0xffffffffu, end, 31), cap);
+    for (uint32_t base = span0; base < span1; base += 32u) {
+        const uint32_t o = base + (uint32_t)lane;
+        int j = 0;
+#pragma unroll
+        for (int step = 16; step > 0; step >>= 1)
+            if (__shfl_sync(0xffffffffu, end, j + step - 1) <= o) j += step;
+        const uint32_t k = o - __shfl_sync(0xffffffffu, start, j);
+        const uint32_t rx = __shfl_sync(0xffffffffu, t.x, j), ry = __shfl_sync(0xffffffffu, t.y, j);
+        const uint32_t gj = __shfl_sync(0xffffffffu, g, j);
+        if (o < span1) {
+            const uint32_t x0 = rx & 0xFFFFu, y0 = rx >> 16, w = (ry & 0xFFFFu) - x0;
+            const uint32_t dy = k / w;
+            tile_out[o] = (y0 + dy) * grid_x + x0 + (k - dy * w);
+            val_out[o] = gj;
         }
+    }
 }
 
 // Coverage mask of one tile instance: bit w is set iff the Gaussian can blend a pixel of consumer warp w's
@@ -99,8 +117,7 @@ __device__ __forceinline__ uint32_t cover_mask(const float4 ga, const float4 gb,
 __global__ void __launch_bounds__(256)
 ranges_and_records_kernel(int R_host, const int32_t* __restrict__ count_dev, const uint32_t* __restrict__ tile_sorted,
                           const uint32_t* __restrict__ point_list, uint32_t grid_x,
-                          const float4* __restrict__ geomA, const float4* __restrict__ geomB,
-                          const float* __restrict__ colors, const float* __restrict__ colors2,
+                          const float4* __restrict__ geom, const float* __restrict__ colors, const float* __restrict__ colors2,
                           uint2* __restrict__ ranges, float4* __restrict__ recA, float4* __restrict__ recB,
                           float4* __restrict__ recC, float4* __restrict__ recD) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -114,7 +131,7 @@ ranges_and_records_kernel(int R_host, const int32_t* __restrict__ count_dev, con
     }
     if (i == R - 1) ranges[tile].y = (uint32_t)R;
     const uint32_t g = __ldg(point_list + i);
-    const float4 ga = __ldg(geomA + g), gb = __ldg(geomB + g);
+    const float4 ga = __ldg(geom + 2 * (size_t)g), gb = __ldg(geom + 2 * (size_t)g + 1);   // one 32-B sector
     recA[i] = make_float4(ga.x, ga.y, __uint_as_float(cover_mask(ga, gb, tile % grid_x, tile / grid_x)), 0.f);
     recB[i] = gb;
     const float* c = colors + 3 * (size_t)g;
@@ -136,8 +153,8 @@ int launch_binning(const sb_settings& s, int P, int R, const float* colors, cons
     if (R <= 0) return SB_OK;
     const int bits = (int)higher_msb((uint32_t)tiles);  // same bit count as the reference sort uses
     { ScopedStage _p(kStEmit, st);
-      emit_instances_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, g.sorted_idx, g.offsets, g.tiles_touched, g.rect,
-                                                             (uint32_t)gx, count_dev ? (uint32_t)R : 0xFFFFFFFFu,
+      emit_instances_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, g.sorted_idx, g.offsets, g.rect, (uint32_t)gx,
+                                                             count_dev ? (uint32_t)R : 0xFFFFFFFFu,
                                                              b.tile_unsorted, b.val_unsorted); }
     SB_LAUNCH_CHECK("emit_instances_kernel");
     { ScopedStage _p(kStTileSort, st);
@@ -148,7 +165,7 @@ int launch_binning(const sb_settings& s, int P, int R, const float* colors, cons
       if (rc != SB_OK) return rc; }
     ScopedStage _p(kStRecords, st);
     ranges_and_records_kernel<<<(R + 255) / 256, 256, 0, st>>>(R, count_dev, b.tile_sorted, b.point_list,
-                                                               (uint32_t)gx, g.geomA, g.geomB, colors, colors2,
+                                                               (uint32_t)gx, g.geom, colors, colors2,
                                                                img.ranges, b.recA, b.recB, b.recC, b.recD);
     SB_LAUNCH_CHECK("ranges_and_records_kernel");
     return SB_OK;

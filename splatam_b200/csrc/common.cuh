@@ -48,19 +48,21 @@ struct Carver {
 };
 
 // ---- per-Gaussian state written by the projection kernel --------------------------------
-// geomA = {pixel x, pixel y, conservative half-extent hx, hy of the contributing ellipse}
-// geomB = {conic.x, conic.y, conic.z, opacity}
-// rect  = {xmin | ymin<<16, xmax | ymax<<16} tile rectangle (getRect, auxiliary.h:46-56)
+// geom[2g]     = geomA = {pixel x, pixel y, conservative half-extent hx, hy of the contributing ellipse}
+// geom[2g + 1] = geomB = {conic.x, conic.y, conic.z, opacity}
+//   one 32-B, 32-B-aligned pair per Gaussian: the record gather reads both halves from one DRAM sector
+// rect = {xmin | ymin<<16, xmax | ymax<<16} tile rectangle (getRect, auxiliary.h:46-56).  Emission takes a Gaussian's
+//   tile count from the scan (offsets[i] - offsets[i-1]), so it gathers only this 8-B entry, and only for Gaussians
+//   that touch a tile; tiles_touched stays a dense 4-B array for the scan's gather.
 struct GeometryWs {
     int32_t*  header;        // [0]=num_rendered  [1]=num_visible  [2]=capacity overflow flag of the sync-free mode (device)
     uint32_t* depth_key;     // [P] float bits of view-space z, kCulledKey if it emits nothing
     uint32_t* tiles_touched; // [P]
-    float4*   geomA;         // [P]
-    float4*   geomB;         // [P]
-    uint2*    rect;          // [P]
+    float4*   geom;          // [2P], written only for Gaussians that touch a tile
+    uint2*    rect;          // [P], written only for Gaussians that touch a tile
     uint32_t* sorted_key;    // [P] depth keys ascending
     uint32_t* sorted_idx;    // [P] Gaussian index in (depth, index) order
-    uint32_t* offsets;       // [P] inclusive scan of tiles_touched in that order
+    uint32_t* offsets;       // [P] inclusive scan of the tile counts in that order
     void*     sort_temp;     // radix_sort.cu scratch (histograms, look-back status, ping-pong pairs)
     size_t    sort_temp_bytes;
     void*     scan_temp;     // CUB inclusive-scan scratch

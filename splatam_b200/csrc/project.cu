@@ -125,8 +125,7 @@ project_kernel(int P,
                float scale_modifier, uint32_t grid_x, uint32_t grid_y, bool prefiltered,
                bool means_al16, bool scales_al16, bool rot_al16,
                int32_t* __restrict__ radii, uint32_t* __restrict__ depth_key,
-               uint32_t* __restrict__ tiles_touched, float4* __restrict__ geomA,
-               float4* __restrict__ geomB, uint2* __restrict__ rect) {
+               uint32_t* __restrict__ tiles_touched, float4* __restrict__ geom, uint2* __restrict__ rect) {
     __shared__ __align__(16) float s_mean[kProjThreads * 3];
     __shared__ __align__(16) float s_scale[kProjThreads * 3];
     __shared__ float s_vm[16], s_pm[16];
@@ -152,8 +151,10 @@ project_kernel(int P,
             // in_frustum(): a culled point with `prefiltered` set traps in the reference (auxiliary.h:156-160).
             if (prefiltered) __trap();
             radii[gidx] = 0;
+#ifndef SB_PROBE_PROJECT_RADII_ONLY
             depth_key[gidx] = kCulledKey;
             tiles_touched[gidx] = 0u;
+#endif
         }
     }
     const uint32_t ball = __ballot_sync(0xffffffffu, front);
@@ -249,12 +250,22 @@ project_kernel(int P,
             }
         }
     }
+#ifdef SB_PROBE_PROJECT_RADII_ONLY
+    {   // tools/stage_bounds.py's variant: every result but the radius stays live (a store that is never taken), so
+        // its time is the arithmetic and the input traffic without the geometry stores
+        const uint32_t h = __float_as_uint(gA.x) ^ __float_as_uint(gA.y) ^ __float_as_uint(gA.z) ^
+                           __float_as_uint(gA.w) ^ __float_as_uint(gB.x) ^ __float_as_uint(gB.y) ^
+                           __float_as_uint(gB.z) ^ __float_as_uint(gB.w) ^ out_rect.x ^ out_rect.y ^ out_key ^ out_tiles;
+        radii[idx] = h == 0x7fc00001u ? -1 : out_radius;
+        return;
+    }
+#endif
     radii[idx] = out_radius;
     depth_key[idx] = out_key;
     tiles_touched[idx] = out_tiles;
-    if (out_tiles != 0u) {          // geomA / geomB / rect are only ever read for Gaussians that touch a tile
-        geomA[idx] = gA;
-        geomB[idx] = gB;
+    if (out_tiles != 0u) {          // geometry and rectangle are only ever read for Gaussians that touch a tile
+        geom[2 * (size_t)idx] = gA;
+        geom[2 * (size_t)idx + 1] = gB;
         rect[idx] = out_rect;
     }
 }
@@ -307,7 +318,7 @@ int launch_project(const sb_settings& s, int P, const float* means3D, const floa
         P, means3D, opacities, scales, reinterpret_cast<const float4*>(rotations), cov3D_precomp,
         s.viewmatrix, s.projmatrix, W, H, s.tanfovx, s.tanfovy, focal_x, focal_y, s.scale_modifier,
         gx, gy, s.prefiltered != 0, al16(means3D), al16(scales), al16(rotations),
-        radii, g.depth_key, g.tiles_touched, g.geomA, g.geomB, g.rect);
+        radii, g.depth_key, g.tiles_touched, g.geom, g.rect);
     SB_LAUNCH_CHECK("project_kernel");
     return SB_OK;
 }
