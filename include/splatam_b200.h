@@ -224,6 +224,22 @@ SB_API int sb_export_binning(const sb_settings* s, int P, int num_rendered,
  *   (16 tx + 8 (w & 1), 16 ty + 4 (w >> 1)) of its tile (tx, ty) -- the only pairs the blend kernels evaluate */
 SB_API int sb_export_cover(const sb_settings* s, int num_rendered, const void* binning_ws, size_t binning_ws_bytes,
                            uint8_t* cover, void* stream);
+/* ---- the rasterizer's radix sort on its own (testing; csrc/radix_sort.cu: the depth sort, the tile sort and the
+ *      mesh-evaluation grid all run it) ---------------------------------------------------------------------------
+ * sb_radix_sort_pairs: stable ascending sort of the n pairs (keys_in[i], vals_in ? vals_in[i] : i) by the key bits
+ *   [begin_bit, end_bit) (8-bit digits, one pass per digit), written to keys_out and vals_out [capacity] (device u32;
+ *   the full keys, not just their sorted bits).  n = capacity, or clamp(*n_dev, 0, capacity) with n_dev (device int32)
+ *   read on the device: the call never synchronises and can be captured in a CUDA graph.  keys_in and vals_in are not
+ *   modified, and nothing is written at or past index n of the outputs.  temp: sb_radix_sort_temp_bytes(capacity,
+ *   end_bit - begin_bit) device bytes, any content; that size never decreases as the capacity grows.
+ * SB_ERR_BAD_ARG, before any launch, for capacity < 0 or >= 2^30, begin_bit < 0, end_bit > 32 and begin_bit >=
+ * end_bit; then SB_OK with nothing launched for capacity 0; then SB_ERR_BAD_ARG for null pointers (NULL vals_in and
+ * n_dev excepted) and an output that is an input or the other output (a pass may write an output while it reads the
+ * inputs); SB_ERR_WORKSPACE for a short temp. */
+SB_API int sb_radix_sort_temp_bytes(int capacity, int bits, size_t* bytes);
+SB_API int sb_radix_sort_pairs(const uint32_t* keys_in, const uint32_t* vals_in, uint32_t* keys_out, uint32_t* vals_out,
+                               int capacity, const int32_t* n_dev, int begin_bit, int end_bit, void* temp,
+                               size_t temp_bytes, void* stream);
 
 /* ---- per-iteration training ops around the rasterizer (SURVEY.md section 8(f) row N3) -----------------
  * sb_adam_step: torch.optim.Adam (no amsgrad / weight decay) over ONE flat parameter buffer whose segments

@@ -149,6 +149,8 @@ _SIGNATURES = {
     "sb_export_binning": (_i, [ctypes.POINTER(SbSettings), _i, _i, _vp, _sz, _vp, _sz, _vp, _sz,
                                _vp, _vp, _vp, _vp, _vp, _vp]),
     "sb_export_cover": (_i, [ctypes.POINTER(SbSettings), _i, _vp, _sz, _vp, _vp]),
+    "sb_radix_sort_temp_bytes": (_i, [_i, _i, ctypes.POINTER(_sz)]),
+    "sb_radix_sort_pairs": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _vp, _sz, _vp]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 

@@ -380,6 +380,27 @@ SB_API int sb_export_cover(const sb_settings* s, int num_rendered, const void* b
     return SB_OK;
 }
 
+SB_API int sb_radix_sort_temp_bytes(int capacity, int bits, size_t* bytes) {
+    if (!bytes || capacity < 0 || capacity >= (1 << 30) || bits < 1 || bits > 32) return SB_ERR_BAD_ARG;
+    *bytes = radix_temp_bytes(capacity, bits);
+    return SB_OK;
+}
+
+SB_API int sb_radix_sort_pairs(const uint32_t* keys_in, const uint32_t* vals_in, uint32_t* keys_out, uint32_t* vals_out,
+                               int capacity, const int32_t* n_dev, int begin_bit, int end_bit, void* temp,
+                               size_t temp_bytes, void* stream) {
+    if (capacity < 0 || capacity >= (1 << 30) || begin_bit < 0 || end_bit > 32 || begin_bit >= end_bit)
+        return SB_ERR_BAD_ARG;
+    if (capacity == 0) return SB_OK;
+    if (!keys_in || !keys_out || !vals_out || !temp) return SB_ERR_BAD_ARG;
+    // a pass may write an output while it reads the inputs, so no output may be an input or the other output
+    if (keys_out == keys_in || vals_out == keys_in || keys_out == vals_out ||
+        (vals_in && (keys_out == vals_in || vals_out == vals_in)))
+        return SB_ERR_BAD_ARG;
+    return radix_sort_pairs(keys_in, vals_in, keys_out, vals_out, capacity, n_dev, begin_bit, end_bit, temp, temp_bytes,
+                            static_cast<cudaStream_t>(stream));
+}
+
 SB_API int sb_profile_begin(void) {
     for (auto& r : g_prof) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
     g_prof.clear();

@@ -55,8 +55,14 @@ RadixTemp radix_layout(void* temp, int capacity, int passes) {
     t.tiles = (capacity + kTileItems - 1) / kTileItems;
     t.hist = c.take<uint32_t>((size_t)kMaxPasses * kBins);
     t.tickets = c.take<uint32_t>(64);
-    t.status = c.take<uint32_t>((size_t)passes * (size_t)(t.tiles > 0 ? t.tiles : 1) * kBins);
+    const int live_tiles = t.tiles > 0 ? t.tiles : 1;
+    t.status = c.take<uint32_t>((size_t)passes * (size_t)live_tiles * kBins);
     t.zero_bytes = c.used();
+    // Past kSmallSortLimit the tiles double in size, so the status words of the tiles in use halve.  Reserve (without
+    // zeroing) up to the small-tile count at the limit, so the temp size never decreases as the capacity grows and a
+    // temp sized for one capacity serves every smaller one.
+    const int reserve_tiles = capacity > kSmallSortLimit ? kSmallSortLimit / (kSortThreads * kItemsSmall) : 0;
+    if (reserve_tiles > live_tiles) c.take<uint32_t>((size_t)passes * (size_t)(reserve_tiles - live_tiles) * kBins);
     t.pk = c.take<uint32_t>((size_t)(capacity > 0 ? capacity : 1));
     t.pv = c.take<uint32_t>((size_t)(capacity > 0 ? capacity : 1));
     t.bytes = c.used();
