@@ -1,5 +1,5 @@
-// radix_sort.cu -- hand-written stable LSD radix sort of (u32 key, u32 value) pairs, 8-bit digits, one kernel per
-// digit pass with decoupled look-back ("onesweep"), for sm_90a.
+// radix_sort.cu -- hand-written stable LSD radix sort of (u32 key, u32 value) pairs, 8-bit digits, three kernels per
+// digit pass (reduce-then-scan), for sm_90a.
 //
 // Where the reference calls cub::DeviceRadixSort::SortPairs on 64-bit (tile | depth) keys over num_rendered pairs
 // (X/cuda_rasterizer/rasterizer_impl.cu:304-309), this repo orders the P Gaussians by their 32 depth bits once
@@ -11,15 +11,19 @@
 //     written or read;
 //   * the input keys are never modified (the depth keys are re-used by the blend and by the key export).
 //
-// Structure of a pass (one CTA = 256 threads x 16 keys = one 4096-key tile, tiles ticketed in launch order):
-//   1. warp-striped coalesced key loads; per-warp stable ranking with __match_any_sync (all lanes holding the same
-//      digit find each other, the lowest lane bumps the warp's bin counter in shared memory);
-//   2. per digit: exclusive prefix over the 8 warps, tile total;
-//   3. per digit (one thread each): decoupled look-back over the predecessor tiles' status words
-//      {2-bit flag | 30-bit count}: publish AGGREGATE, sum predecessors until an INCLUSIVE one, publish INCLUSIVE;
-//   4. keys and values are first scattered inside shared memory into their tile-local sorted order, then written
-//      to global memory in runs (one run per digit), so the global writes are coalesced.
-// A single up-front kernel builds the digit histograms of all passes (global bin bases).
+// A pass over sort tiles of 256 threads x 16 keys (4096 keys; 2048 up to 64K pairs):
+//   1. upsweep: one CTA per tile counts the tile's digits (shared-memory atomics into one histogram per warp) and
+//      writes counts[digit][tile], every entry of a live tile, so nothing is zeroed;
+//   2. scan: one CTA per digit turns its row into the exclusive prefix over the tiles and writes the digit's total;
+//   3. downsweep: one CTA per tile ranks its keys stably (warp-striped coalesced loads; per-warp ranking: the lanes
+//      holding the same digit find each other by one ballot per digit bit, the lowest lane bumps the warp's bin
+//      counter in shared memory), scatters keys and values into their tile-local sorted order in shared memory and
+//      writes them to global memory in runs (one run per digit), so the global writes are coalesced.  A digit's
+//      global base is the exclusive prefix of the digit totals plus its scanned count for this tile.
+// No CTA waits on another, so a pass is deterministic and does not depend on the order CTAs are scheduled in.  The
+// single-kernel pass with decoupled look-back that this replaces made every tile wait on a chain of predecessor tiles'
+// status words (DESIGN.md section 5).
+// Grids are sized by the capacity; every kernel derives the live tile count from n (a device-side count allowed).
 #include "radix_sort.cuh"
 #include "common.cuh"
 
@@ -33,70 +37,83 @@ constexpr int kSortWarps = kSortThreads / 32;
 constexpr int kItemsLarge = 16, kItemsSmall = 8;       // keys per thread: 4096- or 2048-key tiles
 constexpr int kSmallSortLimit = 64 << 10;              // tiny inputs only: 2048-key tiles lose to 4096-key tiles at 1M keys
 constexpr int kMaxPasses = 4;
-constexpr uint32_t kFlagAgg = 1u << 30, kFlagInc = 2u << 30, kValMask = (1u << 30) - 1u;
 
 struct RadixTemp {
-    uint32_t* hist;      // [kMaxPasses][kBins]
-    uint32_t* tickets;   // [64] (one per pass)
-    uint32_t* status;    // [passes][tiles][kBins]
+    uint32_t* totals;    // [kBins] keys per digit
+    uint32_t* counts;    // [kBins][stride]: per-tile digit counts, scanned in place into per-tile digit bases
     uint32_t* pk;        // ping-pong keys   [capacity]
     uint32_t* pv;        // ping-pong values [capacity]
-    size_t zero_bytes;   // hist + tickets + status are contiguous and zeroed per sort
     size_t bytes;
-    int tiles;
+    int tiles, stride;
 };
 
 inline int tile_items_for(int capacity) { return kSortThreads * (capacity <= kSmallSortLimit ? kItemsSmall : kItemsLarge); }
 
-RadixTemp radix_layout(void* temp, int capacity, int passes) {
+RadixTemp radix_layout(void* temp, int capacity) {
     RadixTemp t;
     Carver c(temp);
     const int kTileItems = tile_items_for(capacity);
     t.tiles = (capacity + kTileItems - 1) / kTileItems;
-    t.hist = c.take<uint32_t>((size_t)kMaxPasses * kBins);
-    t.tickets = c.take<uint32_t>(64);
-    const int live_tiles = t.tiles > 0 ? t.tiles : 1;
-    t.status = c.take<uint32_t>((size_t)passes * (size_t)live_tiles * kBins);
-    t.zero_bytes = c.used();
-    // Past kSmallSortLimit the tiles double in size, so the status words of the tiles in use halve.  Reserve (without
-    // zeroing) up to the small-tile count at the limit, so the temp size never decreases as the capacity grows and a
-    // temp sized for one capacity serves every smaller one.
-    const int reserve_tiles = capacity > kSmallSortLimit ? kSmallSortLimit / (kSortThreads * kItemsSmall) : 0;
-    if (reserve_tiles > live_tiles) c.take<uint32_t>((size_t)passes * (size_t)(reserve_tiles - live_tiles) * kBins);
+    // Past kSmallSortLimit the tiles double in size, so the tiles in use halve.  Reserve count columns up to the
+    // small-tile count at the limit, so the temp size never decreases as the capacity grows and a temp sized for one
+    // capacity serves every smaller one.
+    const int reserve_tiles = capacity > kSmallSortLimit ? kSmallSortLimit / (kSortThreads * kItemsSmall) : 1;
+    t.stride = ((t.tiles > reserve_tiles ? t.tiles : reserve_tiles) + 3) & ~3;   // 16-B aligned rows
+    t.totals = c.take<uint32_t>(kBins);
+    t.counts = c.take<uint32_t>((size_t)kBins * (size_t)t.stride);
     t.pk = c.take<uint32_t>((size_t)(capacity > 0 ? capacity : 1));
     t.pv = c.take<uint32_t>((size_t)(capacity > 0 ? capacity : 1));
     t.bytes = c.used();
     return t;
 }
 
-__device__ __forceinline__ uint32_t ld_relaxed(const uint32_t* p) {
-    uint32_t v;
-    asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_relaxed(uint32_t* p, uint32_t v) {
-    asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+__device__ __forceinline__ int live_count(int capacity, const int32_t* n_dev) {
+    return n_dev ? min(*n_dev, capacity) : capacity;
 }
 
-__global__ void __launch_bounds__(256)
-radix_hist_kernel(const uint32_t* __restrict__ keys, int capacity, const int32_t* __restrict__ n_dev, int begin_bit,
-                  int end_bit, int passes, uint32_t* __restrict__ hist) {
-    __shared__ uint32_t sh[kMaxPasses][kBins];
-    for (int i = threadIdx.x; i < kMaxPasses * kBins; i += blockDim.x) (&sh[0][0])[i] = 0u;
-    __syncthreads();
-    const int n = n_dev ? min(*n_dev, capacity) : capacity;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const uint32_t key = __ldg(keys + i);
-        for (int p = 0; p < passes; ++p) {
-            const int lo = begin_bit + 8 * p, width = min(8, end_bit - lo);
-            atomicAdd(&sh[p][(key >> lo) & ((1u << width) - 1u)], 1u);
-        }
+// The lanes of the warp holding the same digit d (mask = the digit's bits): one ballot per digit bit.  The hardware
+// match instruction (__match_any_sync) costs more the more distinct values a warp holds; on random 8-bit digits it
+// made the ranking the longest part of a pass (DESIGN.md section 5).
+__device__ __forceinline__ uint32_t match_digit(uint32_t d, uint32_t mask) {
+    uint32_t peers = 0xffffffffu;
+#pragma unroll
+    for (int b = 0; b < 8; ++b) {
+        if (!((mask >> b) & 1u)) break;   // mask is 2^width - 1, the same in every lane
+        const bool set = (d >> b) & 1u;
+        const uint32_t bal = __ballot_sync(0xffffffffu, set);
+        peers &= set ? bal : ~bal;
     }
+    return peers;
+}
+
+template <int kItems>
+__global__ void __launch_bounds__(kSortThreads)
+radix_upsweep_kernel(const uint32_t* __restrict__ keys_in, int capacity, const int32_t* __restrict__ n_dev, int shift,
+                     uint32_t mask, int stride, uint32_t* __restrict__ counts) {
+    constexpr int kTileItems = kSortThreads * kItems;
+    __shared__ uint32_t s_hist[kSortWarps][kBins];
+    const int tid = threadIdx.x;
+    const int n = live_count(capacity, n_dev);
+    const long long tile_base = (long long)blockIdx.x * kTileItems;
+    if (tile_base >= n) return;
+    const int valid = (int)min((long long)kTileItems, (long long)n - tile_base);
+    for (int i = tid; i < kSortWarps * kBins; i += kSortThreads) (&s_hist[0][0])[i] = 0u;
     __syncthreads();
-    for (int i = threadIdx.x; i < passes * kBins; i += blockDim.x) {
-        const uint32_t v = (&sh[0][0])[i];
-        if (v) atomicAdd(hist + i, v);
+    uint32_t k[kItems];
+#pragma unroll
+    for (int j = 0; j < kItems; ++j) {
+        const int li = j * kSortThreads + tid;
+        k[j] = li < valid ? __ldg(keys_in + tile_base + li) : 0u;
     }
+    uint32_t* const h = s_hist[tid >> 5];   // one histogram per warp: only lanes of one warp contend for a bin
+#pragma unroll
+    for (int j = 0; j < kItems; ++j)
+        if (j * kSortThreads + tid < valid) atomicAdd(&h[(k[j] >> shift) & mask], 1u);
+    __syncthreads();
+    uint32_t c = 0;
+#pragma unroll
+    for (int w = 0; w < kSortWarps; ++w) c += s_hist[w][tid];
+    counts[(size_t)tid * stride + blockIdx.x] = c;
 }
 
 // Exclusive prefix of one value per thread over the 256 threads of the CTA.
@@ -117,12 +134,46 @@ __device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t v, uint32_t* s
     return base + inc - v;
 }
 
+// Row d = blockIdx.x of counts (the live tiles' counts of digit d) -> its exclusive prefix; totals[d] = the row's sum.
+// Each thread takes 4 consecutive tiles per round (one 16-B load: rows start 16-B aligned), 1024 tiles per round.
+__global__ void __launch_bounds__(kSortThreads)
+radix_scan_kernel(int capacity, const int32_t* __restrict__ n_dev, int tile_items, int stride,
+                  uint32_t* __restrict__ counts, uint32_t* __restrict__ totals) {
+    __shared__ uint32_t s_scan[kSortWarps];
+    const int tid = threadIdx.x;
+    const int n = live_count(capacity, n_dev);
+    const int tiles = n > 0 ? (int)(((long long)n + tile_items - 1) / tile_items) : 0;
+    uint32_t* const row = counts + (size_t)blockIdx.x * stride;
+    uint32_t carry = 0;
+    for (int t0 = 0; t0 < tiles; t0 += 4 * kSortThreads) {
+        const int first = t0 + 4 * tid;
+        uint4 v = make_uint4(0u, 0u, 0u, 0u);
+        if (first < tiles) {   // first + 3 < stride: the stride is a multiple of 4
+            v = *reinterpret_cast<const uint4*>(row + first);
+            if (first + 1 >= tiles) v.y = 0u;
+            if (first + 2 >= tiles) v.z = 0u;
+            if (first + 3 >= tiles) v.w = 0u;
+        }
+        const uint32_t sum = v.x + v.y + v.z + v.w;
+        const uint32_t excl = carry + block_exclusive_scan(sum, s_scan);
+        if (first < tiles) row[first] = excl;
+        if (first + 1 < tiles) row[first + 1] = excl + v.x;
+        if (first + 2 < tiles) row[first + 2] = excl + v.x + v.y;
+        if (first + 3 < tiles) row[first + 3] = excl + v.x + v.y + v.z;
+        if (tid == kSortThreads - 1) s_scan[0] = excl + sum;
+        __syncthreads();
+        carry = s_scan[0];
+        __syncthreads();
+    }
+    if (tid == 0) totals[blockIdx.x] = carry;
+}
+
 template <bool IOTA, int kItems>
 __global__ void __launch_bounds__(kSortThreads)
-radix_onesweep_kernel(const uint32_t* __restrict__ keys_in, const uint32_t* __restrict__ vals_in,
-                      uint32_t* __restrict__ keys_out, uint32_t* __restrict__ vals_out, int capacity,
-                      const int32_t* __restrict__ n_dev, int shift, uint32_t mask, const uint32_t* __restrict__ hist,
-                      uint32_t* __restrict__ ticket, uint32_t* __restrict__ status) {
+radix_downsweep_kernel(const uint32_t* __restrict__ keys_in, const uint32_t* __restrict__ vals_in,
+                       uint32_t* __restrict__ keys_out, uint32_t* __restrict__ vals_out, int capacity,
+                       const int32_t* __restrict__ n_dev, int shift, uint32_t mask, int stride,
+                       const uint32_t* __restrict__ counts, const uint32_t* __restrict__ totals) {
     constexpr int kTileItems = kSortThreads * kItems;
     __shared__ uint32_t s_keys[kTileItems];
     __shared__ uint32_t s_vals[kTileItems];
@@ -130,16 +181,16 @@ radix_onesweep_kernel(const uint32_t* __restrict__ keys_in, const uint32_t* __re
     __shared__ uint32_t s_tile_excl[kBins];
     __shared__ uint32_t s_gbase[kBins];
     __shared__ uint32_t s_scan[kSortWarps];
-    __shared__ uint32_t s_tile;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int n = n_dev ? min(*n_dev, capacity) : capacity;
-    if (tid == 0) s_tile = atomicAdd(ticket, 1u);
+    const int n = live_count(capacity, n_dev);
+    const long long tile_base = (long long)blockIdx.x * kTileItems;
+    if (tile_base >= n) return;
+    const int valid = (int)min((long long)kTileItems, (long long)n - tile_base);
+    // this tile's base of digit tid among the keys of that digit, and the digit's total (both from the scan)
+    const uint32_t digit_base = __ldg(counts + (size_t)tid * stride + blockIdx.x);
+    const uint32_t digit_total = __ldg(totals + tid);
     for (int i = tid; i < kSortWarps * kBins; i += kSortThreads) (&s_whist[0][0])[i] = 0u;
     __syncthreads();
-    const uint32_t tile = s_tile;
-    const long long tile_base = (long long)tile * kTileItems;
-    if (tile_base >= n) return;                      // tickets beyond the live range (device-side n)
-    const int valid = (int)min((long long)kTileItems, (long long)n - tile_base);
 
     // 1. load + rank.  Element order inside the tile is (warp, round, lane), i.e. the global index order.
     uint32_t keys[kItems];
@@ -155,7 +206,7 @@ radix_onesweep_kernel(const uint32_t* __restrict__ keys_in, const uint32_t* __re
 #pragma unroll
     for (int j = 0; j < kItems; ++j) {
         const uint32_t d = (keys[j] >> shift) & mask;
-        const uint32_t peers = __match_any_sync(0xffffffffu, d);
+        const uint32_t peers = match_digit(d, mask);
         const int leader = __ffs(peers) - 1;
         uint32_t base = 0;
         if (lane == leader) { base = whist[d]; whist[d] = base + __popc(peers); }
@@ -165,49 +216,17 @@ radix_onesweep_kernel(const uint32_t* __restrict__ keys_in, const uint32_t* __re
     }
     __syncthreads();
 
-    // 2. per digit (thread d): exclusive prefix over the warps, tile total
+    // 2. per digit (thread d): exclusive prefix over the warps, tile total; global base of the digit in this tile
     uint32_t count = 0;
 #pragma unroll
     for (int w = 0; w < kSortWarps; ++w) { const uint32_t c = s_whist[w][tid]; s_whist[w][tid] = count; count += c; }
-
-    // 3. decoupled look-back: number of keys with this digit in all predecessor tiles
-    uint32_t* const my = status + (size_t)tile * kBins + tid;
-    uint32_t prev = 0;
-    if (tile == 0) {
-        st_relaxed(my, kFlagInc | count);
-    } else {
-        st_relaxed(my, kFlagAgg | count);
-        // walk back over the predecessors, kLook status words in flight at a time (the loads are independent, so their
-        // L2 latencies overlap; a strictly serial walk costs one round trip per predecessor tile)
-        constexpr int kLook = 8;
-        long long t = (long long)tile - 1;
-        bool done = false;
-        while (t >= 0 && !done) {
-            const int nb = (int)min((long long)kLook, t + 1);
-            uint32_t sw[kLook];
-#pragma unroll
-            for (int i = 0; i < kLook; ++i)
-                sw[i] = i < nb ? ld_relaxed(status + (size_t)(t - i) * kBins + tid) : 0u;
-#pragma unroll
-            for (int i = 0; i < kLook; ++i) {
-                if (i < nb && !done) {
-                    uint32_t sv = sw[i];
-                    while ((sv >> 30) == 0u) sv = ld_relaxed(status + (size_t)(t - i) * kBins + tid);
-                    prev += sv & kValMask;
-                    done = (sv >> 30) == 2u;
-                }
-            }
-            t -= nb;
-        }
-        st_relaxed(my, kFlagInc | (prev + count));
-    }
     const uint32_t tile_excl = block_exclusive_scan(count, s_scan);
-    const uint32_t hist_excl = block_exclusive_scan(__ldg(hist + tid), s_scan);
+    const uint32_t digit_excl = block_exclusive_scan(digit_total, s_scan);
     s_tile_excl[tid] = tile_excl;
-    s_gbase[tid] = hist_excl + prev - tile_excl;     // global position = s_gbase[digit] + tile-local position
+    s_gbase[tid] = digit_excl + digit_base - tile_excl;   // global position = s_gbase[digit] + tile-local position
     __syncthreads();
 
-    // 4. tile-local scatter in shared memory, then run-wise coalesced global writes
+    // 3. tile-local scatter in shared memory, then run-wise coalesced global writes
 #pragma unroll
     for (int j = 0; j < kItems; ++j) {
         const uint32_t d = (keys[j] >> shift) & mask;
@@ -228,8 +247,8 @@ radix_onesweep_kernel(const uint32_t* __restrict__ keys_in, const uint32_t* __re
 }  // namespace
 
 size_t radix_temp_bytes(int capacity, int bits) {
-    const int passes = (bits + 7) / 8;
-    return radix_layout(nullptr, capacity, passes < 1 ? 1 : passes).bytes;
+    (void)bits;   // the count matrix is re-used by every pass
+    return radix_layout(nullptr, capacity).bytes;
 }
 
 int radix_sort_pairs(const uint32_t* keys_in, const uint32_t* vals_in, uint32_t* keys_out, uint32_t* vals_out,
@@ -239,12 +258,9 @@ int radix_sort_pairs(const uint32_t* keys_in, const uint32_t* vals_in, uint32_t*
     const int passes = (end_bit - begin_bit + 7) / 8;
     if (passes < 1 || passes > kMaxPasses || begin_bit < 0 || end_bit > 32 || capacity >= (1 << 30) || !temp)
         return SB_ERR_BAD_ARG;
-    RadixTemp t = radix_layout(temp, capacity, passes);
+    RadixTemp t = radix_layout(temp, capacity);
     if (temp_bytes < t.bytes) return SB_ERR_WORKSPACE;
-    SB_CUDA_CHECK(cudaMemsetAsync(temp, 0, t.zero_bytes, st));
-    const int hist_blocks = min((capacity + 4 * 256 - 1) / (4 * 256), 132 * 8);   // 132 SMs x 8
-    radix_hist_kernel<<<hist_blocks, 256, 0, st>>>(keys_in, capacity, n_dev, begin_bit, end_bit, passes, t.hist);
-    SB_LAUNCH_CHECK("radix_hist_kernel");
+    const bool small = capacity <= kSmallSortLimit;
     const uint32_t* src_k = keys_in;
     const uint32_t* src_v = vals_in;
     for (int p = 0; p < passes; ++p) {
@@ -254,18 +270,23 @@ int radix_sort_pairs(const uint32_t* keys_in, const uint32_t* vals_in, uint32_t*
         uint32_t* dst_v = to_out ? vals_out : t.pv;
         const int lo = begin_bit + 8 * p, width = min(8, end_bit - lo);
         const uint32_t mask = (1u << width) - 1u;
-        uint32_t* status = t.status + (size_t)p * (size_t)t.tiles * kBins;
+        if (small) radix_upsweep_kernel<kItemsSmall><<<t.tiles, kSortThreads, 0, st>>>(src_k, capacity, n_dev, lo, mask, t.stride, t.counts);
+        else radix_upsweep_kernel<kItemsLarge><<<t.tiles, kSortThreads, 0, st>>>(src_k, capacity, n_dev, lo, mask, t.stride, t.counts);
+        SB_LAUNCH_CHECK("radix_upsweep_kernel");
+        radix_scan_kernel<<<kBins, kSortThreads, 0, st>>>(capacity, n_dev, tile_items_for(capacity), t.stride, t.counts,
+                                                            t.totals);
+        SB_LAUNCH_CHECK("radix_scan_kernel");
 #define SB_SORT_PASS(IOTA, ITEMS)                                                                                   \
-        radix_onesweep_kernel<IOTA, ITEMS><<<t.tiles, kSortThreads, 0, st>>>(src_k, IOTA ? nullptr : src_v, dst_k, dst_v,  \
-                                                                             capacity, n_dev, lo, mask, t.hist + p * kBins, \
-                                                                             t.tickets + p, status)
-        const bool iota = (p == 0 && vals_in == nullptr), small = capacity <= kSmallSortLimit;
+        radix_downsweep_kernel<IOTA, ITEMS><<<t.tiles, kSortThreads, 0, st>>>(src_k, IOTA ? nullptr : src_v, dst_k,    \
+                                                                              dst_v, capacity, n_dev, lo, mask,         \
+                                                                              t.stride, t.counts, t.totals)
+        const bool iota = (p == 0 && vals_in == nullptr);
         if (iota && small) SB_SORT_PASS(true, kItemsSmall);
         else if (iota) SB_SORT_PASS(true, kItemsLarge);
         else if (small) SB_SORT_PASS(false, kItemsSmall);
         else SB_SORT_PASS(false, kItemsLarge);
 #undef SB_SORT_PASS
-        SB_LAUNCH_CHECK("radix_onesweep_kernel");
+        SB_LAUNCH_CHECK("radix_downsweep_kernel");
         src_k = dst_k;
         src_v = dst_v;
     }

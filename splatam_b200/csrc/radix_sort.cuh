@@ -8,9 +8,9 @@
 
 namespace sb {
 
-// Scratch for one sort of up to `capacity` pairs over `bits` key bits (8-bit digits): digit histograms, tile tickets,
-// the decoupled look-back status words of every pass, and one ping-pong pair buffer.  Never decreases as the capacity
-// grows, so a temp sized for one capacity serves every smaller one.
+// Scratch for one sort of up to `capacity` pairs over `bits` key bits (8-bit digits): the per-tile digit counts that
+// every pass re-uses, the digit totals, and one ping-pong pair buffer.  Never decreases as the capacity grows, so a
+// temp sized for one capacity serves every smaller one.
 size_t radix_temp_bytes(int capacity, int bits);
 
 // Stable ascending sort of the n pairs (keys_in[i], vals_in ? vals_in[i] : i) by key bits [begin_bit, end_bit).
