@@ -22,9 +22,10 @@
 //                               back into the matrix.  A lane never spends an iteration on a Gaussian that
 //                               does not cover its pixel: 1.8-2.0x fewer iterations than a warp-lock-stepped walk
 //                               on the 1M-Gaussian bench (tools/lane_window_model.py);
-//   reduce   (lane = Gaussian, two lanes per slot): sweep the slot's 32 pixels, accumulate the nine moment
-//                               sums in registers at full lane utilisation, and flush them with three
-//                               16-byte vector reductions (REDG.E.ADD.F32x4) per (warp, Gaussian).
+//   reduce   (lane = Gaussian, two lanes per slot): sweep the slot's 32 pixels, accumulate raw moments in
+//                               pixel coordinates local to the rectangle and the colour sums in registers at full
+//                               lane utilisation, shift the moments to the Gaussian's centre once per slot, and
+//                               flush them with 16-byte vector reductions (REDG.E.ADD.F32x4) per (warp, Gaussian).
 #include "common.cuh"
 #include "pipeline.cuh"
 
@@ -79,6 +80,51 @@ __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float 
                  : "memory");
 }
 
+// Takes the first slot left in `rest` (bit 31 - s stands for slot s) out of it and returns s, or -1 when `rest` is
+// empty: bfind.shiftamt (SASS FLO.U32.SH) is the leading-zero count, 0xffffffff for 0, and shr.b32 clamps its shift,
+// so the empty case needs no branch.
+__device__ __forceinline__ int pop_slot(uint32_t& rest) {
+    uint32_t s, bit;
+    asm("bfind.shiftamt.u32 %0, %1;" : "=r"(s) : "r"(rest));
+    asm("shr.b32 %0, 0x80000000, %1;" : "=r"(bit) : "r"(s));
+    rest ^= bit;
+    return (int)s;
+}
+
+// Phase timing of the instrumented build (tools/blend_phases.py compiles this file with -DSB_PROBE_BLEND_PHASES;
+// the shipped library has none of it).  Every consumer warp sums clock64() deltas per phase and adds them to
+// g_probe_cycles at its end; each CTA leaves its %globaltimer start and end in g_probe_cta_ns.
+enum ProbePhase { kPhWait, kPhGather, kPhEvaluate, kPhChain, kPhReduce, kNumPhases };
+#ifdef SB_PROBE_BLEND_PHASES
+constexpr int kProbeMaxTiles = 1 << 16;
+__device__ unsigned long long g_probe_cycles[kNumPhases];
+__device__ unsigned long long g_probe_cta_ns[2][kProbeMaxTiles];
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+struct PhaseClock {
+    long long t, acc[kNumPhases];
+    __device__ __forceinline__ void start() {
+        for (int p = 0; p < kNumPhases; ++p) acc[p] = 0;
+        t = clock64();
+    }
+    __device__ __forceinline__ void lap(int p) { const long long n = clock64(); acc[p] += n - t; t = n; }
+    __device__ __forceinline__ void flush(int lane, uint32_t tile) {
+        if (lane != 0) return;
+        for (int p = 0; p < kNumPhases; ++p) atomicAdd(&g_probe_cycles[p], (unsigned long long)acc[p]);
+        if (tile < kProbeMaxTiles) atomicMax(&g_probe_cta_ns[1][tile], globaltimer_ns());
+    }
+};
+#else
+struct PhaseClock {
+    __device__ __forceinline__ void start() {}
+    __device__ __forceinline__ void lap(int) {}
+    __device__ __forceinline__ void flush(int, uint32_t) {}
+};
+#endif
+
 // Per-pixel running state of the back-to-front walk (one lane = one pixel).
 template <int NCH>
 struct PixelState {
@@ -96,10 +142,11 @@ __device__ __forceinline__ void process_window(BwdSmem<NCH, KW>& sm, const int w
                                                const float4 dLa, const float4 dLb, const float T_final,
                                                const float bg_dot, const float bg_dot1, PixelState<NCH>& st,
                                                const float fx0, const float fy0, const float ddelx_dx,
-                                               const float ddely_dy, float* __restrict__ accum) {
+                                               const float ddely_dy, float* __restrict__ accum, PhaseClock& clk) {
     constexpr uint32_t full = 0xffffffffu;
     constexpr int kStride = NCH == 6 ? kAccumStride2 : kAccumStride;
     __syncwarp();
+    clk.lap(kPhGather);
     Cell* const qcol = &sm.q[warp][0][lane];          // this pixel's column, row stride kRow cells
     float* const q3col = &sm.q3[NCH == 6 ? warp : 0][0][lane];
 
@@ -139,44 +186,57 @@ __device__ __forceinline__ void process_window(BwdSmem<NCH, KW>& sm, const int w
         wa = wa_n; q = q_n; col = col_n; ex = ex_n;
     }
 
+    clk.lap(kPhEvaluate);
+
     // ---- chain: each lane walks its own contributors, deepest first (slot order = back to front) ----
+    //      A lane whose contributors are used up steps on an all-zero cell, so the step needs no branch: alpha = 0
+    //      gives ir = 1 exactly (fast_rcp(1) = 1), so T does not change; A (and A1) take the deeper contributor's
+    //      term one step early and then add 0 * 0, which is the value the next contributor would have computed,
+    //      bit for bit (A is never -0: it starts at +0 and a sum of two terms is -0 only if both are).  Only the
+    //      stores are predicated.
     const int iters = (int)__reduce_max_sync(full, (uint32_t)__popc(mymask));
     {
+        uint32_t rest = __brev(mymask);
         // the next contributor's cell is loaded before this one's chain step (hides the shared-memory latency)
-        int so = (mymask != 0u ? __ffs(mymask) - 1 : 0) * kRow;
-        Cell v = qcol[so];
-        float v3 = NCH == 6 ? q3col[so] : 0.f;
+        int s = pop_slot(rest);
+        Cell v = make_float2(0.f, 0.f);
+        float v3 = 0.f;
+        if (s >= 0) {
+            v = qcol[s * kRow];
+            if constexpr (NCH == 6) v3 = q3col[s * kRow];
+        }
         for (int it = 0; it < iters; ++it) {
-            const bool on = mymask != 0u;
-            mymask &= mymask - 1u;
-            const int so_n = (mymask != 0u ? __ffs(mymask) - 1 : 0) * kRow;
-            const Cell v_n = qcol[so_n];
-            const float v3_n = NCH == 6 ? q3col[so_n] : 0.f;
-            if (on) {
-                const float Gop = v.x, cd = v.y;
-                const float alpha = fminf(Gop, 0.99f);
-                const float ir = fast_rcp(1.f - alpha);
-                st.T = st.T * ir;                                     // T = T / (1 - alpha)
-                const float ca = alpha * st.T;                        // dchannel_dcolor
-                const float om = 1.f - st.last_alpha;
-                st.A = fmaf(st.last_alpha, st.last_cd, om * st.A);
-                const float tb = T_final * ir;
-                const float dL_dalpha = fmaf(cd - st.A, st.T, -tb * bg_dot);
-                st.last_cd = cd;
-                if constexpr (NCH == 6) {
-                    const float cd1 = v3;
-                    st.A1 = fmaf(st.last_alpha, st.last_cd1, om * st.A1);
-                    const float dL_dalpha1 = fmaf(cd1 - st.A1, st.T, -tb * bg_dot1);
-                    st.last_cd1 = cd1;
-                    q3col[so] = Gop * dL_dalpha1;
-                }
-                qcol[so] = make_float2(Gop * dL_dalpha, ca);
-                st.last_alpha = alpha;
+            const int s_n = pop_slot(rest);
+            Cell v_n = make_float2(0.f, 0.f);
+            float v3_n = 0.f;
+            if (s_n >= 0) {
+                v_n = qcol[s_n * kRow];
+                if constexpr (NCH == 6) v3_n = q3col[s_n * kRow];
             }
-            so = so_n; v = v_n; v3 = v3_n;
+            const float Gop = v.x, cd = v.y;
+            const float alpha = fminf(Gop, 0.99f);
+            const float ir = fast_rcp(1.f - alpha);
+            st.T = st.T * ir;                                     // T = T / (1 - alpha)
+            const float ca = alpha * st.T;                        // dchannel_dcolor
+            const float om = 1.f - st.last_alpha;
+            st.A = fmaf(st.last_alpha, st.last_cd, om * st.A);
+            const float tb = T_final * ir;
+            const float dL_dalpha = fmaf(cd - st.A, st.T, -tb * bg_dot);
+            st.last_cd = cd;
+            if constexpr (NCH == 6) {
+                const float cd1 = v3;
+                st.A1 = fmaf(st.last_alpha, st.last_cd1, om * st.A1);
+                const float dL_dalpha1 = fmaf(cd1 - st.A1, st.T, -tb * bg_dot1);
+                st.last_cd1 = cd1;
+                if (s >= 0) q3col[s * kRow] = Gop * dL_dalpha1;
+            }
+            if (s >= 0) qcol[s * kRow] = make_float2(Gop * dL_dalpha, ca);
+            st.last_alpha = alpha;
+            s = s_n; v = v_n; v3 = v3_n;
         }
     }
     __syncwarp();
+    clk.lap(kPhChain);
 
     // ---- reduce: lanes (sl, part) = (lane & 15, lane >> 4) sweep pixels [16 part, 16 part + 16) of slot
     //      16 round + sl ----
@@ -190,25 +250,47 @@ __device__ __forceinline__ void process_window(BwdSmem<NCH, KW>& sm, const int w
         const float gxr = wa.x - fx0, gyr = (wa.y - fy0) - (float)(2 * part);
         const Cell* qrow = &sm.q[warp][sc][16 * part];
         const float4* dl = &sm.dL[warp][0][16 * part];
-        float Sw = 0.f, Swx = 0.f, Swy = 0.f, Sxx = 0.f, Sxy = 0.f, Syy = 0.f, C0 = 0.f, C1 = 0.f, C2 = 0.f;
-        float E0 = 0.f, E1 = 0.f, E2 = 0.f, Rx = 0.f, Ry = 0.f;   // NCH == 6 only
+        // Raw moments in pixel coordinates local to the half-rectangle (8x2 pixels) and centred on its middle:
+        // lx = px - 3.5 in [-3.5, 3.5] is a constant of the unrolled row sweep and ly = py - 0.5 = -+0.5 one of the
+        // row, so a pixel costs one add and two FMAs with immediates for all six moment sums (ly^2 = 1/4 makes
+        // sum w ly^2 = Sw / 4, and sum w lx ly is taken per row).  The row loop stays rolled: unrolling both rows
+        // lets the compiler hoist all 16 pixels' loads and spills at <3,16,3>'s 72-register budget.
+        float Sw = 0.f, Sx = 0.f, Sy = 0.f, Sxyl = 0.f, XX = 0.f, C0 = 0.f, C1 = 0.f, C2 = 0.f;
+        float E0 = 0.f, E1 = 0.f, E2 = 0.f, Rw = 0.f, Rly = 0.f, RX = 0.f;   // NCH == 6 only
+#pragma unroll 1
+        for (int row = 0; row < 2; ++row) {
+            const float ly = (float)row - 0.5f;
+            float W = 0.f, X = 0.f, Wr = 0.f;
 #pragma unroll
-        for (int it = 0; it < 16; ++it) {
-            const Cell v = qrow[it];
-            const float4 d = dl[it];
-            const float w = v.x, ca = v.y;
-            const float dx = gxr - (float)(it & 7), dy = gyr - (float)(it >> 3);
-            const float wdx = w * dx, wdy = w * dy;
-            Sw += w; Swx += wdx; Swy += wdy;
-            Sxx = fmaf(wdx, dx, Sxx); Sxy = fmaf(wdx, dy, Sxy); Syy = fmaf(wdy, dy, Syy);
-            C0 = fmaf(ca, d.x, C0); C1 = fmaf(ca, d.y, C1); C2 = fmaf(ca, d.z, C2);
-            if constexpr (NCH == 6) {
-                const float wr = sm.q3[NCH == 6 ? warp : 0][NCH == 6 ? sc : 0][16 * part + it];
-                const float4 d2 = sm.dL[warp][NCH == 6 ? 1 : 0][16 * part + it];
-                Rx = fmaf(wr, dx, Rx); Ry = fmaf(wr, dy, Ry);
-                E0 = fmaf(ca, d2.x, E0); E1 = fmaf(ca, d2.y, E1); E2 = fmaf(ca, d2.z, E2);
+            for (int i = 0; i < 8; ++i) {
+                const int it = 8 * row + i;
+                const Cell v = qrow[it];
+                const float4 d = dl[it];
+                const float w = v.x, ca = v.y;
+                const float lx = (float)i - 3.5f;
+                W += w; X = fmaf(w, lx, X); XX = fmaf(w, lx * lx, XX);
+                C0 = fmaf(ca, d.x, C0); C1 = fmaf(ca, d.y, C1); C2 = fmaf(ca, d.z, C2);
+                if constexpr (NCH == 6) {
+                    const float wr = sm.q3[NCH == 6 ? warp : 0][NCH == 6 ? sc : 0][16 * part + it];
+                    const float4 d2 = sm.dL[warp][NCH == 6 ? 1 : 0][16 * part + it];
+                    Wr += wr; RX = fmaf(wr, lx, RX);
+                    E0 = fmaf(ca, d2.x, E0); E1 = fmaf(ca, d2.y, E1); E2 = fmaf(ca, d2.z, E2);
+                }
             }
+            Sw += W; Sy = fmaf(ly, W, Sy); Sx += X; Sxyl = fmaf(ly, X, Sxyl);
+            if constexpr (NCH == 6) { Rw += Wr; Rly = fmaf(ly, Wr, Rly); }
         }
+        // Moments about the Gaussian's centre (gx, gy) in the same frame, dx = gx - lx, dy = gy - ly.  Shifting the
+        // raw moments cancels terms of size gx^2 Sw, with |gx| <= 3.5 + the splat's reach past the rectangle; the
+        // rounding error is a few ulps of gx^2 Sw, against the ulps of the per-pixel sums it replaces.  Centring
+        // the local frame (rather than taking the corner pixel as 0) keeps gx small when the centre is inside.
+        const float gx = gxr - 3.5f, gy = gyr - 0.5f;
+        float Swx = fmaf(gx, Sw, -Sx), Swy = fmaf(gy, Sw, -Sy);
+        float Sxx = fmaf(gx, Swx - Sx, XX);                       // sum w dx^2
+        float Syy = fmaf(gy, Swy - Sy, 0.25f * Sw);               // sum w dy^2
+        float Sxy = fmaf(gx, Swy, fmaf(-gy, Sx, Sxyl));           // sum w dx dy
+        float Rx = 0.f, Ry = 0.f;
+        if constexpr (NCH == 6) { Rx = fmaf(gx, Rw, -RX); Ry = fmaf(gy, Rw, -Rly); }
         Sw += __shfl_xor_sync(full, Sw, 16);   Swx += __shfl_xor_sync(full, Swx, 16);
         Swy += __shfl_xor_sync(full, Swy, 16); Sxx += __shfl_xor_sync(full, Sxx, 16);
         Sxy += __shfl_xor_sync(full, Sxy, 16); Syy += __shfl_xor_sync(full, Syy, 16);
@@ -237,6 +319,7 @@ __device__ __forceinline__ void process_window(BwdSmem<NCH, KW>& sm, const int w
         }
     }
     __syncwarp();
+    clk.lap(kPhReduce);
 }
 
 template <int NCH, int KW, int kMinBlocks>
@@ -256,6 +339,12 @@ blend_backward_kernel(const uint2* __restrict__ ranges, const float4* __restrict
     const uint2 range = ranges[tile];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
+#ifdef SB_PROBE_BLEND_PHASES
+    if (threadIdx.x == 0 && tile < kProbeMaxTiles) {
+        g_probe_cta_ns[0][tile] = globaltimer_ns();
+        g_probe_cta_ns[1][tile] = 0ull;
+    }
+#endif
     if (threadIdx.x == 0) {
         for (int s = 0; s < kStages; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], kConsumerWarps); }
         sm.nmax = 0u;
@@ -311,10 +400,14 @@ blend_backward_kernel(const uint2* __restrict__ ranges, const float4* __restrict
     st.T = T_final; st.A = 0.f; st.last_alpha = 0.f; st.last_cd = 0.f; st.A1 = 0.f; st.last_cd1 = 0.f;
     int wcount = 0;                                    // survivors in the window (warp-uniform)
     const uint32_t lt_mask = (1u << lane) - 1u;
+    PhaseClock clk;
+    clk.start();
 
     for (int k = 0; k < nb; ++k) {
         const int s = k % kStages;
+        clk.lap(kPhGather);
         mbar_wait(&sm.full[s], (k / kStages) & 1);
+        clk.lap(kPhWait);
         const int hi = m - k * kBatch, cnt = min(kBatch, hi), lo = hi - cnt;
         if (lo < (int)warp_nc) {
             for (int c = 0; c < cnt; c += 32) {
@@ -338,7 +431,7 @@ blend_backward_kernel(const uint2* __restrict__ ranges, const float4* __restrict
                     hit = hit && !take;
                     if (wcount == KW) {
                         process_window<NCH, KW>(sm, warp, lane, KW, pxf, pyf, nc, dLa, dLb, T_final, bg_dot, bg_dot1,
-                                                st, fx0, fy0, ddelx_dx, ddely_dy, accum);
+                                                st, fx0, fy0, ddelx_dx, ddely_dy, accum, clk);
                         wcount = 0;
                     }
                     mask = (ntake == nhit) ? 0u : __ballot_sync(full, hit);
@@ -350,10 +443,28 @@ blend_backward_kernel(const uint2* __restrict__ ranges, const float4* __restrict
     }
     if (wcount > 0)
         process_window<NCH, KW>(sm, warp, lane, wcount, pxf, pyf, nc, dLa, dLb, T_final, bg_dot, bg_dot1, st, fx0,
-                                fy0, ddelx_dx, ddely_dy, accum);
+                                fy0, ddelx_dx, ddely_dy, accum, clk);
+    clk.lap(kPhGather);
+    clk.flush(lane, tile);
 }
 
 }  // namespace
+
+#ifdef SB_PROBE_BLEND_PHASES
+// Instrumented build only: copies the phase totals (kNumPhases values) and the first `ntiles` CTA start / end times
+// to the host, then zeroes the totals.
+extern "C" SB_API int sb_probe_blend_phases(unsigned long long* cycles, unsigned long long* cta_start,
+                                            unsigned long long* cta_end, int ntiles) {
+    if (ntiles < 0 || ntiles > kProbeMaxTiles) return SB_ERR_BAD_ARG;
+    const size_t nt = (size_t)ntiles * sizeof(unsigned long long);
+    if (cudaMemcpyFromSymbol(cycles, g_probe_cycles, sizeof(g_probe_cycles)) != cudaSuccess ||
+        cudaMemcpyFromSymbol(cta_start, g_probe_cta_ns, nt, 0) != cudaSuccess ||
+        cudaMemcpyFromSymbol(cta_end, g_probe_cta_ns, nt, sizeof(g_probe_cta_ns[0])) != cudaSuccess)
+        return SB_ERR_CUDA;
+    const unsigned long long zero[kNumPhases] = {};
+    return cudaMemcpyToSymbol(g_probe_cycles, zero, sizeof(zero)) == cudaSuccess ? SB_OK : SB_ERR_CUDA;
+}
+#endif
 
 int launch_blend_backward(const sb_settings& s, int R, const BinningWs& b, const ImageWs& img,
                           const float* dL_dout_color, const float* dL_dout_color2, float* accum,
