@@ -8,7 +8,8 @@ OBJS := $(CSRC)/abi.o $(CSRC)/radix_sort.o $(CSRC)/project.o $(CSRC)/binning.o $
         $(CSRC)/blend_backward.o $(CSRC)/geometry_backward.o $(CSRC)/train_ops.o $(CSRC)/prepare.o $(CSRC)/sh.o \
         $(CSRC)/map_ops.o $(CSRC)/eval_metrics.o $(CSRC)/ingest.o $(CSRC)/lpips.o \
         $(CSRC)/eval_frames.o $(CSRC)/viewer.o $(CSRC)/mesh.o $(CSRC)/mesh_eval.o $(CSRC)/mesh_render.o \
-        $(CSRC)/icp.o $(CSRC)/loop.o $(CSRC)/reloc.o $(CSRC)/exposure.o $(CSRC)/dynamic.o
+        $(CSRC)/icp.o $(CSRC)/loop.o $(CSRC)/reloc.o $(CSRC)/exposure.o $(CSRC)/dynamic.o \
+        $(CSRC)/navmap.o
 LIB := splatam_b200/libsplatam_b200.so
 
 all: $(LIB) oracle

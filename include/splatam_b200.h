@@ -491,6 +491,37 @@ SB_API int sb_mc_emit(int nx, int ny, int nz, float ox, float oy, float oz, floa
                       const float* color, void* workspace, size_t workspace_bytes, float* vertices, float* colors,
                       int* faces, void* stream);
 
+/* ---- navigation maps: occupancy labels, an exact Euclidean signed distance field and distance queries
+ * (splatam_b200/navmap.py, csrc/navmap.cu; oracle/navmap_numpy.py restates every rule) ---------------------------
+ * The grid is the TSDF volume's: nz x ny x nx samples (x fastest), sample (i, j, k) at origin + voxel * (i, j, k).
+ * Every dimension is at most 8192 and the sample count below 2^31, so every finite squared distance fits in int32 and
+ * every envelope comparison in int64.  Float32 operations are rounded as written.  No host synchronisation.
+ * sb_nav_labels: labels uint8 [nz,ny,nx] from tsdf T and weight W: 0 (unknown) if W < min_weight, else 2 (occupied)
+ *   if T * trunc <= occ_dist, else 1 (free).
+ * sb_esdf: the obstacle set O is the occupied samples, and the unknown ones too when unknown_is_obstacle is 1.
+ *   sd2 int32 [nz,ny,nx] in lattice units: a sample s outside O gets +min over o in O of |s - o|^2, a sample in O
+ *   gets -min over f outside O of |s - f|^2; INT32_MAX everywhere if O is empty, -INT32_MAX everywhere if O is every
+ *   sample.  esdf float32 [nz,ny,nx] in metres: sign(sd2) * (voxel * sqrt((float)|sd2|)), the sentinels +-inf.  The
+ *   transform is exact (integer lower envelopes of parabolas along x, y, then z; workspace sb_esdf_workspace_bytes).
+ * sb_esdf_query: dist [N] and grad [N,3] of the points [N,3] in the esdf.  Per axis u = (p - o) / voxel; a point is
+ *   inside iff every u is finite and 0 <= u <= n - 1, and gets NaN distance and gradient otherwise.  i = min(floor(u),
+ *   n - 2), t = u - i.  With c_zyx the corner esdf[k + z][j + y][i + x] and lerp(a, b, t) = a + t * (b - a):
+ *     e_zy = lerp(c_zy0, c_zy1, tx);  f_z = lerp(e_z0, e_z1, ty);  dist = lerp(f_0, f_1, tz);
+ *     grad_x = lerp(lerp(c_001 - c_000, c_011 - c_010, ty), lerp(c_101 - c_100, c_111 - c_110, ty), tz) / voxel;
+ *     grad_y = lerp(e_01 - e_00, e_11 - e_10, tz) / voxel;  grad_z = (f_1 - f_0) / voxel
+ *   the exact derivative of the interpolant.  If a corner is infinite, dist is the first infinite corner in the
+ *   order c_000, c_001, c_010, ..., c_111 (x fastest) and grad is 0.
+ * SB_ERR_BAD_ARG, before any launch, for null pointers the call reads, a dimension outside [1, 8192] (the query:
+ * [2, 8192]), 2^31 or more samples, a non-finite origin, voxel, trunc, min_weight or occ_dist, a non-positive voxel or
+ * trunc, unknown_is_obstacle outside {0, 1} and N < 0; SB_ERR_WORKSPACE for a short workspace. */
+SB_API int sb_nav_labels(int nx, int ny, int nz, const float* tsdf, const float* weight, float trunc, float min_weight,
+                         float occ_dist, uint8_t* labels, void* stream);
+SB_API int sb_esdf_workspace_bytes(int nx, int ny, int nz, size_t* bytes);
+SB_API int sb_esdf(int nx, int ny, int nz, const uint8_t* labels, float voxel, int unknown_is_obstacle,
+                   void* workspace, size_t workspace_bytes, int* sd2, float* esdf, void* stream);
+SB_API int sb_esdf_query(int nx, int ny, int nz, float ox, float oy, float oz, float voxel, const float* esdf, int N,
+                         const float* points, float* dist, float* grad, void* stream);
+
 /* ---- mesh evaluation: visibility culling and exact nearest neighbours (splatam_b200/mesh_eval.py,
  * csrc/mesh_eval.cu) ---------------------------------------------------------------------------------------------
  * Float32, each operation rounded as written.  No host synchronisation.

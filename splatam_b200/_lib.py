@@ -105,6 +105,10 @@ _SIGNATURES = {
     "sb_mc_workspace_bytes": (_i, [_i, _i, _i, ctypes.POINTER(_sz)]),
     "sb_mc_count": (_i, [_i, _i, _i, _vp, _vp, _f, _vp, _sz, _vp, _vp]),
     "sb_mc_emit": (_i, [_i, _i, _i, _f, _f, _f, _f, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "sb_nav_labels": (_i, [_i, _i, _i, _vp, _vp, _f, _f, _f, _vp, _vp]),
+    "sb_esdf_workspace_bytes": (_i, [_i, _i, _i, ctypes.POINTER(_sz)]),
+    "sb_esdf": (_i, [_i, _i, _i, _vp, _f, _i, _vp, _sz, _vp, _vp, _vp]),
+    "sb_esdf_query": (_i, [_i, _i, _i, _f, _f, _f, _f, _vp, _i, _vp, _vp, _vp, _vp]),
     "sb_points_visible": (_i, [_i, _vp, _i, _i, _i, _vp, _vp, _f, _f, _f, _f, _f, _vp, _vp]),
     "sb_nn_grid_workspace_bytes": (_i, [_i, _i, _i, _i, ctypes.POINTER(_sz)]),
     "sb_nn_grid_build": (_i, [_i, _vp, _f, _f, _f, _f, _i, _i, _i, _vp, _sz, _vp]),

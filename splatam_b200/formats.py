@@ -15,6 +15,8 @@ and the 3DGS-viewer PLY export, byte-compatible with what the reference writes.
 * ``save_mesh_ply`` / ``load_mesh_ply``                      a coloured triangle mesh (splatam_b200/mesh.py) as a
   binary little-endian PLY that MeshLab and Blender open; ``load_mesh_ply`` also reads the ground-truth meshes of the
   datasets (ASCII or binary, extra properties, same-count polygons)
+* ``save_nav_map`` / ``load_nav_map``                        a navigation map (splatam_b200/navmap.py): labels, ESDF
+  and grid in one npz, read back through a checked reader
 """
 import os
 
@@ -247,6 +249,61 @@ def load_exposure(path, num_frames=None, device=None):
         return a
     import torch
     return torch.from_numpy(np.ascontiguousarray(a)).to(device)
+
+
+NAV_MAP_KEYS = ("labels", "esdf", "origin", "voxel_size", "trunc", "min_weight", "occ_dist", "unknown_is_obstacle")
+
+
+def save_nav_map(path, labels, esdf, origin, voxel_size, trunc, min_weight, occ_dist, unknown_is_obstacle):
+    """A navigation map (splatam_b200/navmap.py) as one npz: `labels` uint8 and `esdf` float32, both [nz,ny,nx];
+    `origin` float32 [3]; `voxel_size`, `trunc`, `min_weight` and `occ_dist` as 0-d float32; `unknown_is_obstacle`
+    as 0-d bool.  Returns the path."""
+    lab = np.ascontiguousarray(np.asarray(_host(labels), dtype=np.uint8))
+    e = np.ascontiguousarray(np.asarray(_host(esdf), dtype=np.float32))
+    d = os.path.dirname(os.path.abspath(path))
+    os.makedirs(d, exist_ok=True)
+    f32 = lambda x: np.array(x, dtype=np.float32)
+    with open(path, "wb") as f:
+        np.savez(f, labels=lab, esdf=e, origin=f32(origin).reshape(3), voxel_size=f32(voxel_size), trunc=f32(trunc),
+                 min_weight=f32(min_weight), occ_dist=f32(occ_dist),
+                 unknown_is_obstacle=np.array(bool(unknown_is_obstacle)))
+    return path
+
+
+def load_nav_map(path):
+    """The record of `save_nav_map` as a dict of numpy arrays (the scalars as 0-d arrays).  ValueError naming the key
+    when a key is missing, has another dtype or shape, a label is above 2, the origin is not finite, the voxel size
+    or trunc is not finite and positive, or min_weight or occ_dist is not finite."""
+    want = dict(labels=np.uint8, esdf=np.float32, origin=np.float32, voxel_size=np.float32, trunc=np.float32,
+                min_weight=np.float32, occ_dist=np.float32, unknown_is_obstacle=np.bool_)
+    with np.load(path) as z:
+        missing = [k for k in NAV_MAP_KEYS if k not in z.files]
+        if missing:
+            raise ValueError("%s lacks %s" % (path, ", ".join(missing)))
+        d = {k: np.asarray(z[k]) for k in NAV_MAP_KEYS}
+    for k, t in want.items():
+        if d[k].dtype != t:
+            raise ValueError("%s: %s has dtype %s, expected %s" % (path, k, d[k].dtype, np.dtype(t)))
+    if d["labels"].ndim != 3 or min(d["labels"].shape) < 1:
+        raise ValueError("%s: labels has shape %s, expected [nz,ny,nx]" % (path, d["labels"].shape))
+    if d["esdf"].shape != d["labels"].shape:
+        raise ValueError("%s: esdf has shape %s, labels %s" % (path, d["esdf"].shape, d["labels"].shape))
+    if d["origin"].shape != (3,):
+        raise ValueError("%s: origin has shape %s, expected (3,)" % (path, d["origin"].shape))
+    for k in ("voxel_size", "trunc", "min_weight", "occ_dist", "unknown_is_obstacle"):
+        if d[k].shape != ():
+            raise ValueError("%s: %s has shape %s, expected a scalar" % (path, k, d[k].shape))
+    if d["labels"].size and int(d["labels"].max()) > 2:
+        raise ValueError("%s: labels holds %d, above 2 (occupied)" % (path, int(d["labels"].max())))
+    if not np.all(np.isfinite(d["origin"])):
+        raise ValueError("%s: origin %s is not finite" % (path, d["origin"]))
+    for k in ("voxel_size", "trunc"):
+        if not (np.isfinite(d[k]) and d[k] > 0):
+            raise ValueError("%s: %s %r must be finite and positive" % (path, k, float(d[k])))
+    for k in ("min_weight", "occ_dist"):
+        if not np.isfinite(d[k]):
+            raise ValueError("%s: %s %r must be finite" % (path, k, float(d[k])))
+    return d
 
 
 def rgb_to_spherical_harmonic(rgb):
